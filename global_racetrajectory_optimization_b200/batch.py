@@ -40,7 +40,7 @@ _WS = {}
 
 # mirror of csrc/mincurv_ws.cuh (debugging / tests read intermediate results out of the workspace)
 SLAB_VECTORS = ("H DIAG DFW DBW LFW INVD TII RHOP RHOM PX PY NX NY MX MY XP YP SX SY KREF LB UB F "
-                "T0 T1 T2 T3 T4 T5 ALPHA LU LL RD RHS DX DD DLU DLL SU SL ISU ISL YPAD "
+                "T0 T1 T2 T3 T4 T5 ALPHA LU LL RD RHS DX DD DLU DLL SU SL ISU ISL HBSRC "
                 "S3 S4 L3 L4 KL WK EDX T3K T4K VV IH").split()
 HB_PITCH = 34
 ZB_PITCH = 108

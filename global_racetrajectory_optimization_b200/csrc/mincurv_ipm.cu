@@ -118,6 +118,13 @@ __device__ __forceinline__ uint64_t l2_evict_first_policy() {
     asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol));
     return pol;
 }
+// The band rows of H are read, not streamed: with shared centre lines every instance of a centre line reads the owner's
+// band (32 bands, 8.7 MB, for the 2112 instances of the headline batch), so they keep the normal policy and stay in L2.
+__device__ __forceinline__ uint64_t l2_evict_normal_policy() {
+    uint64_t pol;
+    asm volatile("createpolicy.fractional.L2::evict_normal.b64 %0, 1.0;" : "=l"(pol));
+    return pol;
+}
 __device__ __forceinline__ void tma_load_1d(void *dst, const void *src, unsigned bytes, uint64_t *bar, uint64_t policy) {
     asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1], %2, [%3], %4;"
                  ::"r"(smem_u32(dst)), "l"(src), "r"(bytes), "r"(smem_u32(bar)), "l"(policy) : "memory");
@@ -204,15 +211,15 @@ struct IpShared {
 // so the sweeps read nothing but the streamed units (no per-column global loads on the serial chains).  Columns
 // NA .. 8 ceil(NA / 8) - 1 are padding (pivot 1, nothing else): every unit is a full panel.
 struct Factor {
-    const double *HB;      // band of H, row i: H[i][i .. i+32], [33]: pivot H_ii + D_i (written by factor())
+    const double *HB;      // band of H, row i: H[i][i .. i+32] (read only: possibly another instance's, shared centre lines)
     const double *DD;      // barrier diagonal
     double *LT, *GT;
     int n, NA;
 };
 
-__device__ __forceinline__ Factor make_factor(double *slab, const Layout &L, int n) {
+__device__ __forceinline__ Factor make_factor(double *slab, const Layout &L, int n, const double *HB) {
     Factor F;
-    F.HB = slab + L.o_hb;
+    F.HB = HB;
     F.DD = vec(slab, L, V_DD);
     F.LT = slab + L.o_tiles;
     F.GT = F.LT + (size_t)L.np * LROW;
@@ -229,19 +236,22 @@ __device__ __forceinline__ int blk(int I, int J) { return (I * (I + 1)) / 2 + J;
 //      k0 + 32 + l); (2) eight pivots: d_j by shuffle from lane j, w = 1/d, l = v w, v_{j',j} by shuffle from lane j'
 //      for the in-panel updates; (3) trailing update W'[I][J] = W[I+1][J+1] + (L d)(L)^T on the tensor cores, which also
 //      slides the window by one block (the block row of the eight entering rows starts from zero). ----
-__device__ __noinline__ bool factor_chain(IpShared &sh, const double *__restrict__ HBp, double *__restrict__ LTp, double *__restrict__ GTp, const int NA, const double *__restrict__ g, unsigned tick) {
+__device__ __noinline__ bool factor_chain(IpShared &sh, const double *__restrict__ HBp, const double *__restrict__ DD, double *__restrict__ LTp, double *__restrict__ GTp, const int NA, const double *__restrict__ g, unsigned tick) {
     const int lane = threadIdx.x & 31;
     const int gq = lane >> 2, q = lane & 3;
     const int nunits = (NA + SUB - 1) / SUB;
-    const uint64_t pol = l2_evict_first_policy();
+    const uint64_t pol = l2_evict_normal_policy();
     double W[10][2];
 #pragma unroll
     for (int b = 0; b < 10; ++b) { W[b][0] = 0.0; W[b][1] = 0.0; }
     // right-hand side: gv = g - (L y so far) of row k0 + lane; the entering rows take their g from a block of 32 loaded a
-    // block ahead (a load issued inside the panel step would be waited for right away: the scoreboard is per warp)
+    // block ahead (a load issued inside the panel step would be waited for right away: the scoreboard is per warp).
+    // The barrier diagonal of the panel's own rows comes the same way: ddcur = D of the current block of 32 rows.
     double gv = (lane < NA) ? g[lane] : 0.0;
     double gcur = (32 + lane < NA) ? g[32 + lane] : 0.0;
     double gnext = (64 + lane < NA) ? g[64 + lane] : 0.0;
+    double ddcur = (lane < NA) ? DD[lane] : 0.0;
+    double ddnext = (32 + lane < NA) ? DD[32 + lane] : 0.0;
     bool ok = true;
     if (lane == 0) {
         mbar_expect_tx(&sh.hb_full[tick % HB_SLOTS], HB_UNIT_BYTES);
@@ -254,8 +264,10 @@ __device__ __noinline__ bool factor_chain(IpShared &sh, const double *__restrict
         SEG(8);
         if (t > 0 && (t & 3) == 0) {                  // a new block of 32 rows enters over the next four panels
             gcur = gnext;
-            const int idx = k0 + 64 + lane;
+            ddcur = ddnext;
+            const int idx = k0 + 64 + lane, idd = k0 + 32 + lane;
             gnext = (idx < NA) ? g[idx] : 0.0;
+            ddnext = (idd < NA) ? DD[idd] : 0.0;
         }
         if (lane == 0 && t + 1 < nunits) {            // band rows of the next panel (slot of panel t-1: all lanes are past it)
             const unsigned h2 = (ht + 1) % HB_SLOTS;
@@ -278,6 +290,7 @@ __device__ __noinline__ bool factor_chain(IpShared &sh, const double *__restrict
             const double2 uu = *reinterpret_cast<const double2 *>(&ho.vb[lane * VBP + j]);
             p[j] = uu.x; p[j + 1] = uu.y;
         }
+        const double ddl = __shfl_sync(FULL, ddcur, ((t & 3) << 3) + (lane & 7));     // lanes 0..7: D of row k0 + lane
         PROF_T0(tw0);
         mbar_wait(&sh.hb_full[hs], (ht / HB_SLOTS) & 1u);
         PROF_ADD(14, tw0);
@@ -288,7 +301,10 @@ __device__ __noinline__ bool factor_chain(IpShared &sh, const double *__restrict
             const int d = lane - j;                    // row k0 + lane, column k0 + j: band entry H[k0+j][d]; d = 0: the pivot (with D)
             const bool col_ok = (k0 + j < NA);
             double a1 = 0.0;
-            if (d >= 0 && row_ok && col_ok) a1 = hbg[j * HB_PITCH + ((d == 0) ? HB_PITCH - 1 : d)];
+            if (d >= 0 && row_ok && col_ok) {
+                a1 = hbg[j * HB_PITCH + d];
+                if (d == 0) a1 += ddl;
+            }
             if (d == 0 && !col_ok) a1 = 1.0;           // padding column: unit pivot
             p[j] = (d >= 0) ? a1 - p[j] : 0.0;
             const int d2 = 32 + lane - j;              // entering row k0 + 32 + lane: nonzero for j >= lane only, no updates yet
@@ -501,19 +517,16 @@ __device__ __noinline__ void factor_fill(IpShared &sh, const double *__restrict_
 //      `tick` counts the hand-off units of this CTA so far (slot / parity bookkeeping of the mbarrier rings); the caller
 //      advances it by factor_units(n) afterwards. ----
 __device__ __forceinline__ unsigned factor_units(int n) { return (unsigned)((n - 32 + SUB - 1) / SUB); }
-__device__ __noinline__ bool factor(IpShared &sh, double *slab, const Layout &L, int n, const double *g, unsigned tick) {
-    const Factor F = make_factor(slab, L, n);
+__device__ __noinline__ bool factor(IpShared &sh, double *slab, const Layout &L, int n, const double *HB, const double *g, unsigned tick) {
+    const Factor F = make_factor(slab, L, n, HB);
     const int NA = F.NA;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    double *HBw = slab + L.o_hb;
-#pragma unroll 4
-    for (int i = threadIdx.x; i < NA; i += IP_THREADS) HBw[(size_t)i * HB_PITCH + HB_PITCH - 1] = HBw[(size_t)i * HB_PITCH] + F.DD[i];
     for (int e = threadIdx.x; e < 20 * 32; e += IP_THREADS) sh.s.sfrag[e] = 0.0;
-    fence_proxy_async();        // the pivots above (generic proxy) are read by the bulk copies (async proxy)
-    __syncthreads();
+    fence_proxy_async();        // the band may have been assembled by this kernel (K2b') and the band-row slots were last
+    __syncthreads();            // used by the sweeps, both through the generic proxy; the bulk copies are the async proxy
     PROF_T0(tc0);
     if (warp == 0) {
-        if (!factor_chain(sh, F.HB, F.LT, F.GT, NA, g, tick)) sh.flag = 1;
+        if (!factor_chain(sh, F.HB, F.DD, F.LT, F.GT, NA, g, tick)) sh.flag = 1;
         PROF_ADD(1, tc0);
     } else {
         factor_fill(sh, F.HB, F.LT, F.GT, NA, g, tick);
@@ -847,7 +860,7 @@ __device__ __noinline__ void sweep_backward(IpShared &sh, const double *__restri
 // two warps concurrently: warp 1's separator reduction trails warp 0's forward sweep, then (after the separator solve)
 // warp 1's right-hand side t runs ahead of warp 0's backward sweep.
 __device__ __noinline__ void solve(IpShared &sh, double *slab, const Layout &L, int n, const double *g, double *x, bool fused) {
-    const Factor F = make_factor(slab, L, n);
+    const Factor F = make_factor(slab, L, n, nullptr);      // (the sweeps read the stored factor only)
     const int warp = threadIdx.x >> 5;
     if (threadIdx.x < 4) sh.prog[threadIdx.x] = 0;
     fence_proxy_async();        // the ring area was last accessed through the generic proxy (factor hand-off buffers)
@@ -928,7 +941,7 @@ mincurv_pdip_kernel(int B, int n_max, const int32_t *__restrict__ n_pts, double 
         }
         PROF_T0(tq0);
         double *slab = ws + (size_t)b * L.stride;
-        const double *HB = slab + L.o_hb;
+        const double *HB = ws + (size_t)*band_owner(slab, L) * L.stride + L.o_hb;      // (shared centre lines: the owner's)
         const double *__restrict__ LB = vec(slab, L, V_LB), *__restrict__ UB = vec(slab, L, V_UB), *__restrict__ F = vec(slab, L, V_F);
         double *__restrict__ AL = vec(slab, L, V_ALPHA), *__restrict__ LU = vec(slab, L, V_LU), *__restrict__ LL = vec(slab, L, V_LL), *__restrict__ RD = vec(slab, L, V_RD);
         double *__restrict__ RHS = vec(slab, L, V_RHS), *__restrict__ DX = vec(slab, L, V_DX), *__restrict__ DD = vec(slab, L, V_DD);
@@ -958,14 +971,17 @@ mincurv_pdip_kernel(int B, int n_max, const int32_t *__restrict__ n_pts, double 
         for (int i = threadIdx.x; i < n; i += IP_THREADS) {
             const double gi = G0[i];
             const double lu = fmax(-gi, 0.0) + lam0, ll = fmax(gi, 0.0) + lam0;
+            const double rd = gi + lu - ll;
             LU[i] = lu; LL[i] = ll;
-            RD[i] = gi + lu - ll;
+            RD[i] = rd;
             const double a = AL[i];
             // slacks are carried as variables of their own: recomputing ub - alpha loses them to
             // cancellation once s << eps |alpha| (late iterations), see DESIGN.md
             const double su = UB[i] - a, sl = a - LB[i];
+            const double isu = 1.0 / su, isl = 1.0 / sl;
             SU[i] = su; SL[i] = sl;
-            ISU[i] = 1.0 / su; ISL[i] = 1.0 / sl;
+            ISU[i] = isu; ISL[i] = isl;
+            DD[i] = lu * isu + ll * isl; RHS[i] = -rd + lu - ll;       // barrier diagonal, affine right-hand side
             musum += su * lu + sl * ll;
         }
         musum = block_reduce<0>(musum, sh.red);
@@ -980,28 +996,13 @@ mincurv_pdip_kernel(int B, int n_max, const int32_t *__restrict__ n_pts, double 
         // Every thread owns the elements i = tid + k * 64; the loops take them in groups of VG with all loads of a
         // group issued before the first use (the vectors live in L2/HBM: one element at a time, each trip of a loop
         // paid the full memory latency).
+        // The barrier diagonal DD = lu / su + ll / sl and the affine right-hand side RHS = -rd + lu - ll of an iteration
+        // are computed where their inputs are: by the loop above for the first iteration, by the update pass of the
+        // previous iteration for the others.
         constexpr int VG = 4, VS = VG * IP_THREADS;
         for (it = 0; it < prm.max_iter; ++it) {
-            // ---- barrier diagonal and affine right-hand side ----
-            PROF_T0(tv1);
-#pragma unroll 1
-            for (int i0 = threadIdx.x; i0 < n; i0 += VS) {
-                double lu[VG], ll[VG], isu[VG], isl[VG], rd[VG];
-#pragma unroll
-                for (int k = 0; k < VG; ++k) {
-                    const int i = min(i0 + k * IP_THREADS, n - 1);
-                    lu[k] = LU[i]; ll[k] = LL[i]; isu[k] = ISU[i]; isl[k] = ISL[i]; rd[k] = RD[i];
-                }
-#pragma unroll
-                for (int k = 0; k < VG; ++k) {
-                    const int i = i0 + k * IP_THREADS;
-                    if (i < n) { DD[i] = lu[k] * isu[k] + ll[k] * isl[k]; RHS[i] = -rd[k] + lu[k] - ll[k]; }
-                }
-            }
-            __syncthreads();
-            PROF_ADD(16, tv1);
             PROF_T0(tf0);
-            const bool fok = factor(sh, slab, L, n, RHS, tick);
+            const bool fok = factor(sh, slab, L, n, HB, RHS, tick);
             tick += factor_units(n);
             if (!fok) { result = 3; break; }
             PROF_ADD(10, tf0);
@@ -1115,8 +1116,12 @@ mincurv_pdip_kernel(int B, int n_max, const int32_t *__restrict__ n_pts, double 
                         const double sun = su[k] - ap * dx[k], sln = sl[k] + ap * dx[k];
                         // H dx = rhs - D dx  (M dx = rhs)
                         const double rdn = rd[k] + ap * (rh[k] - dd[k] * dx[k]) + ad * (dlu - dll);
+                        const double isun = 1.0 / sun, isln = 1.0 / sln;
                         AL[i] = an; LU[i] = lun; LL[i] = lln; RD[i] = rdn; SU[i] = sun; SL[i] = sln;
-                        ISU[i] = 1.0 / sun; ISL[i] = 1.0 / sln;
+                        ISU[i] = isun; ISL[i] = isln;
+                        // the next iteration's barrier diagonal and affine right-hand side (the expressions of the
+                        // initial point; unused if this iteration is the last)
+                        DD[i] = lun * isun + lln * isln; RHS[i] = -rdn + lun - lln;
                         musum2 += sun * lun + sln * lln;
                         rdmax = fmax(rdmax, fabs(rdn));
                         dxmax = fmax(dxmax, fabs(dx[k]));
@@ -1281,7 +1286,7 @@ mincurv_pdip_kappa_kernel(int B, int n_max, const int32_t *__restrict__ n_pts, d
             apply_Et(slab, L, n, VV, ETV, t0, t1, t2, t3, t4, t5);
             for (int i = threadIdx.x; i < n; i += IP_THREADS) RHS[i] = -F[i] - ETV[i];
             __syncthreads();
-            const bool fok = factor(sh, slab, L, n, RHS, tick);
+            const bool fok = factor(sh, slab, L, n, slab + L.o_hb, RHS, tick);      // (the band assembled above, own slab)
             tick += factor_units(n);
             if (!fok) {
                 // E^T W E with W = l/s -> 1e12 and beyond is no longer numerically SPD: accept a late iterate, else give up
@@ -1415,12 +1420,12 @@ debug_factor_solve_kernel(int B, int n_max, const int32_t *__restrict__ n_pts, d
         double *slab = ws + (size_t)b * L.stride;
         if (threadIdx.x == 0) sh.flag = 0;
         __syncthreads();
-        const bool ok = factor(sh, slab, L, n, vec(slab, L, V_RHS), tick);
+        const bool ok = factor(sh, slab, L, n, slab + L.o_hb, vec(slab, L, V_RHS), tick);
         tick += factor_units(n);
         solve(sh, slab, L, n, vec(slab, L, V_RHS), vec(slab, L, V_DX), true);
         solve(sh, slab, L, n, vec(slab, L, V_T0), vec(slab, L, V_T1), false);
         // a second factorisation exercises the parity bookkeeping of the rings across calls
-        const bool ok2 = factor(sh, slab, L, n, vec(slab, L, V_T0), tick);
+        const bool ok2 = factor(sh, slab, L, n, slab + L.o_hb, vec(slab, L, V_T0), tick);
         tick += factor_units(n);
         solve(sh, slab, L, n, vec(slab, L, V_T0), vec(slab, L, V_T2), true);
         if (threadIdx.x == 0) status[b] = (ok && ok2) ? 0 : 3;

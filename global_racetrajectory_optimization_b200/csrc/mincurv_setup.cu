@@ -37,6 +37,7 @@ mincurv_setup_kernel(int n_max, const int32_t *__restrict__ n_pts,
         if (threadIdx.x == 0) status[b] = -1;   // unsupported size (see N_MIN)
         return;
     }
+    if (threadIdx.x == 0) *band_owner(slab, L) = b;       // (a follower's is set by mincurv_share_kernel)
     const double wv = w_veh_batch ? w_veh_batch[b] : w_veh;
     const double *rt = reftrack + (size_t)b * n_max * 4;
     const double *nv = normvec + (size_t)b * n_max * 2;
@@ -72,8 +73,8 @@ mincurv_setup_kernel(int n_max, const int32_t *__restrict__ n_pts,
     __syncthreads();
     // Instances that share a centreline (same x, y, normals, spacing: e.g. the width variants of one track) share H, f and
     // k_ref, only the bounds differ: with centre_id the assembly runs once per centreline (the owner, centre_id[b] == b) and
-    // mincurv_share_kernel copies its result into the followers' slabs.  An owner finishes the assembly even when its own
-    // bounds are infeasible (its followers need it).
+    // mincurv_share_kernel copies its O(N) vectors into the followers' slabs; the band of H stays in the owner's slab.  An
+    // owner finishes the assembly even when its own bounds are infeasible (its followers need it).
     const bool follower = centre_id && centre_id[b] != b;
     if (s_flag || follower) {
         if (threadIdx.x == 0) status[b] = s_flag ? 1 : 0;
@@ -128,7 +129,10 @@ mincurv_setup_kernel(int n_max, const int32_t *__restrict__ n_pts,
     if (threadIdx.x == 0 && !s_flag) status[b] = 0;
 }
 
-// followers of a shared centreline: copy what the owner assembled (vectors V_H .. V_KREF, V_F, V_IH and the band of H)
+// followers of a shared centreline: copy the vectors the owner assembled (V_H .. V_KREF, V_F, V_IH) and point the
+// follower at the owner's band of H.  The band is not copied: the interior-point kernel reads it from the owner's slab,
+// so that the instances of one centre line share one copy in L2.  (The curvature-row phase assembles a weighted band in
+// the instance's own slab from the copied vectors.)
 __global__ void __launch_bounds__(256)
 mincurv_share_kernel(int B, int n_max, const int32_t *__restrict__ n_pts, const int32_t *__restrict__ centre_id,
                      double *__restrict__ ws, Layout L, int32_t *__restrict__ status) {
@@ -152,7 +156,7 @@ mincurv_share_kernel(int B, int n_max, const int32_t *__restrict__ n_pts, const 
     copy((size_t)V_H * np, (size_t)(V_KREF - V_H + 1) * np);
     copy((size_t)V_F * np, np);
     copy((size_t)V_IH * np, np);
-    copy(L.o_hb, np * HB_PITCH);
+    if (threadIdx.x == 0) *band_owner(dst, L) = o;
 }
 
 void launch_mincurv_setup(int B, int n_max, const int32_t *n_pts, const double *reftrack, const double *normvec,

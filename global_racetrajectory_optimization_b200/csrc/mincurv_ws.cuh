@@ -3,9 +3,10 @@
 // HBM layout (DESIGN.md section 3): slab b starts at ws + b * stride doubles and holds
 //   [NUM_VEC][np]        O(N) vectors (geometry, linearisation, interior-point iterates)
 //   [n_max][ZB_PITCH]    bands of B_t = Ti diag(w_t) Ti, t = 0..2  (assembly scratch, mincurv_setup.cu)
-//   [np][HB_PITCH]       band of H = E^T E              (row i: H[i][i .. i+32], cyclic)
+//   [np][HB_PITCH]       band of H = E^T E              (row i: H[i][i .. i+32], cyclic; [33] padding)
 //   [np][42] + [np][34]  bordered LDL^T factor of H + D: chain rows [Q - I | L21 | - | w] per panel of eight columns,
 //                        fill rows [G | z | w] (mincurv_ipm.cu)
+// With shared centre lines a follower's band stays in its owner's slab: V_HBSRC says whose band an instance uses.
 #pragma once
 #include "common.cuh"
 
@@ -17,7 +18,7 @@ enum Vec : int {
     V_LB, V_UB, V_F,
     V_T0, V_T1, V_T2, V_T3, V_T4, V_T5,
     V_ALPHA, V_LU, V_LL, V_RD, V_RHS, V_DX, V_DD, V_DLU, V_DLL, V_SU, V_SL,
-    V_ISU, V_ISL, V_YPAD,                                   // reciprocal slacks, padded forward-solve vector
+    V_ISU, V_ISL, V_HBSRC,                                  // reciprocal slacks, band source (band_owner)
     V_S3, V_S4, V_L3, V_L4, V_KL, V_WK, V_EDX, V_T3K, V_T4K, V_VV,   // curvature-row phase (K2b')
     V_IH,                                                   // 1 / h
     NUM_VEC
@@ -57,5 +58,9 @@ struct PdipParams {
 };
 
 __device__ __forceinline__ double *vec(double *slab, const Layout &L, int v) { return slab + (size_t)v * L.np; }
+
+// index of the instance whose slab holds this instance's band of H: its own, or with shared centre lines the owner's
+// (written by mincurv_setup_kernel / mincurv_share_kernel, read by mincurv_pdip_kernel)
+__device__ __forceinline__ int32_t *band_owner(double *slab, const Layout &L) { return reinterpret_cast<int32_t *>(vec(slab, L, V_HBSRC)); }
 
 }  // namespace mc

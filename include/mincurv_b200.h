@@ -106,7 +106,8 @@ int mc_mincurv_solve_batch_ex(int B, int n_max, const int32_t *n_pts,
 
 /* the same for batches in which several instances share a centreline (x, y, normal vectors, h and n_pts identical, only
  * the track widths / vehicle width differ -- e.g. the width variants of one track, main_globaltraj.py:264-271
- * called in a sweep): H, f and k_ref depend on the centreline only, so they are assembled once per centreline and copied.
+ * called in a sweep): H, f and k_ref depend on the centreline only, so they are assembled once per centreline; f and
+ * k_ref are copied to the followers, and the solver reads the owner's band of H (it stays in the owner's workspace slab).
  *   centre_id [B] or NULL : centre_id[b] = index (in this batch) of the instance that owns b's centreline; owners have
  *                           centre_id[b] == b.  NULL: every instance is assembled on its own.  A follower whose owner is
  *                           not an owner itself, is out of range or has another n_pts gets status -1.

@@ -22,7 +22,7 @@ import ctypes
 from global_racetrajectory_optimization_b200 import _lib
 buf = (ctypes.c_ulonglong * 24)()
 _lib.load().mc_debug_read_profile(ctypes.cast(buf, ctypes.c_void_p), 1)
-names = ["v5_update", "chain(w0)", "fwd_sweep", "sep_rhs(w1)", "sep_solve+c(w1)", "sep_ldlt", "solve_pred", "solve_corr", "bwd_sweep", "total", "factor", "nqp", "iters", "fill(w1)", "w0_wait_hb", "v4_steplen", "v1_diag_rhs", "v2_affine", "v3_corr_rhs", "w0_wait_ltempty", "w1_wait_ltfull", "w1_Supdate", "ringwait_w0", "ringwait_w1"]
+names = ["v5_update", "chain(w0)", "fwd_sweep", "sep_rhs(w1)", "sep_solve+c(w1)", "sep_ldlt", "solve_pred", "solve_corr", "bwd_sweep", "total", "factor", "nqp", "iters", "fill(w1)", "w0_wait_hb", "v4_steplen", "v1_diag_rhs(in v5_update)", "v2_affine", "v3_corr_rhs", "w0_wait_ltempty", "w1_wait_ltfull", "w1_Supdate", "ringwait_w0", "ringwait_w1"]
 vals = list(buf)
 nq = max(vals[11], 1)
 print("profile (cycles per QP of CTA 0, %d QPs, %.1f iters/QP):" % (vals[11], vals[12] / nq))
