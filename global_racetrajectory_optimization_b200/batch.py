@@ -55,7 +55,7 @@ def mincurv_slab_layout(n_max: int) -> dict:
     o_hb = o
     o += np_ * HB_PITCH
     o_tiles = o
-    o += np_ * 76
+    o += np_ * 67
     return dict(np=np_, nb_max=nb_max, o_zb=o_zb, o_hb=o_hb, o_tiles=o_tiles, stride=(o + 15) & ~15)
 
 

@@ -20,7 +20,7 @@
 // fp64 pipe, latency-bound on the in-block pivot chains and on the hand-offs between three warp roles.  Here every step offers 64 independent DFMAs per instance and eight
 // instances share an SM, so the fp64 pipe and the issue slots are what is busy.
 //
-// The factor (34 doubles per column of L and of G: 32 entries + the sweeps' per-column scalars) goes to the instance's HBM slab and
+// The factor (per column: the 32 band entries of L + w, the 32 entries of G + z, w) goes to the instance's HBM slab and
 // is streamed back by the triangular sweeps through a shared-memory ring of 8-column units filled by cp.async.bulk
 // (TMA, 1-D) on mbarriers -- the band rows of H reach warp 0 the same way.  Per iteration: factor written once, read
 // three times (the predictor's forward sweep is fused into the factorisation).
@@ -37,7 +37,7 @@ constexpr int VBP = 12;                // pitch of the row-major panel buffers (
 constexpr int FROW = 34;               // pitch of a fill row: [g (32), z, w]
 constexpr int HB_SLOTS = 2;            // band-row units of warp 0 (the next panel's is in flight)
 constexpr int HO_SLOTS = 2;            // panels between warp 0 and warp 1
-constexpr int LROW = 42;               // pitch of a chain-factor row: [Q - I (8), L21 (32), t, w]
+constexpr int LROW = 33;               // pitch of a chain-factor column: its 32 band entries of [Q - I; L21], w (see lt_slot)
 #ifndef MC_LT_SLOTS
 #define MC_LT_SLOTS 3
 #endif
@@ -45,7 +45,7 @@ constexpr int LT_SLOTS = MC_LT_SLOTS;  // sweep rings: warp 0 streams the chain 
 constexpr int GT_SLOTS = 6 - LT_SLOTS;
 constexpr int RING_UNITS = LT_SLOTS + GT_SLOTS;       // mbarriers: [0, LT_SLOTS) warp 0, [LT_SLOTS, RING_UNITS) warp 1
 constexpr int QDEPTH = 16;             // units of z (forward) / t (backward) in flight between the two warps
-constexpr int LT_UNIT_DOUBLES = SUB * LROW;           // 336
+constexpr int LT_UNIT_DOUBLES = SUB * LROW;           // 264 (2112 bytes: one bulk copy, 16-byte multiple)
 constexpr int GT_UNIT_DOUBLES = SUB * FROW;           // 272
 constexpr unsigned HB_UNIT_BYTES = SUB * HB_PITCH * sizeof(double);   // 2176
 
@@ -202,11 +202,13 @@ struct IpShared {
 };
 
 // pointers into the instance slab that the factorisation and the sweeps use.  Factor rows in HBM, one bulk copy per unit
-// of eight rows (every row 16-byte aligned):
-//   LT[k0+j] = [ (Q - I)[0..7][j], L21[0..31][j], -, w_k ]   (pitch 42) the chain factor, one panel of columns k0 .. k0+7
-//              at a time: L21 = the 32 rows of L below the panel, Q = L11^-1 the inverse of the panel's unit-lower block, so
-//              that the panel's triangular solve in the sweeps is a mat-vec too (forward: y1 = Q a1, a2 -= L21 y1;
-//              backward: u = t1 - L21^T x2, x1 = Q^T u).  t = (y - G^T x_S) w: right-hand side of the backward sweep, w = 1/d_k
+// of eight rows (every unit 16-byte aligned):
+//   LT[k0+j] = [ 32 band entries of column j of [Q - I; L21], w_k ]   (pitch 33) the chain factor, one panel of columns
+//              k0 .. k0+7 at a time: L21 = the 32 rows of L below the panel, Q = L11^-1 the inverse of the panel's
+//              unit-lower block, so that the panel's triangular solve in the sweeps is a mat-vec too (forward: y1 = Q a1,
+//              a2 -= L21 y1; backward: u = t1 - L21^T x2, x1 = Q^T u).  w = 1/d_k.  With the rows m = 0..39 of
+//              [Q - I; L21] counted from k0, column j is nonzero for j < m <= j + 32 only (Q - I strictly lower, L with 32
+//              sub-diagonals): exactly 32 entries, kept at lt_slot(j, m).  The sweeps set the other entries to zero by predicate
 //   GT[k]    = [ G[0 .. 31][k],  z_k,  w_k ]                  (pitch 34) z = w y: what the separator's forward part needs
 // so the sweeps read nothing but the streamed units (no per-column global loads on the serial chains).  Columns
 // NA .. 8 ceil(NA / 8) - 1 are padding (pivot 1, nothing else): every unit is a full panel.
@@ -226,6 +228,13 @@ __device__ __forceinline__ Factor make_factor(double *slab, const Layout &L, int
     F.n = n;
     F.NA = n - 32;
     return F;
+}
+
+// slot of entry (c, m), c < m <= c + 32, in a chain unit: the packed order m - c - 1 rotated by 4 c, so that the sweeps'
+// DMMA fragment loads (a column quartet x eight rows, or eight columns x a row quartet) fall on distinct shared-memory banks
+__device__ __forceinline__ int lt_slot(int c, int m) { return LROW * c + ((m + 3 * c - 1) & 31); }
+__device__ __forceinline__ double lt_entry(const double *unit, int c, int m) {
+    return (c < m && m <= c + 32) ? unit[lt_slot(c, m)] : 0.0;
 }
 
 __device__ __forceinline__ int blk(int I, int J) { return (I * (I + 1)) / 2 + J; }      // lower 8x8 block (I >= J) of a 4x4 block grid
@@ -318,6 +327,10 @@ __device__ __noinline__ bool factor_chain(IpShared &sh, const double *__restrict
         double dsave = 1.0, wsave = 1.0, ysave = 0.0;
         double *ltp = LTp + (size_t)k0 * LROW;
         const int wr = (lane >= 8) ? lane - 8 : 24 + lane;      // window row (after the slide) of the row this lane hands over
+        // the eight slots lt_slot(j, 8 + wr) of this lane's L21 entries, recomputed in every panel: hoisted out of the loop
+        // they took eight registers and made the loop spill
+        int wrs;
+        asm volatile("mov.b32 %0, %1;" : "=r"(wrs) : "r"(wr));
 #pragma unroll
         for (int j = 0; j < 8; ++j) {
             const double dj = __shfl_sync(FULL, p[j], j);
@@ -326,7 +339,7 @@ __device__ __noinline__ bool factor_chain(IpShared &sh, const double *__restrict
             const double w = fast_rcp(dj);
             const double lt = p[j] * w, lt2 = p2[j] * w;           // (lanes <= j: lt is not an entry of L; lanes > j: lt2 = 0)
             ho.vb[wr * VBP + j] = (lane >= 8) ? lt : lt2;
-            st_stream(ltp + j * LROW + 8 + wr, (lane >= 8) ? lt : lt2);      // L21: the 32 rows below the panel
+            if (lane >= 8 || lane <= j) st_stream(ltp + lt_slot(j, 8 + wrs), (lane >= 8) ? lt : lt2);      // L21: the band of the 32 rows below the panel
             if (lane < 8 && lane > j) ho.l11[lane * 8 + j] = lt;
             if (lane == j) { dsave = dj; wsave = w; ysave = yj; }
             gv = fma(-lt, yj, gv);                                 // (lanes <= j: gv is dead)
@@ -345,7 +358,7 @@ __device__ __noinline__ bool factor_chain(IpShared &sh, const double *__restrict
         }
         __syncwarp();
         // ---- (2b) Q = L11^-1 (the panel's unit-lower block): with it the panel's triangular solves in the sweeps are mat-vecs.
-        //      LT[k0+j] = [ (Q - I)[0..7][j], L21[0..31][j] (stored above), t, w ] ----
+        //      column j of the unit: the strictly lower part of Q's column j, L21's (stored above), w ----
         {
             const int jq = lane & 7;
             double q8[8];
@@ -357,11 +370,11 @@ __device__ __noinline__ bool factor_chain(IpShared &sh, const double *__restrict
                 q8[m] = sacc;
             }
             if (lane < 8) {
-                double *ltq = LTp + (size_t)(k0 + lane) * LROW;
+                double *ltq = ltp + 36 * lane - 1;     // + m = lt_slot(lane, m) for the rows m < 8 of Q (no wrap)
 #pragma unroll
-                for (int m = 0; m < 8; m += 2)
-                    st_stream(reinterpret_cast<double2 *>(ltq + m), make_double2((m == lane) ? 0.0 : q8[m], (m + 1 == lane) ? 0.0 : q8[m + 1]));
-                st_stream(ltq + 41, wsave);
+                for (int m = 1; m < 8; ++m)
+                    if (m > lane) st_stream(ltq + m, q8[m]);
+                st_stream(ltp + lane * LROW + 32, wsave);
             }
         }
         // ---- (3) trailing update on the tensor cores; the window slides by one block ----
@@ -672,15 +685,15 @@ __device__ __noinline__ void sweep_forward(IpShared &sh, const double *__restric
             gnext = (idx < NA) ? g[idx] : 0.0;
         }
         if ((u & 7) == 0 && u >= 8) prog_wait(sh, &sh.prog[1], u - 8);      // queue slots of units u .. u+7 are free again
-        const double *lt = R.wait(sl) + q * LROW + gq;           // A fragments: column 4 h + q of the panel, row (8 I +) gq
+        const double *lt = R.wait(sl);
         const double ge = __shfl_sync(FULL, gcur, ((u & 3) << 3) + gq);
-        double a[5][2];
+        double a[5][2];                                  // A fragments: column 4 h + q of the panel, row 8 I + gq
 #pragma unroll
         for (int I = 0; I < 5; ++I) {
-            a[I][0] = lt[8 * I];
-            a[I][1] = lt[4 * LROW + 8 * I];
+            a[I][0] = lt_entry(lt, q, 8 * I + gq);
+            a[I][1] = lt_entry(lt, 4 + q, 8 * I + gq);
         }
-        const double wl = lt[(gq - q) * LROW + 41 - gq];        // w of column k0 + gq
+        const double wl = lt[gq * LROW + 32];                    // w of column k0 + gq
         // y1 = a1 + (Q - I) a1: two independent products
         const double b0 = __shfl_sync(FULL, acc[0], 4 * q), b1 = __shfl_sync(FULL, acc[0], 16 + 4 * q);
         double y0[2] = {acc[0], acc[0]}, y1[2] = {0.0, 0.0};
@@ -822,10 +835,10 @@ __device__ __noinline__ void sweep_backward(IpShared &sh, const double *__restri
     int sl = 0, sn = AHEAD % LT_SLOTS;
     for (int i = 0; i < nunits; ++i, sl = (sl == LT_SLOTS - 1) ? 0 : sl + 1, sn = (sn == LT_SLOTS - 1) ? 0 : sn + 1) {
         const int k0 = (U0 - i) * SUB;
-        const double *lt = R.wait(sl) + gq * LROW + q;           // A fragments: column gq of the panel, row 4 c + q
-        double a[10];
+        const double *lt = R.wait(sl);
+        double a[10];                                    // A fragments: column gq of the panel, row 4 c + q
 #pragma unroll
-        for (int c = 0; c < 10; ++c) a[c] = lt[4 * c];
+        for (int c = 0; c < 10; ++c) a[c] = lt_entry(lt, gq, 4 * c + q);
         double c0[2] = {0.0, 0.0}, c1[2] = {0.0, 0.0};
 #pragma unroll
         for (int e = 2; e < 8; e += 2) {

@@ -4,7 +4,7 @@
 //   [NUM_VEC][np]        O(N) vectors (geometry, linearisation, interior-point iterates)
 //   [n_max][ZB_PITCH]    bands of B_t = Ti diag(w_t) Ti, t = 0..2  (assembly scratch, mincurv_setup.cu)
 //   [np][HB_PITCH]       band of H = E^T E              (row i: H[i][i .. i+32], cyclic; [33] padding)
-//   [np][42] + [np][34]  bordered LDL^T factor of H + D: chain rows [Q - I | L21 | - | w] per panel of eight columns,
+//   [np][33] + [np][34]  bordered LDL^T factor of H + D: chain rows [band of (Q - I; L21) | w] per panel of eight columns,
 //                        fill rows [G | z | w] (mincurv_ipm.cu)
 // With shared centre lines a follower's band stays in its owner's slab: V_HBSRC says whose band an instance uses.
 #pragma once
@@ -43,7 +43,7 @@ __host__ __device__ inline Layout make_layout(int n_max) {
     L.o_hb = o;
     o += (size_t)L.np * HB_PITCH;
     L.o_tiles = o;
-    o += (size_t)L.np * 76;
+    o += (size_t)L.np * 67;
     L.stride = (o + 15) & ~(size_t)15;
     return L;
 }
