@@ -9,10 +9,10 @@
 
 namespace mc {
 size_t spline_ws_doubles(int n_max);
-size_t pdip_smem_bytes();
 int pdip_ctas_per_sm();
 int pdip_kappa_ctas_per_sm();
-int launch_debug_factor_solve(int, int, const int32_t *, double *, const Layout &, int32_t *, cudaStream_t);
+int debug_factor_solve_ctas_per_sm();
+int launch_debug_factor_solve(int, int, const int32_t *, double *, const Layout &, int32_t *, int, cudaStream_t);
 int debug_read_profile(unsigned long long *, int);
 void launch_mincurv_setup(int, int, const int32_t *, const double *, const double *, const double *, double,
                           const double *, double, const int32_t *, double *, const Layout &, int32_t *, cudaStream_t);
@@ -133,6 +133,21 @@ static int mincurv_args(const char *who, int B, int n_max, void *workspace, size
     return MC_OK;
 }
 
+// launch shape of a persistent solver kernel: per_sm resident CTAs on every SM, but no more CTAs than instances; the counter
+// that hands out the instances sits behind the slabs
+struct SolverGrid {
+    int grid;
+    int *counter;
+};
+static SolverGrid solver_grid(int B, int n_max, void *workspace, int per_sm) {
+    int dev = 0, sms = 132;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+    int grid = sms * (per_sm > 0 ? per_sm : 1);
+    if (grid > B) grid = B;
+    return {grid, (int *)((char *)workspace + mincurv_slabs_bytes(B, n_max))};
+}
+
 int mc_mincurv_setup_batch_shared(int B, int n_max, const int32_t *n_pts, const double *reftrack, const double *normvec,
                                   const double *h, double w_veh, const double *w_veh_batch, double f_scale,
                                   const int32_t *centre_id, int32_t *status, void *workspace, size_t workspace_bytes,
@@ -176,19 +191,14 @@ int mc_mincurv_pdip_batch(int B, int n_max, const int32_t *n_pts, double *alpha,
     if (const char *e = getenv("MC_DEBUG_PDIP_ETA")) { const double v = atof(e); if (v > 0.5 && v < 1.0) prm.eta = v; }
     if (const char *e = getenv("MC_DEBUG_PDIP_DX_REL")) { const double v = atof(e); if (v >= 0.0) prm.dx_rel = v; }
     if (const char *e = getenv("MC_DEBUG_PDIP_MU_REL")) { const double v = atof(e); if (v > 0.0) prm.mu_rel = v; }   // tolerance experiments only
-    int dev = 0, sms = 132;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     int per_sm = mc::pdip_ctas_per_sm();
     if (const char *e = getenv("MC_DEBUG_PDIP_CTAS_PER_SM")) {      // occupancy experiments only (tools/prof_run.py)
         const int v = atoi(e);
         if (v > 0 && v < per_sm) per_sm = v;
     }
-    int grid = sms * (per_sm > 0 ? per_sm : 1);
-    if (grid > B) grid = B;
-    int *counter = (int *)((char *)workspace + mincurv_slabs_bytes(B, n_max));
+    const SolverGrid g = solver_grid(B, n_max, workspace, per_sm);
     if (mc::launch_mincurv_pdip(B, n_max, n_pts, (double *)workspace, mc::make_layout(n_max), prm, alpha, status, iters,
-                                grid, counter, (cudaStream_t)stream) != 0) {
+                                g.grid, g.counter, (cudaStream_t)stream) != 0) {
         snprintf(g_err, sizeof(g_err), "mincurv_pdip_kernel: cudaFuncSetAttribute failed");
         return MC_ECUDA;
     }
@@ -255,15 +265,9 @@ int mc_mincurv_kappa_batch(int B, int n_max, const int32_t *n_pts, double kappa_
     prm.eta = 0.995;
     prm.dx_rel = 0.0;
     prm.lam0_rel = 1e-2;
-    int dev = 0, sms = 132;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    const int per_sm = mc::pdip_kappa_ctas_per_sm();
-    int grid = sms * (per_sm > 0 ? per_sm : 1);
-    if (grid > B) grid = B;
-    int *counter = (int *)((char *)workspace + mincurv_slabs_bytes(B, n_max));
+    const SolverGrid g = solver_grid(B, n_max, workspace, mc::pdip_kappa_ctas_per_sm());
     if (mc::launch_mincurv_pdip_kappa(B, n_max, n_pts, (double *)workspace, mc::make_layout(n_max), prm, kappa_bound, alpha,
-                                      status, iters, grid, counter, (cudaStream_t)stream) != 0) {
+                                      status, iters, g.grid, g.counter, (cudaStream_t)stream) != 0) {
         snprintf(g_err, sizeof(g_err), "mincurv_pdip_kappa_kernel: cudaFuncSetAttribute failed");
         return MC_ECUDA;
     }
@@ -385,8 +389,6 @@ int mc_iqp_relinearise_batch(int B, int n_max, const int32_t *n_pts, const int32
     return check_cuda("calc_splines_kernel");
 }
 
-/* debug aid: cycle counters of CTA 0 of mincurv_pdip_kernel (16 x uint64): 0 A' assembly, 1 chol, 2 inverse,
- * 3 barrier A, 4 phase B, 5 barrier B, 6 solves, 7 TMA waits (forward), 9 total, 10 factor, 11 QPs, 12 IPM iterations */
 // ------------------------------------------------------------------------------------------------
 size_t mc_vel_profile_workspace_bytes(int B, int V, int n_max) {
     if (B <= 0 || V <= 0 || n_max < 2) return 0;
@@ -540,13 +542,16 @@ int mc_debug_factor_solve(int B, int n_max, const int32_t *n_pts, int32_t *statu
     if (!status) return bad("mc_debug_factor_solve: NULL argument");
     int rc = mincurv_args("mc_debug_factor_solve", B, n_max, workspace, workspace_bytes);
     if (rc) return rc;
-    if (mc::launch_debug_factor_solve(B, n_max, n_pts, (double *)workspace, mc::make_layout(n_max), status, (cudaStream_t)stream) != 0)
+    const SolverGrid g = solver_grid(B, n_max, workspace, mc::debug_factor_solve_ctas_per_sm());
+    if (mc::launch_debug_factor_solve(B, n_max, n_pts, (double *)workspace, mc::make_layout(n_max), status, g.grid,
+                                      (cudaStream_t)stream) != 0)
         return bad("mc_debug_factor_solve: cudaFuncSetAttribute failed");
     return check_cuda("debug_factor_solve_kernel");
 }
 
-int mc_debug_read_profile(unsigned long long *host_out16, int reset) {
-    return mc::debug_read_profile(host_out16, reset) == 0 ? MC_OK : MC_ECUDA;
+// debug aid: the cycle counters of CTA 0 of mincurv_pdip_kernel, slots as in enum ProfSlot of mincurv_ipm.cu
+int mc_debug_read_profile(unsigned long long *host_out24, int reset) {
+    return mc::debug_read_profile(host_out24, reset) == 0 ? MC_OK : MC_ECUDA;
 }
 
 int mc_iqp_finish_batch(int B, int n_max, int n_cap, int iter, int iters_min, double curv_error_allowed, int fixed_iters,

@@ -130,10 +130,29 @@ __device__ __forceinline__ void tma_load_1d(void *dst, const void *src, unsigned
                  ::"r"(smem_u32(dst)), "l"(src), "r"(bytes), "r"(smem_u32(bar)), "l"(policy) : "memory");
 }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async;" ::: "memory"); }
-__device__ __forceinline__ void named_bar_sync(int id, int nthreads) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory"); }
 
+// cycle counters of the instrumented build (-DMC_PROFILE), accumulated by CTA 0 and read by mc_debug_read_profile; slots
+// 3, 4 and 16 are not written.  tools/prof_run.py names the slots in this order.
+enum ProfSlot {
+    PROF_UPDATE = 0,                                     // update pass: step, residuals, next barrier diagonal and rhs
+    PROF_CHAIN = 1,                                      // factor_chain (warp 0)
+    PROF_FWD_SWEEPS = 2,                                 // sweep_forward + sweep_sep_rhs (corrector; the predictor's is fused)
+    PROF_SEP_LDLT = 5,                                   // separator block and its LDL^T
+    PROF_SOLVE_PRED = 6, PROF_SOLVE_CORR = 7,            // solve: predictor, corrector
+    PROF_BWD_SWEEPS = 8,                                 // sweep_sep_solve + sweep_backward
+    PROF_TOTAL = 9, PROF_FACTOR = 10,                    // whole instance; factor
+    PROF_NQP = 11, PROF_ITERS = 12,                      // counts: instances, interior-point iterations
+    PROF_FILL = 13,                                      // factor_fill (warp 1)
+    PROF_W0_WAIT_HB = 14,                                // warp 0 waiting for the band rows of H
+    PROF_STEPLEN = 15,                                   // corrector step lengths
+    PROF_AFFINE = 17, PROF_CORR_RHS = 18,                // affine step lengths and centring; corrector right-hand side
+    PROF_W0_WAIT_HO_EMPTY = 19, PROF_W1_WAIT_HO_FULL = 20,   // hand-off waits: warp 0 for a free slot, warp 1 for a panel
+    PROF_W1_UPDATE = 21,                                 // warp 1: trailing update of G and S
+    PROF_RING_WAIT_W0 = 22, PROF_RING_WAIT_W1 = 23,      // sweep ring waits: warp 0 (chain units), warp 1 (fill units)
+    PROF_SLOTS = 24
+};
 #ifdef MC_PROFILE
-__device__ unsigned long long g_prof[24];
+__device__ unsigned long long g_prof[PROF_SLOTS];
 #define PROF_T0(name) const long long name = clock64()
 #define PROF_ADD(slot, t0) do { if (blockIdx.x == 0 && threadIdx.x == 0) atomicAdd(&g_prof[slot], (unsigned long long)(clock64() - (t0))); } while (0)
 #define PROF_ADD1(slot, t0) do { if (blockIdx.x == 0 && threadIdx.x == 32) atomicAdd(&g_prof[slot], (unsigned long long)(clock64() - (t0))); } while (0)
@@ -164,8 +183,6 @@ __device__ __forceinline__ double fast_rcp(double d) {
     e = fma(-d, x, 1.0);
     return fma(x, e, x);
 }
-// x with its high word ANDed with m (m = 0: a denormal of magnitude < 2^-1022, i.e. zero for every purpose here;
-// m = ~0: x).  One LOP3 instead of a 64-bit select: resets the accumulators of the lane whose row enters the window.
 
 // one panel (eight columns) handed from warp 0 to warp 1
 struct Handoff {
@@ -216,18 +233,12 @@ struct Factor {
     const double *HB;      // band of H, row i: H[i][i .. i+32] (read only: possibly another instance's, shared centre lines)
     const double *DD;      // barrier diagonal
     double *LT, *GT;
-    int n, NA;
+    int NA;
 };
 
 __device__ __forceinline__ Factor make_factor(double *slab, const Layout &L, int n, const double *HB) {
-    Factor F;
-    F.HB = HB;
-    F.DD = vec(slab, L, V_DD);
-    F.LT = slab + L.o_tiles;
-    F.GT = F.LT + (size_t)L.np * LROW;
-    F.n = n;
-    F.NA = n - 32;
-    return F;
+    double *LT = slab + L.o_tiles;
+    return {HB, vec(slab, L, V_DD), LT, LT + (size_t)L.np * LROW, n - 32};
 }
 
 // slot of entry (c, m), c < m <= c + 32, in a chain unit: the packed order m - c - 1 rotated by 4 c, so that the sweeps'
@@ -245,7 +256,7 @@ __device__ __forceinline__ int blk(int I, int J) { return (I * (I + 1)) / 2 + J;
 //      k0 + 32 + l); (2) eight pivots: d_j by shuffle from lane j, w = 1/d, l = v w, v_{j',j} by shuffle from lane j'
 //      for the in-panel updates; (3) trailing update W'[I][J] = W[I+1][J+1] + (L d)(L)^T on the tensor cores, which also
 //      slides the window by one block (the block row of the eight entering rows starts from zero). ----
-__device__ __noinline__ bool factor_chain(IpShared &sh, const double *__restrict__ HBp, const double *__restrict__ DD, double *__restrict__ LTp, double *__restrict__ GTp, const int NA, const double *__restrict__ g, unsigned tick) {
+__device__ __noinline__ bool factor_chain(IpShared &sh, const double *__restrict__ HBp, const double *__restrict__ DD, double *__restrict__ LTp, const int NA, const double *__restrict__ g, unsigned tick) {
     const int lane = threadIdx.x & 31;
     const int gq = lane >> 2, q = lane & 3;
     const int nunits = (NA + SUB - 1) / SUB;
@@ -285,7 +296,7 @@ __device__ __noinline__ bool factor_chain(IpShared &sh, const double *__restrict
         }
         PROF_T0(tw1);
         if (ht >= (unsigned)HO_SLOTS) mbar_wait(&sh.ho_empty[ls], ((ht / HO_SLOTS) - 1u) & 1u);
-        PROF_ADD(19, tw1);
+        PROF_ADD(PROF_W0_WAIT_HO_EMPTY, tw1);
         Handoff &ho = sh.u.f.ho[ls];
         SEG(9);
         // ---- (1) block column 0 of the window -> row layout, through the (still free) fragment area of the hand-off slot
@@ -302,7 +313,7 @@ __device__ __noinline__ bool factor_chain(IpShared &sh, const double *__restrict
         const double ddl = __shfl_sync(FULL, ddcur, ((t & 3) << 3) + (lane & 7));     // lanes 0..7: D of row k0 + lane
         PROF_T0(tw0);
         mbar_wait(&sh.hb_full[hs], (ht / HB_SLOTS) & 1u);
-        PROF_ADD(14, tw0);
+        PROF_ADD(PROF_W0_WAIT_HB, tw0);
         const double *hbg = sh.u.f.hb[hs];
         const bool row_ok = (k0 + lane < NA), row2_ok = (lane < 8) && (k0 + 32 + lane < NA);
 #pragma unroll
@@ -414,7 +425,7 @@ __device__ __noinline__ bool factor_chain(IpShared &sh, const double *__restrict
 //      DMMA C fragments, panel by forward substitution with the panel's unit-lower block, trailing update
 //      G'[:, J] = G[:, J+1] + G_panel L^T and S -= (G_panel w) G_panel^T on the tensor cores; also the separator part of
 //      the fused forward substitution  gS -= G (w y) ----
-__device__ __noinline__ void factor_fill(IpShared &sh, const double *__restrict__ HBp, double *__restrict__ LTp, double *__restrict__ GTp, const int NA, const double *__restrict__ g, unsigned tick) {
+__device__ __noinline__ void factor_fill(IpShared &sh, const double *__restrict__ HBp, double *__restrict__ GTp, const int NA, const double *__restrict__ g, unsigned tick) {
     const int lane = threadIdx.x & 31;
     const int gq = lane >> 2, q = lane & 3;
     const int nunits = (NA + SUB - 1) / SUB;
@@ -458,7 +469,7 @@ __device__ __noinline__ void factor_fill(IpShared &sh, const double *__restrict_
         __syncwarp();
         PROF_T0(tw2);
         mbar_wait_relaxed(&sh.ho_full[ls], (ht / HO_SLOTS) & 1u);
-        PROF_ADD1(20, tw2);
+        PROF_ADD1(PROF_W1_WAIT_HO_FULL, tw2);
         const Handoff &ho = sh.u.f.ho[ls];
         // ---- the panel: g_j -= sum_{m<j} g_m L[k0+j][k0+m] ----
 #pragma unroll
@@ -520,7 +531,7 @@ __device__ __noinline__ void factor_fill(IpShared &sh, const double *__restrict_
                 *reinterpret_cast<double2 *>(&sh.s.sfrag[(blk(I, J) * 32 + lane) * 2]) = make_double2(c2[J][0], c2[J][1]);
         }
         __syncwarp();
-        PROF_ADD1(21, tw3);
+        PROF_ADD1(PROF_W1_UPDATE, tw3);
         if (lane == 0) mbar_arrive(&sh.ho_empty[ls]);
     }
     sh.gs[lane] = g[NA + lane] - gsacc;
@@ -539,11 +550,11 @@ __device__ __noinline__ bool factor(IpShared &sh, double *slab, const Layout &L,
     __syncthreads();            // used by the sweeps, both through the generic proxy; the bulk copies are the async proxy
     PROF_T0(tc0);
     if (warp == 0) {
-        if (!factor_chain(sh, F.HB, F.DD, F.LT, F.GT, NA, g, tick)) sh.flag = 1;
-        PROF_ADD(1, tc0);
+        if (!factor_chain(sh, F.HB, F.DD, F.LT, NA, g, tick)) sh.flag = 1;
+        PROF_ADD(PROF_CHAIN, tc0);
     } else {
-        factor_fill(sh, F.HB, F.LT, F.GT, NA, g, tick);
-        PROF_ADD1(13, tc0);
+        factor_fill(sh, F.HB, F.GT, NA, g, tick);
+        PROF_ADD1(PROF_FILL, tc0);
     }
     PROF_T0(tc1);
     // ---- separator: S = M[sep, sep] + D_S - G D^-1 G^T, LDL^T in place (warp 1) ----
@@ -605,34 +616,51 @@ __device__ __noinline__ bool factor(IpShared &sh, double *slab, const Layout &L,
         if (!ok) sh.flag = 1;
     }
     __syncthreads();
-    PROF_ADD(5, tc1);
+    PROF_ADD(PROF_SEP_LDLT, tc1);
     return sh.flag == 0;
 }
 
-// ---- sweep ring: one warp consumes 8-column units streamed HBM -> shared by bulk copies it issues itself ----
+// ---- sweep ring: one warp consumes the 8-column units of a factor stream in order (from unit 0 up, or from the last unit
+//      down), streamed HBM -> shared by bulk copies it issues itself; AHEAD units are in flight.  prime() before the loop;
+//      per unit i: wait(), refill(i) by lane 0 once every lane is done with the unit (the unit AHEAD further on goes into
+//      the slot of unit i - 1), next() with the loop counter: the cursors walk the slots cyclically, no modulo. ----
 template <int SLOTS, int BASE, int UNIT_DOUBLES, int WHO>
 struct RingT {
+    static constexpr int AHEAD = SLOTS - 1;
     IpShared &sh;
     double *buf;
     unsigned phase;
     uint64_t pol;
-    __device__ RingT(IpShared &s, double *b) : sh(s), buf(b), phase(s.ring_phase[WHO]), pol(l2_evict_first_policy()) {}
-    // unit -> slot `sl` (the callers walk the slots cyclically: no modulo on the serial paths)
-    __device__ __forceinline__ void issue(int unit, int sl, const double *rows) {
+    const double *rows;        // the unit stream: units 0 .. nunits - 1, taken from unit 0 up or (down) from the last one
+    int nunits, last;
+    bool down;
+    int sl, sn;                // slots of the next unit to consume and of the next refill
+    __device__ RingT(IpShared &s, double *b, const double *r, int nu, bool dn)
+        : sh(s), buf(b), phase(s.ring_phase[WHO]), pol(l2_evict_first_policy()), rows(r), nunits(nu), last(nu - 1), down(dn), sl(0), sn(AHEAD) {}
+    __device__ __forceinline__ int unit(int i) const { return down ? last - i : i; }      // the i-th unit in order
+    __device__ __forceinline__ void issue(int u, int slot) {
         const unsigned bytes = (unsigned)(UNIT_DOUBLES * sizeof(double));
-        mbar_expect_tx(&sh.ring_full[BASE + sl], bytes);
-        tma_load_1d(buf + sl * UNIT_DOUBLES, rows + (size_t)unit * UNIT_DOUBLES, bytes, &sh.ring_full[BASE + sl], pol);
+        mbar_expect_tx(&sh.ring_full[BASE + slot], bytes);
+        tma_load_1d(buf + slot * UNIT_DOUBLES, rows + (size_t)u * UNIT_DOUBLES, bytes, &sh.ring_full[BASE + slot], pol);
     }
-    __device__ __forceinline__ const double *wait(int sl) {
+    __device__ __forceinline__ void prime() {
+        if ((threadIdx.x & 31) == 0) for (int i = 0; i < AHEAD && i < nunits; ++i) issue(unit(i), i);
+    }
+    __device__ __forceinline__ const double *wait() {
 #ifdef MC_PROFILE
         const long long tw = clock64();
 #endif
         mbar_wait(&sh.ring_full[BASE + sl], (phase >> sl) & 1u);
 #ifdef MC_PROFILE
-        if (blockIdx.x == 0 && (threadIdx.x & 31) == 0) atomicAdd(&g_prof[22 + WHO], (unsigned long long)(clock64() - tw));
+        if (blockIdx.x == 0 && (threadIdx.x & 31) == 0) atomicAdd(&g_prof[PROF_RING_WAIT_W0 + WHO], (unsigned long long)(clock64() - tw));
 #endif
         phase ^= 1u << sl;
         return buf + sl * UNIT_DOUBLES;
+    }
+    __device__ __forceinline__ void refill(int i) { if (i + AHEAD < nunits) issue(down ? unit(i) - AHEAD : unit(i) + AHEAD, sn); }
+    __device__ __forceinline__ void next() {
+        sl = (sl == SLOTS - 1) ? 0 : sl + 1;
+        sn = (sn == SLOTS - 1) ? 0 : sn + 1;
     }
     __device__ __forceinline__ void close() { sh.ring_phase[WHO] = phase; }
 };
@@ -663,21 +691,18 @@ __device__ __forceinline__ void prog_wait(IpShared &sh, const int *p, int need) 
 // a[k0 + 8 I + gq], I = 0..3; B operands (a1, y1 at index 4 h + q) come by shuffle.
 // z = w y goes to warp 1 (sweep_sep_rhs runs one unit behind) through the queue sw.q, and into the fill rows (GT[k][32])
 // for the backward half of the solve.
-__device__ __noinline__ void sweep_forward(IpShared &sh, const double *__restrict__ HBp, double *__restrict__ LTp, double *__restrict__ GTp, const int NA, const double *__restrict__ g) {
+__device__ __noinline__ void sweep_forward(IpShared &sh, double *__restrict__ LTp, double *__restrict__ GTp, const int NA, const double *__restrict__ g) {
     const int lane = threadIdx.x & 31;
     const int gq = lane >> 2, q = lane & 3;
     const int nunits = (NA + SUB - 1) / SUB;
-    constexpr int AHEAD = LT_SLOTS - 1;
-    LtRing R(sh, &sh.u.sw.lt[0][0]);
-    if (lane == 0)
-        for (int u = 0; u < AHEAD && u < nunits; ++u) R.issue(u, u, LTp);
+    LtRing R(sh, &sh.u.sw.lt[0][0], LTp, nunits, false);
+    R.prime();
     double acc[4];
 #pragma unroll
     for (int I = 0; I < 4; ++I) acc[I] = (8 * I + gq < NA) ? g[8 * I + gq] : 0.0;
     double gcur = (32 + lane < NA) ? g[32 + lane] : 0.0;       // g of the rows that enter over the next four panels,
     double gnext = (64 + lane < NA) ? g[64 + lane] : 0.0;      // and the block after it (loaded a block ahead)
-    int sl = 0, sn = AHEAD % LT_SLOTS;            // slots of unit u and of unit u + AHEAD
-    for (int u = 0; u < nunits; ++u, sl = (sl == LT_SLOTS - 1) ? 0 : sl + 1, sn = (sn == LT_SLOTS - 1) ? 0 : sn + 1) {
+    for (int u = 0; u < nunits; ++u, R.next()) {
         const int k0 = u * SUB;
         if (u > 0 && (u & 3) == 0) {
             gcur = gnext;
@@ -685,7 +710,7 @@ __device__ __noinline__ void sweep_forward(IpShared &sh, const double *__restric
             gnext = (idx < NA) ? g[idx] : 0.0;
         }
         if ((u & 7) == 0 && u >= 8) prog_wait(sh, &sh.prog[1], u - 8);      // queue slots of units u .. u+7 are free again
-        const double *lt = R.wait(sl);
+        const double *lt = R.wait();
         const double ge = __shfl_sync(FULL, gcur, ((u & 3) << 3) + gq);
         double a[5][2];                                  // A fragments: column 4 h + q of the panel, row 8 I + gq
 #pragma unroll
@@ -719,28 +744,22 @@ __device__ __noinline__ void sweep_forward(IpShared &sh, const double *__restric
 #pragma unroll
         for (int I = 0; I < 4; ++I) acc[I] = nw[I];
         __syncwarp();
-        if (lane == 0) {
-            prog_publish(&sh.prog[0], u + 1);
-            if (u + AHEAD < nunits) R.issue(u + AHEAD, sn, LTp);
-        }
+        if (lane == 0) { prog_publish(&sh.prog[0], u + 1); R.refill(u); }
     }
     R.close();
     fence_proxy_async();        // z (generic-proxy stores) is read back through bulk copies (async proxy)
 }
 
 // separator part of the forward sweep (warp 1, one unit behind warp 0):  gs = g_S - G z
-__device__ __noinline__ void sweep_sep_rhs(IpShared &sh, const double *__restrict__ HBp, double *__restrict__ LTp, double *__restrict__ GTp, const int NA, const double *__restrict__ g) {
+__device__ __noinline__ void sweep_sep_rhs(IpShared &sh, double *__restrict__ GTp, const int NA, const double *__restrict__ g) {
     const int lane = threadIdx.x & 31;
     const int nunits = (NA + SUB - 1) / SUB;
-    constexpr int AHEAD = GT_SLOTS - 1;
-    GtRing R(sh, &sh.u.sw.gt[0][0]);
-    if (lane == 0)
-        for (int u = 0; u < AHEAD && u < nunits; ++u) R.issue(u, u, GTp);
+    GtRing R(sh, &sh.u.sw.gt[0][0], GTp, nunits, false);
+    R.prime();
     double s0 = 0.0, s1 = 0.0;
     const double gsl = g[NA + lane];
-    int sl = 0, sn = AHEAD % GT_SLOTS;
-    for (int u = 0; u < nunits; ++u, sl = (sl == GT_SLOTS - 1) ? 0 : sl + 1, sn = (sn == GT_SLOTS - 1) ? 0 : sn + 1) {
-        const double *gt = R.wait(sl) + lane;
+    for (int u = 0; u < nunits; ++u, R.next()) {
+        const double *gt = R.wait() + lane;
         prog_wait<true>(sh, &sh.prog[0], u + 1);
         const double *zq = &sh.u.sw.q[(u & (QDEPTH - 1)) * SUB];       // (padding columns: z = 0, g = 0)
 #pragma unroll
@@ -749,10 +768,7 @@ __device__ __noinline__ void sweep_sep_rhs(IpShared &sh, const double *__restric
             s1 = fma(gt[(s2 + 1) * FROW], zq[s2 + 1], s1);
         }
         __syncwarp();
-        if (lane == 0) {
-            prog_publish(&sh.prog[1], u + 1);
-            if (u + AHEAD < nunits) R.issue(u + AHEAD, sn, GTp);
-        }
+        if (lane == 0) { prog_publish(&sh.prog[1], u + 1); R.refill(u); }
     }
     R.close();
     sh.gs[lane] = gsl - (s0 + s1);
@@ -760,14 +776,11 @@ __device__ __noinline__ void sweep_sep_rhs(IpShared &sh, const double *__restric
 
 // separator solve and the right-hand side of the backward sweep (warp 1, ahead of warp 0's sweep_backward):
 //   x_S = S^-1 gs;   t = (y - G^T x_S) w = z - w G^T x_S, from the last unit down, handed over through the queue sw.q
-__device__ __noinline__ void sweep_sep_solve(IpShared &sh, const double *__restrict__ HBp, double *__restrict__ LTp, double *__restrict__ GTp, const int NA, double *__restrict__ x) {
+__device__ __noinline__ void sweep_sep_solve(IpShared &sh, double *__restrict__ GTp, const int NA, double *__restrict__ x) {
     const int lane = threadIdx.x & 31;
     const int nunits = (NA + SUB - 1) / SUB;
-    constexpr int AHEAD = GT_SLOTS - 1;
-    GtRing R(sh, &sh.u.sw.gt[0][0]);
-    const int U0 = nunits - 1;
-    if (lane == 0)
-        for (int i = 0; i < AHEAD && i < nunits; ++i) R.issue(U0 - i, i, GTp);
+    GtRing R(sh, &sh.u.sw.gt[0][0], GTp, nunits, true);
+    R.prime();
     double a = sh.gs[lane];
 #pragma unroll 4
     for (int k = 0; k < 32; ++k) {
@@ -788,11 +801,10 @@ __device__ __noinline__ void sweep_sep_solve(IpShared &sh, const double *__restr
     double xq[8];
 #pragma unroll
     for (int i = 0; i < 8; ++i) xq[i] = __shfl_sync(FULL, a, 8 * qr + i);
-    int sl = 0, sn = AHEAD % GT_SLOTS;
-    for (int i = 0; i < nunits; ++i, sl = (sl == GT_SLOTS - 1) ? 0 : sl + 1, sn = (sn == GT_SLOTS - 1) ? 0 : sn + 1) {
-        const int k = (U0 - i) * SUB + kl;
+    for (int i = 0; i < nunits; ++i, R.next()) {
+        const int k = R.unit(i) * SUB + kl;
         if ((i & 7) == 0 && i >= 8) prog_wait<true>(sh, &sh.prog[2], i - 8);      // queue slots of the next eight units are free again
-        const double *gt = R.wait(sl) + kl * FROW;
+        const double *gt = R.wait() + kl * FROW;
         const double2 zw = *reinterpret_cast<const double2 *>(&gt[32]);
         double c0 = 0.0, c1 = 0.0;
 #pragma unroll
@@ -806,10 +818,7 @@ __device__ __noinline__ void sweep_sep_solve(IpShared &sh, const double *__restr
         c += __shfl_xor_sync(FULL, c, 16);
         if (qr == 0) sh.u.sw.q[(i & (QDEPTH - 1)) * SUB + kl] = (k < NA) ? fma(-c, zw.y, zw.x) : 0.0;      // (padding rows: t = 0)
         __syncwarp();
-        if (lane == 0) {
-            prog_publish(&sh.prog[3], i + 1);
-            if (i + AHEAD < nunits) R.issue(U0 - i - AHEAD, sn, GTp);
-        }
+        if (lane == 0) { prog_publish(&sh.prog[3], i + 1); R.refill(i); }
     }
     R.close();
 }
@@ -820,22 +829,18 @@ __device__ __noinline__ void sweep_sep_solve(IpShared &sh, const double *__restr
 // x's come out in C layout (lane (gq, .): row k0 + gq) and move over by shuffle.  Only the two products with the previous
 // panel's x and the two with u are on the chain from panel to panel; the other six are issued ahead of them.
 // t comes from warp 1 (sweep_sep_solve, running ahead) through the queue sw.q.
-__device__ __noinline__ void sweep_backward(IpShared &sh, const double *__restrict__ HBp, double *__restrict__ LTp, double *__restrict__ GTp, const int NA, double *__restrict__ x) {
+__device__ __noinline__ void sweep_backward(IpShared &sh, double *__restrict__ LTp, const int NA, double *__restrict__ x) {
     const int lane = threadIdx.x & 31;
     const int gq = lane >> 2, q = lane & 3;
     const int nunits = (NA + SUB - 1) / SUB;
-    constexpr int AHEAD = LT_SLOTS - 1;
-    LtRing R(sh, &sh.u.sw.lt[0][0]);
-    const int U0 = nunits - 1;
-    if (lane == 0)
-        for (int i = 0; i < AHEAD && i < nunits; ++i) R.issue(U0 - i, i, LTp);
+    LtRing R(sh, &sh.u.sw.lt[0][0], LTp, nunits, true);
+    R.prime();
     double nbx[8];
 #pragma unroll
     for (int i = 0; i < 8; ++i) nbx[i] = 0.0;
-    int sl = 0, sn = AHEAD % LT_SLOTS;
-    for (int i = 0; i < nunits; ++i, sl = (sl == LT_SLOTS - 1) ? 0 : sl + 1, sn = (sn == LT_SLOTS - 1) ? 0 : sn + 1) {
-        const int k0 = (U0 - i) * SUB;
-        const double *lt = R.wait(sl);
+    for (int i = 0; i < nunits; ++i, R.next()) {
+        const int k0 = R.unit(i) * SUB;
+        const double *lt = R.wait();
         double a[10];                                    // A fragments: column gq of the panel, row 4 c + q
 #pragma unroll
         for (int c = 0; c < 10; ++c) a[c] = lt_entry(lt, gq, 4 * c + q);
@@ -861,10 +866,7 @@ __device__ __noinline__ void sweep_backward(IpShared &sh, const double *__restri
         nbx[0] = -__shfl_sync(FULL, x1, 4 * q);
         nbx[1] = -__shfl_sync(FULL, x1, 16 + 4 * q);
         __syncwarp();
-        if (lane == 0) {
-            prog_publish(&sh.prog[2], i + 1);
-            if (i + AHEAD < nunits) R.issue(U0 - i - AHEAD, sn, LTp);
-        }
+        if (lane == 0) { prog_publish(&sh.prog[2], i + 1); R.refill(i); }
     }
     R.close();
 }
@@ -880,16 +882,16 @@ __device__ __noinline__ void solve(IpShared &sh, double *slab, const Layout &L, 
     __syncthreads();
     if (!fused) {
         PROF_T0(t0);
-        if (warp == 0) sweep_forward(sh, F.HB, F.LT, F.GT, F.NA, g);
-        else sweep_sep_rhs(sh, F.HB, F.LT, F.GT, F.NA, g);
+        if (warp == 0) sweep_forward(sh, F.LT, F.GT, F.NA, g);
+        else sweep_sep_rhs(sh, F.GT, F.NA, g);
         __syncthreads();
-        PROF_ADD1(2, t0);
+        PROF_ADD1(PROF_FWD_SWEEPS, t0);
     }
     PROF_T0(t3);
-    if (warp == 1) sweep_sep_solve(sh, F.HB, F.LT, F.GT, F.NA, x);
-    else sweep_backward(sh, F.HB, F.LT, F.GT, F.NA, x);
+    if (warp == 1) sweep_sep_solve(sh, F.GT, F.NA, x);
+    else sweep_backward(sh, F.LT, F.NA, x);
     __syncthreads();
-    PROF_ADD1(8, t3);
+    PROF_ADD1(PROF_BWD_SWEEPS, t3);
 }
 
 // banded cyclic mat-vec out = H v (real-indexed)
@@ -911,7 +913,10 @@ __device__ void band_matvec(const double *__restrict__ HB, const double *__restr
     }
 }
 
-__device__ __forceinline__ void ip_init_shared(IpShared &sh) {
+// the CTA's state in dynamic shared memory, its mbarriers initialised
+__device__ __forceinline__ IpShared &ip_init_shared() {
+    extern __shared__ __align__(16) unsigned char smem_raw[];
+    IpShared &sh = *reinterpret_cast<IpShared *>(smem_raw);
     if (threadIdx.x == 0) {
         for (int i = 0; i < HB_SLOTS; ++i) mbar_init(&sh.hb_full[i], 1);
         for (int i = 0; i < HO_SLOTS; ++i) { mbar_init(&sh.ho_full[i], 1); mbar_init(&sh.ho_empty[i], 1); }
@@ -920,14 +925,43 @@ __device__ __forceinline__ void ip_init_shared(IpShared &sh) {
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     __syncthreads();
+    return sh;
 }
+
+// the next instance for this CTA: handed out dynamically (iteration counts differ between instances)
+__device__ __forceinline__ int next_instance(IpShared &sh, int *work_counter) {
+    __syncthreads();
+    if (threadIdx.x == 0) sh.next = atomicAdd(work_counter, 1);
+    __syncthreads();
+    return sh.next;
+}
+
+// alpha, status and the iteration count of instance b (the curvature-row phase adds its iterations to the box phase's)
+template <bool ADD_ITERS>
+__device__ __forceinline__ void write_instance(double *aout, int n, int n_max, const double *AL, int b, int result, int it,
+                                               int32_t *status, int32_t *iters_out) {
+    __syncthreads();
+    for (int i = threadIdx.x; i < n_max; i += IP_THREADS) aout[i] = (i < n) ? AL[i] : 0.0;
+    if (threadIdx.x == 0) {
+        status[b] = result;
+        if (iters_out) iters_out[b] = ADD_ITERS ? iters_out[b] + it : it;
+    }
+}
+
+// ---- Mehrotra's scalar steps: the affine step length min(1, 1 / max-ratio); the centring target sigma mu with
+//      sigma = (mu_aff / mu)^3, mu_aff = the complementarity after the affine step, a polynomial in (ap, ad), over m products;
+//      the damped step length min(1, eta / max-ratio) ----
+__device__ __forceinline__ double affine_step(double r) { return (r > 1.0) ? 1.0 / r : 1.0; }
+__device__ __forceinline__ double centring(double c00, double c01, double c10, double c11, double ap, double ad, double mu, double m) {
+    const double sigma = (c00 + ad * c01 + ap * c10 + ap * ad * c11) / m / mu;
+    return sigma * sigma * sigma * mu;
+}
+__device__ __forceinline__ double damped_step(double eta, double r) { return (eta < r) ? eta / r : 1.0; }
 
 __global__ void __launch_bounds__(IP_THREADS, 8)
 mincurv_pdip_kernel(int B, int n_max, const int32_t *__restrict__ n_pts, double *__restrict__ ws, Layout L,
                     PdipParams prm, double *__restrict__ alpha_out, int32_t *__restrict__ status,
                     int32_t *__restrict__ iters_out, int *__restrict__ work_counter) {
-    extern __shared__ __align__(16) unsigned char smem_raw[];
-    IpShared &sh = *reinterpret_cast<IpShared *>(smem_raw);
 #ifdef MC_DEBUG_SM_LIMIT       // contention experiments: only the first MC_DEBUG_SM_LIMIT SMs take work (full occupancy on those)
     {
         unsigned smid;
@@ -935,16 +969,9 @@ mincurv_pdip_kernel(int B, int n_max, const int32_t *__restrict__ n_pts, double 
         if (smid >= MC_DEBUG_SM_LIMIT) return;
     }
 #endif
-    ip_init_shared(sh);
+    IpShared &sh = ip_init_shared();
     unsigned tick = 0;      // hand-off units of the factorisations so far (uniform across the CTA)
-
-    for (;;) {
-        // instances are handed out dynamically (iteration counts differ between instances)
-        __syncthreads();
-        if (threadIdx.x == 0) sh.next = atomicAdd(work_counter, 1);
-        __syncthreads();
-        const int b = sh.next;
-        if (b >= B) break;
+    for (int b; (b = next_instance(sh, work_counter)) < B;) {
         const int n = n_pts ? n_pts[b] : n_max;
         double *aout = alpha_out + (size_t)b * n_max;
         if (status[b] != 0) {
@@ -1018,10 +1045,10 @@ mincurv_pdip_kernel(int B, int n_max, const int32_t *__restrict__ n_pts, double 
             const bool fok = factor(sh, slab, L, n, HB, RHS, tick);
             tick += factor_units(n);
             if (!fok) { result = 3; break; }
-            PROF_ADD(10, tf0);
+            PROF_ADD(PROF_FACTOR, tf0);
             PROF_T0(ts0);
             solve(sh, slab, L, n, RHS, DX, true);
-            PROF_ADD(6, ts0);
+            PROF_ADD(PROF_SOLVE_PRED, ts0);
             // ---- affine direction: step lengths 1 / max-ratio; mu_aff as a polynomial in (ap, ad) ----
             PROF_T0(tv2);
             double rp = 0.0, rdl = 0.0, c00 = 0.0, c01 = 0.0, c10 = 0.0, c11 = 0.0;
@@ -1049,14 +1076,11 @@ mincurv_pdip_kernel(int B, int n_max, const int32_t *__restrict__ n_pts, double 
             }
             rp = block_reduce<1>(rp, sh.red);
             rdl = block_reduce<1>(rdl, sh.red);
-            double ap = (rp > 1.0) ? 1.0 / rp : 1.0, ad = (rdl > 1.0) ? 1.0 / rdl : 1.0;
+            double ap = affine_step(rp), ad = affine_step(rdl);
             c00 = block_reduce<0>(c00, sh.red); c01 = block_reduce<0>(c01, sh.red);
             c10 = block_reduce<0>(c10, sh.red); c11 = block_reduce<0>(c11, sh.red);
-            const double mua = (c00 + ad * c01 + ap * c10 + ap * ad * c11) / (2.0 * n);
-            double sigma = mua / mu;
-            sigma = sigma * sigma * sigma;
-            const double smu = sigma * mu;
-            PROF_ADD(17, tv2);
+            const double smu = centring(c00, c01, c10, c11, ap, ad, mu, 2.0 * n);
+            PROF_ADD(PROF_AFFINE, tv2);
             PROF_T0(tv3);
             // ---- corrector right-hand side ----
 #pragma unroll 1
@@ -1080,10 +1104,10 @@ mincurv_pdip_kernel(int B, int n_max, const int32_t *__restrict__ n_pts, double 
                 }
             }
             __syncthreads();
-            PROF_ADD(18, tv3);
+            PROF_ADD(PROF_CORR_RHS, tv3);
             PROF_T0(ts1);
             solve(sh, slab, L, n, RHS, DX, false);
-            PROF_ADD(7, ts1);
+            PROF_ADD(PROF_SOLVE_CORR, ts1);
             PROF_T0(tv4);
             rp = 0.0; rdl = 0.0;
 #pragma unroll 1
@@ -1105,9 +1129,9 @@ mincurv_pdip_kernel(int B, int n_max, const int32_t *__restrict__ n_pts, double 
             }
             rp = block_reduce<1>(rp, sh.red);
             rdl = block_reduce<1>(rdl, sh.red);
-            ap = (prm.eta < rp) ? prm.eta / rp : 1.0;       // min(1, eta / max-ratio)
-            ad = (prm.eta < rdl) ? prm.eta / rdl : 1.0;
-            PROF_ADD(15, tv4);
+            ap = damped_step(prm.eta, rp);
+            ad = damped_step(prm.eta, rdl);
+            PROF_ADD(PROF_STEPLEN, tv4);
             PROF_T0(tv5);
             double musum2 = 0.0, rdmax = 0.0, dxmax = 0.0, amax = 0.0;
             constexpr int VG2 = 2, VS2 = VG2 * IP_THREADS;        // 13 input vectors: groups of two
@@ -1144,7 +1168,7 @@ mincurv_pdip_kernel(int B, int n_max, const int32_t *__restrict__ n_pts, double 
             }
             mu = block_reduce<0>(musum2, sh.red) / (2.0 * n);
             rdmax = block_reduce<1>(rdmax, sh.red);
-            PROF_ADD(0, tv5);
+            PROF_ADD(PROF_UPDATE, tv5);
             // weakly active bounds converge like sqrt(mu): also require that the step itself has become small
             bool settled = true;
             if (prm.dx_rel > 0.0 && mu <= prm.mu_rel * mu0) {
@@ -1155,26 +1179,18 @@ mincurv_pdip_kernel(int B, int n_max, const int32_t *__restrict__ n_pts, double 
             if (mu <= prm.mu_rel * mu0 && rdmax <= rd_tol && settled) { result = 0; ++it; break; }
             if (mu <= 1e-4 * prm.mu_rel * mu0) { result = (rdmax <= 1e3 * rd_tol) ? 0 : 2; ++it; break; }   // complementarity exhausted
         }
-        __syncthreads();
-        for (int i = threadIdx.x; i < n_max; i += IP_THREADS) aout[i] = (i < n) ? AL[i] : 0.0;
-        if (threadIdx.x == 0) {
-            status[b] = result;
-            if (iters_out) iters_out[b] = it;
-        }
-        PROF_ADD(9, tq0);
+        write_instance<false>(aout, n, n_max, AL, b, result, it, status, iters_out);
+        PROF_ADD(PROF_TOTAL, tq0);
 #ifdef MC_PROFILE
-        if (blockIdx.x == 0 && threadIdx.x == 0) { atomicAdd(&g_prof[11], 1ull); atomicAdd(&g_prof[12], (unsigned long long)it); }
+        if (blockIdx.x == 0 && threadIdx.x == 0) { atomicAdd(&g_prof[PROF_NQP], 1ull); atomicAdd(&g_prof[PROF_ITERS], (unsigned long long)it); }
 #endif
     }
 }
 
-size_t pdip_smem_bytes() { return sizeof(IpShared); }
-
 int debug_read_profile(unsigned long long *host_out, int reset) {
 #ifdef MC_PROFILE
-    if (cudaMemcpyFromSymbol(host_out, g_prof, sizeof(unsigned long long) * 24) != cudaSuccess) return -1;
-    if (const char *e = getenv("MC_PROFILE_SEGMENTS")) {       // tools/prof_run.py: sub-phase counters of one panel
-        (void)e;
+    if (cudaMemcpyFromSymbol(host_out, g_prof, sizeof(unsigned long long) * PROF_SLOTS) != cudaSuccess) return -1;
+    if (getenv("MC_PROFILE_SEGMENTS")) {       // tools/prof_run.py: sub-phase counters of one panel
         unsigned long long seg[32];
         if (cudaMemcpyFromSymbol(seg, g_seg, sizeof(seg)) == cudaSuccess) {
             fprintf(stderr, "segments:");
@@ -1184,13 +1200,13 @@ int debug_read_profile(unsigned long long *host_out, int reset) {
     }
     if (reset) {
         unsigned long long z[32] = {0};
-        if (cudaMemcpyToSymbol(g_prof, z, sizeof(unsigned long long) * 24) != cudaSuccess) return -1;
+        if (cudaMemcpyToSymbol(g_prof, z, sizeof(unsigned long long) * PROF_SLOTS) != cudaSuccess) return -1;
         cudaMemcpyToSymbol(g_seg, z, sizeof(z));
     }
     return 0;
 #else
     (void)reset;
-    for (int i = 0; i < 24; ++i) host_out[i] = 0ull;
+    for (int i = 0; i < PROF_SLOTS; ++i) host_out[i] = 0ull;
     return 0;
 #endif
 }
@@ -1203,16 +1219,22 @@ static int ctas_per_sm(K kernel) {
     return nb > 0 ? nb : 1;
 }
 
+// launches a solver kernel (CTA state in dynamic shared memory); its work counter, if it has one, starts from zero
+template <typename... P, typename... A>
+static int launch_solver(void (*kernel)(P...), int grid, int *work_counter, cudaStream_t stream, A... args) {
+    // (per launch: the attribute is per device and a process may drive several)
+    cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(IpShared));
+    if (e != cudaSuccess) return (int)e;
+    if (work_counter) cudaMemsetAsync(work_counter, 0, sizeof(int), stream);
+    kernel<<<grid, IP_THREADS, sizeof(IpShared), stream>>>(args...);
+    return 0;
+}
+
 int pdip_ctas_per_sm() { return ctas_per_sm(mincurv_pdip_kernel); }
 
 int launch_mincurv_pdip(int B, int n_max, const int32_t *n_pts, double *ws, const Layout &L, const PdipParams &prm,
                         double *alpha, int32_t *status, int32_t *iters, int grid, int *work_counter, cudaStream_t stream) {
-    // (per launch: the attribute is per device and a process may drive several)
-    cudaError_t e = cudaFuncSetAttribute(mincurv_pdip_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(IpShared));
-    if (e != cudaSuccess) return (int)e;
-    cudaMemsetAsync(work_counter, 0, sizeof(int), stream);
-    mincurv_pdip_kernel<<<grid, IP_THREADS, sizeof(IpShared), stream>>>(B, n_max, n_pts, ws, L, prm, alpha, status, iters, work_counter);
-    return 0;
+    return launch_solver(mincurv_pdip_kernel, grid, work_counter, stream, B, n_max, n_pts, ws, L, prm, alpha, status, iters, work_counter);
 }
 
 // ================================================================================================
@@ -1227,16 +1249,9 @@ __global__ void __launch_bounds__(IP_THREADS, 8)
 mincurv_pdip_kappa_kernel(int B, int n_max, const int32_t *__restrict__ n_pts, double *__restrict__ ws, Layout L,
                           PdipParams prm, double kb, double *__restrict__ alpha_out, int32_t *__restrict__ status,
                           int32_t *__restrict__ iters_out, int *__restrict__ work_counter) {
-    extern __shared__ __align__(16) unsigned char smem_raw[];
-    IpShared &sh = *reinterpret_cast<IpShared *>(smem_raw);
-    ip_init_shared(sh);
+    IpShared &sh = ip_init_shared();
     unsigned tick = 0;
-    for (;;) {
-        __syncthreads();
-        if (threadIdx.x == 0) sh.next = atomicAdd(work_counter, 1);
-        __syncthreads();
-        const int b = sh.next;
-        if (b >= B) break;
+    for (int b; (b = next_instance(sh, work_counter)) < B;) {
         if (status[b] != 4) continue;
         const int n = n_pts ? n_pts[b] : n_max;
         double *aout = alpha_out + (size_t)b * n_max;
@@ -1326,13 +1341,10 @@ mincurv_pdip_kappa_kernel(int B, int n_max, const int32_t *__restrict__ n_pts, d
             }
             rp = block_reduce<1>(rp, sh.red);
             rdl = block_reduce<1>(rdl, sh.red);
-            double ap = (rp > 1.0) ? 1.0 / rp : 1.0, ad = (rdl > 1.0) ? 1.0 / rdl : 1.0;
+            double ap = affine_step(rp), ad = affine_step(rdl);
             c00 = block_reduce<0>(c00, sh.red); c01 = block_reduce<0>(c01, sh.red);
             c10 = block_reduce<0>(c10, sh.red); c11 = block_reduce<0>(c11, sh.red);
-            const double mua = (c00 + ad * c01 + ap * c10 + ap * ad * c11) / m4;
-            double sigma = mua / mu;
-            sigma = sigma * sigma * sigma;
-            const double smu = sigma * mu;
+            const double smu = centring(c00, c01, c10, c11, ap, ad, mu, m4);
             // ---- corrector right-hand side ----
             for (int i = threadIdx.x; i < n; i += IP_THREADS) {
                 const double su = SU[i], sl = SL[i], lu = LU[i], ll = LL[i], dx = DX[i], isu = ISU[i], isl = ISL[i];
@@ -1365,8 +1377,8 @@ mincurv_pdip_kappa_kernel(int B, int n_max, const int32_t *__restrict__ n_pts, d
             }
             rp = block_reduce<1>(rp, sh.red);
             rdl = block_reduce<1>(rdl, sh.red);
-            ap = (prm.eta < rp) ? prm.eta / rp : 1.0;
-            ad = (prm.eta < rdl) ? prm.eta / rdl : 1.0;
+            ap = damped_step(prm.eta, rp);
+            ad = damped_step(prm.eta, rdl);
             double musum2 = 0.0;
             rpmax = 0.0;
             for (int i = threadIdx.x; i < n; i += IP_THREADS) {
@@ -1395,24 +1407,15 @@ mincurv_pdip_kappa_kernel(int B, int n_max, const int32_t *__restrict__ n_pts, d
             if (mu <= prm.mu_rel * mu0 && rdmax <= rd_tol && rpmax <= 1e-8 * kb) { result = 0; ++it; break; }
             if (mu <= 1e-2 * prm.mu_rel * mu0) { result = (rdmax <= 1e3 * rd_tol && rpmax <= 1e-6 * kb) ? 0 : 2; ++it; break; }
         }
-        __syncthreads();
-        for (int i = threadIdx.x; i < n_max; i += IP_THREADS) aout[i] = (i < n) ? AL[i] : 0.0;
-        if (threadIdx.x == 0) {
-            status[b] = result;
-            if (iters_out) iters_out[b] += it;
-        }
+        write_instance<true>(aout, n, n_max, AL, b, result, it, status, iters_out);
     }
 }
 
 int launch_mincurv_pdip_kappa(int B, int n_max, const int32_t *n_pts, double *ws, const Layout &L, const PdipParams &prm,
                               double kappa_bound, double *alpha, int32_t *status, int32_t *iters, int grid, int *work_counter,
                               cudaStream_t stream) {
-    cudaError_t e = cudaFuncSetAttribute(mincurv_pdip_kappa_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(IpShared));
-    if (e != cudaSuccess) return (int)e;
-    cudaMemsetAsync(work_counter, 0, sizeof(int), stream);
-    mincurv_pdip_kappa_kernel<<<grid, IP_THREADS, sizeof(IpShared), stream>>>(B, n_max, n_pts, ws, L, prm, kappa_bound, alpha,
-                                                                             status, iters, work_counter);
-    return 0;
+    return launch_solver(mincurv_pdip_kappa_kernel, grid, work_counter, stream, B, n_max, n_pts, ws, L, prm, kappa_bound, alpha, status,
+                         iters, work_counter);
 }
 
 int pdip_kappa_ctas_per_sm() { return ctas_per_sm(mincurv_pdip_kappa_kernel); }
@@ -1424,9 +1427,7 @@ int pdip_kappa_ctas_per_sm() { return ctas_per_sm(mincurv_pdip_kappa_kernel); }
 __global__ void __launch_bounds__(IP_THREADS, 8)
 debug_factor_solve_kernel(int B, int n_max, const int32_t *__restrict__ n_pts, double *__restrict__ ws, Layout L,
                           int32_t *__restrict__ status) {
-    extern __shared__ __align__(16) unsigned char smem_raw[];
-    IpShared &sh = *reinterpret_cast<IpShared *>(smem_raw);
-    ip_init_shared(sh);
+    IpShared &sh = ip_init_shared();
     unsigned tick = 0;
     for (int b = blockIdx.x; b < B; b += gridDim.x) {
         const int n = n_pts ? n_pts[b] : n_max;
@@ -1446,12 +1447,10 @@ debug_factor_solve_kernel(int B, int n_max, const int32_t *__restrict__ n_pts, d
     }
 }
 
-int launch_debug_factor_solve(int B, int n_max, const int32_t *n_pts, double *ws, const Layout &L, int32_t *status, cudaStream_t stream) {
-    cudaError_t e = cudaFuncSetAttribute(debug_factor_solve_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(IpShared));
-    if (e != cudaSuccess) return (int)e;
-    const int grid = B < 1056 ? B : 1056;          // 132 SMs x 8 resident CTAs on an H100
-    debug_factor_solve_kernel<<<grid, IP_THREADS, sizeof(IpShared), stream>>>(B, n_max, n_pts, ws, L, status);
-    return 0;
+int debug_factor_solve_ctas_per_sm() { return ctas_per_sm(debug_factor_solve_kernel); }
+
+int launch_debug_factor_solve(int B, int n_max, const int32_t *n_pts, double *ws, const Layout &L, int32_t *status, int grid, cudaStream_t stream) {
+    return launch_solver(debug_factor_solve_kernel, grid, nullptr, stream, B, n_max, n_pts, ws, L, status);
 }
 
 }  // namespace mc

@@ -20,12 +20,16 @@ print("prof_run", Bn, N, f"{dt*1e3:.2f} ms {Bn/dt:.0f} QP/s status", np.bincount
 
 import ctypes
 from global_racetrajectory_optimization_b200 import _lib
+# the written slots of the cycle counters, in the order of enum ProfSlot in csrc/mincurv_ipm.cu
+PROF_TOTAL, PROF_NQP, PROF_ITERS = 9, 11, 12
+CYCLE_SLOTS = [(0, "update"), (1, "chain(w0)"), (2, "fwd_sweeps"), (5, "sep_ldlt"), (6, "solve_pred"), (7, "solve_corr"),
+               (8, "bwd_sweeps"), (9, "total"), (10, "factor"), (13, "fill(w1)"), (14, "w0_wait_hb"), (15, "steplen"),
+               (17, "affine"), (18, "corr_rhs"), (19, "w0_wait_ho_empty"), (20, "w1_wait_ho_full"), (21, "w1_update"),
+               (22, "ringwait_w0"), (23, "ringwait_w1")]
 buf = (ctypes.c_ulonglong * 24)()
 _lib.load().mc_debug_read_profile(ctypes.cast(buf, ctypes.c_void_p), 1)
-names = ["v5_update", "chain(w0)", "fwd_sweep", "sep_rhs(w1)", "sep_solve+c(w1)", "sep_ldlt", "solve_pred", "solve_corr", "bwd_sweep", "total", "factor", "nqp", "iters", "fill(w1)", "w0_wait_hb", "v4_steplen", "v1_diag_rhs(in v5_update)", "v2_affine", "v3_corr_rhs", "w0_wait_ltempty", "w1_wait_ltfull", "w1_Supdate", "ringwait_w0", "ringwait_w1"]
 vals = list(buf)
-nq = max(vals[11], 1)
-print("profile (cycles per QP of CTA 0, %d QPs, %.1f iters/QP):" % (vals[11], vals[12] / nq))
-for k, nm in enumerate(names):
-    if nm != "-" and (k < 11 or k > 12):
-        print("  %-9s %12.0f  %5.1f%%" % (nm, vals[k] / nq, 100.0 * vals[k] / max(vals[9], 1)))
+nq = max(vals[PROF_NQP], 1)
+print("profile (cycles per QP of CTA 0, %d QPs, %.1f iters/QP):" % (vals[PROF_NQP], vals[PROF_ITERS] / nq))
+for k, nm in CYCLE_SLOTS:
+    print("  %-16s %12.0f  %5.1f%%" % (nm, vals[k] / nq, 100.0 * vals[k] / max(vals[PROF_TOTAL], 1)))
