@@ -227,6 +227,133 @@ def shared_centre_ids(group: torch.Tensor) -> torch.Tensor:
     return first[inv].to(torch.int32)
 
 
+def _chunk_centre_ids(centre_id, s, e, B):
+    # owners are addressed inside the chunk: the first instance of the chunk with the same owner takes the role
+    if centre_id is None:
+        return None
+    return centre_id if (s == 0 and e == B) else shared_centre_ids(centre_id[s:e])
+
+
+class _MinCurvDiff(torch.autograd.Function):
+    """alpha of the min-curvature QP as a function of the widths; see opt_min_curv_diff."""
+
+    @staticmethod
+    def forward(ctx, widths, w_veh_t, centre, normvec, h, kappa_bound, w_scalar, n_pts, centre_id, chunk, f_scale, strict):
+        lib = _lib.load()
+        B, n_max, _ = centre.shape
+        dev = centre.device
+        reftrack = torch.cat((centre, widths), dim=2).contiguous()
+        alpha = torch.empty((B, n_max), dtype=torch.float64, device=dev)
+        cerr = torch.empty((B,), dtype=torch.float64, device=dev)
+        kmax = torch.empty((B,), dtype=torch.float64, device=dev)
+        status = torch.empty((B,), dtype=torch.int32, device=dev)
+        iters = torch.empty((B,), dtype=torch.int32, device=dev)
+        sens = torch.empty((B, 2, n_max), dtype=torch.float64, device=dev)
+        grad_status = torch.empty((B,), dtype=torch.int32, device=dev)
+        ws = _workspace("mincurv", lib.mc_mincurv_workspace_bytes(chunk, n_max), dev)
+        for s in range(0, B, chunk):
+            e = min(B, s + chunk)
+            rc = lib.mc_mincurv_solve_batch_sens(e - s, n_max, _ptr(n_pts[s:e]) if n_pts is not None else None,
+                                                 _ptr(reftrack[s:e]), _ptr(normvec[s:e]), _ptr(h[s:e]), float(kappa_bound),
+                                                 w_scalar, _ptr(w_veh_t[s:e]) if w_veh_t is not None else None, f_scale,
+                                                 _ptr(_chunk_centre_ids(centre_id, s, e, B)), _ptr(alpha[s:e]), _ptr(cerr[s:e]),
+                                                 _ptr(kmax[s:e]), _ptr(status[s:e]), _ptr(iters[s:e]), _ptr(sens[s:e]),
+                                                 _ptr(grad_status[s:e]), _ptr(ws), ws.numel(), _stream())
+            _lib.check(rc, "mc_mincurv_solve_batch_sens")
+        ctx.save_for_backward(widths, centre, normvec, h, w_veh_t, n_pts, centre_id, sens, grad_status)
+        ctx.w_scalar, ctx.chunk, ctx.f_scale, ctx.strict = w_scalar, chunk, f_scale, strict
+        ctx.mark_non_differentiable(cerr, kmax, status, iters, grad_status)
+        return alpha, cerr, kmax, status, iters, grad_status
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, grad_alpha, *_unused):
+        widths, centre, normvec, h, w_veh_t, n_pts, centre_id, sens, grad_status = ctx.saved_tensors
+        lib = _lib.load()
+        B, n_max, _ = centre.shape
+        dev = centre.device
+        grad_alpha = grad_alpha.to(dtype=torch.float64).contiguous()
+        wanted = (grad_alpha != 0).any(dim=1)
+
+        def refuse(gs, what):
+            bad = wanted & (gs != 0)
+            if ctx.strict and bool(bad.any()):
+                idx = bad.nonzero().flatten()
+                raise _lib.MinCurvLibError(
+                    f"opt_min_curv_diff: no width gradient for {idx.numel()} instance(s) {what} (first: {idx[:8].tolist()}, "
+                    f"grad_status {gs[idx[:8]].tolist()}); strict=False gives them zero gradients")
+        refuse(grad_status, "with a nonzero upstream gradient")
+        gs = grad_status.clone()            # (the adjoint sets 3 where its factorisation breaks down)
+        reftrack = torch.cat((centre, widths), dim=2).contiguous()
+        gwr = torch.empty((B, n_max), dtype=torch.float64, device=dev)
+        gwl = torch.empty((B, n_max), dtype=torch.float64, device=dev)
+        gwv = torch.empty((B,), dtype=torch.float64, device=dev)
+        chunk = ctx.chunk
+        ws = _workspace("mincurv", lib.mc_mincurv_workspace_bytes(chunk, n_max), dev)
+        for s in range(0, B, chunk):
+            e = min(B, s + chunk)
+            rc = lib.mc_mincurv_adjoint_batch(e - s, n_max, _ptr(n_pts[s:e]) if n_pts is not None else None, _ptr(reftrack[s:e]),
+                                              _ptr(normvec[s:e]), _ptr(h[s:e]), ctx.w_scalar,
+                                              _ptr(w_veh_t[s:e]) if w_veh_t is not None else None, ctx.f_scale,
+                                              _ptr(_chunk_centre_ids(centre_id, s, e, B)), _ptr(sens[s:e]), _ptr(gs[s:e]),
+                                              _ptr(grad_alpha[s:e]), _ptr(gwr[s:e]), _ptr(gwl[s:e]), _ptr(gwv[s:e]), _ptr(ws),
+                                              ws.numel(), _stream())
+            _lib.check(rc, "mc_mincurv_adjoint_batch")
+        refuse(gs, "whose adjoint factorisation broke down")
+        return (torch.stack((gwr, gwl), dim=2), gwv if w_veh_t is not None else None) + (None,) * 10
+
+
+@_device_guard
+def opt_min_curv_diff(centre: torch.Tensor, widths: torch.Tensor, normvec: torch.Tensor, h: torch.Tensor, kappa_bound: float,
+                      w_veh: Union[float, torch.Tensor], n_pts: Optional[torch.Tensor] = None,
+                      centre_id: Optional[torch.Tensor] = None, max_chunk: Optional[int] = None,
+                      f_scale: Optional[float] = None, strict: bool = True) -> dict:
+    """opt_min_curv_batch with alpha differentiable with respect to the track widths and the vehicle width (autograd).
+
+    centre [B, n_max, 2] (x, y) and widths [B, n_max, 2] (w_tr_right, w_tr_left) make up the reftrack of
+    opt_min_curv_batch; w_veh is a float or a [B] tensor.  Returns the dict of opt_min_curv_batch (alpha, curv_error_max,
+    kappa_lin_max, status, iters: the same values) plus grad_status [B] (int32).  alpha carries a grad_fn: backward() /
+    torch.autograd.grad give dL/dwidths [B, n_max, 2] and, for a tensor w_veh, dL/dw_veh, at the cost of one assembly, one
+    factorisation and one solve per instance (implicit differentiation of the KKT conditions, DESIGN.md section 3.10).
+    centre, normvec and h are constants: they must not require grad.
+    grad_status: 0 = the gradient is computed; 4 = the curvature rows were active (solved by the curvature-row phase),
+    not supported; otherwise the solve's status (1, 2, 3, -1).  strict=True: backward raises if an instance with a
+    nonzero upstream gradient has grad_status != 0 (or its adjoint factorisation breaks down); strict=False: such
+    instances get zero gradients."""
+    _require_cuda()
+    lib = _lib.load()
+    for t, name in ((centre, "centre"), (normvec, "normvec"), (h, "h")):
+        if isinstance(t, torch.Tensor) and t.requires_grad:
+            raise ValueError(f"opt_min_curv_diff: {name} is a constant (no gradient with respect to it); detach it")
+    centre = _f64(centre, "centre")
+    widths = _f64(widths, "widths")
+    normvec = _f64(normvec, "normvec")
+    h = _f64(h, "h")
+    B, n_max, two = centre.shape
+    if two != 2 or widths.shape != (B, n_max, 2) or normvec.shape != (B, n_max, 2) or h.shape != (B, n_max):
+        raise RuntimeError("opt_min_curv_diff: centre and widths must be [B, n_max, 2], normvec [B, n_max, 2], h [B, n_max]")
+    if n_max < N_MIN:
+        raise NotImplementedError(f"closed tracks with fewer than {N_MIN} points are not supported by the banded solver")
+    dev = centre.device
+    n_pts = _npts(n_pts, B, dev)
+    if isinstance(w_veh, torch.Tensor):
+        if w_veh.numel() != B:
+            raise ValueError("w_veh tensor must have one entry per track")
+        w_scalar, w_veh_t = 0.0, w_veh.to(device=dev, dtype=torch.float64).reshape(B).contiguous()
+    else:
+        w_scalar, w_veh_t = float(w_veh), None
+    if centre_id is not None:
+        if centre_id.shape != (B,):
+            raise ValueError("centre_id must be [B]")
+        centre_id = centre_id.to(device=dev, dtype=torch.int32).contiguous()
+    per_item = lib.mc_mincurv_workspace_bytes(1, n_max)
+    chunk = _chunk(B, per_item, dev) if max_chunk is None else min(B, max_chunk)
+    alpha, cerr, kmax, status, iters, grad_status = _MinCurvDiff.apply(
+        widths, w_veh_t, centre, normvec, h, float(kappa_bound), w_scalar, n_pts, centre_id, chunk,
+        float(F_SCALE if f_scale is None else f_scale), bool(strict))
+    return dict(alpha=alpha, curv_error_max=cerr, kappa_lin_max=kmax, status=status, iters=iters, grad_status=grad_status)
+
+
 @_device_guard
 def opt_shortest_path_batch(reftrack: torch.Tensor, normvec: torch.Tensor, w_veh: Union[float, torch.Tensor],
                             n_pts: Optional[torch.Tensor] = None) -> dict:

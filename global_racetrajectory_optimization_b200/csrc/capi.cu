@@ -5,6 +5,7 @@
 #include <cstring>
 
 #include "../../include/mincurv_b200.h"
+#include "mincurv_sens.h"
 #include "mincurv_ws.cuh"
 
 namespace mc {
@@ -12,6 +13,11 @@ size_t spline_ws_doubles(int n_max);
 int pdip_ctas_per_sm();
 int pdip_kappa_ctas_per_sm();
 int debug_factor_solve_ctas_per_sm();
+int adjoint_ctas_per_sm();
+int launch_mincurv_adjoint(int, int, const int32_t *, const double *, double, const double *, double *, const Layout &,
+                           const double *, const double *, int32_t *, double *, double *, double *, int, int *, cudaStream_t);
+void launch_mincurv_sens_export(int, int, const int32_t *, double *, const Layout &, const int32_t *, double *, int32_t *,
+                                cudaStream_t);
 int launch_debug_factor_solve(int, int, const int32_t *, double *, const Layout &, int32_t *, int, cudaStream_t);
 int debug_read_profile(unsigned long long *, int);
 void launch_mincurv_setup(int, int, const int32_t *, const double *, const double *, const double *, double,
@@ -232,12 +238,11 @@ int mc_mincurv_solve_batch_ex(int B, int n_max, const int32_t *n_pts, const doub
                                          alpha, curv_error_max, kappa_lin_max, status, iters, workspace, workspace_bytes, stream);
 }
 
-int mc_mincurv_solve_batch_shared(int B, int n_max, const int32_t *n_pts, const double *reftrack, const double *normvec,
-                                  const double *h, double kappa_bound, double w_veh, const double *w_veh_batch, double f_scale,
-                                  const int32_t *centre_id, double *alpha, double *curv_error_max, double *kappa_lin_max,
-                                  int32_t *status, int32_t *iters, void *workspace, size_t workspace_bytes, void *stream) {
-    if (!reftrack || !normvec || !h || !alpha || !curv_error_max || !status)
-        return bad("mc_mincurv_solve_batch: NULL argument");
+// setup -> pdip -> finalize -> (export of the sensitivity data) -> kappa -> finalize; sens == NULL: no export
+static int mincurv_solve(int B, int n_max, const int32_t *n_pts, const double *reftrack, const double *normvec, const double *h,
+                         double kappa_bound, double w_veh, const double *w_veh_batch, double f_scale, const int32_t *centre_id,
+                         double *alpha, double *curv_error_max, double *kappa_lin_max, int32_t *status, int32_t *iters,
+                         double *sens, int32_t *grad_status, void *workspace, size_t workspace_bytes, void *stream) {
     int rc = mc_mincurv_setup_batch_shared(B, n_max, n_pts, reftrack, normvec, h, w_veh, w_veh_batch, f_scale, centre_id, status,
                                            workspace, workspace_bytes, stream);
     if (rc) return rc;
@@ -246,11 +251,67 @@ int mc_mincurv_solve_batch_shared(int B, int n_max, const int32_t *n_pts, const 
     rc = mc_mincurv_finalize_batch(B, n_max, n_pts, alpha, kappa_bound, curv_error_max, kappa_lin_max, status, workspace,
                                    workspace_bytes, stream);
     if (rc) return rc;
+    if (sens) {
+        // the box phase's final iterate, before the curvature-row phase takes over the status-4 slabs
+        mc::launch_mincurv_sens_export(B, n_max, n_pts, (double *)workspace, mc::make_layout(n_max), status, sens, grad_status,
+                                       (cudaStream_t)stream);
+        rc = check_cuda("mincurv_sens_export_kernel");
+        if (rc) return rc;
+    }
     // instances whose box-only optimum violates the curvature rows (status 4) are re-solved with the rows
     rc = mc_mincurv_kappa_batch(B, n_max, n_pts, kappa_bound, alpha, status, iters, workspace, workspace_bytes, stream);
     if (rc) return rc;
     return mc_mincurv_finalize_batch(B, n_max, n_pts, alpha, kappa_bound, curv_error_max, kappa_lin_max, status, workspace,
                                      workspace_bytes, stream);
+}
+
+int mc_mincurv_solve_batch_shared(int B, int n_max, const int32_t *n_pts, const double *reftrack, const double *normvec,
+                                  const double *h, double kappa_bound, double w_veh, const double *w_veh_batch, double f_scale,
+                                  const int32_t *centre_id, double *alpha, double *curv_error_max, double *kappa_lin_max,
+                                  int32_t *status, int32_t *iters, void *workspace, size_t workspace_bytes, void *stream) {
+    if (!reftrack || !normvec || !h || !alpha || !curv_error_max || !status)
+        return bad("mc_mincurv_solve_batch: NULL argument");
+    return mincurv_solve(B, n_max, n_pts, reftrack, normvec, h, kappa_bound, w_veh, w_veh_batch, f_scale, centre_id, alpha,
+                         curv_error_max, kappa_lin_max, status, iters, nullptr, nullptr, workspace, workspace_bytes, stream);
+}
+
+int mc_mincurv_solve_batch_sens(int B, int n_max, const int32_t *n_pts, const double *reftrack, const double *normvec,
+                                const double *h, double kappa_bound, double w_veh, const double *w_veh_batch, double f_scale,
+                                const int32_t *centre_id, double *alpha, double *curv_error_max, double *kappa_lin_max,
+                                int32_t *status, int32_t *iters, double *sens, int32_t *grad_status, void *workspace,
+                                size_t workspace_bytes, void *stream) {
+    if (!reftrack || !normvec || !h || !alpha || !curv_error_max || !status || !sens || !grad_status)
+        return bad("mc_mincurv_solve_batch_sens: NULL argument");
+    if (!(f_scale > 0.0)) return bad("mc_mincurv_solve_batch_sens: f_scale must be positive");
+    int rc = mincurv_args("mc_mincurv_solve_batch_sens", B, n_max, workspace, workspace_bytes);
+    if (rc) return rc;
+    return mincurv_solve(B, n_max, n_pts, reftrack, normvec, h, kappa_bound, w_veh, w_veh_batch, f_scale, centre_id, alpha,
+                         curv_error_max, kappa_lin_max, status, iters, sens, grad_status, workspace, workspace_bytes, stream);
+}
+
+int mc_mincurv_adjoint_batch(int B, int n_max, const int32_t *n_pts, const double *reftrack, const double *normvec,
+                             const double *h, double w_veh, const double *w_veh_batch, double f_scale, const int32_t *centre_id,
+                             const double *sens, int32_t *grad_status, const double *grad_alpha, double *grad_w_right,
+                             double *grad_w_left, double *grad_w_veh, void *workspace, size_t workspace_bytes, void *stream) {
+    if (!reftrack || !normvec || !h || !sens || !grad_status || !grad_alpha || !grad_w_right || !grad_w_left || !grad_w_veh)
+        return bad("mc_mincurv_adjoint_batch: NULL argument");
+    if (!(f_scale > 0.0)) return bad("mc_mincurv_adjoint_batch: f_scale must be positive");
+    int rc = mincurv_args("mc_mincurv_adjoint_batch", B, n_max, workspace, workspace_bytes);
+    if (rc) return rc;
+    const mc::Layout L = mc::make_layout(n_max);
+    // the band of H and the bounds are rebuilt in the slabs; the assembly's status words (the forward pass's, recorded in
+    // grad_status) go to grad_w_right, which the adjoint kernel overwrites
+    mc::launch_mincurv_setup(B, n_max, n_pts, reftrack, normvec, h, w_veh, w_veh_batch, f_scale, centre_id, (double *)workspace, L,
+                             reinterpret_cast<int32_t *>(grad_w_right), (cudaStream_t)stream);
+    rc = check_cuda("mincurv_setup_kernel");
+    if (rc) return rc;
+    const SolverGrid g = solver_grid(B, n_max, workspace, mc::adjoint_ctas_per_sm());
+    if (mc::launch_mincurv_adjoint(B, n_max, n_pts, reftrack, w_veh, w_veh_batch, (double *)workspace, L, sens, grad_alpha,
+                                   grad_status, grad_w_right, grad_w_left, grad_w_veh, g.grid, g.counter, (cudaStream_t)stream) != 0) {
+        snprintf(g_err, sizeof(g_err), "mincurv_adjoint_kernel: cudaFuncSetAttribute failed");
+        return MC_ECUDA;
+    }
+    return check_cuda("mincurv_adjoint_kernel");
 }
 
 int mc_mincurv_kappa_batch(int B, int n_max, const int32_t *n_pts, double kappa_bound, double *alpha, int32_t *status,

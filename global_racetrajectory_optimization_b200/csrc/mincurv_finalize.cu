@@ -66,6 +66,31 @@ mincurv_finalize_kernel(int n_max, const int32_t *__restrict__ n_pts, double *__
     }
 }
 
+// Export for the width sensitivities (K2d, mincurv_ipm.cu), run between the first finalize pass and the curvature-row
+// phase: the box phase's final ratios sens[b][0][i] = lu / su, sens[b][1][i] = ll / sl, and grad_status[b] = the status
+// at that point (0: solved by the box phase; 4: goes to the curvature-row phase; otherwise the solve's failure status).
+// Zeros for every instance with grad_status != 0 and beyond n.
+__global__ void __launch_bounds__(256)
+mincurv_sens_export_kernel(int n_max, const int32_t *__restrict__ n_pts, double *__restrict__ ws, Layout L,
+                           const int32_t *__restrict__ status, double *__restrict__ sens, int32_t *__restrict__ grad_status) {
+    const int b = blockIdx.x;
+    const int st = status[b];
+    const int n = (st == 0) ? (n_pts ? n_pts[b] : n_max) : 0;
+    double *slab = ws + (size_t)b * L.stride;
+    const double *LU = vec(slab, L, V_LU), *LL = vec(slab, L, V_LL), *SU = vec(slab, L, V_SU), *SL = vec(slab, L, V_SL);
+    double *du = sens + (size_t)b * 2 * n_max, *dl = du + n_max;
+    for (int i = threadIdx.x; i < n_max; i += blockDim.x) {
+        du[i] = (i < n) ? LU[i] / SU[i] : 0.0;
+        dl[i] = (i < n) ? LL[i] / SL[i] : 0.0;
+    }
+    if (threadIdx.x == 0) grad_status[b] = st;
+}
+
+void launch_mincurv_sens_export(int B, int n_max, const int32_t *n_pts, double *ws, const Layout &L, const int32_t *status,
+                                double *sens, int32_t *grad_status, cudaStream_t stream) {
+    mincurv_sens_export_kernel<<<B, 256, 0, stream>>>(n_max, n_pts, ws, L, status, sens, grad_status);
+}
+
 void launch_mincurv_finalize(int B, int n_max, const int32_t *n_pts, double *ws, const Layout &L, const double *alpha,
                              double kappa_bound, double *curv_error_max, double *kappa_lin_max, int32_t *status,
                              cudaStream_t stream) {

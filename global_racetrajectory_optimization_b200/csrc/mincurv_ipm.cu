@@ -1453,4 +1453,83 @@ int launch_debug_factor_solve(int B, int n_max, const int32_t *n_pts, double *ws
     return launch_solver(debug_factor_solve_kernel, grid, nullptr, stream, B, n_max, n_pts, ws, L, status);
 }
 
+// ================================================================================================
+// K2d -- width sensitivities of the box-only QP (DESIGN.md section 3.10): implicit differentiation of its KKT conditions
+// at the interior-point solution.  With the final ratios d_u = lu / su, d_l = ll / sl of the forward solve (`sens`,
+// mincurv_sens_export_kernel) and an upstream gradient g of alpha:
+//   (H + D) v = g,  D = d_u + d_l;   dL/dub = d_u v,  dL/dlb = d_l v
+// and ub = w_right - w_veh / 2, lb = -w_left + w_veh / 2 (mincurv_setup_kernel P1).  A collapsed box (ub - lb < 2 FIX_EPS,
+// replaced by mid -+ FIX_EPS) follows mid = (w_right - w_left) / 2: both widths get +-(dL/dub + dL/dlb) / 2, w_veh nothing.
+// One factorisation and one solve per instance; the band of H is read from the owner's slab as in mincurv_pdip_kernel.
+// Instances with grad_status != 0 get zeros; a non-positive pivot sets grad_status 3 (zeros too).
+// ================================================================================================
+__global__ void __launch_bounds__(IP_THREADS, 8)
+mincurv_adjoint_kernel(int B, int n_max, const int32_t *__restrict__ n_pts, const double *__restrict__ reftrack, double w_veh,
+                       const double *__restrict__ w_veh_batch, double *__restrict__ ws, Layout L, const double *__restrict__ sens,
+                       const double *__restrict__ grad_alpha, int32_t *__restrict__ grad_status,
+                       double *__restrict__ grad_w_right, double *__restrict__ grad_w_left, double *__restrict__ grad_w_veh,
+                       int *__restrict__ work_counter) {
+    IpShared &sh = ip_init_shared();
+    unsigned tick = 0;
+    for (int b; (b = next_instance(sh, work_counter)) < B;) {
+        const int n = n_pts ? n_pts[b] : n_max;
+        double *gwr = grad_w_right + (size_t)b * n_max, *gwl = grad_w_left + (size_t)b * n_max;
+        bool ok = grad_status[b] == 0;
+        if (ok) {
+            double *slab = ws + (size_t)b * L.stride;
+            const double *HB = ws + (size_t)*band_owner(slab, L) * L.stride + L.o_hb;      // (shared centre lines: the owner's)
+            const double *__restrict__ DU = sens + (size_t)b * 2 * n_max, *__restrict__ DL = DU + n_max;
+            const double *__restrict__ GA = grad_alpha + (size_t)b * n_max;
+            double *__restrict__ RHS = vec(slab, L, V_RHS), *__restrict__ DX = vec(slab, L, V_DX), *__restrict__ DD = vec(slab, L, V_DD);
+            if (threadIdx.x == 0) sh.flag = 0;
+            for (int i = threadIdx.x; i < L.np; i += IP_THREADS) {
+                if (i < n) DD[i] = DU[i] + DL[i];
+                RHS[i] = (i < n) ? GA[i] : 0.0;
+            }
+            ok = factor(sh, slab, L, n, HB, RHS, tick);
+            tick += factor_units(n);
+            if (ok) {
+                solve(sh, slab, L, n, RHS, DX, true);
+                const double wv = w_veh_batch ? w_veh_batch[b] : w_veh;
+                const double *rt = reftrack + (size_t)b * n_max * 4;
+                double gv = 0.0;
+                for (int i = threadIdx.x; i < n_max; i += IP_THREADS) {
+                    double gr = 0.0, gl = 0.0;
+                    if (i < n) {
+                        const double v = DX[i], gu = DU[i] * v, glb = DL[i] * v;
+                        const double2 ww = *reinterpret_cast<const double2 *>(rt + (size_t)i * 4 + 2);
+                        const double ub = ww.x - 0.5 * wv, lb = -(ww.y - 0.5 * wv);      // (the expressions of the setup)
+                        if (ub - lb < 2.0 * FIX_EPS) {
+                            gr = 0.5 * (gu + glb);
+                            gl = -gr;
+                        } else {
+                            gr = gu;
+                            gl = -glb;
+                            gv += 0.5 * (glb - gu);
+                        }
+                    }
+                    gwr[i] = gr;
+                    gwl[i] = gl;
+                }
+                gv = block_reduce<0>(gv, sh.red);
+                if (threadIdx.x == 0) grad_w_veh[b] = gv;
+                continue;
+            }
+            if (threadIdx.x == 0) grad_status[b] = 3;
+        }
+        for (int i = threadIdx.x; i < n_max; i += IP_THREADS) { gwr[i] = 0.0; gwl[i] = 0.0; }
+        if (threadIdx.x == 0) grad_w_veh[b] = 0.0;
+    }
+}
+
+int adjoint_ctas_per_sm() { return ctas_per_sm(mincurv_adjoint_kernel); }
+
+int launch_mincurv_adjoint(int B, int n_max, const int32_t *n_pts, const double *reftrack, double w_veh, const double *w_veh_batch,
+                           double *ws, const Layout &L, const double *sens, const double *grad_alpha, int32_t *grad_status,
+                           double *grad_w_right, double *grad_w_left, double *grad_w_veh, int grid, int *work_counter,
+                           cudaStream_t stream) {
+    return launch_solver(mincurv_adjoint_kernel, grid, work_counter, stream, B, n_max, n_pts, reftrack, w_veh, w_veh_batch, ws, L, sens,
+                         grad_alpha, grad_status, grad_w_right, grad_w_left, grad_w_veh, work_counter);
+}
+
 }  // namespace mc

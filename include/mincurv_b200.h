@@ -139,6 +139,9 @@ int mc_mincurv_pdip_batch(int B, int n_max, const int32_t *n_pts, double *alpha,
 int mc_mincurv_finalize_batch(int B, int n_max, const int32_t *n_pts, const double *alpha, double kappa_bound,
                               double *curv_error_max, double *kappa_lin_max, int32_t *status,
                               void *workspace, size_t workspace_bytes, void *stream);
+/* Width sensitivities of this QP (alpha differentiated with respect to w_tr_right, w_tr_left and w_veh by one more
+ * factorisation per instance): see global_racetrajectory_optimization_b200/csrc/mincurv_sens.h and DESIGN.md 3.10. */
+
 /* Fourth stage, run by mc_mincurv_solve_batch between two finalize passes: re-solves every instance flagged
  * status 4 (curvature rows violated by the box-only optimum) as the full QP tph hands to quadprog, rows
  * |k_ref + E alpha| <= kappa_bound included; leaves all other instances untouched. */
