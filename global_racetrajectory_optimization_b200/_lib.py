@@ -27,6 +27,10 @@ _SIGS = {
     "mc_mincurv_solve_batch_shared": (_c_int, [_c_int, _c_int, _vp, _vp, _vp, _vp, _c_dbl, _c_dbl, _vp, _c_dbl, _vp, _vp, _vp,
                                                _vp, _vp, _vp, _vp, _sz, _vp]),
     "mc_mincurv_setup_batch_shared": (_c_int, [_c_int, _c_int, _vp, _vp, _vp, _vp, _c_dbl, _vp, _c_dbl, _vp, _vp, _vp, _sz, _vp]),
+    "mc_mincurv_solve_batch_sens": (_c_int, [_c_int, _c_int, _vp, _vp, _vp, _vp, _c_dbl, _c_dbl, _vp, _c_dbl, _vp, _vp, _vp, _vp,
+                                             _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
+    "mc_mincurv_adjoint_batch": (_c_int, [_c_int, _c_int, _vp, _vp, _vp, _vp, _c_dbl, _vp, _c_dbl, _vp, _vp, _vp, _vp, _vp, _vp,
+                                          _vp, _vp, _sz, _vp]),
     "mc_mincurv_setup_batch_ex": (_c_int, [_c_int, _c_int, _vp, _vp, _vp, _vp, _c_dbl, _vp, _c_dbl, _vp, _vp, _sz, _vp]),
     "mc_mincurv_setup_batch": (_c_int, [_c_int, _c_int, _vp, _vp, _vp, _vp, _c_dbl, _vp, _vp, _vp, _sz, _vp]),
     "mc_mincurv_pdip_batch": (_c_int, [_c_int, _c_int, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
@@ -68,15 +72,6 @@ _SIGS = {
 
 EXPORTED_SYMBOLS = tuple(_SIGS)
 
-# width sensitivities (csrc/mincurv_sens.h, batch.opt_min_curv_diff): exported by the same library, declared in their own
-# header and bound from their own table
-_SENS_SIGS = {
-    "mc_mincurv_solve_batch_sens": (_c_int, [_c_int, _c_int, _vp, _vp, _vp, _vp, _c_dbl, _c_dbl, _vp, _c_dbl, _vp, _vp, _vp, _vp,
-                                             _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
-    "mc_mincurv_adjoint_batch": (_c_int, [_c_int, _c_int, _vp, _vp, _vp, _vp, _c_dbl, _vp, _c_dbl, _vp, _vp, _vp, _vp, _vp, _vp,
-                                          _vp, _vp, _sz, _vp]),
-}
-
 
 class MinCurvLibError(RuntimeError):
     pass
@@ -98,7 +93,7 @@ def load(build_if_missing: bool = True):
         raise MinCurvLibError(f"{path} is missing: build it with `python -m global_racetrajectory_optimization_b200.build` "
                               "(there is no CPU fallback for this path)")
     lib = ctypes.CDLL(path)
-    for name, (res, args) in {**_SIGS, **_SENS_SIGS}.items():
+    for name, (res, args) in _SIGS.items():
         fn = getattr(lib, name)
         fn.restype = res
         fn.argtypes = args

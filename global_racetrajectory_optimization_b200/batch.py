@@ -13,6 +13,7 @@ from __future__ import annotations
 import ctypes
 import functools
 import math
+from types import SimpleNamespace
 from typing import Optional, Union
 
 import torch
@@ -67,6 +68,11 @@ def _require_cuda() -> None:
 
 def _ptr(t: Optional[torch.Tensor]):
     return ctypes.c_void_p(t.data_ptr()) if t is not None else None
+
+
+def _rows_ptr(t: Optional[torch.Tensor], s: int, e: int):
+    """Pointer to rows s:e of t (the instances of one chunked launch); NULL for an absent tensor."""
+    return _ptr(t[s:e]) if t is not None else None
 
 
 def _stream():
@@ -150,11 +156,11 @@ def calc_splines_batch(xy: torch.Tensor, n_pts: Optional[torch.Tensor] = None,
 
 
 def _wveh(w_veh, B, dev):
+    """(scalar, None) for a number, (0.0, [B] float64 tensor) for a tensor: the w_veh / w_veh_batch pair of the C-ABI."""
     if isinstance(w_veh, torch.Tensor):
-        wb = w_veh.to(device=dev, dtype=torch.float64).contiguous()
-        if wb.numel() != B:
+        if w_veh.numel() != B:
             raise ValueError("w_veh tensor must have one entry per track")
-        return 0.0, wb
+        return 0.0, w_veh.to(device=dev, dtype=torch.float64).reshape(B).contiguous()
     return float(w_veh), None
 
 
@@ -162,6 +168,38 @@ def _chunk(B: int, per_item_bytes: int, device) -> int:
     free, _ = torch.cuda.mem_get_info(device)
     budget = max(int(free * 0.6), per_item_bytes)
     return max(1, min(B, budget // max(per_item_bytes, 1)))
+
+
+def _mincurv_inputs(tracks: dict, shape_error: str, n_pts, w_veh, centre_id, max_chunk, f_scale) -> SimpleNamespace:
+    """The checked and normalised inputs of opt_min_curv_batch and opt_min_curv_diff.  tracks: name -> (tensor, cols), every
+    tensor [B, n_max, cols] ([B, n_max] for cols None; the first fixes B and n_max).  Returns a namespace of the tracks as
+    contiguous float64 CUDA tensors, B, n_max, dev, n_pts, w_scalar and w_batch (see _wveh), centre_id (int32 or None),
+    f_scale (None: F_SCALE) and chunk, the instances per launch."""
+    t = {name: _f64(x, name) for name, (x, _) in tracks.items()}
+    first = next(iter(t.values()))
+    B, n_max = first.shape[:2]
+    if any(t[name].shape != (B, n_max) + ((cols,) if cols else ()) for name, (_, cols) in tracks.items()):
+        raise RuntimeError(shape_error)
+    if n_max < N_MIN:
+        raise NotImplementedError(f"closed tracks with fewer than {N_MIN} points are not supported by the banded solver")
+    dev = first.device
+    n_pts = _npts(n_pts, B, dev)
+    w_scalar, w_batch = _wveh(w_veh, B, dev)
+    if centre_id is not None:
+        if centre_id.shape != (B,):
+            raise ValueError("centre_id must be [B]")
+        centre_id = centre_id.to(device=dev, dtype=torch.int32).contiguous()
+    per_item = _lib.load().mc_mincurv_workspace_bytes(1, n_max)
+    return SimpleNamespace(**t, B=B, n_max=n_max, dev=dev, n_pts=n_pts, w_scalar=w_scalar, w_batch=w_batch,
+                           centre_id=centre_id, f_scale=float(F_SCALE if f_scale is None else f_scale),
+                           chunk=_chunk(B, per_item, dev) if max_chunk is None else min(B, max_chunk))
+
+
+def _mincurv_results(B: int, n_max: int, dev) -> dict:
+    """Buffers for the per-instance results of a solve, in the order of the C-ABI."""
+    f64, i32 = dict(dtype=torch.float64, device=dev), dict(dtype=torch.int32, device=dev)
+    return dict(alpha=torch.empty((B, n_max), **f64), curv_error_max=torch.empty((B,), **f64),
+                kappa_lin_max=torch.empty((B,), **f64), status=torch.empty((B,), **i32), iters=torch.empty((B,), **i32))
 
 
 @_device_guard
@@ -177,44 +215,12 @@ def opt_min_curv_batch(reftrack: torch.Tensor, normvec: torch.Tensor, h: torch.T
     (owners: centre_id[b] == b).  H, f and k_ref are then assembled once per centreline (same results, less work);
     shared_centre_ids() builds the tensor from group labels."""
     _require_cuda()
-    lib = _lib.load()
-    reftrack = _f64(reftrack, "reftrack")
-    normvec = _f64(normvec, "normvec")
-    h = _f64(h, "h")
-    B, n_max, four = reftrack.shape
-    if four != 4 or normvec.shape != (B, n_max, 2) or h.shape != (B, n_max):
-        raise RuntimeError("Array size of reftrack should be the same as normvectors!")
-    if n_max < N_MIN:
-        raise NotImplementedError(f"closed tracks with fewer than {N_MIN} points are not supported by the banded solver")
-    dev = reftrack.device
-    n_pts = _npts(n_pts, B, dev)
-    w_scalar, w_batch = _wveh(w_veh, B, dev)
-    alpha = torch.empty((B, n_max), dtype=torch.float64, device=dev)
-    cerr = torch.empty((B,), dtype=torch.float64, device=dev)
-    kmax = torch.empty((B,), dtype=torch.float64, device=dev)
-    status = torch.empty((B,), dtype=torch.int32, device=dev)
-    iters = torch.empty((B,), dtype=torch.int32, device=dev)
-    per_item = lib.mc_mincurv_workspace_bytes(1, n_max)
-    chunk = _chunk(B, per_item, dev) if max_chunk is None else min(B, max_chunk)
-    ws = _workspace("mincurv", lib.mc_mincurv_workspace_bytes(chunk, n_max), dev)
-    if centre_id is not None:
-        if centre_id.shape != (B,):
-            raise ValueError("centre_id must be [B]")
-        centre_id = centre_id.to(device=dev, dtype=torch.int32).contiguous()
-    for s in range(0, B, chunk):
-        e = min(B, s + chunk)
-        cid = None
-        if centre_id is not None:
-            # owners are addressed inside the chunk: the first instance of the chunk with the same owner takes the role
-            cid = centre_id if (s == 0 and e == B) else shared_centre_ids(centre_id[s:e])
-        rc = lib.mc_mincurv_solve_batch_shared(e - s, n_max, _ptr(n_pts[s:e]) if n_pts is not None else None,
-                                               _ptr(reftrack[s:e]), _ptr(normvec[s:e]), _ptr(h[s:e]), float(kappa_bound),
-                                               w_scalar, _ptr(w_batch[s:e]) if w_batch is not None else None,
-                                               float(F_SCALE if f_scale is None else f_scale), _ptr(cid),
-                                               _ptr(alpha[s:e]), _ptr(cerr[s:e]), _ptr(kmax[s:e]), _ptr(status[s:e]),
-                                               _ptr(iters[s:e]), _ptr(ws), ws.numel(), _stream())
-        _lib.check(rc, "mc_mincurv_solve_batch_shared")
-    return dict(alpha=alpha, curv_error_max=cerr, kappa_lin_max=kmax, status=status, iters=iters)
+    a = _mincurv_inputs(dict(reftrack=(reftrack, 4), normvec=(normvec, 2), h=(h, None)),
+                        "Array size of reftrack should be the same as normvectors!", n_pts, w_veh, centre_id, max_chunk, f_scale)
+    out = _mincurv_results(a.B, a.n_max, a.dev)
+    _mincurv_launch("mc_mincurv_solve_batch_shared", a.chunk, a.n_pts, a.reftrack, a.normvec, a.h, float(kappa_bound),
+                    a.w_scalar, a.w_batch, a.f_scale, a.centre_id, *out.values())
+    return out
 
 
 def shared_centre_ids(group: torch.Tensor) -> torch.Tensor:
@@ -234,32 +240,36 @@ def _chunk_centre_ids(centre_id, s, e, B):
     return centre_id if (s == 0 and e == B) else shared_centre_ids(centre_id[s:e])
 
 
+def _mincurv_launch(entry: str, chunk: int, n_pts, reftrack, normvec, h, kappa_bound, w_scalar, w_batch, f_scale, centre_id,
+                    *outputs) -> None:
+    """Runs the C-ABI entry mc_mincurv_solve_batch_shared, mc_mincurv_solve_batch_sens or mc_mincurv_adjoint_batch on
+    chunks of at most chunk instances.  The arguments are the entry's own in its order, outputs the per-instance tensors
+    after centre_id; kappa_bound is None for the adjoint, which takes none."""
+    lib = _lib.load()
+    B, n_max = h.shape
+    ws = _workspace("mincurv", lib.mc_mincurv_workspace_bytes(chunk, n_max), h.device)
+    kb = () if kappa_bound is None else (kappa_bound,)
+    for s in range(0, B, chunk):
+        e = min(B, s + chunk)
+        cid = _chunk_centre_ids(centre_id, s, e, B)
+        rc = getattr(lib, entry)(e - s, n_max, _rows_ptr(n_pts, s, e), _ptr(reftrack[s:e]), _ptr(normvec[s:e]), _ptr(h[s:e]),
+                                 *kb, w_scalar, _rows_ptr(w_batch, s, e), f_scale, _ptr(cid),
+                                 *(_ptr(t[s:e]) for t in outputs), _ptr(ws), ws.numel(), _stream())
+        _lib.check(rc, entry)
+
+
 class _MinCurvDiff(torch.autograd.Function):
     """alpha of the min-curvature QP as a function of the widths; see opt_min_curv_diff."""
 
     @staticmethod
     def forward(ctx, widths, w_veh_t, centre, normvec, h, kappa_bound, w_scalar, n_pts, centre_id, chunk, f_scale, strict):
-        lib = _lib.load()
         B, n_max, _ = centre.shape
-        dev = centre.device
         reftrack = torch.cat((centre, widths), dim=2).contiguous()
-        alpha = torch.empty((B, n_max), dtype=torch.float64, device=dev)
-        cerr = torch.empty((B,), dtype=torch.float64, device=dev)
-        kmax = torch.empty((B,), dtype=torch.float64, device=dev)
-        status = torch.empty((B,), dtype=torch.int32, device=dev)
-        iters = torch.empty((B,), dtype=torch.int32, device=dev)
-        sens = torch.empty((B, 2, n_max), dtype=torch.float64, device=dev)
-        grad_status = torch.empty((B,), dtype=torch.int32, device=dev)
-        ws = _workspace("mincurv", lib.mc_mincurv_workspace_bytes(chunk, n_max), dev)
-        for s in range(0, B, chunk):
-            e = min(B, s + chunk)
-            rc = lib.mc_mincurv_solve_batch_sens(e - s, n_max, _ptr(n_pts[s:e]) if n_pts is not None else None,
-                                                 _ptr(reftrack[s:e]), _ptr(normvec[s:e]), _ptr(h[s:e]), float(kappa_bound),
-                                                 w_scalar, _ptr(w_veh_t[s:e]) if w_veh_t is not None else None, f_scale,
-                                                 _ptr(_chunk_centre_ids(centre_id, s, e, B)), _ptr(alpha[s:e]), _ptr(cerr[s:e]),
-                                                 _ptr(kmax[s:e]), _ptr(status[s:e]), _ptr(iters[s:e]), _ptr(sens[s:e]),
-                                                 _ptr(grad_status[s:e]), _ptr(ws), ws.numel(), _stream())
-            _lib.check(rc, "mc_mincurv_solve_batch_sens")
+        alpha, cerr, kmax, status, iters = _mincurv_results(B, n_max, centre.device).values()
+        sens = torch.empty((B, 2, n_max), dtype=torch.float64, device=centre.device)
+        grad_status = torch.empty((B,), dtype=torch.int32, device=centre.device)
+        _mincurv_launch("mc_mincurv_solve_batch_sens", chunk, n_pts, reftrack, normvec, h, kappa_bound, w_scalar, w_veh_t,
+                        f_scale, centre_id, alpha, cerr, kmax, status, iters, sens, grad_status)
         ctx.save_for_backward(widths, centre, normvec, h, w_veh_t, n_pts, centre_id, sens, grad_status)
         ctx.w_scalar, ctx.chunk, ctx.f_scale, ctx.strict = w_scalar, chunk, f_scale, strict
         ctx.mark_non_differentiable(cerr, kmax, status, iters, grad_status)
@@ -269,7 +279,6 @@ class _MinCurvDiff(torch.autograd.Function):
     @torch.autograd.function.once_differentiable
     def backward(ctx, grad_alpha, *_unused):
         widths, centre, normvec, h, w_veh_t, n_pts, centre_id, sens, grad_status = ctx.saved_tensors
-        lib = _lib.load()
         B, n_max, _ = centre.shape
         dev = centre.device
         grad_alpha = grad_alpha.to(dtype=torch.float64).contiguous()
@@ -288,17 +297,8 @@ class _MinCurvDiff(torch.autograd.Function):
         gwr = torch.empty((B, n_max), dtype=torch.float64, device=dev)
         gwl = torch.empty((B, n_max), dtype=torch.float64, device=dev)
         gwv = torch.empty((B,), dtype=torch.float64, device=dev)
-        chunk = ctx.chunk
-        ws = _workspace("mincurv", lib.mc_mincurv_workspace_bytes(chunk, n_max), dev)
-        for s in range(0, B, chunk):
-            e = min(B, s + chunk)
-            rc = lib.mc_mincurv_adjoint_batch(e - s, n_max, _ptr(n_pts[s:e]) if n_pts is not None else None, _ptr(reftrack[s:e]),
-                                              _ptr(normvec[s:e]), _ptr(h[s:e]), ctx.w_scalar,
-                                              _ptr(w_veh_t[s:e]) if w_veh_t is not None else None, ctx.f_scale,
-                                              _ptr(_chunk_centre_ids(centre_id, s, e, B)), _ptr(sens[s:e]), _ptr(gs[s:e]),
-                                              _ptr(grad_alpha[s:e]), _ptr(gwr[s:e]), _ptr(gwl[s:e]), _ptr(gwv[s:e]), _ptr(ws),
-                                              ws.numel(), _stream())
-            _lib.check(rc, "mc_mincurv_adjoint_batch")
+        _mincurv_launch("mc_mincurv_adjoint_batch", ctx.chunk, n_pts, reftrack, normvec, h, None, ctx.w_scalar, w_veh_t,
+                        ctx.f_scale, centre_id, sens, gs, grad_alpha, gwr, gwl, gwv)
         refuse(gs, "whose adjoint factorisation broke down")
         return (torch.stack((gwr, gwl), dim=2), gwv if w_veh_t is not None else None) + (None,) * 10
 
@@ -321,36 +321,15 @@ def opt_min_curv_diff(centre: torch.Tensor, widths: torch.Tensor, normvec: torch
     nonzero upstream gradient has grad_status != 0 (or its adjoint factorisation breaks down); strict=False: such
     instances get zero gradients."""
     _require_cuda()
-    lib = _lib.load()
     for t, name in ((centre, "centre"), (normvec, "normvec"), (h, "h")):
         if isinstance(t, torch.Tensor) and t.requires_grad:
             raise ValueError(f"opt_min_curv_diff: {name} is a constant (no gradient with respect to it); detach it")
-    centre = _f64(centre, "centre")
-    widths = _f64(widths, "widths")
-    normvec = _f64(normvec, "normvec")
-    h = _f64(h, "h")
-    B, n_max, two = centre.shape
-    if two != 2 or widths.shape != (B, n_max, 2) or normvec.shape != (B, n_max, 2) or h.shape != (B, n_max):
-        raise RuntimeError("opt_min_curv_diff: centre and widths must be [B, n_max, 2], normvec [B, n_max, 2], h [B, n_max]")
-    if n_max < N_MIN:
-        raise NotImplementedError(f"closed tracks with fewer than {N_MIN} points are not supported by the banded solver")
-    dev = centre.device
-    n_pts = _npts(n_pts, B, dev)
-    if isinstance(w_veh, torch.Tensor):
-        if w_veh.numel() != B:
-            raise ValueError("w_veh tensor must have one entry per track")
-        w_scalar, w_veh_t = 0.0, w_veh.to(device=dev, dtype=torch.float64).reshape(B).contiguous()
-    else:
-        w_scalar, w_veh_t = float(w_veh), None
-    if centre_id is not None:
-        if centre_id.shape != (B,):
-            raise ValueError("centre_id must be [B]")
-        centre_id = centre_id.to(device=dev, dtype=torch.int32).contiguous()
-    per_item = lib.mc_mincurv_workspace_bytes(1, n_max)
-    chunk = _chunk(B, per_item, dev) if max_chunk is None else min(B, max_chunk)
+    a = _mincurv_inputs(dict(centre=(centre, 2), widths=(widths, 2), normvec=(normvec, 2), h=(h, None)),
+                        "opt_min_curv_diff: centre and widths must be [B, n_max, 2], normvec [B, n_max, 2], h [B, n_max]",
+                        n_pts, w_veh, centre_id, max_chunk, f_scale)
     alpha, cerr, kmax, status, iters, grad_status = _MinCurvDiff.apply(
-        widths, w_veh_t, centre, normvec, h, float(kappa_bound), w_scalar, n_pts, centre_id, chunk,
-        float(F_SCALE if f_scale is None else f_scale), bool(strict))
+        a.widths, a.w_batch, a.centre, a.normvec, a.h, float(kappa_bound), a.w_scalar, a.n_pts, a.centre_id, a.chunk,
+        a.f_scale, bool(strict))
     return dict(alpha=alpha, curv_error_max=cerr, kappa_lin_max=kmax, status=status, iters=iters, grad_status=grad_status)
 
 
@@ -685,14 +664,13 @@ def vel_profile_batch(kappa: torch.Tensor, el_lengths: torch.Tensor, ggv, ax_max
     ws = _workspace("velprofile", lib.mc_vel_profile_workspace_bytes(chunk, V, n_max), dev)
     for s in range(0, B, chunk):
         e = min(B, s + chunk)
-        rc = lib.mc_vel_profile_batch_ex(e - s, n_max, _ptr(n_pts[s:e]) if n_pts is not None else None, _ptr(kappa[s:e]),
-                                         _ptr(el_lengths[s:e]), _ptr(mu[s:e]) if mu is not None else None, V, _ptr(scale_t),
-                                         _ptr(vmax_t), v_scalar, int(ggv_t.shape[0]), _ptr(ggv_t), int(mach_t.shape[0]),
-                                         _ptr(mach_t), float(dyn_model_exp), float(drag_coeff), float(m_veh), fw,
+        rc = lib.mc_vel_profile_batch_ex(e - s, n_max, _rows_ptr(n_pts, s, e), _ptr(kappa[s:e]), _ptr(el_lengths[s:e]),
+                                         _rows_ptr(mu, s, e), V, _ptr(scale_t), _ptr(vmax_t), v_scalar, int(ggv_t.shape[0]),
+                                         _ptr(ggv_t), int(mach_t.shape[0]), _ptr(mach_t), float(dyn_model_exp),
+                                         float(drag_coeff), float(m_veh), fw,
                                          int(VP_DECEL_SLICE_UPPER if decel_slice_upper is None else decel_slice_upper),
-                                         _ptr(vx[s:e]) if vx is not None else None, _ptr(ax[s:e]) if ax is not None else None,
-                                         _ptr(t[s:e]) if t is not None else None, _ptr(laptime[s:e]), _ptr(status[s:e]),
-                                         _ptr(ws), ws.numel(), _stream())
+                                         _rows_ptr(vx, s, e), _rows_ptr(ax, s, e), _rows_ptr(t, s, e), _ptr(laptime[s:e]),
+                                         _ptr(status[s:e]), _ptr(ws), ws.numel(), _stream())
         _lib.check(rc, "mc_vel_profile_batch_ex")
     out = dict(laptime=laptime, status=status)
     if want_profiles:
@@ -796,12 +774,11 @@ def min_bound_dists_batch(xy: torch.Tensor, psi: torch.Tensor, bound1: torch.Ten
     dev = xy.device
     out = torch.zeros((B, n_traj_max), dtype=torch.float64, device=dev)
     n_traj, nb1, nb2 = _npts(n_traj, B, dev), _npts(nb1, B, dev), _npts(nb2, B, dev)
-    sl = lambda t, s, e: _ptr(t[s:e]) if t is not None else None
     for s in range(0, B, _GRID_Y_MAX):           # the track index is the y dimension of the launch grid
         e = min(B, s + _GRID_Y_MAX)
-        rc = lib.mc_min_bound_dists_batch(e - s, n_traj_max, sl(n_traj, s, e), _ptr(xy[s:e]), _ptr(psi[s:e]),
-                                          int(bound1.shape[1]), sl(nb1, s, e), _ptr(bound1[s:e]), int(bound2.shape[1]),
-                                          sl(nb2, s, e), _ptr(bound2[s:e]), int(bound1.shape[2]), float(length_veh),
+        rc = lib.mc_min_bound_dists_batch(e - s, n_traj_max, _rows_ptr(n_traj, s, e), _ptr(xy[s:e]), _ptr(psi[s:e]),
+                                          int(bound1.shape[1]), _rows_ptr(nb1, s, e), _ptr(bound1[s:e]), int(bound2.shape[1]),
+                                          _rows_ptr(nb2, s, e), _ptr(bound2[s:e]), int(bound1.shape[2]), float(length_veh),
                                           float(width_veh), _ptr(out[s:e]), _stream())
         _lib.check(rc, "mc_min_bound_dists_batch")
     return out
@@ -907,9 +884,8 @@ def check_normals_crossing_batch(track: torch.Tensor, normvec: torch.Tensor, hor
     crossing = torch.zeros((B,), dtype=torch.int32, device=dev)
     for s in range(0, B, _GRID_Y_MAX):
         e = min(B, s + _GRID_Y_MAX)
-        rc = lib.mc_check_normals_crossing_batch(e - s, n_max, _ptr(n_pts[s:e]) if n_pts is not None else None,
-                                                 _ptr(track[s:e]), _ptr(normvec[s:e]), int(horizon), _ptr(crossing[s:e]),
-                                                 _stream())
+        rc = lib.mc_check_normals_crossing_batch(e - s, n_max, _rows_ptr(n_pts, s, e), _ptr(track[s:e]), _ptr(normvec[s:e]),
+                                                 int(horizon), _ptr(crossing[s:e]), _stream())
         _lib.check(rc, "mc_check_normals_crossing_batch")
     return crossing != 0
 

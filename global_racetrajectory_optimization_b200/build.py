@@ -11,7 +11,7 @@ CSRC = os.path.join(_HERE, "csrc")
 LIB_PATH = os.path.join(_HERE, "libmincurv_b200.so")
 SOURCES = ["capi.cu", "mincurv_setup.cu", "mincurv_ipm.cu", "mincurv_finalize.cu", "splines.cu", "shortest_path.cu",
            "vel_profile.cu", "traj_check.cu", "synth.cu", "prep_track.cu"]
-HEADERS = ["common.cuh", "mincurv_ws.cuh", "mincurv_ops.cuh", "mincurv_sens.h", "vel_profile_core.cuh", "traj_check_core.cuh", os.path.join("..", "..", "include", "mincurv_b200.h")]
+HEADERS = ["common.cuh", "mincurv_ws.cuh", "mincurv_ops.cuh", "vel_profile_core.cuh", "traj_check_core.cuh", os.path.join("..", "..", "include", "mincurv_b200.h")]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "-shared"]
 

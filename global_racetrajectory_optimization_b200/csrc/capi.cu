@@ -5,7 +5,6 @@
 #include <cstring>
 
 #include "../../include/mincurv_b200.h"
-#include "mincurv_sens.h"
 #include "mincurv_ws.cuh"
 
 namespace mc {
@@ -238,11 +237,14 @@ int mc_mincurv_solve_batch_ex(int B, int n_max, const int32_t *n_pts, const doub
                                          alpha, curv_error_max, kappa_lin_max, status, iters, workspace, workspace_bytes, stream);
 }
 
-// setup -> pdip -> finalize -> (export of the sensitivity data) -> kappa -> finalize; sens == NULL: no export
+// setup -> pdip -> finalize -> (export of the sensitivity data) -> kappa -> finalize; sens == NULL: no export.  Every
+// argument is checked before the first launch: the pointers here, f_scale and the sizes by the setup stage.
 static int mincurv_solve(int B, int n_max, const int32_t *n_pts, const double *reftrack, const double *normvec, const double *h,
                          double kappa_bound, double w_veh, const double *w_veh_batch, double f_scale, const int32_t *centre_id,
                          double *alpha, double *curv_error_max, double *kappa_lin_max, int32_t *status, int32_t *iters,
                          double *sens, int32_t *grad_status, void *workspace, size_t workspace_bytes, void *stream) {
+    if (!reftrack || !normvec || !h || !alpha || !curv_error_max || !status)
+        return bad("mc_mincurv_solve_batch: NULL argument");
     int rc = mc_mincurv_setup_batch_shared(B, n_max, n_pts, reftrack, normvec, h, w_veh, w_veh_batch, f_scale, centre_id, status,
                                            workspace, workspace_bytes, stream);
     if (rc) return rc;
@@ -269,8 +271,6 @@ int mc_mincurv_solve_batch_shared(int B, int n_max, const int32_t *n_pts, const 
                                   const double *h, double kappa_bound, double w_veh, const double *w_veh_batch, double f_scale,
                                   const int32_t *centre_id, double *alpha, double *curv_error_max, double *kappa_lin_max,
                                   int32_t *status, int32_t *iters, void *workspace, size_t workspace_bytes, void *stream) {
-    if (!reftrack || !normvec || !h || !alpha || !curv_error_max || !status)
-        return bad("mc_mincurv_solve_batch: NULL argument");
     return mincurv_solve(B, n_max, n_pts, reftrack, normvec, h, kappa_bound, w_veh, w_veh_batch, f_scale, centre_id, alpha,
                          curv_error_max, kappa_lin_max, status, iters, nullptr, nullptr, workspace, workspace_bytes, stream);
 }
@@ -280,11 +280,7 @@ int mc_mincurv_solve_batch_sens(int B, int n_max, const int32_t *n_pts, const do
                                 const int32_t *centre_id, double *alpha, double *curv_error_max, double *kappa_lin_max,
                                 int32_t *status, int32_t *iters, double *sens, int32_t *grad_status, void *workspace,
                                 size_t workspace_bytes, void *stream) {
-    if (!reftrack || !normvec || !h || !alpha || !curv_error_max || !status || !sens || !grad_status)
-        return bad("mc_mincurv_solve_batch_sens: NULL argument");
-    if (!(f_scale > 0.0)) return bad("mc_mincurv_solve_batch_sens: f_scale must be positive");
-    int rc = mincurv_args("mc_mincurv_solve_batch_sens", B, n_max, workspace, workspace_bytes);
-    if (rc) return rc;
+    if (!sens || !grad_status) return bad("mc_mincurv_solve_batch_sens: NULL argument");
     return mincurv_solve(B, n_max, n_pts, reftrack, normvec, h, kappa_bound, w_veh, w_veh_batch, f_scale, centre_id, alpha,
                          curv_error_max, kappa_lin_max, status, iters, sens, grad_status, workspace, workspace_bytes, stream);
 }
@@ -293,21 +289,17 @@ int mc_mincurv_adjoint_batch(int B, int n_max, const int32_t *n_pts, const doubl
                              const double *h, double w_veh, const double *w_veh_batch, double f_scale, const int32_t *centre_id,
                              const double *sens, int32_t *grad_status, const double *grad_alpha, double *grad_w_right,
                              double *grad_w_left, double *grad_w_veh, void *workspace, size_t workspace_bytes, void *stream) {
-    if (!reftrack || !normvec || !h || !sens || !grad_status || !grad_alpha || !grad_w_right || !grad_w_left || !grad_w_veh)
+    if (!sens || !grad_status || !grad_alpha || !grad_w_right || !grad_w_left || !grad_w_veh)
         return bad("mc_mincurv_adjoint_batch: NULL argument");
-    if (!(f_scale > 0.0)) return bad("mc_mincurv_adjoint_batch: f_scale must be positive");
-    int rc = mincurv_args("mc_mincurv_adjoint_batch", B, n_max, workspace, workspace_bytes);
-    if (rc) return rc;
-    const mc::Layout L = mc::make_layout(n_max);
     // the band of H and the bounds are rebuilt in the slabs; the assembly's status words (the forward pass's, recorded in
     // grad_status) go to grad_w_right, which the adjoint kernel overwrites
-    mc::launch_mincurv_setup(B, n_max, n_pts, reftrack, normvec, h, w_veh, w_veh_batch, f_scale, centre_id, (double *)workspace, L,
-                             reinterpret_cast<int32_t *>(grad_w_right), (cudaStream_t)stream);
-    rc = check_cuda("mincurv_setup_kernel");
+    int rc = mc_mincurv_setup_batch_shared(B, n_max, n_pts, reftrack, normvec, h, w_veh, w_veh_batch, f_scale, centre_id,
+                                           reinterpret_cast<int32_t *>(grad_w_right), workspace, workspace_bytes, stream);
     if (rc) return rc;
     const SolverGrid g = solver_grid(B, n_max, workspace, mc::adjoint_ctas_per_sm());
-    if (mc::launch_mincurv_adjoint(B, n_max, n_pts, reftrack, w_veh, w_veh_batch, (double *)workspace, L, sens, grad_alpha,
-                                   grad_status, grad_w_right, grad_w_left, grad_w_veh, g.grid, g.counter, (cudaStream_t)stream) != 0) {
+    if (mc::launch_mincurv_adjoint(B, n_max, n_pts, reftrack, w_veh, w_veh_batch, (double *)workspace, mc::make_layout(n_max),
+                                   sens, grad_alpha, grad_status, grad_w_right, grad_w_left, grad_w_veh, g.grid, g.counter,
+                                   (cudaStream_t)stream) != 0) {
         snprintf(g_err, sizeof(g_err), "mincurv_adjoint_kernel: cudaFuncSetAttribute failed");
         return MC_ECUDA;
     }

@@ -139,8 +139,44 @@ int mc_mincurv_pdip_batch(int B, int n_max, const int32_t *n_pts, double *alpha,
 int mc_mincurv_finalize_batch(int B, int n_max, const int32_t *n_pts, const double *alpha, double kappa_bound,
                               double *curv_error_max, double *kappa_lin_max, int32_t *status,
                               void *workspace, size_t workspace_bytes, void *stream);
-/* Width sensitivities of this QP (alpha differentiated with respect to w_tr_right, w_tr_left and w_veh by one more
- * factorisation per instance): see global_racetrajectory_optimization_b200/csrc/mincurv_sens.h and DESIGN.md 3.10. */
+
+/* Width sensitivities of this QP: alpha differentiated with respect to w_tr_right, w_tr_left and w_veh by one more
+ * factorisation per instance (batch.opt_min_curv_diff; DESIGN.md section 3.10 has the derivation).
+ * Only instances solved by the box-only phase have a gradient.  grad_status[b] (int32):
+ *   0  solved by the box-only phase (status 0): gradients are computed
+ *   4  the box-only optimum violated the curvature rows and the curvature-row phase re-solved it: not supported
+ *   1, 2, 3, -1  the forward solve's status (infeasible, iteration cap, breakdown, unsupported size)
+ *   3  also: a non-positive pivot in the adjoint factorisation
+ * Every unsupported instance gets zero gradients.  The widths are differentiated, the centre line, h, f_scale and
+ * kappa_bound are constants.
+ *
+ * mc_mincurv_solve_batch_sens: mc_mincurv_solve_batch_shared (same arguments, bit-identical alpha, curv_error_max,
+ * kappa_lin_max, status, iters) that also exports what the backward pass needs, 16 bytes per point:
+ *   sens        [B][2][n_max] : lu / su and ll / sl, the box phase's final multiplier-to-slack ratios of the upper and
+ *                               lower bounds (zero beyond n_pts[b] and for grad_status != 0)
+ *   grad_status [B]           : see above; recorded after the box phase, before the curvature-row phase
+ *
+ * mc_mincurv_adjoint_batch: vector-Jacobian product of alpha with respect to the widths: for an upstream gradient
+ * grad_alpha [B][n_max] of a loss L,
+ *   grad_w_right [B][n_max] = dL / dw_tr_right,  grad_w_left [B][n_max] = dL / dw_tr_left,  grad_w_veh [B] = dL / dw_veh
+ * (per instance; the scalar w_veh's gradient is their sum).  Geometry, widths, w_veh / w_veh_batch, f_scale and centre_id
+ * must be those of the mc_mincurv_solve_batch_sens call that produced sens and grad_status.  The assembly is re-run in
+ * the workspace, then one factorisation of H + diag(sens[0] + sens[1]) and one solve per instance; nothing has to
+ * survive in the workspace between the two calls.  grad_status is read, and set to 3 where the factorisation breaks
+ * down.  grad_w_right also serves as scratch of the assembly's status words before it is written. */
+int mc_mincurv_solve_batch_sens(int B, int n_max, const int32_t *n_pts,
+                                const double *reftrack, const double *normvec, const double *h,
+                                double kappa_bound, double w_veh, const double *w_veh_batch, double f_scale,
+                                const int32_t *centre_id,
+                                double *alpha, double *curv_error_max, double *kappa_lin_max,
+                                int32_t *status, int32_t *iters, double *sens, int32_t *grad_status,
+                                void *workspace, size_t workspace_bytes, void *stream);
+int mc_mincurv_adjoint_batch(int B, int n_max, const int32_t *n_pts,
+                             const double *reftrack, const double *normvec, const double *h,
+                             double w_veh, const double *w_veh_batch, double f_scale, const int32_t *centre_id,
+                             const double *sens, int32_t *grad_status, const double *grad_alpha,
+                             double *grad_w_right, double *grad_w_left, double *grad_w_veh,
+                             void *workspace, size_t workspace_bytes, void *stream);
 
 /* Fourth stage, run by mc_mincurv_solve_batch between two finalize passes: re-solves every instance flagged
  * status 4 (curvature rows violated by the box-only optimum) as the full QP tph hands to quadprog, rows

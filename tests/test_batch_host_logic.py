@@ -1,46 +1,12 @@
-"""CPU tests (-m "not gpu") of the host logic above the C-ABI: every batched wrapper is run against a recording stand-in
-of libmincurv_b200.so (no compute: each entry point only checks its argument count against the ctypes signature table and
-returns MC_OK), with CPU tensors in place of device buffers.  Catches arity / ordering / chunking mistakes in batch.py and
-globaltraj.py without a GPU; the numerical behaviour is covered by the -m gpu tests."""
+"""CPU tests (-m "not gpu") of the host logic above the C-ABI: every batched wrapper is run against the recording stand-in
+of libmincurv_b200.so in fake_lib.py, with CPU tensors in place of device buffers.  Catches arity / ordering / chunking
+mistakes in batch.py and globaltraj.py without a GPU; the numerical behaviour is covered by the -m gpu tests."""
 import numpy as np
 import pytest
 import torch
 
+from fake_lib import FakeLib, fake  # noqa: F401  (fake: the fixture)
 from global_racetrajectory_optimization_b200 import _lib, batch as B_, globaltraj
-
-
-class FakeLib:
-    def __init__(self):
-        self.calls = []
-
-    def __getattr__(self, name):
-        if name not in _lib._SIGS:
-            raise AttributeError(name)
-        res, args = _lib._SIGS[name]
-
-        def fn(*a):
-            assert len(a) == len(args), f"{name}: {len(a)} arguments passed, {len(args)} declared"
-            self.calls.append((name, a))
-            if name.endswith("_workspace_bytes"):
-                return 4096
-            return 0
-        return fn
-
-
-@pytest.fixture()
-def fake(monkeypatch):
-    lib = FakeLib()
-    monkeypatch.setattr(_lib, "load", lambda build_if_missing=True: lib)
-    monkeypatch.setattr(_lib, "check", lambda rc, what: None)
-    monkeypatch.setattr(B_, "_require_cuda", lambda: None)
-    monkeypatch.setattr(B_, "_f64", lambda t, name: t.contiguous())
-    monkeypatch.setattr(B_, "_stream", lambda: None)
-    monkeypatch.setattr(B_, "_chunk", lambda B, per_item, dev: max(1, B // 2))      # force the chunked paths
-    monkeypatch.setattr(B_, "_WS", {})
-    # the stand-in writes nothing: what the wrappers allocate with torch.empty would be uninitialised memory (a NaN in
-    # alpha used to reach create_raceline_batch's capacity estimate from time to time)
-    monkeypatch.setattr(torch, "empty", lambda *a, **k: torch.zeros(*a, **k))
-    return lib
 
 
 def _names(lib):
@@ -55,6 +21,9 @@ def test_every_wrapper_matches_the_signature_table(fake):
     res = B_.opt_min_curv_batch(rt, nv, h, 0.12, torch.full((B,), 2.0, dtype=torch.float64), n_pts=npts)
     assert _names(fake).count("mc_mincurv_solve_batch_shared") == 3                     # 5 tracks in chunks of 2
     assert res["alpha"].shape == (B, n)
+    widths = rt[:, :, 2:].clone().requires_grad_()
+    B_.opt_min_curv_diff(rt[:, :, :2], widths, nv, h, 0.12, 2.0, n_pts=npts)["alpha"].sum().backward()
+    assert widths.grad.shape == (B, n, 2)
     alpha = torch.zeros((B, n), dtype=torch.float64)      # (the stand-in library writes nothing: outputs are uninitialised)
     B_.opt_shortest_path_batch(rt, nv, 2.0, n_pts=npts)
     rl = B_.create_raceline_batch(rt, nv, alpha, 2.0, n_pts=npts)

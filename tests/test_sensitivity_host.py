@@ -1,6 +1,6 @@
 """CPU tests (-m "not gpu") of the width sensitivities: the oracle's exact active-set VJP (tests/qp_sens.py) against
 central finite differences of the oracle's own Goldfarb-Idnani solves, the argument validation of the two C entries
-without a GPU, and the host logic of batch.opt_min_curv_diff against a recording stand-in of the library."""
+without a GPU, and the host logic of batch.opt_min_curv_diff against the recording stand-in of the library (fake_lib.py)."""
 import ctypes
 
 import numpy as np
@@ -8,6 +8,7 @@ import pytest
 import torch
 
 import qp_sens as Q
+from fake_lib import fake  # noqa: F401  (the fixture)
 from global_racetrajectory_optimization_b200 import _lib, batch as B_
 
 
@@ -104,39 +105,6 @@ def test_sensitivity_entries_validate_their_arguments_without_gpu():
     assert solve(alpha=None) == -1 and solve(st=None) == -1
     for k in ("ga", "gwr", "gwl", "gwv", "rt", "nv", "h"):
         assert adjoint(**{k: None}) == -1
-
-
-class _FakeLib:
-    """Checks every call's arity against the signature tables and records it; computes nothing."""
-
-    def __init__(self):
-        self.calls = []
-
-    def __getattr__(self, name):
-        sigs = {**_lib._SIGS, **_lib._SENS_SIGS}
-        if name not in sigs:
-            raise AttributeError(name)
-        res, args = sigs[name]
-
-        def fn(*a):
-            assert len(a) == len(args), f"{name}: {len(a)} arguments passed, {len(args)} declared"
-            self.calls.append((name, a))
-            return 4096 if name.endswith("_workspace_bytes") else 0
-        return fn
-
-
-@pytest.fixture()
-def fake(monkeypatch):
-    lib = _FakeLib()
-    monkeypatch.setattr(_lib, "load", lambda build_if_missing=True: lib)
-    monkeypatch.setattr(_lib, "check", lambda rc, what: None)
-    monkeypatch.setattr(B_, "_require_cuda", lambda: None)
-    monkeypatch.setattr(B_, "_f64", lambda t, name: t.contiguous())
-    monkeypatch.setattr(B_, "_stream", lambda: None)
-    monkeypatch.setattr(B_, "_chunk", lambda B, per_item, dev: max(1, B // 2))
-    monkeypatch.setattr(B_, "_WS", {})
-    monkeypatch.setattr(torch, "empty", lambda *a, **k: torch.zeros(*a, **k))     # (the stand-in writes nothing)
-    return lib
 
 
 def test_opt_min_curv_diff_chunks_forward_and_backward_alike(fake):
