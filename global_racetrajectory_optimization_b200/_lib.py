@@ -4,77 +4,65 @@ from __future__ import annotations
 
 import ctypes
 import os
+import re
 
 from . import build as _build
 
-_c_int = ctypes.c_int
-_c_dbl = ctypes.c_double
-_vp = ctypes.c_void_p
-_sz = ctypes.c_size_t
-
 _LIB = None
-
-_SIGS = {
-    "mc_version": (_c_int, []),
-    "mc_last_error": (ctypes.c_char_p, []),
-    "mc_calc_splines_workspace_bytes": (_sz, [_c_int, _c_int]),
-    "mc_calc_splines_batch": (_c_int, [_c_int, _c_int, _vp, _vp, _c_int, _vp, _c_int, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
-    "mc_mincurv_workspace_bytes": (_sz, [_c_int, _c_int]),
-    "mc_mincurv_solve_batch": (_c_int, [_c_int, _c_int, _vp, _vp, _vp, _vp, _c_dbl, _c_dbl, _vp, _vp, _vp, _vp, _vp, _vp,
-                                        _vp, _sz, _vp]),
-    "mc_mincurv_solve_batch_ex": (_c_int, [_c_int, _c_int, _vp, _vp, _vp, _vp, _c_dbl, _c_dbl, _vp, _c_dbl, _vp, _vp, _vp, _vp,
-                                           _vp, _vp, _sz, _vp]),
-    "mc_mincurv_solve_batch_shared": (_c_int, [_c_int, _c_int, _vp, _vp, _vp, _vp, _c_dbl, _c_dbl, _vp, _c_dbl, _vp, _vp, _vp,
-                                               _vp, _vp, _vp, _vp, _sz, _vp]),
-    "mc_mincurv_setup_batch_shared": (_c_int, [_c_int, _c_int, _vp, _vp, _vp, _vp, _c_dbl, _vp, _c_dbl, _vp, _vp, _vp, _sz, _vp]),
-    "mc_mincurv_solve_batch_sens": (_c_int, [_c_int, _c_int, _vp, _vp, _vp, _vp, _c_dbl, _c_dbl, _vp, _c_dbl, _vp, _vp, _vp, _vp,
-                                             _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
-    "mc_mincurv_adjoint_batch": (_c_int, [_c_int, _c_int, _vp, _vp, _vp, _vp, _c_dbl, _vp, _c_dbl, _vp, _vp, _vp, _vp, _vp, _vp,
-                                          _vp, _vp, _sz, _vp]),
-    "mc_mincurv_setup_batch_ex": (_c_int, [_c_int, _c_int, _vp, _vp, _vp, _vp, _c_dbl, _vp, _c_dbl, _vp, _vp, _sz, _vp]),
-    "mc_mincurv_setup_batch": (_c_int, [_c_int, _c_int, _vp, _vp, _vp, _vp, _c_dbl, _vp, _vp, _vp, _sz, _vp]),
-    "mc_mincurv_pdip_batch": (_c_int, [_c_int, _c_int, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
-    "mc_mincurv_finalize_batch": (_c_int, [_c_int, _c_int, _vp, _vp, _c_dbl, _vp, _vp, _vp, _vp, _sz, _vp]),
-    "mc_mincurv_kappa_batch": (_c_int, [_c_int, _c_int, _vp, _c_dbl, _vp, _vp, _vp, _vp, _sz, _vp]),
-    "mc_shortest_path_workspace_bytes": (_sz, [_c_int, _c_int]),
-    "mc_shortest_path_solve_batch": (_c_int, [_c_int, _c_int, _vp, _vp, _vp, _c_dbl, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
-    "mc_create_raceline_workspace_bytes": (_sz, [_c_int, _c_int]),
-    "mc_create_raceline_batch": (_c_int, [_c_int, _c_int, _vp, _vp, _c_int, _vp, _vp, _c_dbl, _c_int, _vp, _vp, _vp, _vp,
-                                          _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
-    "mc_calc_head_curv_batch": (_c_int, [_c_int, _c_int, _vp, _vp, _c_int, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
-    "mc_iqp_relinearise_workspace_bytes": (_sz, [_c_int, _c_int, _c_int]),
-    "mc_iqp_relinearise_batch": (_c_int, [_c_int, _c_int, _vp, _vp, _vp, _vp, _vp, _c_dbl, _c_int, _vp, _vp, _vp, _vp,
-                                          _sz, _vp]),
-    "mc_scale_alpha_batch": (_c_int, [_c_int, _c_int, _vp, _vp, _c_dbl, _vp]),
-    "mc_iqp_finish_batch": (_c_int, [_c_int, _c_int, _c_int, _c_int, _c_int, _c_dbl, _c_int, _c_int] + [_vp] * 16),
-    "mc_vel_profile_workspace_bytes": (_sz, [_c_int, _c_int, _c_int]),
-    "mc_vel_profile_batch": (_c_int, [_c_int, _c_int, _vp, _vp, _vp, _vp, _c_int, _vp, _vp, _c_dbl, _c_int, _vp, _c_int, _vp,
-                                      _c_dbl, _c_dbl, _c_dbl, _c_int, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
-    "mc_vel_profile_batch_ex": (_c_int, [_c_int, _c_int, _vp, _vp, _vp, _vp, _c_int, _vp, _vp, _c_dbl, _c_int, _vp, _c_int, _vp,
-                                         _c_dbl, _c_dbl, _c_dbl, _c_int, _c_int, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
-    "mc_calc_ax_t_profile_batch": (_c_int, [_c_int, _c_int, _vp, _vp, _c_int, _vp, _vp, _c_dbl, _vp, _vp, _vp]),
-    "mc_interp_track_workspace_bytes": (_sz, [_c_int, _c_int]),
-    "mc_interp_track_batch": (_c_int, [_c_int, _c_int, _vp, _vp, _c_int, _vp, _c_dbl, _c_int, _c_dbl, _c_int, _vp, _vp, _vp,
-                                       _sz, _vp]),
-    "mc_min_bound_dists_batch": (_c_int, [_c_int, _c_int, _vp, _vp, _vp, _c_int, _vp, _vp, _c_int, _vp, _vp, _c_int, _c_dbl,
-                                          _c_dbl, _vp, _vp]),
-    "mc_traj_extrema_batch": (_c_int, [_c_int, _c_int, _vp, _vp, _vp, _vp, _vp, _c_dbl, _c_dbl, _vp, _vp]),
-    "mc_assemble_trajectory_batch": (_c_int, [_c_int, _c_int, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _c_int, _vp, _vp, _vp, _vp]),
-    "mc_check_normals_crossing_batch": (_c_int, [_c_int, _c_int, _vp, _vp, _vp, _c_int, _vp, _vp]),
-    "mc_prep_track_workspace_bytes": (_sz, [_c_int, _c_int, _c_int]),
-    "mc_prep_track_batch": (_c_int, [_c_int, _c_int, _vp, _vp, _c_int, _c_dbl, _c_dbl, _c_dbl, _c_dbl, _c_int, _c_int, _vp, _vp, _vp,
-                                     _vp, _sz, _vp]),
-    "mc_polygon_length_batch": (_c_int, [_c_int, _c_int, _vp, _vp, _c_int, _vp, _vp, _c_int, _c_dbl, _vp, _vp]),
-    "mc_jitter_widths_batch": (_c_int, [_c_int, _c_int, _vp, _c_int, _vp, _vp, _vp, _c_dbl, _vp, _vp, _vp]),
-    "mc_debug_read_profile": (_c_int, [_vp, _c_int]),
-    "mc_debug_factor_solve": (_c_int, [_c_int, _c_int, _vp, _vp, _vp, _sz, _vp]),
-}
-
-EXPORTED_SYMBOLS = tuple(_SIGS)
 
 
 class MinCurvLibError(RuntimeError):
     pass
+
+
+def _c_source(path: str) -> str:
+    """The C source in path without its comments and preprocessor lines."""
+    with open(path) as f:
+        txt = re.sub(r"/\*.*?\*/|//[^\n]*", " ", f.read(), flags=re.S)
+    return re.sub(r"^[ \t]*#[^\n]*", "", txt, flags=re.M)
+
+
+_SCALARS = {"int": ctypes.c_int, "double": ctypes.c_double, "size_t": ctypes.c_size_t}
+
+
+def _ctype(c: str, decl: str, ret: bool = False):
+    c = " ".join(c.replace("*", " * ").split())
+    if ret and c == "const char *":
+        return ctypes.c_char_p
+    if c.endswith("*"):
+        return ctypes.c_void_p
+    if c not in _SCALARS:
+        raise MinCurvLibError(f"{decl}: no ctypes type for the C type '{c}'")
+    return _SCALARS[c]
+
+
+def header_signatures(path: str) -> dict:
+    """name -> (restype, argtypes) of every declaration `ret mc_name(type name, ...);` in the C header at path."""
+    sigs = {}
+    for ret, name, args in re.findall(r"([\w\s*]+?)\b(mc_\w+)\s*\(([^)]*)\)\s*;", _c_source(path)):
+        params = [] if args.strip() in ("", "void") else [re.sub(r"\w+\s*$", "", p) for p in args.split(",")]
+        sigs[name] = (_ctype(ret, name, ret=True), [_ctype(p, name) for p in params])
+    return sigs
+
+
+_SIGS = header_signatures(_build.HEADER)
+EXPORTED_SYMBOLS = tuple(_SIGS)
+
+
+def slab_mirror():
+    """The names of enum Vec in csrc/mincurv_ws.cuh without V_ (the O(N) vectors at the head of a minimum-curvature
+    workspace slab, in slab order) and the constexpr ints of csrc/common.cuh, so that the host reads the layout the
+    kernels were compiled with."""
+    enum = re.search(r"enum\s+Vec\b[^{]*\{([^}]*)\}", _c_source(os.path.join(_build.CSRC, "mincurv_ws.cuh"))).group(1)
+    names = []
+    for i, (name, value) in enumerate(re.findall(r"(\w+)\s*(?:=\s*(\d+))?", enum)):
+        if name == "NUM_VEC":
+            break
+        if not name.startswith("V_") or (value and int(value) != i):
+            raise MinCurvLibError(f"enum Vec: cannot mirror entry {i} '{name}'")
+        names.append(name[2:])
+    consts = re.findall(r"constexpr\s+int\s+(\w+)\s*=\s*(\d+)\s*;", _c_source(os.path.join(_build.CSRC, "common.cuh")))
+    return names, {k: int(v) for k, v in consts}
 
 
 def lib_path() -> str:

@@ -20,8 +20,11 @@ import torch
 
 from . import _lib
 
-_GRID_Y_MAX = 65535  # tracks per launch of the kernels that put the track index on gridDim.y
-N_MIN = 80          # smallest closed track the banded solver supports (csrc/common.cuh N_MIN)
+# the workspace layout of the minimum-curvature path as the kernels were compiled with it (csrc/mincurv_ws.cuh,
+# csrc/common.cuh): debugging and tests read intermediate results out of the workspace
+SLAB_VECTORS, _CONSTS = _lib.slab_mirror()
+HB_PITCH, ZB_PITCH = _CONSTS["HB_PITCH"], _CONSTS["ZB_PITCH"]
+N_MIN = _CONSTS["N_MIN"]     # smallest closed track the banded solver supports
 STATUS_TEXT = {
     0: "ok",
     1: "Problem not solvable, track might be too small to run with current safety distance!",
@@ -39,17 +42,10 @@ VP_DECEL_SLICE_UPPER = 1    # tph.calc_vel_profile (closed): half of the doubled
 
 _WS = {}
 
-# mirror of csrc/mincurv_ws.cuh (debugging / tests read intermediate results out of the workspace)
-SLAB_VECTORS = ("H DIAG DFW DBW LFW INVD TII RHOP RHOM PX PY NX NY MX MY XP YP SX SY KREF LB UB F "
-                "T0 T1 T2 T3 T4 T5 ALPHA LU LL RD RHS DX DD DLU DLL SU SL ISU ISL HBSRC "
-                "S3 S4 L3 L4 KL WK EDX T3K T4K VV IH").split()
-HB_PITCH = 34
-ZB_PITCH = 108
-
 
 def mincurv_slab_layout(n_max: int) -> dict:
+    """make_layout of csrc/mincurv_ws.cuh: offsets of one instance's slab, in doubles."""
     np_ = ((n_max + 31) // 32) * 32 + 64
-    nb_max = max(1, (n_max - 32 + 31) // 32)
     o = len(SLAB_VECTORS) * np_
     o_zb = o
     o += n_max * ZB_PITCH
@@ -57,7 +53,7 @@ def mincurv_slab_layout(n_max: int) -> dict:
     o += np_ * HB_PITCH
     o_tiles = o
     o += np_ * 67
-    return dict(np=np_, nb_max=nb_max, o_zb=o_zb, o_hb=o_hb, o_tiles=o_tiles, stride=(o + 15) & ~15)
+    return dict(np=np_, o_zb=o_zb, o_hb=o_hb, o_tiles=o_tiles, stride=(o + 15) & ~15)
 
 
 def _require_cuda() -> None:
@@ -774,13 +770,10 @@ def min_bound_dists_batch(xy: torch.Tensor, psi: torch.Tensor, bound1: torch.Ten
     dev = xy.device
     out = torch.zeros((B, n_traj_max), dtype=torch.float64, device=dev)
     n_traj, nb1, nb2 = _npts(n_traj, B, dev), _npts(nb1, B, dev), _npts(nb2, B, dev)
-    for s in range(0, B, _GRID_Y_MAX):           # the track index is the y dimension of the launch grid
-        e = min(B, s + _GRID_Y_MAX)
-        rc = lib.mc_min_bound_dists_batch(e - s, n_traj_max, _rows_ptr(n_traj, s, e), _ptr(xy[s:e]), _ptr(psi[s:e]),
-                                          int(bound1.shape[1]), _rows_ptr(nb1, s, e), _ptr(bound1[s:e]), int(bound2.shape[1]),
-                                          _rows_ptr(nb2, s, e), _ptr(bound2[s:e]), int(bound1.shape[2]), float(length_veh),
-                                          float(width_veh), _ptr(out[s:e]), _stream())
-        _lib.check(rc, "mc_min_bound_dists_batch")
+    rc = lib.mc_min_bound_dists_batch(B, n_traj_max, _ptr(n_traj), _ptr(xy), _ptr(psi), int(bound1.shape[1]), _ptr(nb1),
+                                      _ptr(bound1), int(bound2.shape[1]), _ptr(nb2), _ptr(bound2), int(bound1.shape[2]),
+                                      float(length_veh), float(width_veh), _ptr(out), _stream())
+    _lib.check(rc, "mc_min_bound_dists_batch")
     return out
 
 
@@ -882,11 +875,9 @@ def check_normals_crossing_batch(track: torch.Tensor, normvec: torch.Tensor, hor
     if horizon >= smallest:
         raise RuntimeError("Horizon of %i points is too large for a track with %i points, reduce horizon!" % (horizon, smallest))
     crossing = torch.zeros((B,), dtype=torch.int32, device=dev)
-    for s in range(0, B, _GRID_Y_MAX):
-        e = min(B, s + _GRID_Y_MAX)
-        rc = lib.mc_check_normals_crossing_batch(e - s, n_max, _rows_ptr(n_pts, s, e), _ptr(track[s:e]), _ptr(normvec[s:e]),
-                                                 int(horizon), _ptr(crossing[s:e]), _stream())
-        _lib.check(rc, "mc_check_normals_crossing_batch")
+    rc = lib.mc_check_normals_crossing_batch(B, n_max, _ptr(n_pts), _ptr(track), _ptr(normvec), int(horizon), _ptr(crossing),
+                                             _stream())
+    _lib.check(rc, "mc_check_normals_crossing_batch")
     return crossing != 0
 
 

@@ -2,16 +2,18 @@
 loader when the shared library is missing or older than its sources."""
 from __future__ import annotations
 
+import glob
 import os
 import shutil
 import subprocess
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(_HERE, "csrc")
+INCLUDE = os.path.join(os.path.dirname(_HERE), "include")
+HEADER = os.path.join(INCLUDE, "mincurv_b200.h")      # the C-ABI; _lib derives its ctypes signatures from it
 LIB_PATH = os.path.join(_HERE, "libmincurv_b200.so")
-SOURCES = ["capi.cu", "mincurv_setup.cu", "mincurv_ipm.cu", "mincurv_finalize.cu", "splines.cu", "shortest_path.cu",
-           "vel_profile.cu", "traj_check.cu", "synth.cu", "prep_track.cu"]
-HEADERS = ["common.cuh", "mincurv_ws.cuh", "mincurv_ops.cuh", "vel_profile_core.cuh", "traj_check_core.cuh", os.path.join("..", "..", "include", "mincurv_b200.h")]
+SOURCES = sorted(glob.glob(os.path.join(CSRC, "*.cu")))
+HEADERS = sorted(glob.glob(os.path.join(CSRC, "*.cuh")) + glob.glob(os.path.join(INCLUDE, "*.h")))
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "-shared"]
 
@@ -27,8 +29,7 @@ def needs_build() -> bool:
     if not os.path.exists(LIB_PATH):
         return True
     t = os.path.getmtime(LIB_PATH)
-    deps = [os.path.join(CSRC, s) for s in SOURCES + HEADERS]
-    return any(os.path.getmtime(d) > t for d in deps)
+    return any(os.path.getmtime(d) > t for d in SOURCES + HEADERS)
 
 
 PROFILE_LIB_PATH = os.path.join(_HERE, "libmincurv_b200_prof.so")
@@ -38,7 +39,7 @@ def build_profile(verbose: bool = False, extra=(), out=None) -> str:
     """Instrumented build (-DMC_PROFILE: cycle counters inside the interior-point kernel, read with mc_debug_read_profile);
     a separate file, loaded only when MC_B200_LIB points at it (tools/prof_run.py).  Never the product library."""
     out = out or PROFILE_LIB_PATH
-    cmd = [_nvcc(), *NVCC_FLAGS, "-DMC_PROFILE", *extra, "-o", out, *[os.path.join(CSRC, s) for s in SOURCES]]
+    cmd = [_nvcc(), *NVCC_FLAGS, "-DMC_PROFILE", *extra, "-o", out, *SOURCES]
     if verbose:
         cmd.insert(1, "-Xptxas=-v")
     subprocess.check_call(cmd)
@@ -48,7 +49,7 @@ def build_profile(verbose: bool = False, extra=(), out=None) -> str:
 def build(force: bool = False, verbose: bool = False) -> str:
     if not force and not needs_build():
         return LIB_PATH
-    cmd = [_nvcc(), *NVCC_FLAGS, "-o", LIB_PATH, *[os.path.join(CSRC, s) for s in SOURCES]]
+    cmd = [_nvcc(), *NVCC_FLAGS, "-o", LIB_PATH, *SOURCES]
     if verbose:
         cmd.insert(1, "-Xptxas=-v")
     subprocess.check_call(cmd)

@@ -1,5 +1,6 @@
 // extern "C" boundary of libmincurv_b200.so -- see include/mincurv_b200.h for the contract and the
 // reference call sites each entry point replaces.
+#include <cstdarg>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -79,23 +80,20 @@ static int check_cuda(const char *what) {
     }
     return MC_OK;
 }
-static int bad(const char *msg) {
-    snprintf(g_err, sizeof(g_err), "%s", msg);
+__attribute__((format(printf, 1, 2))) static int bad(const char *fmt, ...) {
+    va_list ap;
+    va_start(ap, fmt);
+    vsnprintf(g_err, sizeof(g_err), fmt, ap);
+    va_end(ap);
     return MC_EINVAL;
+}
+static int small_workspace(const char *who) {
+    snprintf(g_err, sizeof(g_err), "%s: workspace too small", who);
+    return MC_EWORKSPACE;
 }
 static size_t align256(size_t b) { return (b + 255) & ~(size_t)255; }
 
 extern "C" {
-
-int mc_mincurv_kappa_batch(int, int, const int32_t *, double, double *, int32_t *, int32_t *, void *, size_t, void *);
-int mc_mincurv_solve_batch_shared(int, int, const int32_t *, const double *, const double *, const double *, double, double,
-                                  const double *, double, const int32_t *, double *, double *, double *, int32_t *, int32_t *, void *, size_t,
-                                  void *);
-int mc_mincurv_solve_batch_ex(int, int, const int32_t *, const double *, const double *, const double *, double, double,
-                              const double *, double, double *, double *, double *, int32_t *, int32_t *, void *, size_t, void *);
-int mc_vel_profile_batch_ex(int, int, const int32_t *, const double *, const double *, const double *, int, const double *,
-                            const double *, double, int, const double *, int, const double *, double, double, double, int, int,
-                            double *, double *, double *, double *, int32_t *, void *, size_t, void *);
 
 int mc_version(void) { return 100; }
 const char *mc_last_error(void) { return g_err; }
@@ -111,10 +109,8 @@ int mc_calc_splines_batch(int B, int n_max, const int32_t *n_pts, const double *
                           double *normvec, double *h_out, void *workspace, size_t workspace_bytes, void *stream) {
     if (B <= 0 || n_max < 3 || !xy || (xy_stride != 2 && xy_stride != 4)) return bad("mc_calc_splines_batch: bad argument");
     if ((coeffs_x == nullptr) != (coeffs_y == nullptr)) return bad("mc_calc_splines_batch: coeffs_x/coeffs_y must both be given or both NULL");
-    if (!workspace || workspace_bytes < mc_calc_splines_workspace_bytes(B, n_max)) {
-        snprintf(g_err, sizeof(g_err), "mc_calc_splines_batch: workspace too small");
-        return MC_EWORKSPACE;
-    }
+    if (!workspace || workspace_bytes < mc_calc_splines_workspace_bytes(B, n_max))
+        return small_workspace("mc_calc_splines_batch");
     mc::launch_calc_splines(B, n_max, n_pts, xy, xy_stride, el_lengths, use_dist_scaling, coeffs_x, coeffs_y, normvec,
                             h_out, (double *)workspace, (cudaStream_t)stream);
     return check_cuda("mc_calc_splines_batch");
@@ -130,11 +126,8 @@ size_t mc_mincurv_workspace_bytes(int B, int n_max) {
 
 static int mincurv_args(const char *who, int B, int n_max, void *workspace, size_t workspace_bytes) {
     if (B <= 0) return bad("mincurv: B <= 0");
-    if (n_max < mc::N_MIN) return bad("mincurv: n_max below the supported minimum (80 points)");
-    if (!workspace || workspace_bytes < mc_mincurv_workspace_bytes(B, n_max)) {
-        snprintf(g_err, sizeof(g_err), "%s: workspace too small", who);
-        return MC_EWORKSPACE;
-    }
+    if (n_max < mc::N_MIN) return bad("mincurv: n_max below the supported minimum (%d points)", mc::N_MIN);
+    if (!workspace || workspace_bytes < mc_mincurv_workspace_bytes(B, n_max)) return small_workspace(who);
     return MC_OK;
 }
 
@@ -338,10 +331,8 @@ int mc_shortest_path_solve_batch(int B, int n_max, const int32_t *n_pts, const d
                                  void *workspace, size_t workspace_bytes, void *stream) {
     if (B <= 0 || n_max < 3 || !reftrack || !normvec || !alpha || !status)
         return bad("mc_shortest_path_solve_batch: bad argument");
-    if (!workspace || workspace_bytes < mc_shortest_path_workspace_bytes(B, n_max)) {
-        snprintf(g_err, sizeof(g_err), "mc_shortest_path_solve_batch: workspace too small");
-        return MC_EWORKSPACE;
-    }
+    if (!workspace || workspace_bytes < mc_shortest_path_workspace_bytes(B, n_max))
+        return small_workspace("mc_shortest_path_solve_batch");
     if (mc::launch_shortest_path(B, n_max, n_pts, reftrack, normvec, w_veh, w_veh_batch, alpha, status, iters,
                                  (double *)workspace, (cudaStream_t)stream) != 0) {
         snprintf(g_err, sizeof(g_err), "shortest_path_kernel: launch configuration failed");
@@ -363,10 +354,8 @@ int mc_create_raceline_batch(int B, int n_max, const int32_t *n_pts, const doubl
         !(stepsize_interp > 0.0) || !coeffs_x || !coeffs_y || !spline_lengths || !n_out || !raceline_interp ||
         !spline_inds || !t_values || !s_interp || !el_lengths_interp)
         return bad("mc_create_raceline_batch: bad argument");
-    if (!workspace || workspace_bytes < mc_create_raceline_workspace_bytes(B, n_max)) {
-        snprintf(g_err, sizeof(g_err), "mc_create_raceline_batch: workspace too small");
-        return MC_EWORKSPACE;
-    }
+    if (!workspace || workspace_bytes < mc_create_raceline_workspace_bytes(B, n_max))
+        return small_workspace("mc_create_raceline_batch");
     mc::launch_create_raceline(B, n_max, n_pts, refline, ref_stride, normvec, alpha, stepsize_interp, n_out_max,
                                coeffs_x, coeffs_y, spline_lengths, n_out, raceline_interp, spline_inds, t_values,
                                s_interp, el_lengths_interp, psi, kappa, (double *)workspace, (cudaStream_t)stream);
@@ -417,10 +406,7 @@ int mc_iqp_relinearise_batch(int B, int n_max, const int32_t *n_pts, const int32
         return bad("mc_iqp_relinearise_batch: bad argument");
     size_t off[10];
     const size_t need = iqp_ws_parts(B, n_max, n_max_new, off);
-    if (!workspace || workspace_bytes < need) {
-        snprintf(g_err, sizeof(g_err), "mc_iqp_relinearise_batch: workspace too small");
-        return MC_EWORKSPACE;
-    }
+    if (!workspace || workspace_bytes < need) return small_workspace("mc_iqp_relinearise_batch");
     char *w = (char *)workspace;
     cudaStream_t s = (cudaStream_t)stream;
     double *spl = (double *)(w + off[0]);
@@ -470,10 +456,8 @@ int mc_vel_profile_batch_ex(int B, int n_max, const int32_t *n_pts, const double
     if (filt_window > 1 && (filt_window % 2 == 0 || filt_window >= n_max))
         return bad("mc_vel_profile_batch: filt_window must be odd (tph: 'Window width of moving average filter must be odd!')");
     if ((size_t)B * V > (size_t)0x7fffffff - 256) return bad("mc_vel_profile_batch: too many profiles in one call");
-    if (!workspace || workspace_bytes < mc_vel_profile_workspace_bytes(B, V, n_max)) {
-        snprintf(g_err, sizeof(g_err), "mc_vel_profile_batch: workspace too small");
-        return MC_EWORKSPACE;
-    }
+    if (!workspace || workspace_bytes < mc_vel_profile_workspace_bytes(B, V, n_max))
+        return small_workspace("mc_vel_profile_batch");
     if (mc::launch_vel_profile(B, V, n_max, n_pts, kappa, el_lengths, mu, ggv_scale, v_max_batch, v_max, n_ggv, ggv, n_mach,
                                ax_max_machines, dyn_model_exp, drag_coeff, m_veh, filt_window, decel_slice_upper != 0, vx, ax, t,
                                laptime, status, (double *)workspace, (cudaStream_t)stream) != 0)
@@ -502,10 +486,8 @@ int mc_interp_track_batch(int B, int n_max, const int32_t *n_pts, const double *
     if (B <= 0 || n_max < 2 || !pts || (stride != 2 && stride != 4) || !(stepsize_approx > 0.0) || n_out_max <= 0 || !out ||
         !n_out || (normvec && (stride != 4 || (width_col != 2 && width_col != 3))))
         return bad("mc_interp_track_batch: bad argument");
-    if (!workspace || workspace_bytes < mc_interp_track_workspace_bytes(B, n_max)) {
-        snprintf(g_err, sizeof(g_err), "mc_interp_track_batch: workspace too small");
-        return MC_EWORKSPACE;
-    }
+    if (!workspace || workspace_bytes < mc_interp_track_workspace_bytes(B, n_max))
+        return small_workspace("mc_interp_track_batch");
     mc::launch_interp_track(B, n_max, n_pts, pts, stride, normvec, normal_sign, normvec ? width_col : 2, stepsize_approx,
                             n_out_max, out, n_out, (double *)workspace, (cudaStream_t)stream);
     return check_cuda("interp_track_kernel");
@@ -514,7 +496,7 @@ int mc_interp_track_batch(int B, int n_max, const int32_t *n_pts, const double *
 int mc_min_bound_dists_batch(int B, int n_traj_max, const int32_t *n_traj, const double *xy, const double *psi, int nb1_max,
                              const int32_t *nb1, const double *bound1, int nb2_max, const int32_t *nb2, const double *bound2,
                              int bound_stride, double length_veh, double width_veh, double *min_dists, void *stream) {
-    if (B <= 0 || B > 65535 || n_traj_max <= 0 || !xy || !psi || !bound1 || !bound2 || nb1_max <= 0 || nb2_max <= 0 ||
+    if (B <= 0 || n_traj_max <= 0 || !xy || !psi || !bound1 || !bound2 || nb1_max <= 0 || nb2_max <= 0 ||
         bound_stride < 2 || !min_dists)
         return bad("mc_min_bound_dists_batch: bad argument");
     mc::launch_min_bound_dists(B, n_traj_max, n_traj, xy, psi, nb1_max, nb1, bound1, nb2_max, nb2, bound2, bound_stride,
@@ -542,7 +524,7 @@ int mc_assemble_trajectory_batch(int B, int n_max, const int32_t *n_traj, const 
 
 int mc_check_normals_crossing_batch(int B, int n_max, const int32_t *n_pts, const double *track, const double *normvec,
                                     int horizon, int32_t *crossing, void *stream) {
-    if (B <= 0 || B > 65535 || n_max < 3 || !track || !normvec || horizon < 1 || !crossing)
+    if (B <= 0 || n_max < 3 || !track || !normvec || horizon < 1 || !crossing)
         return bad("mc_check_normals_crossing_batch: bad argument");
     mc::launch_normals_crossing(B, n_max, n_pts, track, normvec, horizon, crossing, (cudaStream_t)stream);
     return check_cuda("normals_crossing_kernel");
@@ -561,10 +543,8 @@ int mc_prep_track_batch(int B, int n_raw_max, const int32_t *n_raw, const double
         n_out_max < 4 || !reftrack_interp || !n_out)
         return bad("mc_prep_track_batch: bad argument");
     if (k_reg != 3) return bad("mc_prep_track_batch: only cubic splines (k_reg = 3, the reference's setting) are implemented");
-    if (!workspace || workspace_bytes < mc_prep_track_workspace_bytes(B, n_raw_max, n_int_max)) {
-        snprintf(g_err, sizeof(g_err), "mc_prep_track_batch: workspace too small");
-        return MC_EWORKSPACE;
-    }
+    if (!workspace || workspace_bytes < mc_prep_track_workspace_bytes(B, n_raw_max, n_int_max))
+        return small_workspace("mc_prep_track_batch");
     mc::launch_prep_track(B, n_raw_max, n_raw, track, s_reg, stepsize_prep, stepsize_reg, min_width, n_int_max, n_out_max,
                           reftrack_interp, n_out, smoothing_lambda, (double *)workspace, (cudaStream_t)stream);
     return check_cuda("prep_track_kernel");

@@ -21,8 +21,15 @@ constexpr int ZB_PITCH = 108;    // per-point scratch row of the assembly: three
 constexpr int HBW = 32;          // half-bandwidth kept of H = E^T E (truncation error ~1e-10 on alpha)
 constexpr int HB_PITCH = 34;     // 33 used, padded so that a row is a multiple of 16 bytes
 constexpr int N_MIN = 80;        // smallest supported closed track (band must not wrap onto itself)
-constexpr double F_SCALE_DEFAULT = 2.0;  // tph: f carries a factor 2 that H does not (SURVEY.md A.3); run-time parameter f_scale of mc_mincurv_setup_batch_ex
 constexpr double FIX_EPS = 1e-8; // half-width given to variables whose box has collapsed (lb == ub)
+
+// Kernels that put the track index on blockIdx.y see at most 65535 tracks per launch: launch(b0, nb) is called for
+// consecutive chunks of nb <= 65535 tracks starting at track b0, and offsets its pointers by b0.
+template <class Launch>
+inline void for_grid_y_chunks(int B, Launch &&launch) {
+    constexpr int GRID_Y_MAX = 65535;
+    for (int b0 = 0; b0 < B; b0 += GRID_Y_MAX) launch(b0, B - b0 < GRID_Y_MAX ? B - b0 : GRID_Y_MAX);
+}
 
 __device__ __forceinline__ int wrapi(int i, int n) {
     i %= n;

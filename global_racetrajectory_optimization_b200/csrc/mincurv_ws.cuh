@@ -27,7 +27,6 @@ enum Vec : int {
 struct Layout {
     int n_max;
     int np;          // padded vector length (multiple of 32, >= n_max + 64)
-    int nb_max;      // (n_max - 32) / 32 rounded up (kept for the Python mirror of the layout)
     size_t o_zb, o_hb, o_tiles, stride;   // in doubles
 };
 
@@ -35,8 +34,6 @@ __host__ __device__ inline Layout make_layout(int n_max) {
     Layout L;
     L.n_max = n_max;
     L.np = ((n_max + 31) / 32) * 32 + 64;
-    L.nb_max = (n_max - 32 + 31) / 32;
-    if (L.nb_max < 1) L.nb_max = 1;
     size_t o = (size_t)NUM_VEC * L.np;
     L.o_zb = o;
     o += (size_t)n_max * ZB_PITCH;

@@ -425,13 +425,12 @@ void launch_create_raceline(int B, int n_max, const int32_t *n_pts, const double
 void launch_head_curv(int B, int n_max, const double *cx, const double *cy, int n_eval_max, const int32_t *n_eval,
                       const int32_t *ind, const double *t, double *psi, double *kappa, double *dkappa,
                       cudaStream_t stream) {
-    for (int b0 = 0; b0 < B; b0 += 65535) {         // the track index is gridDim.y (<= 65535 per launch)
-        const int nb = (B - b0 < 65535) ? B - b0 : 65535;
+    for_grid_y_chunks(B, [&](int b0, int nb) {
         const size_t oe = (size_t)b0 * n_eval_max, oc = (size_t)b0 * n_max * 4;
         dim3 grid((n_eval_max + 255) / 256, nb);
         head_curv_kernel<<<grid, 256, 0, stream>>>(n_max, cx + oc, cy + oc, n_eval_max, n_eval ? n_eval + b0 : nullptr, ind + oe,
                                                    t + oe, psi + oe, kappa ? kappa + oe : nullptr, dkappa ? dkappa + oe : nullptr);
-    }
+    });
 }
 void launch_iqp_new_reftrack(int B, int n_max, const int32_t *n_pts, const int32_t *active, const double *reftrack,
                              const double *normvec, const double *alpha, int n_max_new, const int32_t *n_new,
@@ -495,11 +494,10 @@ void launch_iqp_finish(int B, int n_max, int n_cap, int it, int iters_min, doubl
 }
 
 void launch_scale_alpha(int B, int n_max, double *alpha, const double *scale_batch, double scale, cudaStream_t stream) {
-    for (int b0 = 0; b0 < B; b0 += 65535) {         // the track index is gridDim.y (<= 65535 per launch)
-        const int nb = (B - b0 < 65535) ? B - b0 : 65535;
+    for_grid_y_chunks(B, [&](int b0, int nb) {
         dim3 grid((n_max + 255) / 256, nb);
         scale_alpha_kernel<<<grid, 256, 0, stream>>>(n_max, alpha + (size_t)b0 * n_max, scale_batch ? scale_batch + b0 : nullptr, scale);
-    }
+    });
 }
 
 }  // namespace mc

@@ -127,9 +127,14 @@ __global__ void __launch_bounds__(MB_THREADS) min_bound_dists_kernel(int n_traj_
 void launch_min_bound_dists(int B, int n_traj_max, const int32_t *n_traj, const double *xy, const double *psi, int nb_max1,
                             const int32_t *nb1, const double *bound1, int nb_max2, const int32_t *nb2, const double *bound2,
                             int bstride, double length_veh, double width_veh, double *min_dists, cudaStream_t stream) {
-    dim3 grid((n_traj_max + MB_THREADS - 1) / MB_THREADS, B);
-    min_bound_dists_kernel<<<grid, MB_THREADS, 0, stream>>>(n_traj_max, n_traj, xy, psi, nb_max1, nb1, bound1, nb_max2, nb2,
-                                                            bound2, bstride, length_veh, width_veh, min_dists);
+    for_grid_y_chunks(B, [&](int b0, int nb) {
+        const size_t ot = (size_t)b0 * n_traj_max;
+        dim3 grid((n_traj_max + MB_THREADS - 1) / MB_THREADS, nb);
+        min_bound_dists_kernel<<<grid, MB_THREADS, 0, stream>>>(
+            n_traj_max, n_traj ? n_traj + b0 : nullptr, xy + 2 * ot, psi + ot, nb_max1, nb1 ? nb1 + b0 : nullptr,
+            bound1 + (size_t)b0 * nb_max1 * bstride, nb_max2, nb2 ? nb2 + b0 : nullptr, bound2 + (size_t)b0 * nb_max2 * bstride,
+            bstride, length_veh, width_veh, min_dists + ot);
+    });
 }
 
 // ---- extrema tested by check_traj ---------------------------------------------------------------------------------
@@ -220,8 +225,11 @@ __global__ void __launch_bounds__(128) normals_crossing_kernel(int n_max, const 
 void launch_normals_crossing(int B, int n_max, const int32_t *n_pts, const double *track, const double *normvec, int horizon,
                              int32_t *crossing, cudaStream_t stream) {
     cudaMemsetAsync(crossing, 0, (size_t)B * sizeof(int32_t), stream);
-    dim3 grid((n_max + 127) / 128, B);
-    normals_crossing_kernel<<<grid, 128, 0, stream>>>(n_max, n_pts, track, normvec, horizon, crossing);
+    for_grid_y_chunks(B, [&](int b0, int nb) {
+        dim3 grid((n_max + 127) / 128, nb);
+        normals_crossing_kernel<<<grid, 128, 0, stream>>>(n_max, n_pts ? n_pts + b0 : nullptr, track + (size_t)b0 * n_max * 4,
+                                                          normvec + (size_t)b0 * n_max * 2, horizon, crossing + b0);
+    });
 }
 
 }  // namespace mc

@@ -13,6 +13,7 @@
  *   - all arrays are float64 unless stated, batch-major, row-major, padded to n_max points per track;
  *     n_pts[b] (int32, may be NULL => every track has n_max points) is the true size of track b;
  *   - `stream` is a cudaStream_t passed as void*; calls are asynchronous and stream-ordered;
+ *   - arguments are int, double, size_t or pointers: the package's ctypes binding is parsed from these declarations;
  *   - return value: 0 = ok, <0 = bad argument (-1), CUDA error (-2), workspace too small (-3);
  *   - per-instance results are reported in status[b] (int32):
  *       0 ok | 1 track too narrow ("Problem not solvable, track might be too small ...", tph RuntimeError)

@@ -84,17 +84,16 @@ def test_shared_centre_ids_and_their_chunking(fake, monkeypatch):
         B_.opt_min_curv_batch(rt, nv, h, 0.12, 2.0, centre_id=cid[:4])
 
 
-def test_launches_with_the_track_index_on_grid_y_are_chunked(fake, monkeypatch):
-    monkeypatch.setattr(B_, "_GRID_Y_MAX", 2)
-    B, n = 5, 100
+def test_launches_with_the_track_index_on_grid_y_take_the_whole_batch(fake):
+    """The library splits these launches into chunks of at most 65535 tracks (gridDim.y) itself: one call per batch."""
+    B, n = 65535 + 7, 3
     rt = torch.rand((B, n, 4), dtype=torch.float64)
     nv = torch.rand((B, n, 2), dtype=torch.float64)
-    B_.check_normals_crossing_batch(rt, nv, 10)
-    B_.min_bound_dists_batch(torch.rand((B, 50, 2), dtype=torch.float64), torch.rand((B, 50), dtype=torch.float64), rt, rt,
+    B_.check_normals_crossing_batch(rt, nv, 1)
+    B_.min_bound_dists_batch(torch.rand((B, 1, 2), dtype=torch.float64), torch.rand((B, 1), dtype=torch.float64), rt, rt,
                              4.7, 2.0)
-    sizes = [c[1][0] for c in fake.calls if c[0] == "mc_check_normals_crossing_batch"]
-    assert sizes == [2, 2, 1]
-    assert [c[1][0] for c in fake.calls if c[0] == "mc_min_bound_dists_batch"] == [2, 2, 1]
+    assert [c[1][0] for c in fake.calls if c[0] == "mc_check_normals_crossing_batch"] == [B]
+    assert [c[1][0] for c in fake.calls if c[0] == "mc_min_bound_dists_batch"] == [B]
 
 
 @pytest.mark.parametrize("opt_type", ["mincurv", "shortest_path"])

@@ -127,6 +127,45 @@ def test_assemble_trajectory_matches_main_globaltraj(golden):
         assert np.all(out[i, want.shape[0]:].cpu().numpy() == 0.0)
 
 
+def _ring_tracks(B, K=7):
+    """B small closed tracks cycling through K ring shapes of 16 points (radius 10-11 m, outward normals): even shapes are
+    narrow, odd ones reach past the centre on the left, where the normals cross.  7 does not divide 65535, so the rows
+    after a 65535-track chunk boundary differ from the first rows of the batch, and so do the per-track counts."""
+    g = torch.Generator().manual_seed(5)
+    ang = torch.arange(16, dtype=torch.float64) * (2 * np.pi / 16)
+    normal = torch.stack((ang.cos(), ang.sin()), dim=1).expand(K, 16, 2)
+    centre = normal * (10.0 + torch.rand((K, 16, 1), generator=g, dtype=torch.float64))
+    w_left = torch.where(torch.arange(K) % 2 == 1, 12.0, 2.0).to(torch.float64)[:, None].expand(K, 16)
+    widths = torch.stack((torch.full((K, 16), 2.0, dtype=torch.float64), w_left), dim=2)
+    psi = torch.rand((K, 8), generator=g, dtype=torch.float64) * 6.0 - 3.0
+    k = torch.arange(B) % K
+    b = torch.arange(B, dtype=torch.int32)
+    dev = torch.device("cuda")
+    return dict(track=torch.cat((centre, widths), dim=2)[k].to(dev), normvec=normal[k].contiguous().to(dev),
+                xy=centre[:, ::2][k].contiguous().to(dev), psi=psi[k].to(dev),
+                bound_r=(centre + normal * widths[:, :, :1])[k].to(dev), bound_l=(centre - normal * widths[:, :, 1:])[k].to(dev),
+                n_pts=(12 + b % 4).to(dev), n_traj=(5 + b % 4).to(dev), nb1=(16 - b % 11).to(dev), nb2=(16 - b % 9).to(dev))
+
+
+def _ring_checks(t, rows=slice(None)):
+    r = {k: v[rows].contiguous() for k, v in t.items()}
+    md = B_.min_bound_dists_batch(r["xy"], r["psi"], r["bound_r"], r["bound_l"], 4.7, 2.0, n_traj=r["n_traj"], nb1=r["nb1"],
+                                  nb2=r["nb2"])
+    return md, B_.check_normals_crossing_batch(r["track"], r["normvec"], 3, n_pts=r["n_pts"])
+
+
+def test_batches_beyond_the_grid_y_limit_match_a_small_batch():
+    """min_bound_dists and check_normals_crossing put the track index on gridDim.y, at most 65535 per launch; the library
+    runs larger batches in chunks.  The rows on both sides of the chunk boundary equal a run of the same rows alone."""
+    B = 65535 + 7
+    t = _ring_tracks(B)
+    md, crossing = _ring_checks(t)
+    rows = slice(65535 - 3, B)
+    md_small, crossing_small = _ring_checks(t, rows)
+    assert torch.equal(md[rows], md_small) and torch.equal(crossing[rows], crossing_small)
+    assert bool((md_small[:, :5] > 0).all()) and bool(crossing_small.any()) and not bool(crossing_small.all())
+
+
 def test_check_normals_crossing_batch_vs_oracle(golden):
     """tph.check_normals_crossing (prep_track.py:57-59; tph restatement, parity unpinned) on widened fixtures."""
     import global_racetrajectory_optimization_b200 as tph

@@ -36,6 +36,34 @@ def test_library_exports_every_declared_symbol():
     assert lib.mc_version() >= 100
 
 
+def test_ctypes_signatures_are_parsed_from_the_header(tmp_path):
+    c_int, c_dbl, vp = ctypes.c_int, ctypes.c_double, ctypes.c_void_p
+    sigs = _lib._SIGS
+    assert sigs["mc_last_error"] == (ctypes.c_char_p, [])
+    assert sigs["mc_mincurv_workspace_bytes"] == (ctypes.c_size_t, [c_int, c_int])
+    res, args = sigs["mc_mincurv_solve_batch_shared"]
+    assert res is c_int and len(args) == 19 and [k for k, a in enumerate(args) if a is c_dbl] == [6, 7, 9]
+    assert args[-2] is ctypes.c_size_t and args.count(c_int) == 2
+    assert sigs["mc_iqp_finish_batch"] == (c_int, [c_int] * 5 + [c_dbl, c_int, c_int] + [vp] * 16)
+    bad = tmp_path / "bad.h"
+    bad.write_text("/* a comment */\n#define X 1\nint mc_ok(const int32_t *p, double d);\nint mc_bad(int n, float x);\n")
+    with pytest.raises(_lib.MinCurvLibError, match="mc_bad.*float"):
+        _lib.header_signatures(str(bad))
+    bad.write_text("int mc_ok(const int32_t *p, double d);\n")
+    assert _lib.header_signatures(str(bad)) == {"mc_ok": (c_int, [vp, c_dbl])}
+
+
+@pytest.mark.parametrize("n", [80, 81, 129, 257, 1000, 2000])
+def test_slab_layout_mirror_matches_the_library(n):
+    """batch's slab layout (read from csrc/mincurv_ws.cuh and csrc/common.cuh) against the library's workspace size: for 32
+    instances the slabs are a multiple of 256 bytes, and the work counter adds 256."""
+    from global_racetrajectory_optimization_b200 import batch as B_
+    lib = _lib.load()
+    assert B_.mincurv_slab_layout(n)["stride"] == lib.mc_mincurv_workspace_bytes(32, n) // 256 - 1
+    assert lib.mc_mincurv_workspace_bytes(1, B_.N_MIN) > 0 and lib.mc_mincurv_workspace_bytes(1, B_.N_MIN - 1) == 0
+    assert B_.SLAB_VECTORS[0] == "H" and B_.SLAB_VECTORS[-1] == "IH"
+
+
 def test_workspace_queries_and_argument_validation_without_gpu():
     lib = _lib.load()
     assert lib.mc_mincurv_workspace_bytes(4, 1000) > 4 * 1000 * 34 * 8
