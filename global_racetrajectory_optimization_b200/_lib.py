@@ -47,6 +47,11 @@ def header_signatures(path: str) -> dict:
 
 _SIGS = header_signatures(_build.HEADER)
 EXPORTED_SYMBOLS = tuple(_SIGS)
+# the shortest path's sensitivity entries (batch.opt_shortest_path_diff): exported by the same library, declared in a header
+# of their own; load() binds them with the rest
+_SP_SENS_SIGS = header_signatures(_build.SP_SENS_HEADER)
+SP_SENS_SYMBOLS = tuple(_SP_SENS_SIGS)
+_SIGS.update(_SP_SENS_SIGS)
 
 
 def slab_mirror():

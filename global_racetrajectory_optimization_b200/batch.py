@@ -254,6 +254,15 @@ def _mincurv_launch(entry: str, chunk: int, n_pts, reftrack, normvec, h, kappa_b
         _lib.check(rc, entry)
 
 
+def _refuse(strict: bool, wanted: torch.Tensor, gs: torch.Tensor, who: str, what: str) -> None:
+    """strict: raise if an instance with a nonzero upstream gradient (wanted [B]) has grad_status gs != 0."""
+    bad = wanted & (gs != 0)
+    if strict and bool(bad.any()):
+        idx = bad.nonzero().flatten()
+        raise _lib.MinCurvLibError(f"{who} for {idx.numel()} instance(s) {what} (first: {idx[:8].tolist()}, "
+                                   f"grad_status {gs[idx[:8]].tolist()}); strict=False gives them zero gradients")
+
+
 class _MinCurvDiff(torch.autograd.Function):
     """alpha of the min-curvature QP as a function of the widths; see opt_min_curv_diff."""
 
@@ -279,15 +288,8 @@ class _MinCurvDiff(torch.autograd.Function):
         dev = centre.device
         grad_alpha = grad_alpha.to(dtype=torch.float64).contiguous()
         wanted = (grad_alpha != 0).any(dim=1)
-
-        def refuse(gs, what):
-            bad = wanted & (gs != 0)
-            if ctx.strict and bool(bad.any()):
-                idx = bad.nonzero().flatten()
-                raise _lib.MinCurvLibError(
-                    f"opt_min_curv_diff: no width gradient for {idx.numel()} instance(s) {what} (first: {idx[:8].tolist()}, "
-                    f"grad_status {gs[idx[:8]].tolist()}); strict=False gives them zero gradients")
-        refuse(grad_status, "with a nonzero upstream gradient")
+        who = "opt_min_curv_diff: no width gradient"
+        _refuse(ctx.strict, wanted, grad_status, who, "with a nonzero upstream gradient")
         gs = grad_status.clone()            # (the adjoint sets 3 where its factorisation breaks down)
         reftrack = torch.cat((centre, widths), dim=2).contiguous()
         gwr = torch.empty((B, n_max), dtype=torch.float64, device=dev)
@@ -295,7 +297,7 @@ class _MinCurvDiff(torch.autograd.Function):
         gwv = torch.empty((B,), dtype=torch.float64, device=dev)
         _mincurv_launch("mc_mincurv_adjoint_batch", ctx.chunk, n_pts, reftrack, normvec, h, None, ctx.w_scalar, w_veh_t,
                         ctx.f_scale, centre_id, sens, gs, grad_alpha, gwr, gwl, gwv)
-        refuse(gs, "whose adjoint factorisation broke down")
+        _refuse(ctx.strict, wanted, gs, who, "whose adjoint factorisation broke down")
         return (torch.stack((gwr, gwl), dim=2), gwv if w_veh_t is not None else None) + (None,) * 10
 
 
@@ -335,14 +337,9 @@ def opt_shortest_path_batch(reftrack: torch.Tensor, normvec: torch.Tensor, w_veh
     """Batched tph.opt_shortest_path.  Returns dict(alpha, status, iters)."""
     _require_cuda()
     lib = _lib.load()
-    reftrack = _f64(reftrack, "reftrack")
-    normvec = _f64(normvec, "normvec")
-    B, n_max, four = reftrack.shape
-    if four != 4 or normvec.shape != (B, n_max, 2):
-        raise RuntimeError("Array size of reftrack should be the same as normvectors!")
+    reftrack, normvec, n_pts, w_scalar, w_batch = _shortest_path_inputs(reftrack, normvec, w_veh, n_pts)
+    B, n_max, _ = reftrack.shape
     dev = reftrack.device
-    n_pts = _npts(n_pts, B, dev)
-    w_scalar, w_batch = _wveh(w_veh, B, dev)
     alpha = torch.empty((B, n_max), dtype=torch.float64, device=dev)
     status = torch.empty((B,), dtype=torch.int32, device=dev)
     iters = torch.empty((B,), dtype=torch.int32, device=dev)
@@ -351,6 +348,82 @@ def opt_shortest_path_batch(reftrack: torch.Tensor, normvec: torch.Tensor, w_veh
                                           _ptr(alpha), _ptr(status), _ptr(iters), _ptr(ws), ws.numel(), _stream())
     _lib.check(rc, "mc_shortest_path_solve_batch")
     return dict(alpha=alpha, status=status, iters=iters)
+
+
+def _shortest_path_inputs(reftrack, normvec, w_veh, n_pts):
+    """The checked inputs of opt_shortest_path_batch and opt_shortest_path_diff: reftrack [B, n_max, 4] and normvec
+    [B, n_max, 2] as contiguous float64 CUDA tensors, n_pts (int32 or None) and the w_veh pair of _wveh."""
+    reftrack = _f64(reftrack, "reftrack")
+    normvec = _f64(normvec, "normvec")
+    B, n_max, four = reftrack.shape
+    if four != 4 or normvec.shape != (B, n_max, 2):
+        raise RuntimeError("Array size of reftrack should be the same as normvectors!")
+    return (reftrack, normvec, _npts(n_pts, B, reftrack.device)) + _wveh(w_veh, B, reftrack.device)
+
+
+class _ShortestPathDiff(torch.autograd.Function):
+    """alpha of the shortest-path QP as a function of the reftrack, the normals and w_veh; see opt_shortest_path_diff."""
+
+    @staticmethod
+    def forward(ctx, reftrack, normvec, w_veh_t, w_scalar, n_pts, strict):
+        lib = _lib.load()
+        B, n_max, _ = reftrack.shape
+        f64, i32 = dict(dtype=torch.float64, device=reftrack.device), dict(dtype=torch.int32, device=reftrack.device)
+        alpha, status, iters = torch.empty((B, n_max), **f64), torch.empty((B,), **i32), torch.empty((B,), **i32)
+        sens, grad_status = torch.empty((B, 2, n_max), **f64), torch.empty((B,), **i32)
+        ws = _workspace("shortest", lib.mc_shortest_path_workspace_bytes(B, n_max), reftrack.device)
+        rc = lib.mc_shortest_path_solve_batch_sens(B, n_max, _ptr(n_pts), _ptr(reftrack), _ptr(normvec), w_scalar,
+                                                   _ptr(w_veh_t), _ptr(alpha), _ptr(status), _ptr(iters), _ptr(sens),
+                                                   _ptr(grad_status), _ptr(ws), ws.numel(), _stream())
+        _lib.check(rc, "mc_shortest_path_solve_batch_sens")
+        ctx.save_for_backward(reftrack, normvec, w_veh_t, n_pts, alpha, sens, grad_status)
+        ctx.w_scalar, ctx.strict = w_scalar, strict
+        ctx.mark_non_differentiable(status, iters, grad_status)
+        return alpha, status, iters, grad_status
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, grad_alpha, *_unused):
+        reftrack, normvec, w_veh_t, n_pts, alpha, sens, grad_status = ctx.saved_tensors
+        lib = _lib.load()
+        B, n_max, _ = reftrack.shape
+        f64 = dict(dtype=torch.float64, device=reftrack.device)
+        grad_alpha = grad_alpha.to(dtype=torch.float64).contiguous()
+        wanted = (grad_alpha != 0).any(dim=1)
+        who = "opt_shortest_path_diff: no gradient"
+        _refuse(ctx.strict, wanted, grad_status, who, "with a nonzero upstream gradient")
+        gs = grad_status.clone()            # (the adjoint sets 3 where its solution is not finite)
+        need_rt, need_nv, need_wv = ctx.needs_input_grad[:3]
+        grt = torch.empty((B, n_max, 4), **f64)
+        gnv = torch.empty((B, n_max, 2), **f64) if need_nv else None
+        gwv = torch.empty((B,), **f64) if need_wv else None
+        ws = _workspace("shortest", lib.mc_shortest_path_workspace_bytes(B, n_max), reftrack.device)
+        rc = lib.mc_shortest_path_adjoint_batch(B, n_max, _ptr(n_pts), _ptr(reftrack), _ptr(normvec), ctx.w_scalar,
+                                                _ptr(w_veh_t), _ptr(alpha), _ptr(sens), _ptr(gs), _ptr(grad_alpha), _ptr(grt),
+                                                _ptr(gnv), _ptr(gwv), _ptr(ws), ws.numel(), _stream())
+        _lib.check(rc, "mc_shortest_path_adjoint_batch")
+        _refuse(ctx.strict, wanted, gs, who, "whose adjoint solution is not finite")
+        return grt if need_rt else None, gnv, gwv, None, None, None
+
+
+@_device_guard
+def opt_shortest_path_diff(reftrack: torch.Tensor, normvec: torch.Tensor, w_veh: Union[float, torch.Tensor],
+                           n_pts: Optional[torch.Tensor] = None, strict: bool = True) -> dict:
+    """opt_shortest_path_batch with alpha differentiable with respect to the reftrack, the normals and the vehicle width
+    (autograd).
+
+    Returns the dict of opt_shortest_path_batch (alpha, status, iters: the same values) plus grad_status [B] (int32).
+    alpha carries a grad_fn: backward() / torch.autograd.grad give dL/dreftrack [B, n_max, 4] (x, y at fixed normals,
+    w_tr_right, w_tr_left), dL/dnormvec [B, n_max, 2] and, for a tensor w_veh, dL/dw_veh, at the cost of one cyclic
+    tridiagonal solve per instance (implicit differentiation of the KKT conditions, DESIGN.md section 3.11).  Any of the
+    three may be a constant.  Widths whose bound tph clamps to 0.001 m get zero gradients.
+    grad_status: 0 = the gradient is computed; otherwise the solve's status (2, 3, -1).  strict=True: backward raises if
+    an instance with a nonzero upstream gradient has grad_status != 0 (or a non-finite adjoint solution); strict=False:
+    such instances get zero gradients."""
+    _require_cuda()
+    reftrack, normvec, n_pts, w_scalar, w_batch = _shortest_path_inputs(reftrack, normvec, w_veh, n_pts)
+    alpha, status, iters, grad_status = _ShortestPathDiff.apply(reftrack, normvec, w_batch, w_scalar, n_pts, bool(strict))
+    return dict(alpha=alpha, status=status, iters=iters, grad_status=grad_status)
 
 
 def _closed_polygon_length(pts: torch.Tensor, n_pts: Optional[torch.Tensor], normvec: Optional[torch.Tensor] = None,

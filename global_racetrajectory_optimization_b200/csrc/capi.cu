@@ -7,6 +7,7 @@
 
 #include "../../include/mincurv_b200.h"
 #include "mincurv_ws.cuh"
+#include "shortest_path_sens.h"
 
 namespace mc {
 size_t spline_ws_doubles(int n_max);
@@ -45,6 +46,11 @@ void launch_iqp_finish(int, int, int, int, int, double, int, int, int32_t *, con
 size_t shortest_path_ws_doubles(int n_max);
 int launch_shortest_path(int, int, const int32_t *, const double *, const double *, double, const double *, double *,
                          int32_t *, int32_t *, double *, cudaStream_t);
+void launch_shortest_path_sens_export(int, int, const int32_t *, const int32_t *, const double *, double *, int32_t *,
+                                      cudaStream_t);
+void launch_shortest_path_adjoint(int, int, const int32_t *, const double *, const double *, double, const double *,
+                                  const double *, const double *, int32_t *, const double *, double *, double *, double *,
+                                  double *, cudaStream_t);
 size_t vel_profile_ws_doubles(int n_max);
 int launch_vel_profile(int, int, int, const int32_t *, const double *, const double *, const double *, const double *,
                        const double *, double, int, const double *, int, const double *, double, double, double, int, int,
@@ -339,6 +345,34 @@ int mc_shortest_path_solve_batch(int B, int n_max, const int32_t *n_pts, const d
         return MC_ECUDA;
     }
     return check_cuda("shortest_path_kernel");
+}
+
+int mc_shortest_path_solve_batch_sens(int B, int n_max, const int32_t *n_pts, const double *reftrack, const double *normvec,
+                                      double w_veh, const double *w_veh_batch, double *alpha, int32_t *status, int32_t *iters,
+                                      double *sens, int32_t *grad_status, void *workspace, size_t workspace_bytes,
+                                      void *stream) {
+    if (!sens || !grad_status) return bad("mc_shortest_path_solve_batch_sens: NULL argument");
+    int rc = mc_shortest_path_solve_batch(B, n_max, n_pts, reftrack, normvec, w_veh, w_veh_batch, alpha, status, iters,
+                                          workspace, workspace_bytes, stream);
+    if (rc) return rc;
+    // the workspace still holds the final iterate
+    mc::launch_shortest_path_sens_export(B, n_max, n_pts, status, (const double *)workspace, sens, grad_status,
+                                         (cudaStream_t)stream);
+    return check_cuda("shortest_path_sens_export_kernel");
+}
+
+int mc_shortest_path_adjoint_batch(int B, int n_max, const int32_t *n_pts, const double *reftrack, const double *normvec,
+                                   double w_veh, const double *w_veh_batch, const double *alpha, const double *sens,
+                                   int32_t *grad_status, const double *grad_alpha, double *grad_reftrack, double *grad_normvec,
+                                   double *grad_w_veh, void *workspace, size_t workspace_bytes, void *stream) {
+    if (B <= 0 || n_max < 3 || !reftrack || !normvec || !alpha || !sens || !grad_status || !grad_alpha || !grad_reftrack)
+        return bad("mc_shortest_path_adjoint_batch: bad argument");
+    if (!workspace || workspace_bytes < mc_shortest_path_workspace_bytes(B, n_max))
+        return small_workspace("mc_shortest_path_adjoint_batch");
+    mc::launch_shortest_path_adjoint(B, n_max, n_pts, reftrack, normvec, w_veh, w_veh_batch, alpha, sens, grad_status,
+                                     grad_alpha, grad_reftrack, grad_normvec, grad_w_veh, (double *)workspace,
+                                     (cudaStream_t)stream);
+    return check_cuda("shortest_path_adjoint_kernel");
 }
 
 // ------------------------------------------------------------------------------------------------

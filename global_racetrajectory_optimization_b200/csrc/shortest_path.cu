@@ -202,4 +202,111 @@ int launch_shortest_path(int B, int n_max, const int32_t *n_pts, const double *r
     return 0;
 }
 
+// ---- sensitivities (csrc/shortest_path_sens.h, DESIGN.md section 3.11) ----
+// Run right after shortest_path_kernel on the same workspace: the final iterate's lu / su and ll / sl, the diagonal D of
+// M = H + D that the backward pass factorises, and grad_status = status.
+__global__ void __launch_bounds__(128)
+shortest_path_sens_export_kernel(int B, int n_max, const int32_t *__restrict__ n_pts, const int32_t *__restrict__ status,
+                                 const double *__restrict__ ws, double *__restrict__ sens, int32_t *__restrict__ grad_status) {
+    const int b = blockIdx.x * blockDim.x + threadIdx.x;
+    if (b >= B) return;
+    const int n = n_pts ? n_pts[b] : n_max;
+    const int st = status[b];
+    const bool ok = st == MC_STATUS_OK && n >= 3 && n <= n_max;
+    const SpView w{const_cast<double *>(ws), (size_t)B, (size_t)n_max * B, b};
+    double *du = sens + (size_t)b * 2 * n_max, *dl = du + n_max;
+#pragma unroll 1
+    for (int i = 0; i < n_max; ++i) {
+        const bool in = ok && i < n;
+        du[i] = in ? w(SP_LU, i) / w(SP_SU, i) : 0.0;
+        dl[i] = in ? w(SP_LL, i) / w(SP_SL, i) : 0.0;
+    }
+    grad_status[b] = st;
+}
+
+// Vector-Jacobian product of alpha: v = (H + D)^-1 grad_alpha by the forward's cyclic solve, then the gradients with
+// respect to f, H, and the bounds, chained to the centre line, the normals and the widths (DESIGN.md section 3.11).
+__global__ void __launch_bounds__(128)
+shortest_path_adjoint_kernel(int B, int n_max, const int32_t *__restrict__ n_pts, const double *__restrict__ reftrack,
+                             const double *__restrict__ normvec, double w_veh, const double *__restrict__ w_veh_batch,
+                             const double *__restrict__ alpha, const double *__restrict__ sens, int32_t *__restrict__ grad_status,
+                             const double *__restrict__ grad_alpha, double *__restrict__ grad_reftrack,
+                             double *__restrict__ grad_normvec, double *__restrict__ grad_w_veh, double *__restrict__ ws) {
+    const int b = blockIdx.x * blockDim.x + threadIdx.x;
+    if (b >= B) return;
+    const int n = n_pts ? n_pts[b] : n_max;
+    double *grt = grad_reftrack + (size_t)b * n_max * 4;
+    double *gnv = grad_normvec ? grad_normvec + (size_t)b * n_max * 2 : nullptr;
+    const bool sized = n >= 3 && n <= n_max;
+    bool ok = sized && grad_status[b] == MC_STATUS_OK;
+    const SpView w{ws, (size_t)B, (size_t)n_max * B, b};
+    const double *rt = reftrack + (size_t)b * n_max * 4;
+    const double *nv = normvec + (size_t)b * n_max * 2;
+    const double *a = alpha + (size_t)b * n_max;
+    const double *du = sens + (size_t)b * 2 * n_max, *dl = du + n_max;
+    if (ok) {
+        const double *g = grad_alpha + (size_t)b * n_max;
+        for (int i = 0; i < n; ++i) {
+            const int ip1 = (i + 1 == n) ? 0 : i + 1;
+            const double nx = nv[2 * i], ny = nv[2 * i + 1];
+            w(SP_DG, i) = 4.0 * (nx * nx + ny * ny);
+            w(SP_OFF, i) = -2.0 * (nx * nv[2 * ip1] + ny * nv[2 * ip1 + 1]);
+            w(SP_DD, i) = du[i] + dl[i];
+            w(SP_RHS, i) = g[i];
+        }
+        cyc_solve(w, n, true);
+        for (int i = 0; i < n; ++i) ok = ok && isfinite(w(SP_X, i));
+        if (!ok) grad_status[b] = MC_STATUS_BREAKDOWN;
+    }
+    if (!sized) grad_status[b] = -1;
+    const double wv = w_veh_batch ? w_veh_batch[b] : w_veh;
+    double gwv = 0.0;
+    for (int i = 0; i < n_max; ++i) {
+        if (!ok || i >= n) {
+            grt[4 * i] = grt[4 * i + 1] = grt[4 * i + 2] = grt[4 * i + 3] = 0.0;
+            if (gnv) gnv[2 * i] = gnv[2 * i + 1] = 0.0;
+            continue;
+        }
+        const int im1 = (i == 0) ? n - 1 : i - 1, ip1 = (i + 1 == n) ? 0 : i + 1;
+        const double v = w(SP_X, i), vm = w(SP_X, im1), vp = w(SP_X, ip1);
+        const double nx = nv[2 * i], ny = nv[2 * i + 1];
+        const double nxm = nv[2 * im1], nym = nv[2 * im1 + 1], nxp = nv[2 * ip1], nyp = nv[2 * ip1 + 1];
+        // dL/df_i = -v_i  ->  the centre line (f_j = 2 n_j.(2 p_j - p_{j+1} - p_{j-1}))
+        grt[4 * i] = -(4.0 * nx * v - 2.0 * nxm * vm - 2.0 * nxp * vp);
+        grt[4 * i + 1] = -(4.0 * ny * v - 2.0 * nym * vm - 2.0 * nyp * vp);
+        // dL/dub = d_u v, dL/dlb = d_l v; a clamped bound (the forward's test dr < 0.001) does not move with the widths
+        const double dr = rt[4 * i + 2] - 0.5 * wv, dlw = rt[4 * i + 3] - 0.5 * wv;
+        const double gub = (dr < 0.001) ? 0.0 : du[i] * v, glb = (dlw < 0.001) ? 0.0 : dl[i] * v;
+        grt[4 * i + 2] = gub;
+        grt[4 * i + 3] = -glb;
+        gwv += 0.5 * (glb - gub);
+        if (gnv) {
+            // dL/dH_ii = -v_i a_i, dL/dH_{i,i+1} = -(v_i a_{i+1} + v_{i+1} a_i) (both symmetric entries), dL/df_i = -v_i
+            const double ai = a[i];
+            const double gd = -v * ai, go = -(v * a[ip1] + vp * ai), gom = -(vm * ai + v * a[im1]);
+            const double cx = 2.0 * rt[4 * i] - rt[4 * ip1] - rt[4 * im1], cy = 2.0 * rt[4 * i + 1] - rt[4 * ip1 + 1] - rt[4 * im1 + 1];
+            gnv[2 * i] = 8.0 * nx * gd - 2.0 * nxp * go - 2.0 * nxm * gom - 2.0 * cx * v;
+            gnv[2 * i + 1] = 8.0 * ny * gd - 2.0 * nyp * go - 2.0 * nym * gom - 2.0 * cy * v;
+        }
+    }
+    if (grad_w_veh) grad_w_veh[b] = ok ? gwv : 0.0;
+}
+
+void launch_shortest_path_sens_export(int B, int n_max, const int32_t *n_pts, const int32_t *status, const double *ws,
+                                      double *sens, int32_t *grad_status, cudaStream_t stream) {
+    const int threads = 128;
+    shortest_path_sens_export_kernel<<<(B + threads - 1) / threads, threads, 0, stream>>>(B, n_max, n_pts, status, ws, sens,
+                                                                                         grad_status);
+}
+
+void launch_shortest_path_adjoint(int B, int n_max, const int32_t *n_pts, const double *reftrack, const double *normvec,
+                                  double w_veh, const double *w_veh_batch, const double *alpha, const double *sens,
+                                  int32_t *grad_status, const double *grad_alpha, double *grad_reftrack, double *grad_normvec,
+                                  double *grad_w_veh, double *ws, cudaStream_t stream) {
+    const int threads = 128;
+    shortest_path_adjoint_kernel<<<(B + threads - 1) / threads, threads, 0, stream>>>(
+        B, n_max, n_pts, reftrack, normvec, w_veh, w_veh_batch, alpha, sens, grad_status, grad_alpha, grad_reftrack,
+        grad_normvec, grad_w_veh, ws);
+}
+
 }  // namespace mc
