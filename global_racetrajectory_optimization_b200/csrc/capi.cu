@@ -23,7 +23,7 @@ int launch_debug_factor_solve(int, int, const int32_t *, double *, const Layout 
 int debug_read_profile(unsigned long long *, int);
 void launch_mincurv_setup(int, int, const int32_t *, const double *, const double *, const double *, double,
                           const double *, double, const int32_t *, double *, const Layout &, int32_t *, cudaStream_t);
-int launch_mincurv_pdip(int, int, const int32_t *, double *, const Layout &, const PdipParams &, double *, int32_t *,
+int launch_mincurv_pdip(int, int, const int32_t *, double *, const Layout &, const PdipParams &, int, double *, int32_t *,
                         int32_t *, int, int *, cudaStream_t);
 int launch_mincurv_pdip_kappa(int, int, const int32_t *, double *, const Layout &, const PdipParams &, double, double *,
                               int32_t *, int32_t *, int, int *, cudaStream_t);
@@ -98,6 +98,8 @@ static int small_workspace(const char *who) {
     return MC_EWORKSPACE;
 }
 static size_t align256(size_t b) { return (b + 255) & ~(size_t)255; }
+static constexpr int PDIP_SLICE_DEFAULT = 8;      // DESIGN.md section 3.3: the predictor of the remaining iterations is
+                                                  // no better than chance after 4 iterations, within one iteration after 8
 
 extern "C" {
 
@@ -125,9 +127,10 @@ int mc_calc_splines_batch(int B, int n_max, const int32_t *n_pts, const double *
 // ------------------------------------------------------------------------------------------------
 static size_t mincurv_slabs_bytes(int B, int n_max) { return align256((size_t)B * mc::make_layout(n_max).stride * sizeof(double)); }
 
+static_assert(mc::SCHED_INTS * sizeof(int) <= 256, "the counters behind the slabs");
 size_t mc_mincurv_workspace_bytes(int B, int n_max) {
     if (B <= 0 || n_max < mc::N_MIN) return 0;
-    return mincurv_slabs_bytes(B, n_max) + 256;      // + the work counter of the persistent solver kernels
+    return mincurv_slabs_bytes(B, n_max) + 256;      // + the work counters of the persistent solver kernels (SCHED_INTS)
 }
 
 static int mincurv_args(const char *who, int B, int n_max, void *workspace, size_t workspace_bytes) {
@@ -200,8 +203,11 @@ int mc_mincurv_pdip_batch(int B, int n_max, const int32_t *n_pts, double *alpha,
         const int v = atoi(e);
         if (v > 0 && v < per_sm) per_sm = v;
     }
+    // iterations before an instance is parked in the sliced schedule (DESIGN.md section 3.3); 0: every instance to the end
+    int slice = PDIP_SLICE_DEFAULT;
+    if (const char *e = getenv("MC_DEBUG_PDIP_SLICE")) { const int v = atoi(e); if (v >= 0) slice = v; }   // A/B runs and tests
     const SolverGrid g = solver_grid(B, n_max, workspace, per_sm);
-    if (mc::launch_mincurv_pdip(B, n_max, n_pts, (double *)workspace, mc::make_layout(n_max), prm, alpha, status, iters,
+    if (mc::launch_mincurv_pdip(B, n_max, n_pts, (double *)workspace, mc::make_layout(n_max), prm, slice, alpha, status, iters,
                                 g.grid, g.counter, (cudaStream_t)stream) != 0) {
         snprintf(g_err, sizeof(g_err), "mincurv_pdip_kernel: cudaFuncSetAttribute failed");
         return MC_ECUDA;

@@ -216,6 +216,7 @@ struct IpShared {
     int prog[4];                                      // sweep progress (units done): forward w0, w1; backward w0, w1
     int flag;
     int next;                                         // next instance index (dynamic work distribution)
+    int resumed;                                      // ... a parked one (sliced schedule of mincurv_pdip_kernel)
 };
 
 // pointers into the instance slab that the factorisation and the sweeps use.  Factor rows in HBM, one bulk copy per unit
@@ -936,6 +937,95 @@ __device__ __forceinline__ int next_instance(IpShared &sh, int *work_counter) {
     return sh.next;
 }
 
+// ---- sliced schedule of the box phase (DESIGN.md section 3.3), one launch: every instance first runs for at most
+//      `slice` iterations; an instance that has not stopped by then is PARKED: its scalars go to its slab (the V_PARK
+//      vector), it gets a bucket = its predicted remaining work, and its index is appended to that bucket.  Once no
+//      instance is left unstarted, a CTA takes the parked ones from the fullest bucket down (greedy longest-first), so that
+//      the launch's tail holds short remainders instead of whole instances.  No CTA waits for another: a CTA parks before
+//      it looks for work and leaves only when every bucket is empty, so whatever is parked is taken by a running CTA.
+//      Only the order of the work changes: each instance runs the same iterations. ----
+constexpr int V_PARK = V_VV;           // the curvature-row phase's scratch vector: free while the box phase runs
+enum ParkSlot {                        // doubles of V_PARK
+    PARK_MU = 0, PARK_MU0 = 1, PARK_RDTOL = 2, PARK_IT = 3,     // the iteration's state besides the slab vectors
+    PARK_TRACE = 8,                    // -DMC_TAIL_TRACE: [start, end] of the first part and of the resumed part
+                                       //   (%globaltimer), iterations, SM of the first part, iteration count at parking,
+                                       //   predicted remaining iterations
+    PARK_MU_HIST = 16,                 // -DMC_TAIL_TRACE: mu after iteration 1, 2, ...
+    PARK_LIST = 64                     // ints: entry k of slab r = 1 + the r-th instance parked in bucket k (0: not yet)
+};
+constexpr int PARK_BUCKETS = 24;
+// the ints behind the slabs (SCHED_INTS of them, zeroed before the launch): the work counter, per bucket the instances
+// parked in it and the instances taken from it
+enum SchedSlot { SCHED_WORK = 0, SCHED_COUNT = 8, SCHED_TAKEN = 40 };
+static_assert(SCHED_WORK < SCHED_COUNT && SCHED_COUNT + PARK_BUCKETS <= SCHED_TAKEN && SCHED_TAKEN + PARK_BUCKETS <= SCHED_INTS,
+              "the schedule's counters behind the slabs");
+static_assert(PARK_MU_HIST + 40 <= PARK_LIST && PARK_LIST + PARK_BUCKETS / 2 <= N_MIN + 64, "V_PARK slots within a vector");
+
+__device__ __forceinline__ double *park_slots(double *ws, const Layout &L, int b) { return vec(ws + (size_t)b * L.stride, L, V_PARK); }
+__device__ __forceinline__ int *park_list(double *ws, const Layout &L, int r) { return reinterpret_cast<int *>(park_slots(ws, L, r) + PARK_LIST); }
+__device__ __forceinline__ int ld_relaxed(const int *p) {
+    int v;
+    asm volatile("ld.relaxed.gpu.global.s32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
+    return v;
+}
+
+// bucket of a parked instance: its predicted remaining iterations, from the rate of mu over the last iteration,
+//   r = ceil(log(target / mu) / log(mu / mu_prev)) + 1  clipped to [1, left],
+// times its size relative to n_max (ragged batches)
+__device__ __forceinline__ int park_bucket(double mu, double mu_prev, double target, int left, int n, int n_max) {
+    double r = left;
+    if (mu <= target) r = 1.0;
+    else if (mu < mu_prev) r = ceil(log(target / mu) / log(mu / mu_prev)) + 1.0;
+    r = fmin(fmax(r, 1.0), (double)left);
+    return min(PARK_BUCKETS - 1, (int)ceil(r * n / n_max));
+}
+
+// thread 0, after the whole CTA's stores of the instance's vectors (a barrier before): park instance b in bucket k
+__device__ __forceinline__ void park(int *sched, double *ws, const Layout &L, int b, int k) {
+    __threadfence();                                   // the slab and the scalars before the entry that publishes them
+    const int r = atomicAdd(&sched[SCHED_COUNT + k], 1);
+    atomicExch(&park_list(ws, L, r)[k], b + 1);
+}
+
+// the next work item of this CTA: an unstarted instance while there are any, then a parked one from the fullest bucket
+// down (sh.flag_resume = 1); B when there is neither
+__device__ __forceinline__ int next_work(IpShared &sh, int *sched, double *ws, const Layout &L, int B) {
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        int b = B, resumed = 0;
+        if (ld_relaxed(&sched[SCHED_WORK]) < B) b = atomicAdd(&sched[SCHED_WORK], 1);
+        if (b >= B) {
+            b = B;
+            for (int k = PARK_BUCKETS - 1; k >= 0 && !resumed; --k) {
+                int t = ld_relaxed(&sched[SCHED_TAKEN + k]);
+                while (t < ld_relaxed(&sched[SCHED_COUNT + k])) {      // (counts only grow: entry t exists or is coming)
+                    const int seen = atomicCAS(&sched[SCHED_TAKEN + k], t, t + 1);
+                    if (seen != t) { t = seen; continue; }
+                    // the parking CTA increments the count and then writes the entry, with no wait in between
+                    const int *e = &park_list(ws, L, t)[k];
+                    int v = 0;
+                    for (int spin = 0; spin < (1 << 24) && (v = ld_relaxed(e)) == 0; ++spin) __nanosleep(64);
+                    __threadfence();
+                    if (v > 0) { b = v - 1; resumed = 1; }
+                    break;
+                }
+            }
+        }
+        sh.next = b;
+        sh.resumed = resumed;
+    }
+    __syncthreads();
+    return sh.next;
+}
+
+#ifdef MC_TAIL_TRACE
+__device__ __forceinline__ double trace_clock() {
+    unsigned long long t;
+    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+    return __longlong_as_double((long long)t);
+}
+#endif
+
 // alpha, status and the iteration count of instance b (the curvature-row phase adds its iterations to the box phase's)
 template <bool ADD_ITERS>
 __device__ __forceinline__ void write_instance(double *aout, int n, int n_max, const double *AL, int b, int result, int it,
@@ -958,10 +1048,13 @@ __device__ __forceinline__ double centring(double c00, double c01, double c10, d
 }
 __device__ __forceinline__ double damped_step(double eta, double r) { return (eta < r) ? eta / r : 1.0; }
 
+// slice == 0: every instance runs to the end.  slice > 0: the sliced schedule (instances parked after `slice` iterations,
+// resumed longest first).  sched: the SCHED_INTS counters behind the slabs, zeroed before the launch, and (slice > 0) the
+// PARK_LIST entries of every slab zeroed too.
 __global__ void __launch_bounds__(IP_THREADS, 8)
 mincurv_pdip_kernel(int B, int n_max, const int32_t *__restrict__ n_pts, double *__restrict__ ws, Layout L,
-                    PdipParams prm, double *__restrict__ alpha_out, int32_t *__restrict__ status,
-                    int32_t *__restrict__ iters_out, int *__restrict__ work_counter) {
+                    PdipParams prm, int slice, double *__restrict__ alpha_out, int32_t *__restrict__ status,
+                    int32_t *__restrict__ iters_out, int *__restrict__ sched) {
 #ifdef MC_DEBUG_SM_LIMIT       // contention experiments: only the first MC_DEBUG_SM_LIMIT SMs take work (full occupancy on those)
     {
         unsigned smid;
@@ -971,15 +1064,28 @@ mincurv_pdip_kernel(int B, int n_max, const int32_t *__restrict__ n_pts, double 
 #endif
     IpShared &sh = ip_init_shared();
     unsigned tick = 0;      // hand-off units of the factorisations so far (uniform across the CTA)
-    for (int b; (b = next_instance(sh, work_counter)) < B;) {
+    for (int b; (b = next_work(sh, sched, ws, L, B)) < B;) {
+        const bool resume = sh.resumed;
         const int n = n_pts ? n_pts[b] : n_max;
         double *aout = alpha_out + (size_t)b * n_max;
-        if (status[b] != 0) {
+        if (!resume && status[b] != 0) {
             for (int i = threadIdx.x; i < n_max; i += IP_THREADS) aout[i] = 0.0;
             if (iters_out && threadIdx.x == 0) iters_out[b] = 0;
             continue;
         }
         PROF_T0(tq0);
+#ifdef MC_TAIL_TRACE
+        if (threadIdx.x == 0) {
+            double *PK = park_slots(ws, L, b);
+            if (!resume) {
+                unsigned smid;
+                asm volatile("mov.u32 %0, %%smid;" : "=r"(smid));
+                PK[PARK_TRACE + 2] = 0.0; PK[PARK_TRACE + 3] = 0.0; PK[PARK_TRACE + 5] = smid;
+                PK[PARK_TRACE + 6] = 0.0; PK[PARK_TRACE + 7] = 0.0;
+            }
+            PK[PARK_TRACE + (resume ? 2 : 0)] = trace_clock();
+        }
+#endif
         double *slab = ws + (size_t)b * L.stride;
         const double *HB = ws + (size_t)*band_owner(slab, L) * L.stride + L.o_hb;      // (shared centre lines: the owner's)
         const double *__restrict__ LB = vec(slab, L, V_LB), *__restrict__ UB = vec(slab, L, V_UB), *__restrict__ F = vec(slab, L, V_F);
@@ -989,47 +1095,54 @@ mincurv_pdip_kernel(int B, int n_max, const int32_t *__restrict__ n_pts, double 
         double *__restrict__ ISU = vec(slab, L, V_ISU), *__restrict__ ISL = vec(slab, L, V_ISL);
         double *G0 = vec(slab, L, V_T0);
         if (threadIdx.x == 0) sh.flag = 0;
-
-        // ---------------- initial point: box centre, multipliers from the gradient ----------------
-        for (int i = threadIdx.x; i < n; i += IP_THREADS) AL[i] = 0.5 * (LB[i] + UB[i]);
-        __syncthreads();
-        band_matvec(HB, AL, G0, n);
-        __syncthreads();
-        double gmax = 0.0, fmaxv = 0.0;
+        double mu0, rd_tol, mu;
+        int it;
+        if (resume) {                  // a parked instance: its vectors are in the slab, its scalars in V_PARK
+            const double *PK = park_slots(ws, L, b);
+            mu = PK[PARK_MU]; mu0 = PK[PARK_MU0]; rd_tol = PK[PARK_RDTOL]; it = (int)PK[PARK_IT];
+        } else {
+            // ---------------- initial point: box centre, multipliers from the gradient ----------------
+            for (int i = threadIdx.x; i < n; i += IP_THREADS) AL[i] = 0.5 * (LB[i] + UB[i]);
+            __syncthreads();
+            band_matvec(HB, AL, G0, n);
+            __syncthreads();
+            double gmax = 0.0, fmaxv = 0.0;
 #pragma unroll 1
-        for (int i = threadIdx.x; i < n; i += IP_THREADS) {
-            const double gi = G0[i] + F[i];
-            G0[i] = gi;
-            gmax = fmax(gmax, fabs(gi));
-            fmaxv = fmax(fmaxv, fabs(F[i]));
-        }
-        gmax = block_reduce<1>(gmax, sh.red);
-        fmaxv = block_reduce<1>(fmaxv, sh.red);
-        const double lam0 = prm.lam0_rel * gmax + 1e-300;
-        double musum = 0.0;
+            for (int i = threadIdx.x; i < n; i += IP_THREADS) {
+                const double gi = G0[i] + F[i];
+                G0[i] = gi;
+                gmax = fmax(gmax, fabs(gi));
+                fmaxv = fmax(fmaxv, fabs(F[i]));
+            }
+            gmax = block_reduce<1>(gmax, sh.red);
+            fmaxv = block_reduce<1>(fmaxv, sh.red);
+            const double lam0 = prm.lam0_rel * gmax + 1e-300;
+            double musum = 0.0;
 #pragma unroll 1
-        for (int i = threadIdx.x; i < n; i += IP_THREADS) {
-            const double gi = G0[i];
-            const double lu = fmax(-gi, 0.0) + lam0, ll = fmax(gi, 0.0) + lam0;
-            const double rd = gi + lu - ll;
-            LU[i] = lu; LL[i] = ll;
-            RD[i] = rd;
-            const double a = AL[i];
-            // slacks are carried as variables of their own: recomputing ub - alpha loses them to
-            // cancellation once s << eps |alpha| (late iterations), see DESIGN.md
-            const double su = UB[i] - a, sl = a - LB[i];
-            const double isu = 1.0 / su, isl = 1.0 / sl;
-            SU[i] = su; SL[i] = sl;
-            ISU[i] = isu; ISL[i] = isl;
-            DD[i] = lu * isu + ll * isl; RHS[i] = -rd + lu - ll;       // barrier diagonal, affine right-hand side
-            musum += su * lu + sl * ll;
+            for (int i = threadIdx.x; i < n; i += IP_THREADS) {
+                const double gi = G0[i];
+                const double lu = fmax(-gi, 0.0) + lam0, ll = fmax(gi, 0.0) + lam0;
+                const double rd = gi + lu - ll;
+                LU[i] = lu; LL[i] = ll;
+                RD[i] = rd;
+                const double a = AL[i];
+                // slacks are carried as variables of their own: recomputing ub - alpha loses them to
+                // cancellation once s << eps |alpha| (late iterations), see DESIGN.md
+                const double su = UB[i] - a, sl = a - LB[i];
+                const double isu = 1.0 / su, isl = 1.0 / sl;
+                SU[i] = su; SL[i] = sl;
+                ISU[i] = isu; ISL[i] = isl;
+                DD[i] = lu * isu + ll * isl; RHS[i] = -rd + lu - ll;       // barrier diagonal, affine right-hand side
+                musum += su * lu + sl * ll;
+            }
+            musum = block_reduce<0>(musum, sh.red);
+            mu0 = musum / (2.0 * n);
+            rd_tol = prm.rd_rel * (fmaxv + gmax) + 1e-300;
+            mu = mu0;
+            it = 0;
         }
-        musum = block_reduce<0>(musum, sh.red);
-        const double mu0 = musum / (2.0 * n);
-        const double rd_tol = prm.rd_rel * (fmaxv + gmax) + 1e-300;
-        double mu = mu0;
-        int it = 0;
-        int result = 2;   // max-iter unless we converge
+        int result = -1;               // still running
+        const int it_end = (slice > 0 && !resume) ? min(slice, prm.max_iter) : prm.max_iter;
 
         // Vector phases: the reciprocals 1/s_u, 1/s_l are state (ISU, ISL), so one interior-point iteration
         // costs four divisions per variable; step lengths come from max-ratios (no division per element).
@@ -1040,7 +1153,7 @@ mincurv_pdip_kernel(int B, int n_max, const int32_t *__restrict__ n_pts, double 
         // are computed where their inputs are: by the loop above for the first iteration, by the update pass of the
         // previous iteration for the others.
         constexpr int VG = 4, VS = VG * IP_THREADS;
-        for (it = 0; it < prm.max_iter; ++it) {
+        for (; it < it_end; ++it) {
             PROF_T0(tf0);
             const bool fok = factor(sh, slab, L, n, HB, RHS, tick);
             tick += factor_units(n);
@@ -1166,9 +1279,16 @@ mincurv_pdip_kernel(int B, int n_max, const int32_t *__restrict__ n_pts, double 
                     }
                 }
             }
+            if (threadIdx.x == 0) park_slots(ws, L, b)[PARK_MU] = mu;      // mu before this iteration (read when parking)
             mu = block_reduce<0>(musum2, sh.red) / (2.0 * n);
             rdmax = block_reduce<1>(rdmax, sh.red);
             PROF_ADD(PROF_UPDATE, tv5);
+#ifdef MC_TAIL_TRACE
+            if (threadIdx.x == 0 && it < PARK_LIST - PARK_MU_HIST) {
+                park_slots(ws, L, b)[PARK_MU_HIST + it] = mu;
+                park_slots(ws, L, b)[PARK_MU0] = mu0;
+            }
+#endif
             // weakly active bounds converge like sqrt(mu): also require that the step itself has become small
             bool settled = true;
             if (prm.dx_rel > 0.0 && mu <= prm.mu_rel * mu0) {
@@ -1179,7 +1299,29 @@ mincurv_pdip_kernel(int B, int n_max, const int32_t *__restrict__ n_pts, double 
             if (mu <= prm.mu_rel * mu0 && rdmax <= rd_tol && settled) { result = 0; ++it; break; }
             if (mu <= 1e-4 * prm.mu_rel * mu0) { result = (rdmax <= 1e3 * rd_tol) ? 0 : 2; ++it; break; }   // complementarity exhausted
         }
+        if (result < 0 && it < prm.max_iter) {        // the slice is over: park the instance
+            if (threadIdx.x == 0) {
+                double *PK = park_slots(ws, L, b);
+                const double mu_prev = PK[PARK_MU];     // the rate of the last iteration predicts the remaining ones
+                PK[PARK_MU] = mu; PK[PARK_MU0] = mu0; PK[PARK_RDTOL] = rd_tol; PK[PARK_IT] = it;
+#ifdef MC_TAIL_TRACE
+                PK[PARK_TRACE + 1] = trace_clock();
+                PK[PARK_TRACE + 6] = it;
+                PK[PARK_TRACE + 7] = park_bucket(mu, mu_prev, prm.mu_rel * mu0, prm.max_iter - it, n, n);
+#endif
+                park(sched, ws, L, b, park_bucket(mu, mu_prev, prm.mu_rel * mu0, prm.max_iter - it, n, n_max));
+            }
+            continue;
+        }
+        if (result < 0) result = 2;                    // iteration cap
         write_instance<false>(aout, n, n_max, AL, b, result, it, status, iters_out);
+#ifdef MC_TAIL_TRACE
+        if (threadIdx.x == 0) {
+            double *PK = park_slots(ws, L, b);
+            PK[PARK_TRACE + (resume ? 3 : 1)] = trace_clock();
+            PK[PARK_TRACE + 4] = it;
+        }
+#endif
         PROF_ADD(PROF_TOTAL, tq0);
 #ifdef MC_PROFILE
         if (blockIdx.x == 0 && threadIdx.x == 0) { atomicAdd(&g_prof[PROF_NQP], 1ull); atomicAdd(&g_prof[PROF_ITERS], (unsigned long long)it); }
@@ -1232,9 +1374,14 @@ static int launch_solver(void (*kernel)(P...), int grid, int *work_counter, cuda
 
 int pdip_ctas_per_sm() { return ctas_per_sm(mincurv_pdip_kernel); }
 
-int launch_mincurv_pdip(int B, int n_max, const int32_t *n_pts, double *ws, const Layout &L, const PdipParams &prm,
-                        double *alpha, int32_t *status, int32_t *iters, int grid, int *work_counter, cudaStream_t stream) {
-    return launch_solver(mincurv_pdip_kernel, grid, work_counter, stream, B, n_max, n_pts, ws, L, prm, alpha, status, iters, work_counter);
+// slice > 0 and more instances than CTAs: the sliced schedule (one launch, no grid-wide wait: the CTAs need not all be resident)
+int launch_mincurv_pdip(int B, int n_max, const int32_t *n_pts, double *ws, const Layout &L, const PdipParams &prm, int slice,
+                        double *alpha, int32_t *status, int32_t *iters, int grid, int *sched, cudaStream_t stream) {
+    if (B <= grid) slice = 0;
+    cudaMemsetAsync(sched, 0, SCHED_INTS * sizeof(int), stream);
+    if (slice > 0)      // the PARK_LIST entries of every slab
+        cudaMemset2DAsync(ws + (size_t)V_PARK * L.np + PARK_LIST, L.stride * sizeof(double), 0, PARK_BUCKETS * sizeof(int), B, stream);
+    return launch_solver(mincurv_pdip_kernel, grid, nullptr, stream, B, n_max, n_pts, ws, L, prm, slice, alpha, status, iters, sched);
 }
 
 // ================================================================================================

@@ -45,6 +45,10 @@ __host__ __device__ inline Layout make_layout(int n_max) {
     return L;
 }
 
+// ints behind the slabs (within the 256 bytes there): the work counter of the persistent solver kernels and the schedule
+// of the box phase's two launches (mincurv_ipm.cu)
+constexpr int SCHED_INTS = 64;
+
 struct PdipParams {
     int max_iter;
     double mu_rel;     // stop when mu <= mu_rel * mu0 ...
