@@ -20,7 +20,7 @@
 // fp64 pipe, latency-bound on the in-block pivot chains and on the hand-offs between three warp roles.  Here every step offers 64 independent DFMAs per instance and eight
 // instances share an SM, so the fp64 pipe and the issue slots are what is busy.
 //
-// The factor (per column: the 32 band entries of L + w, the 32 entries of G + z, w) goes to the instance's HBM slab and
+// The factor (per column: the 32 band entries of L + w, the 32 entries of G + w) goes to the instance's HBM slab and
 // is streamed back by the triangular sweeps through a shared-memory ring of 8-column units filled by cp.async.bulk
 // (TMA, 1-D) on mbarriers -- the band rows of H reach warp 0 the same way.  Per iteration: factor written once, read
 // three times (the predictor's forward sweep is fused into the factorisation).
@@ -34,7 +34,7 @@ constexpr unsigned FULL = 0xffffffffu;
 constexpr int IP_THREADS = 64;
 constexpr int SUB = 8;                 // columns per hand-off / streaming unit
 constexpr int VBP = 12;                // pitch of the row-major panel buffers (conflict-free DMMA fragment loads, 16-byte rows)
-constexpr int FROW = 34;               // pitch of a fill row: [g (32), z, w]
+constexpr int FROW = 33;               // pitch of a fill row: [g (32), w]
 constexpr int HB_SLOTS = 2;            // band-row units of warp 0 (the next panel's is in flight)
 constexpr int HO_SLOTS = 2;            // panels between warp 0 and warp 1
 constexpr int LROW = 33;               // pitch of a chain-factor column: its 32 band entries of [Q - I; L21], w (see lt_slot)
@@ -46,7 +46,7 @@ constexpr int GT_SLOTS = 6 - LT_SLOTS;
 constexpr int RING_UNITS = LT_SLOTS + GT_SLOTS;       // mbarriers: [0, LT_SLOTS) warp 0, [LT_SLOTS, RING_UNITS) warp 1
 constexpr int QDEPTH = 16;             // units of z (forward) / t (backward) in flight between the two warps
 constexpr int LT_UNIT_DOUBLES = SUB * LROW;           // 264 (2112 bytes: one bulk copy, 16-byte multiple)
-constexpr int GT_UNIT_DOUBLES = SUB * FROW;           // 272
+constexpr int GT_UNIT_DOUBLES = SUB * FROW;           // 264 (2112 bytes, like a chain unit)
 constexpr unsigned HB_UNIT_BYTES = SUB * HB_PITCH * sizeof(double);   // 2176
 
 __device__ __forceinline__ void dmma(double (&c)[2], double a, double b) {
@@ -227,19 +227,22 @@ struct IpShared {
 //              a2 -= L21 y1; backward: u = t1 - L21^T x2, x1 = Q^T u).  w = 1/d_k.  With the rows m = 0..39 of
 //              [Q - I; L21] counted from k0, column j is nonzero for j < m <= j + 32 only (Q - I strictly lower, L with 32
 //              sub-diagonals): exactly 32 entries, kept at lt_slot(j, m).  The sweeps set the other entries to zero by predicate
-//   GT[k]    = [ G[0 .. 31][k],  z_k,  w_k ]                  (pitch 34) z = w y: what the separator's forward part needs
-// so the sweeps read nothing but the streamed units (no per-column global loads on the serial chains).  Columns
-// NA .. 8 ceil(NA / 8) - 1 are padding (pivot 1, nothing else): every unit is a full panel.
+//   GT[k]    = [ G[0 .. 31][k],  w_k ]                        (pitch 33)
+// so warp 0's sweeps read nothing but the streamed units (no per-column global loads on the serial chains).  z = w y, what
+// the separator's part of the backward half needs, is a vector of its own behind GT: the forward half of every solve
+// writes it, eight adjacent columns per store (full sectors); inside the fill rows it was an 8-byte store into each
+// 264-byte row long after the row had been written.  Columns NA .. 8 ceil(NA / 8) - 1 are padding (pivot 1, nothing
+// else): every unit is a full panel.
 struct Factor {
     const double *HB;      // band of H, row i: H[i][i .. i+32] (read only: possibly another instance's, shared centre lines)
     const double *DD;      // barrier diagonal
-    double *LT, *GT;
+    double *LT, *GT, *Z;
     int NA;
 };
 
 __device__ __forceinline__ Factor make_factor(double *slab, const Layout &L, int n, const double *HB) {
-    double *LT = slab + L.o_tiles;
-    return {HB, vec(slab, L, V_DD), LT, LT + (size_t)L.np * LROW, n - 32};
+    double *LT = slab + L.o_tiles, *GT = LT + (size_t)L.np * LROW;
+    return {HB, vec(slab, L, V_DD), LT, GT, GT + (size_t)L.np * FROW, n - 32};
 }
 
 // slot of entry (c, m), c < m <= c + 32, in a chain unit: the packed order m - c - 1 rotated by 4 c, so that the sweeps'
@@ -426,7 +429,7 @@ __device__ __noinline__ bool factor_chain(IpShared &sh, const double *__restrict
 //      DMMA C fragments, panel by forward substitution with the panel's unit-lower block, trailing update
 //      G'[:, J] = G[:, J+1] + G_panel L^T and S -= (G_panel w) G_panel^T on the tensor cores; also the separator part of
 //      the fused forward substitution  gS -= G (w y) ----
-__device__ __noinline__ void factor_fill(IpShared &sh, const double *__restrict__ HBp, double *__restrict__ GTp, const int NA, const double *__restrict__ g, unsigned tick) {
+__device__ __noinline__ void factor_fill(IpShared &sh, const double *__restrict__ HBp, double *__restrict__ GTp, double *__restrict__ Zp, const int NA, const double *__restrict__ g, unsigned tick) {
     const int lane = threadIdx.x & 31;
     const int gq = lane >> 2, q = lane & 3;
     const int nunits = (NA + SUB - 1) / SUB;
@@ -485,7 +488,8 @@ __device__ __noinline__ void factor_fill(IpShared &sh, const double *__restrict_
         }
         if (lane < 8) {
             const double w = ho.w[lane];
-            *reinterpret_cast<double2 *>(gtp + lane * FROW + 32) = make_double2(w * ho.y[lane], w);      // [z, w]
+            st_stream(gtp + lane * FROW + 32, w);
+            Zp[k0 + lane] = w * ho.y[lane];            // z of the predictor (the fused forward half)
         }
 #pragma unroll
         for (int j = 0; j < 8; j += 2) *reinterpret_cast<double2 *>(&gb[lane * VBP + j]) = make_double2(gp[j], gp[j + 1]);
@@ -554,7 +558,7 @@ __device__ __noinline__ bool factor(IpShared &sh, double *slab, const Layout &L,
         if (!factor_chain(sh, F.HB, F.DD, F.LT, NA, g, tick)) sh.flag = 1;
         PROF_ADD(PROF_CHAIN, tc0);
     } else {
-        factor_fill(sh, F.HB, F.GT, NA, g, tick);
+        factor_fill(sh, F.HB, F.GT, F.Z, NA, g, tick);
         PROF_ADD1(PROF_FILL, tc0);
     }
     PROF_T0(tc1);
@@ -690,9 +694,9 @@ __device__ __forceinline__ void prog_wait(IpShared &sh, const int *p, int need) 
 //   y1 = a1 + (Q - I) a1,   a[k0+8 .. k0+39] -= L21 y1       (rows k0+32 .. k0+39 enter with g).
 // The window a lives in DMMA C fragments (every column of the 8 x 8 tile carries the same vector): lane (gq, q) holds
 // a[k0 + 8 I + gq], I = 0..3; B operands (a1, y1 at index 4 h + q) come by shuffle.
-// z = w y goes to warp 1 (sweep_sep_rhs runs one unit behind) through the queue sw.q, and into the fill rows (GT[k][32])
-// for the backward half of the solve.
-__device__ __noinline__ void sweep_forward(IpShared &sh, double *__restrict__ LTp, double *__restrict__ GTp, const int NA, const double *__restrict__ g) {
+// z = w y goes to warp 1 (sweep_sep_rhs runs one unit behind) through the queue sw.q, and to the vector Z for the backward
+// half of the solve.
+__device__ __noinline__ void sweep_forward(IpShared &sh, double *__restrict__ LTp, double *__restrict__ Zp, const int NA, const double *__restrict__ g) {
     const int lane = threadIdx.x & 31;
     const int gq = lane >> 2, q = lane & 3;
     const int nunits = (NA + SUB - 1) / SUB;
@@ -740,7 +744,7 @@ __device__ __noinline__ void sweep_forward(IpShared &sh, double *__restrict__ LT
             const bool in = (k0 + gq < NA);
             const double z = in ? y * wl : 0.0;
             sh.u.sw.q[(u & (QDEPTH - 1)) * SUB + gq] = z;
-            if (in) GTp[(size_t)(k0 + gq) * FROW + 32] = z;
+            if (in) Zp[k0 + gq] = z;
         }
 #pragma unroll
         for (int I = 0; I < 4; ++I) acc[I] = nw[I];
@@ -748,7 +752,7 @@ __device__ __noinline__ void sweep_forward(IpShared &sh, double *__restrict__ LT
         if (lane == 0) { prog_publish(&sh.prog[0], u + 1); R.refill(u); }
     }
     R.close();
-    fence_proxy_async();        // z (generic-proxy stores) is read back through bulk copies (async proxy)
+    fence_proxy_async();        // the ring slots, read through the generic proxy, are refilled by the backward sweep's bulk copies
 }
 
 // separator part of the forward sweep (warp 1, one unit behind warp 0):  gs = g_S - G z
@@ -776,8 +780,9 @@ __device__ __noinline__ void sweep_sep_rhs(IpShared &sh, double *__restrict__ GT
 }
 
 // separator solve and the right-hand side of the backward sweep (warp 1, ahead of warp 0's sweep_backward):
-//   x_S = S^-1 gs;   t = (y - G^T x_S) w = z - w G^T x_S, from the last unit down, handed over through the queue sw.q
-__device__ __noinline__ void sweep_sep_solve(IpShared &sh, double *__restrict__ GTp, const int NA, double *__restrict__ x) {
+//   x_S = S^-1 gs;   t = (y - G^T x_S) w = z - w G^T x_S, from the last unit down, handed over through the queue sw.q.
+// z comes from the vector the forward half wrote (plain loads, one unit ahead: it was written in this launch)
+__device__ __noinline__ void sweep_sep_solve(IpShared &sh, double *__restrict__ GTp, const double *Zp, const int NA, double *__restrict__ x) {
     const int lane = threadIdx.x & 31;
     const int nunits = (NA + SUB - 1) / SUB;
     GtRing R(sh, &sh.u.sw.gt[0][0], GTp, nunits, true);
@@ -802,22 +807,24 @@ __device__ __noinline__ void sweep_sep_solve(IpShared &sh, double *__restrict__ 
     double xq[8];
 #pragma unroll
     for (int i = 0; i < 8; ++i) xq[i] = __shfl_sync(FULL, a, 8 * qr + i);
+    double znext = 0.0;
+    if (nunits > 0 && R.unit(0) * SUB + kl < NA) znext = Zp[R.unit(0) * SUB + kl];
     for (int i = 0; i < nunits; ++i, R.next()) {
         const int k = R.unit(i) * SUB + kl;
+        const double z = znext;
+        if (i + 1 < nunits && R.unit(i + 1) * SUB + kl < NA) znext = Zp[R.unit(i + 1) * SUB + kl];
         if ((i & 7) == 0 && i >= 8) prog_wait<true>(sh, &sh.prog[2], i - 8);      // queue slots of the next eight units are free again
-        const double *gt = R.wait() + kl * FROW;
-        const double2 zw = *reinterpret_cast<const double2 *>(&gt[32]);
+        const double *gt = R.wait() + kl * FROW;      // (pitch 33: scalar loads, on distinct banks)
         double c0 = 0.0, c1 = 0.0;
 #pragma unroll
         for (int e = 0; e < 8; e += 2) {
-            const double2 gg = *reinterpret_cast<const double2 *>(&gt[8 * qr + e]);
-            c0 = fma(gg.x, xq[e], c0);
-            c1 = fma(gg.y, xq[e + 1], c1);
+            c0 = fma(gt[8 * qr + e], xq[e], c0);
+            c1 = fma(gt[8 * qr + e + 1], xq[e + 1], c1);
         }
         double c = c0 + c1;
         c += __shfl_xor_sync(FULL, c, 8);
         c += __shfl_xor_sync(FULL, c, 16);
-        if (qr == 0) sh.u.sw.q[(i & (QDEPTH - 1)) * SUB + kl] = (k < NA) ? fma(-c, zw.y, zw.x) : 0.0;      // (padding rows: t = 0)
+        if (qr == 0) sh.u.sw.q[(i & (QDEPTH - 1)) * SUB + kl] = (k < NA) ? fma(-c, gt[32], z) : 0.0;      // (padding rows: t = 0)
         __syncwarp();
         if (lane == 0) { prog_publish(&sh.prog[3], i + 1); R.refill(i); }
     }
@@ -883,13 +890,13 @@ __device__ __noinline__ void solve(IpShared &sh, double *slab, const Layout &L, 
     __syncthreads();
     if (!fused) {
         PROF_T0(t0);
-        if (warp == 0) sweep_forward(sh, F.LT, F.GT, F.NA, g);
+        if (warp == 0) sweep_forward(sh, F.LT, F.Z, F.NA, g);
         else sweep_sep_rhs(sh, F.GT, F.NA, g);
         __syncthreads();
         PROF_ADD1(PROF_FWD_SWEEPS, t0);
     }
     PROF_T0(t3);
-    if (warp == 1) sweep_sep_solve(sh, F.GT, F.NA, x);
+    if (warp == 1) sweep_sep_solve(sh, F.GT, F.Z, F.NA, x);
     else sweep_backward(sh, F.LT, F.NA, x);
     __syncthreads();
     PROF_ADD1(PROF_BWD_SWEEPS, t3);
@@ -1047,6 +1054,15 @@ __device__ __forceinline__ double centring(double c00, double c01, double c10, d
     return sigma * sigma * sigma * mu;
 }
 __device__ __forceinline__ double damped_step(double eta, double r) { return (eta < r) ? eta / r : 1.0; }
+// the corrector's complementarity terms tu = sigma mu - s_u l_u + dx dl_u, tl = sigma mu - s_l l_l - dx dl_l of the affine
+// direction dx (isu = 1 / s_u, isl = 1 / s_l).  Recomputed by every pass that needs them rather than stored: the same
+// expression on the same inputs gives the same bits in each of them.
+__device__ __forceinline__ void corrector_terms(double smu, double su, double sl, double lu, double ll, double dx, double isu,
+                                                double isl, double &tu, double &tl) {
+    const double dlu = lu * (dx * isu - 1.0), dll = -ll * (1.0 + dx * isl);
+    tu = smu - su * lu + dx * dlu;
+    tl = smu - sl * ll - dx * dll;
+}
 
 // slice == 0: every instance runs to the end.  slice > 0: the sliced schedule (instances parked after `slice` iterations,
 // resumed longest first).  sched: the SCHED_INTS counters behind the slabs, zeroed before the launch, and (slice > 0) the
@@ -1090,9 +1106,8 @@ mincurv_pdip_kernel(int B, int n_max, const int32_t *__restrict__ n_pts, double 
         const double *HB = ws + (size_t)*band_owner(slab, L) * L.stride + L.o_hb;      // (shared centre lines: the owner's)
         const double *__restrict__ LB = vec(slab, L, V_LB), *__restrict__ UB = vec(slab, L, V_UB), *__restrict__ F = vec(slab, L, V_F);
         double *__restrict__ AL = vec(slab, L, V_ALPHA), *__restrict__ LU = vec(slab, L, V_LU), *__restrict__ LL = vec(slab, L, V_LL), *__restrict__ RD = vec(slab, L, V_RD);
-        double *__restrict__ RHS = vec(slab, L, V_RHS), *__restrict__ DX = vec(slab, L, V_DX), *__restrict__ DD = vec(slab, L, V_DD);
-        double *__restrict__ TU = vec(slab, L, V_DLU), *__restrict__ TL = vec(slab, L, V_DLL), *__restrict__ SU = vec(slab, L, V_SU), *__restrict__ SL = vec(slab, L, V_SL);
-        double *__restrict__ ISU = vec(slab, L, V_ISU), *__restrict__ ISL = vec(slab, L, V_ISL);
+        double *__restrict__ RHS = vec(slab, L, V_RHS), *__restrict__ DX = vec(slab, L, V_DX), *__restrict__ DXA = vec(slab, L, V_DXA);
+        double *__restrict__ DD = vec(slab, L, V_DD), *__restrict__ SU = vec(slab, L, V_SU), *__restrict__ SL = vec(slab, L, V_SL);
         double *G0 = vec(slab, L, V_T0);
         if (threadIdx.x == 0) sh.flag = 0;
         double mu0, rd_tol, mu;
@@ -1131,7 +1146,6 @@ mincurv_pdip_kernel(int B, int n_max, const int32_t *__restrict__ n_pts, double 
                 const double su = UB[i] - a, sl = a - LB[i];
                 const double isu = 1.0 / su, isl = 1.0 / sl;
                 SU[i] = su; SL[i] = sl;
-                ISU[i] = isu; ISL[i] = isl;
                 DD[i] = lu * isu + ll * isl; RHS[i] = -rd + lu - ll;       // barrier diagonal, affine right-hand side
                 musum += su * lu + sl * ll;
             }
@@ -1144,14 +1158,17 @@ mincurv_pdip_kernel(int B, int n_max, const int32_t *__restrict__ n_pts, double 
         int result = -1;               // still running
         const int it_end = (slice > 0 && !resume) ? min(slice, prm.max_iter) : prm.max_iter;
 
-        // Vector phases: the reciprocals 1/s_u, 1/s_l are state (ISU, ISL), so one interior-point iteration
-        // costs four divisions per variable; step lengths come from max-ratios (no division per element).
+        // Vector phases: the state of an iteration is alpha, s_u, s_l, l_u, l_l, r_d (AL SU SL LU LL RD) and the next
+        // factorisation's DD and RHS; within it the affine direction DXA and the combined one DX.  Everything else is
+        // recomputed where it is used, which costs less than its memory traffic: the reciprocals 1/s_u, 1/s_l (IEEE
+        // divisions: the same bits in every pass) and the corrector terms tu, tl (corrector_terms).  Step lengths come
+        // from max-ratios.  RHS carries the corrector's right-hand side from its pass to the update pass.
         // Every thread owns the elements i = tid + k * 64; the loops take them in groups of VG with all loads of a
         // group issued before the first use (the vectors live in L2/HBM: one element at a time, each trip of a loop
         // paid the full memory latency).
         // The barrier diagonal DD = lu / su + ll / sl and the affine right-hand side RHS = -rd + lu - ll of an iteration
         // are computed where their inputs are: by the loop above for the first iteration, by the update pass of the
-        // previous iteration for the others.
+        // previous iteration for the others.  A parked instance resumes from the state alone.
         constexpr int VG = 4, VS = VG * IP_THREADS;
         for (; it < it_end; ++it) {
             PROF_T0(tf0);
@@ -1160,23 +1177,24 @@ mincurv_pdip_kernel(int B, int n_max, const int32_t *__restrict__ n_pts, double 
             if (!fok) { result = 3; break; }
             PROF_ADD(PROF_FACTOR, tf0);
             PROF_T0(ts0);
-            solve(sh, slab, L, n, RHS, DX, true);
+            solve(sh, slab, L, n, RHS, DXA, true);
             PROF_ADD(PROF_SOLVE_PRED, ts0);
             // ---- affine direction: step lengths 1 / max-ratio; mu_aff as a polynomial in (ap, ad) ----
             PROF_T0(tv2);
             double rp = 0.0, rdl = 0.0, c00 = 0.0, c01 = 0.0, c10 = 0.0, c11 = 0.0;
 #pragma unroll 1
             for (int i0 = threadIdx.x; i0 < n; i0 += VS) {
-                double su[VG], sl[VG], lu[VG], ll[VG], dx[VG], isu[VG], isl[VG];
+                double su[VG], sl[VG], lu[VG], ll[VG], dx[VG];
 #pragma unroll
                 for (int k = 0; k < VG; ++k) {
                     const int i = min(i0 + k * IP_THREADS, n - 1);
-                    su[k] = SU[i]; sl[k] = SL[i]; lu[k] = LU[i]; ll[k] = LL[i]; dx[k] = DX[i]; isu[k] = ISU[i]; isl[k] = ISL[i];
+                    su[k] = SU[i]; sl[k] = SL[i]; lu[k] = LU[i]; ll[k] = LL[i]; dx[k] = DXA[i];
                 }
 #pragma unroll
                 for (int k = 0; k < VG; ++k) {
                     if (i0 + k * IP_THREADS < n) {
-                        const double p = dx[k] * isu[k], m = dx[k] * isl[k];
+                        const double isu = 1.0 / su[k], isl = 1.0 / sl[k];
+                        const double p = dx[k] * isu, m = dx[k] * isl;
                         rp = fmax(rp, fmax(p, -m));                 // s_u - a dx >= 0, s_l + a dx >= 0
                         rdl = fmax(rdl, fmax(1.0 - p, 1.0 + m));    // dlu / lu = -1 + p, dll / ll = -1 - m
                         const double dlu = lu[k] * (p - 1.0), dll = -ll[k] * (1.0 + m);
@@ -1198,21 +1216,20 @@ mincurv_pdip_kernel(int B, int n_max, const int32_t *__restrict__ n_pts, double 
             // ---- corrector right-hand side ----
 #pragma unroll 1
             for (int i0 = threadIdx.x; i0 < n; i0 += VS) {
-                double su[VG], sl[VG], lu[VG], ll[VG], dx[VG], isu[VG], isl[VG], rd[VG];
+                double su[VG], sl[VG], lu[VG], ll[VG], dx[VG], rd[VG];
 #pragma unroll
                 for (int k = 0; k < VG; ++k) {
                     const int i = min(i0 + k * IP_THREADS, n - 1);
-                    su[k] = SU[i]; sl[k] = SL[i]; lu[k] = LU[i]; ll[k] = LL[i]; dx[k] = DX[i]; isu[k] = ISU[i]; isl[k] = ISL[i]; rd[k] = RD[i];
+                    su[k] = SU[i]; sl[k] = SL[i]; lu[k] = LU[i]; ll[k] = LL[i]; dx[k] = DXA[i]; rd[k] = RD[i];
                 }
 #pragma unroll
                 for (int k = 0; k < VG; ++k) {
                     const int i = i0 + k * IP_THREADS;
                     if (i < n) {
-                        const double dlu = lu[k] * (dx[k] * isu[k] - 1.0), dll = -ll[k] * (1.0 + dx[k] * isl[k]);
-                        const double tu = smu - su[k] * lu[k] + dx[k] * dlu;
-                        const double tl = smu - sl[k] * ll[k] - dx[k] * dll;
-                        TU[i] = tu; TL[i] = tl;
-                        RHS[i] = -rd[k] - tu * isu[k] + tl * isl[k];
+                        const double isu = 1.0 / su[k], isl = 1.0 / sl[k];
+                        double tu, tl;
+                        corrector_terms(smu, su[k], sl[k], lu[k], ll[k], dx[k], isu, isl, tu, tl);
+                        RHS[i] = -rd[k] - tu * isu + tl * isl;
                     }
                 }
             }
@@ -1225,17 +1242,20 @@ mincurv_pdip_kernel(int B, int n_max, const int32_t *__restrict__ n_pts, double 
             rp = 0.0; rdl = 0.0;
 #pragma unroll 1
             for (int i0 = threadIdx.x; i0 < n; i0 += VS) {
-                double lu[VG], ll[VG], dx[VG], isu[VG], isl[VG], tu[VG], tl[VG];
+                double su[VG], sl[VG], lu[VG], ll[VG], dxa[VG], dx[VG];
 #pragma unroll
                 for (int k = 0; k < VG; ++k) {
                     const int i = min(i0 + k * IP_THREADS, n - 1);
-                    lu[k] = LU[i]; ll[k] = LL[i]; dx[k] = DX[i]; isu[k] = ISU[i]; isl[k] = ISL[i]; tu[k] = TU[i]; tl[k] = TL[i];
+                    su[k] = SU[i]; sl[k] = SL[i]; lu[k] = LU[i]; ll[k] = LL[i]; dxa[k] = DXA[i]; dx[k] = DX[i];
                 }
 #pragma unroll
                 for (int k = 0; k < VG; ++k) {
                     if (i0 + k * IP_THREADS < n) {
-                        const double dlu = (tu[k] + lu[k] * dx[k]) * isu[k], dll = (tl[k] - ll[k] * dx[k]) * isl[k];
-                        rp = fmax(rp, fmax(dx[k] * isu[k], -dx[k] * isl[k]));
+                        const double isu = 1.0 / su[k], isl = 1.0 / sl[k];
+                        double tu, tl;
+                        corrector_terms(smu, su[k], sl[k], lu[k], ll[k], dxa[k], isu, isl, tu, tl);
+                        const double dlu = (tu + lu[k] * dx[k]) * isu, dll = (tl - ll[k] * dx[k]) * isl;
+                        rp = fmax(rp, fmax(dx[k] * isu, -dx[k] * isl));
                         rdl = fmax(rdl, fmax(-dlu / lu[k], -dll / ll[k]));
                     }
                 }
@@ -1247,28 +1267,30 @@ mincurv_pdip_kernel(int B, int n_max, const int32_t *__restrict__ n_pts, double 
             PROF_ADD(PROF_STEPLEN, tv4);
             PROF_T0(tv5);
             double musum2 = 0.0, rdmax = 0.0, dxmax = 0.0, amax = 0.0;
-            constexpr int VG2 = 2, VS2 = VG2 * IP_THREADS;        // 13 input vectors: groups of two
+            constexpr int VG2 = 2, VS2 = VG2 * IP_THREADS;        // 10 input vectors: groups of two
 #pragma unroll 1
             for (int i0 = threadIdx.x; i0 < n; i0 += VS2) {
-                double su[VG2], sl[VG2], lu[VG2], ll[VG2], dx[VG2], isu[VG2], isl[VG2], tu[VG2], tl[VG2], al[VG2], rd[VG2], rh[VG2], dd[VG2];
+                double su[VG2], sl[VG2], lu[VG2], ll[VG2], dxa[VG2], dx[VG2], al[VG2], rd[VG2], rh[VG2], dd[VG2];
 #pragma unroll
                 for (int k = 0; k < VG2; ++k) {
                     const int i = min(i0 + k * IP_THREADS, n - 1);
-                    su[k] = SU[i]; sl[k] = SL[i]; lu[k] = LU[i]; ll[k] = LL[i]; dx[k] = DX[i]; isu[k] = ISU[i]; isl[k] = ISL[i];
-                    tu[k] = TU[i]; tl[k] = TL[i]; al[k] = AL[i]; rd[k] = RD[i]; rh[k] = RHS[i]; dd[k] = DD[i];
+                    su[k] = SU[i]; sl[k] = SL[i]; lu[k] = LU[i]; ll[k] = LL[i]; dxa[k] = DXA[i]; dx[k] = DX[i];
+                    al[k] = AL[i]; rd[k] = RD[i]; rh[k] = RHS[i]; dd[k] = DD[i];
                 }
 #pragma unroll
                 for (int k = 0; k < VG2; ++k) {
                     const int i = i0 + k * IP_THREADS;
                     if (i < n) {
-                        const double dlu = (tu[k] + lu[k] * dx[k]) * isu[k], dll = (tl[k] - ll[k] * dx[k]) * isl[k];
+                        const double isu = 1.0 / su[k], isl = 1.0 / sl[k];
+                        double tu, tl;
+                        corrector_terms(smu, su[k], sl[k], lu[k], ll[k], dxa[k], isu, isl, tu, tl);
+                        const double dlu = (tu + lu[k] * dx[k]) * isu, dll = (tl - ll[k] * dx[k]) * isl;
                         const double an = al[k] + ap * dx[k], lun = lu[k] + ad * dlu, lln = ll[k] + ad * dll;
                         const double sun = su[k] - ap * dx[k], sln = sl[k] + ap * dx[k];
                         // H dx = rhs - D dx  (M dx = rhs)
                         const double rdn = rd[k] + ap * (rh[k] - dd[k] * dx[k]) + ad * (dlu - dll);
                         const double isun = 1.0 / sun, isln = 1.0 / sln;
                         AL[i] = an; LU[i] = lun; LL[i] = lln; RD[i] = rdn; SU[i] = sun; SL[i] = sln;
-                        ISU[i] = isun; ISL[i] = isln;
                         // the next iteration's barrier diagonal and affine right-hand side (the expressions of the
                         // initial point; unused if this iteration is the last)
                         DD[i] = lun * isun + lln * isln; RHS[i] = -rdn + lun - lln;

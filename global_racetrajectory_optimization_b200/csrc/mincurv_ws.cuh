@@ -4,8 +4,8 @@
 //   [NUM_VEC][np]        O(N) vectors (geometry, linearisation, interior-point iterates)
 //   [n_max][ZB_PITCH]    bands of B_t = Ti diag(w_t) Ti, t = 0..2  (assembly scratch, mincurv_setup.cu)
 //   [np][HB_PITCH]       band of H = E^T E              (row i: H[i][i .. i+32], cyclic; [33] padding)
-//   [np][33] + [np][34]  bordered LDL^T factor of H + D: chain rows [band of (Q - I; L21) | w] per panel of eight columns,
-//                        fill rows [G | z | w] (mincurv_ipm.cu)
+//   [np][33] + [np][33] + [np]  bordered LDL^T factor of H + D: chain rows [band of (Q - I; L21) | w] per panel of eight
+//                        columns, fill rows [G | w], and z = w y of the last forward substitution (mincurv_ipm.cu)
 // With shared centre lines a follower's band stays in its owner's slab: V_HBSRC says whose band an instance uses.
 #pragma once
 #include "common.cuh"
@@ -17,8 +17,8 @@ enum Vec : int {
     V_PX, V_PY, V_NX, V_NY, V_MX, V_MY, V_XP, V_YP, V_SX, V_SY, V_KREF,
     V_LB, V_UB, V_F,
     V_T0, V_T1, V_T2, V_T3, V_T4, V_T5,
-    V_ALPHA, V_LU, V_LL, V_RD, V_RHS, V_DX, V_DD, V_DLU, V_DLL, V_SU, V_SL,
-    V_ISU, V_ISL, V_HBSRC,                                  // reciprocal slacks, band source (band_owner)
+    V_ALPHA, V_LU, V_LL, V_RD, V_RHS, V_DX, V_DXA, V_DD, V_DLU, V_DLL, V_SU, V_SL,   // (DXA: the box phase's affine direction)
+    V_ISU, V_ISL, V_HBSRC,                                  // reciprocal slacks (K2b'), band source (band_owner)
     V_S3, V_S4, V_L3, V_L4, V_KL, V_WK, V_EDX, V_T3K, V_T4K, V_VV,   // curvature-row phase (K2b')
     V_IH,                                                   // 1 / h
     NUM_VEC
