@@ -52,6 +52,10 @@ EXPORTED_SYMBOLS = tuple(_SIGS)
 _SP_SENS_SIGS = header_signatures(_build.SP_SENS_HEADER)
 SP_SENS_SYMBOLS = tuple(_SP_SENS_SIGS)
 _SIGS.update(_SP_SENS_SIGS)
+# the lap time's sensitivity entries (batch.vel_profile_diff): the same library, a header of their own; load() binds them
+# too, but they stay out of _SIGS (the table of the public header and the shortest path's entries)
+LAP_SENS_SIGS = header_signatures(_build.LAP_SENS_HEADER)
+LAP_SENS_SYMBOLS = tuple(LAP_SENS_SIGS)
 
 
 def slab_mirror():
@@ -86,7 +90,7 @@ def load(build_if_missing: bool = True):
         raise MinCurvLibError(f"{path} is missing: build it with `python -m global_racetrajectory_optimization_b200.build` "
                               "(there is no CPU fallback for this path)")
     lib = ctypes.CDLL(path)
-    for name, (res, args) in _SIGS.items():
+    for name, (res, args) in {**_SIGS, **LAP_SENS_SIGS}.items():
         fn = getattr(lib, name)
         fn.restype = res
         fn.argtypes = args

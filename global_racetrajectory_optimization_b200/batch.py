@@ -496,6 +496,82 @@ def _create_raceline_once(lib, refline, normvec, alpha, stepsize_interp, n_pts, 
     return out
 
 
+_RL_KEYS = ("raceline_interp", "kappa", "el_lengths_interp", "coeffs_x", "coeffs_y", "spline_lengths", "n_out",
+            "spline_inds", "t_values", "s_interp", "psi")
+
+
+class _CreateRacelineDiff(torch.autograd.Function):
+    """raceline_interp, kappa and el_lengths_interp of create_raceline as functions of alpha, the reference line and the
+    normals; see create_raceline_diff."""
+
+    @staticmethod
+    def forward(ctx, refline, normvec, alpha, stepsize_interp, n_pts, n_out_max, strict):
+        out = create_raceline_batch(refline, normvec, alpha, stepsize_interp, n_pts=n_pts, n_out_max=n_out_max)
+        res = tuple(out[k] for k in _RL_KEYS)
+        ctx.save_for_backward(normvec, alpha, n_pts, out["coeffs_x"], out["coeffs_y"], out["spline_lengths"], out["n_out"],
+                              out["spline_inds"], out["t_values"])
+        ctx.ref_cols, ctx.strict = refline.shape[2], strict
+        ctx.mark_non_differentiable(*res[3:])
+        ctx.set_materialize_grads(False)
+        return res
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, g_ri, g_kappa, g_el, *_unused):
+        normvec, alpha, n_pts, cx, cy, sl, n_out, si, tv = ctx.saved_tensors
+        lib = _lib.load()
+        B, n_max = alpha.shape
+        f64 = dict(dtype=torch.float64, device=alpha.device)
+        g_ri, g_kappa, g_el = (None if g is None else g.to(**f64).contiguous() for g in (g_ri, g_kappa, g_el))
+        wanted = torch.zeros((B,), dtype=torch.bool, device=alpha.device)
+        for g in (g_ri, g_kappa, g_el):
+            if g is not None:
+                wanted |= (g.reshape(B, -1) != 0).any(dim=1)
+        # n_out <= 0: an overflow of an explicit n_out_max (-points needed) or an inactive track: nothing to differentiate
+        _refuse(ctx.strict, wanted, (n_out <= 0).to(torch.int32), "create_raceline_diff: no gradient",
+                "with n_out <= 0 (overflow of n_out_max or an inactive track)")
+        need_ref, need_nv, _ = ctx.needs_input_grad[:3]
+        g_alpha = torch.empty((B, n_max), **f64)
+        g_ref = torch.empty((B, n_max, 2), **f64) if need_ref else None
+        g_nv = torch.empty((B, n_max, 2), **f64) if need_nv else None
+        chunk = _chunk(B, lib.mc_create_raceline_adjoint_workspace_bytes(1, n_max), alpha.device)
+        ws = _workspace("raceline_adjoint", lib.mc_create_raceline_adjoint_workspace_bytes(chunk, n_max), alpha.device)
+        n_out_max = si.shape[1]
+        for s in range(0, B, chunk):
+            e = min(B, s + chunk)
+            rc = lib.mc_create_raceline_adjoint_batch(e - s, n_max, _rows_ptr(n_pts, s, e), _ptr(normvec[s:e]),
+                                                      _ptr(alpha[s:e]), n_out_max, _ptr(cx[s:e]), _ptr(cy[s:e]),
+                                                      _ptr(sl[s:e]), _ptr(n_out[s:e]), _ptr(si[s:e]), _ptr(tv[s:e]),
+                                                      _rows_ptr(g_ri, s, e), _rows_ptr(g_kappa, s, e),
+                                                      _rows_ptr(g_el, s, e), _ptr(g_alpha[s:e]), _rows_ptr(g_ref, s, e),
+                                                      _rows_ptr(g_nv, s, e), _ptr(ws), ws.numel(), _stream())
+            _lib.check(rc, "mc_create_raceline_adjoint_batch")
+        if g_ref is not None and ctx.ref_cols != 2:               # the width columns of a reftrack: no influence
+            g_ref = torch.cat((g_ref, torch.zeros((B, n_max, ctx.ref_cols - 2), **f64)), dim=2)
+        return g_ref, g_nv, g_alpha if ctx.needs_input_grad[2] else None, None, None, None, None
+
+
+@_device_guard
+def create_raceline_diff(refline: torch.Tensor, normvec: torch.Tensor, alpha: torch.Tensor, stepsize_interp: float,
+                         n_pts: Optional[torch.Tensor] = None, n_out_max: Optional[int] = None, strict: bool = True) -> dict:
+    """create_raceline_batch with raceline_interp, kappa and el_lengths_interp differentiable with respect to alpha, the
+    reference line (x, y; the width columns of a [B, n, 4] reftrack get zeros) and the normals (autograd).
+
+    Returns the dict of create_raceline_batch (the same values).  Every other entry, psi included, is not differentiable.
+    The derivative holds n_out and every station's spline segment at the forward's; one CTA per track walks the
+    stations, the lengths and the moment system backwards (DESIGN.md section 3.12).  Any input may be a constant.
+    strict=True: backward raises for a track with n_out <= 0 (an overflow of an explicit n_out_max, or an inactive track)
+    that received a nonzero upstream gradient; strict=False: such tracks get zero gradients."""
+    _require_cuda()
+    refline, normvec, alpha = _f64(refline, "refline"), _f64(normvec, "normvec"), _f64(alpha, "alpha")
+    B, n_max, cols = refline.shape
+    if cols not in (2, 4) or normvec.shape != (B, n_max, 2) or alpha.shape != (B, n_max):
+        raise RuntimeError("create_raceline_diff: refline must be [B, n_max, 2 or 4], normvec [B, n_max, 2], alpha [B, n_max]")
+    res = _CreateRacelineDiff.apply(refline, normvec, alpha, float(stepsize_interp), _npts(n_pts, B, refline.device),
+                                    n_out_max, bool(strict))
+    return dict(zip(_RL_KEYS, res))
+
+
 @_device_guard
 def calc_head_curv_batch(coeffs_x: torch.Tensor, coeffs_y: torch.Tensor, ind_spls: torch.Tensor, t_spls: torch.Tensor,
                          n_eval: Optional[torch.Tensor] = None, calc_curv: bool = True, calc_dcurv: bool = False):
@@ -745,6 +821,91 @@ def vel_profile_batch(kappa: torch.Tensor, el_lengths: torch.Tensor, ggv, ax_max
     if want_profiles:
         out.update(vx=vx, ax=ax, t=t)
     return out
+
+
+class _VelProfileDiff(torch.autograd.Function):
+    """laptime and vx of the velocity profile as functions of kappa and el_lengths; see vel_profile_diff."""
+
+    @staticmethod
+    def forward(ctx, kappa, el_lengths, n_pts, ggv_t, mach_t, v_max, drag_coeff, m_veh, dyn_model_exp, fw, dsu, strict):
+        res = vel_profile_batch(kappa, el_lengths, ggv_t, mach_t, v_max, drag_coeff, m_veh, dyn_model_exp,
+                                fw if fw > 1 else None, n_pts=n_pts, decel_slice_upper=dsu)
+        laptime, status = res["laptime"][:, 0], res["status"][:, 0]
+        vx, ax, t = res["vx"][:, 0], res["ax"][:, 0], res["t"][:, 0]
+        grad_status = status.clone()
+        ctx.save_for_backward(kappa, el_lengths, n_pts, ggv_t, mach_t, grad_status)
+        ctx.params = (v_max, dyn_model_exp, drag_coeff, m_veh, fw, dsu)
+        ctx.strict = strict
+        ctx.mark_non_differentiable(ax, t, status, grad_status)
+        ctx.set_materialize_grads(False)
+        return laptime, vx, ax, t, status, grad_status
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, grad_laptime, grad_vx, *_unused):
+        kappa, el_lengths, n_pts, ggv_t, mach_t, grad_status = ctx.saved_tensors
+        v_max, dyn_model_exp, drag_coeff, m_veh, fw, dsu = ctx.params
+        lib = _lib.load()
+        B, n_max = kappa.shape
+        f64 = dict(dtype=torch.float64, device=kappa.device)
+        grad_laptime = None if grad_laptime is None else grad_laptime.to(**f64).contiguous()
+        grad_vx = None if grad_vx is None else grad_vx.to(**f64).contiguous()
+        wanted = torch.zeros((B,), dtype=torch.bool, device=kappa.device)
+        if grad_laptime is not None:
+            wanted |= grad_laptime != 0
+        if grad_vx is not None:
+            wanted |= (grad_vx != 0).any(dim=1)
+        who = "vel_profile_diff: no gradient"
+        _refuse(ctx.strict, wanted, grad_status, who, "with a nonzero upstream gradient")
+        need_k, need_e = ctx.needs_input_grad[:2]
+        gk = torch.empty((B, n_max), **f64) if need_k else None
+        ge = torch.empty((B, n_max), **f64) if need_e else None
+        gs = torch.empty((B,), dtype=torch.int32, device=kappa.device)
+        chunk = _chunk(B, lib.mc_vel_profile_adjoint_workspace_bytes(1, n_max), kappa.device)
+        ws = _workspace("velprofile_adjoint", lib.mc_vel_profile_adjoint_workspace_bytes(chunk, n_max), kappa.device)
+        for s in range(0, B, chunk):
+            e = min(B, s + chunk)
+            rc = lib.mc_vel_profile_adjoint_batch(e - s, n_max, _rows_ptr(n_pts, s, e), _ptr(kappa[s:e]),
+                                                  _ptr(el_lengths[s:e]), v_max, int(ggv_t.shape[0]), _ptr(ggv_t),
+                                                  int(mach_t.shape[0]), _ptr(mach_t), dyn_model_exp, drag_coeff, m_veh, fw,
+                                                  dsu, _rows_ptr(grad_laptime, s, e), _rows_ptr(grad_vx, s, e),
+                                                  _rows_ptr(gk, s, e), _rows_ptr(ge, s, e), _ptr(gs[s:e]), _ptr(ws),
+                                                  ws.numel(), _stream())
+            _lib.check(rc, "mc_vel_profile_adjoint_batch")
+        _refuse(ctx.strict, wanted, gs, who, "whose gradient is not finite")
+        return (gk, ge) + (None,) * 10
+
+
+@_device_guard
+def vel_profile_diff(kappa: torch.Tensor, el_lengths: torch.Tensor, ggv, ax_max_machines, v_max: float, drag_coeff: float,
+                     m_veh: float, dyn_model_exp: float = 1.0, filt_window: Optional[int] = None,
+                     n_pts: Optional[torch.Tensor] = None, decel_slice_upper: Optional[int] = None,
+                     strict: bool = True) -> dict:
+    """vel_profile_batch for one profile per track (no ggv scales, one top speed, no mu) with the lap time and the speed
+    profile differentiable with respect to kappa and el_lengths (autograd).
+
+    Returns dict(laptime [B], vx [B, n_max], ax [B, n_max], t [B, n_max + 1], status [B], grad_status [B]): the values of
+    vel_profile_batch with V = 1.  laptime and vx carry a grad_fn; backward() / torch.autograd.grad give dL/dkappa and
+    dL/del_lengths [B, n_max] (zero beyond n_pts) at the cost of running the profile again with a tape and walking it
+    backwards, one thread per track (DESIGN.md section 3.12).  The derivative is that of the function the forward
+    evaluates, with its discrete decisions (phase starts, which limit wins each min, table segments, the v_max clip)
+    frozen.  Chain it to create_raceline_batch's kappa / el_lengths_interp with n_pts=rl["n_out"].
+    grad_status: 0 = the gradient is computed; 3 = a non-finite lap time or gradient; for an inactive slot (n_pts < 2)
+    the forward's status.  strict=True: backward raises if an instance with a nonzero upstream gradient has
+    grad_status != 0; strict=False: such instances get zero gradients."""
+    _require_cuda()
+    dev = kappa.device
+    if isinstance(v_max, torch.Tensor) or hasattr(v_max, "__len__"):
+        raise ValueError("vel_profile_diff: v_max must be one number (no per-variant top speeds)")
+    if filt_window is not None and int(filt_window) % 2 != 1:
+        raise RuntimeError("Window width of moving average filter must be odd!")
+    kappa_t, el_t = _f64(kappa, "kappa"), _f64(el_lengths, "el_lengths")
+    laptime, vx, ax, t, status, grad_status = _VelProfileDiff.apply(
+        kappa_t, el_t, _npts(n_pts, kappa_t.shape[0], dev), _table(ggv, 3, "ggv", dev),
+        _table(ax_max_machines, 2, "ax_max_machines", dev), float(v_max), float(drag_coeff), float(m_veh),
+        float(dyn_model_exp), 0 if filt_window is None else int(filt_window),
+        int(VP_DECEL_SLICE_UPPER if decel_slice_upper is None else decel_slice_upper), bool(strict))
+    return dict(laptime=laptime, vx=vx, ax=ax, t=t, status=status, grad_status=grad_status)
 
 
 def lap_time_matrix_batch(kappa: torch.Tensor, el_lengths: torch.Tensor, ggv, ax_max_machines, ggv_scales, top_speeds,

@@ -12,6 +12,7 @@ CSRC = os.path.join(_HERE, "csrc")
 INCLUDE = os.path.join(os.path.dirname(_HERE), "include")
 HEADER = os.path.join(INCLUDE, "mincurv_b200.h")      # the C-ABI; _lib derives its ctypes signatures from it
 SP_SENS_HEADER = os.path.join(CSRC, "shortest_path_sens.h")     # the shortest path's sensitivity entries, bound the same way
+LAP_SENS_HEADER = os.path.join(CSRC, "lap_time_sens.h")         # the lap time's sensitivity entries, bound the same way
 LIB_PATH = os.path.join(_HERE, "libmincurv_b200.so")
 SOURCES = sorted(glob.glob(os.path.join(CSRC, "*.cu")))
 HEADERS = sorted(glob.glob(os.path.join(CSRC, "*.cuh")) + glob.glob(os.path.join(CSRC, "*.h")) +

@@ -8,6 +8,7 @@
 #include "../../include/mincurv_b200.h"
 #include "mincurv_ws.cuh"
 #include "shortest_path_sens.h"
+#include "lap_time_sens.h"
 
 namespace mc {
 size_t spline_ws_doubles(int n_max);
@@ -57,6 +58,15 @@ int launch_vel_profile(int, int, int, const int32_t *, const double *, const dou
                        double *, double *, double *, double *, int32_t *, double *, cudaStream_t);
 void launch_ax_t_profile(int, int, const int32_t *, const double *, int, const double *, const double *, double, double *,
                          double *, cudaStream_t);
+size_t vel_profile_adjoint_ws_doubles(int n_max);
+size_t create_raceline_adjoint_ws_doubles(int n_max);
+void launch_create_raceline_adjoint(int, int, const int32_t *, const double *, const double *, int, const double *,
+                                    const double *, const double *, const int32_t *, const int32_t *, const double *,
+                                    const double *, const double *, const double *, double *, double *, double *, double *,
+                                    cudaStream_t);
+int launch_vel_profile_adjoint(int, int, const int32_t *, const double *, const double *, double, int, const double *, int,
+                               const double *, double, double, double, int, int, const double *, const double *, double *,
+                               double *, int32_t *, double *, cudaStream_t);
 size_t interp_track_ws_doubles(int n_max);
 void launch_interp_track(int, int, const int32_t *, const double *, int, const double *, double, int, double, int, double *,
                          int32_t *, double *, cudaStream_t);
@@ -503,6 +513,56 @@ int mc_vel_profile_batch_ex(int B, int n_max, const int32_t *n_pts, const double
                                laptime, status, (double *)workspace, (cudaStream_t)stream) != 0)
         return bad("mc_vel_profile_batch: ggv / ax_max_machines tables are limited to 256 rows");
     return check_cuda("vel_profile_kernel");
+}
+
+size_t mc_create_raceline_adjoint_workspace_bytes(int B, int n_max) {
+    if (B <= 0 || n_max < 3) return 0;
+    return align256((size_t)B * mc::create_raceline_adjoint_ws_doubles(n_max) * sizeof(double));
+}
+
+int mc_create_raceline_adjoint_batch(int B, int n_max, const int32_t *n_pts, const double *normvec, const double *alpha,
+                                     int n_out_max, const double *coeffs_x, const double *coeffs_y,
+                                     const double *spline_lengths, const int32_t *n_out, const int32_t *spline_inds,
+                                     const double *t_values, const double *grad_raceline, const double *grad_kappa,
+                                     const double *grad_el_lengths, double *grad_alpha, double *grad_refline,
+                                     double *grad_normvec, void *workspace, size_t workspace_bytes, void *stream) {
+    if (B <= 0 || n_max < 3 || n_out_max < 1 || !normvec || !alpha || !coeffs_x || !coeffs_y || !spline_lengths ||
+        !n_out || !spline_inds || !t_values || !grad_alpha)
+        return bad("mc_create_raceline_adjoint_batch: bad argument");
+    if (B > 65535 * 1024) return bad("mc_create_raceline_adjoint_batch: too many tracks in one call");
+    if (!workspace || workspace_bytes < mc_create_raceline_adjoint_workspace_bytes(B, n_max))
+        return small_workspace("mc_create_raceline_adjoint_batch");
+    mc::launch_create_raceline_adjoint(B, n_max, n_pts, normvec, alpha, n_out_max, coeffs_x, coeffs_y, spline_lengths, n_out,
+                                       spline_inds, t_values, grad_raceline, grad_kappa, grad_el_lengths, grad_alpha,
+                                       grad_refline, grad_normvec, (double *)workspace, (cudaStream_t)stream);
+    return check_cuda("create_raceline_adjoint_kernel");
+}
+
+size_t mc_vel_profile_adjoint_workspace_bytes(int B, int n_max) {
+    if (B <= 0 || n_max < 2) return 0;
+    return align256((size_t)B * mc::vel_profile_adjoint_ws_doubles(n_max) * sizeof(double));
+}
+
+int mc_vel_profile_adjoint_batch(int B, int n_max, const int32_t *n_pts, const double *kappa, const double *el_lengths,
+                                 double v_max, int n_ggv, const double *ggv, int n_mach, const double *ax_max_machines,
+                                 double dyn_model_exp, double drag_coeff, double m_veh, int filt_window,
+                                 int decel_slice_upper, const double *grad_laptime, const double *grad_vx,
+                                 double *grad_kappa, double *grad_el_lengths, int32_t *grad_status,
+                                 void *workspace, size_t workspace_bytes, void *stream) {
+    if (B <= 0 || n_max < 2 || !kappa || !el_lengths || !ggv || !ax_max_machines || !grad_status || n_ggv < 1 ||
+        n_mach < 1 || !(m_veh > 0.0) || !(dyn_model_exp > 0.0) || !(v_max > 0.0))
+        return bad("mc_vel_profile_adjoint_batch: bad argument");
+    if (filt_window > 1 && (filt_window % 2 == 0 || filt_window >= n_max))
+        return bad("mc_vel_profile_adjoint_batch: filt_window must be odd and smaller than n_max");
+    if ((size_t)B > (size_t)0x7fffffff - 256) return bad("mc_vel_profile_adjoint_batch: too many profiles in one call");
+    if (!workspace || workspace_bytes < mc_vel_profile_adjoint_workspace_bytes(B, n_max))
+        return small_workspace("mc_vel_profile_adjoint_batch");
+    if (mc::launch_vel_profile_adjoint(B, n_max, n_pts, kappa, el_lengths, v_max, n_ggv, ggv, n_mach, ax_max_machines,
+                                       dyn_model_exp, drag_coeff, m_veh, filt_window, decel_slice_upper != 0, grad_laptime,
+                                       grad_vx, grad_kappa, grad_el_lengths, grad_status, (double *)workspace,
+                                       (cudaStream_t)stream) != 0)
+        return bad("mc_vel_profile_adjoint_batch: ggv / ax_max_machines tables are limited to 256 rows");
+    return check_cuda("vel_profile_adjoint_kernel");
 }
 
 int mc_calc_ax_t_profile_batch(int P, int n_max, const int32_t *n_pts, const double *vx, int vx_pitch,

@@ -405,6 +405,184 @@ __global__ void scale_alpha_kernel(int n_max, double *__restrict__ alpha, const 
 }
 
 // ---------------------------------------------------------------------------------------------
+// K3d -- vector-Jacobian product of create_raceline_kernel (DESIGN.md section 3.12).  n_out and every station's segment
+// are held at the forward's (read from its outputs, not searched again).  One CTA per track, like the forward:
+//   1. station terms: per segment j one thread sums, in station order, the terms of its stations (point, kappa, and
+//      t = (i total / no - CUM[j-1]) / sl[j]; every el_i is total / no): the adjoints of the coefficients of j, of
+//      sl[j], of CUM[j-1] and a share of the adjoint of total (no atomics);
+//   2. lengths: the cumulative sum reversed (a suffix scan, the forward's chunked scan backwards), then the 15-sample
+//      polylines back onto the coefficients;
+//   3. moments: the coefficients give the adjoint of the moments gm and a direct part of the point adjoint; the moment
+//      system m = A^-1 6 D2 p has A = circ(1, 4, 1) and D2 circulant, so they commute and the adjoint of p through m,
+//      6 D2 A^-1 gm, is what the forward's own solve (closed_spline: PCR or chunked, shared or global scratch) returns for
+//      the input points gm.
+// ---------------------------------------------------------------------------------------------
+enum CraVec : int { G_SL = 0, G_CUM, G_C0X, G_C1X, G_C2X, G_C3X, G_C0Y, G_C1Y, G_C2Y, G_C3Y, G_NUM };
+
+size_t create_raceline_adjoint_ws_doubles(int n_max) { return (size_t)(S_NUM + G_NUM) * spl_np(n_max); }
+
+struct CraAdjArgs {
+    int n_max, n_out_max;
+    const int32_t *n_pts, *n_out, *spline_inds;
+    const double *normvec, *alpha, *coeffs_x, *coeffs_y, *spline_lengths, *t_values;
+    const double *g_raceline, *g_kappa, *g_el;
+    double *g_alpha, *g_refline, *g_normvec, *ws;
+};
+
+__global__ void __launch_bounds__(256) create_raceline_adjoint_kernel(const CraAdjArgs a) {
+    const int b = blockIdx.x;
+    const int n = a.n_pts ? a.n_pts[b] : a.n_max;
+    const int no = a.n_out[b];
+    const size_t row = (size_t)b * a.n_max;
+    __shared__ double s_part[256];
+    const bool ok = n >= 3 && n <= a.n_max && no > 0 && no <= a.n_out_max;
+    for (int i = threadIdx.x + (ok ? n : 0); i < a.n_max; i += blockDim.x) {      // padding / unsupported track: zeros
+        a.g_alpha[row + i] = 0.0;
+        if (a.g_refline) { a.g_refline[2 * (row + i)] = 0.0; a.g_refline[2 * (row + i) + 1] = 0.0; }
+        if (a.g_normvec) { a.g_normvec[2 * (row + i)] = 0.0; a.g_normvec[2 * (row + i) + 1] = 0.0; }
+    }
+    if (!ok) return;
+    const int np = spl_np(a.n_max);
+    extern __shared__ __align__(16) double spl_sm[];
+    double *sv = (spline_smem_bytes(a.n_max) <= SPL_SMEM_LIMIT) ? spl_sm : a.ws + (size_t)b * (S_NUM + G_NUM) * np;
+    double *G = a.ws + (size_t)b * (S_NUM + G_NUM) * np + (size_t)S_NUM * np;
+    double *GSL = G + G_SL * np, *GCUM = G + G_CUM * np;
+    const double *cx = a.coeffs_x + row * 4, *cy = a.coeffs_y + row * 4, *sl = a.spline_lengths + row;
+    const size_t orow = (size_t)b * a.n_out_max;
+    const int32_t *si = a.spline_inds + orow;
+    const double *tv = a.t_values + orow;
+    const double inv_no = 1.0 / (double)no;
+
+    // ---- 1. station terms, one thread per segment ----
+    double g_total = 0.0;
+    for (int j = threadIdx.x; j < n; j += blockDim.x) {
+        int lo = 0, hi = no;                                   // first station of segment j (spline_inds is sorted)
+        while (lo < hi) { const int mid = (lo + hi) >> 1; if (si[mid] < j) lo = mid + 1; else hi = mid; }
+        const double4 ax = *reinterpret_cast<const double4 *>(cx + (size_t)j * 4);
+        const double4 ay = *reinterpret_cast<const double4 *>(cy + (size_t)j * 4);
+        const double sj = sl[j];
+        double gx[4] = {0.0, 0.0, 0.0, 0.0}, gy[4] = {0.0, 0.0, 0.0, 0.0}, gsl = 0.0, gcum = 0.0;
+        for (int i = lo; i < no && si[i] == j; ++i) {
+            const double t = tv[i], t2 = t * t, t3 = t2 * t;
+            const double gpx = a.g_raceline ? a.g_raceline[2 * (orow + i)] : 0.0;
+            const double gpy = a.g_raceline ? a.g_raceline[2 * (orow + i) + 1] : 0.0;
+            const double gk = a.g_kappa ? a.g_kappa[orow + i] : 0.0;
+            const double xd = ax.y + 2.0 * ax.z * t + 3.0 * ax.w * t2, yd = ay.y + 2.0 * ay.z * t + 3.0 * ay.w * t2;
+            const double xdd = 2.0 * ax.z + 6.0 * ax.w * t, ydd = 2.0 * ay.z + 6.0 * ay.w * t;
+            double gxd = 0.0, gyd = 0.0, gxdd = 0.0, gydd = 0.0;
+            if (gk != 0.0) {                                   // kappa = (xd ydd - yd xdd) / q^1.5
+                const double q = xd * xd + yd * yd, q15 = q * sqrt(q);
+                const double kap = (xd * ydd - yd * xdd) / q15;
+                gxd = gk * (ydd / q15 - 3.0 * kap * xd / q);
+                gyd = gk * (-xdd / q15 - 3.0 * kap * yd / q);
+                gxdd = -gk * yd / q15;
+                gydd = gk * xd / q15;
+            }
+            gx[0] += gpx; gx[1] += gpx * t + gxd; gx[2] += gpx * t2 + 2.0 * t * gxd + 2.0 * gxdd;
+            gx[3] += gpx * t3 + 3.0 * t2 * gxd + 6.0 * t * gxdd;
+            gy[0] += gpy; gy[1] += gpy * t + gyd; gy[2] += gpy * t2 + 2.0 * t * gyd + 2.0 * gydd;
+            gy[3] += gpy * t3 + 3.0 * t2 * gyd + 6.0 * t * gydd;
+            const double gt = gpx * xd + gpy * yd + gxd * xdd + gyd * ydd + 6.0 * (gxdd * ax.w + gydd * ay.w);
+            // t = (i total / no - CUM[j-1]) / sl[j];  el_i = total / no
+            g_total += gt * (double)i * inv_no / sj + (a.g_el ? a.g_el[orow + i] : 0.0) * inv_no;
+            gcum -= gt / sj;
+            gsl -= gt * t / sj;
+        }
+        G[G_C0X * np + j] = gx[0]; G[G_C1X * np + j] = gx[1]; G[G_C2X * np + j] = gx[2]; G[G_C3X * np + j] = gx[3];
+        G[G_C0Y * np + j] = gy[0]; G[G_C1Y * np + j] = gy[1]; G[G_C2Y * np + j] = gy[2]; G[G_C3Y * np + j] = gy[3];
+        GSL[j] = gsl;
+        if (j > 0) GCUM[j - 1] = gcum;
+    }
+    s_part[threadIdx.x] = g_total;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        double s = 0.0;
+        for (int t = 0; t < (int)blockDim.x; ++t) s += s_part[t];
+        GCUM[n - 1] = s;                                       // total = CUM[n - 1]
+    }
+    __syncthreads();
+    // ---- 2. lengths: GSL[i] += sum_{k >= i} GCUM[k] (chunk per thread + suffix scan of the chunk sums) ----
+    const int chunk = (n + blockDim.x - 1) / blockDim.x;
+    const int c0 = threadIdx.x * chunk, c1 = min(c0 + chunk, n);
+    double part = 0.0;
+    for (int i = c0; i < c1; ++i) part += GCUM[i];
+    s_part[threadIdx.x] = part;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        double run = 0.0;
+        for (int t = (int)blockDim.x - 1; t >= 0; --t) { const double v = s_part[t]; s_part[t] = run; run += v; }
+    }
+    __syncthreads();
+    double run = s_part[threadIdx.x];
+    for (int i = c1 - 1; i >= c0; --i) { run += GCUM[i]; GSL[i] += run; }
+    __syncthreads();
+    //      the 15-sample polyline of segment i (tph.calc_spline_lengths) onto its coefficients
+    for (int i = threadIdx.x; i < n; i += blockDim.x) {
+        const double4 ax = *reinterpret_cast<const double4 *>(cx + (size_t)i * 4);
+        const double4 ay = *reinterpret_cast<const double4 *>(cy + (size_t)i * 4);
+        const double g = GSL[i];
+        double gx[4] = {0.0, 0.0, 0.0, 0.0}, gy[4] = {0.0, 0.0, 0.0, 0.0};
+        double xprev = ax.x, yprev = ay.x, tp[4] = {1.0, 0.0, 0.0, 0.0};
+        for (int s = 1; s < 15; ++s) {
+            const double t = (s == 14) ? 1.0 : (double)s * (1.0 / 14.0);
+            const double t2 = t * t, t3 = t2 * t;
+            const double x = ax.x + ax.y * t + ax.z * t2 + ax.w * t3;
+            const double y = ay.x + ay.y * t + ay.z * t2 + ay.w * t3;
+            const double dx = x - xprev, dy = y - yprev, len = sqrt(dx * dx + dy * dy);
+            if (len > 0.0) {
+                const double ux = g * dx / len, uy = g * dy / len;
+                const double tc[4] = {1.0, t, t2, t3};
+#pragma unroll
+                for (int k = 1; k < 4; ++k) { gx[k] += ux * (tc[k] - tp[k]); gy[k] += uy * (tc[k] - tp[k]); }
+            }
+            tp[1] = t; tp[2] = t2; tp[3] = t3;
+            xprev = x; yprev = y;
+        }
+        G[G_C1X * np + i] += gx[1]; G[G_C2X * np + i] += gx[2]; G[G_C3X * np + i] += gx[3];
+        G[G_C1Y * np + i] += gy[1]; G[G_C2Y * np + i] += gy[2]; G[G_C3Y * np + i] += gy[3];
+    }
+    __syncthreads();
+    // ---- 3. coefficients -> moments (into the points of the spline scratch) and the direct part of the points ----
+    //      c0 = p_i, c1 = p_i+1 - p_i - (2 m_i + m_i+1) / 6, c2 = m_i / 2, c3 = (m_i+1 - m_i) / 6
+    double *H = sv, *PX = sv + np, *PY = sv + 2 * np;
+    for (int i = threadIdx.x; i < n; i += blockDim.x) {
+        const int im = (i == 0) ? n - 1 : i - 1;
+        PX[i] = -G[G_C1X * np + i] / 3.0 + 0.5 * G[G_C2X * np + i] - G[G_C3X * np + i] / 6.0
+                - G[G_C1X * np + im] / 6.0 + G[G_C3X * np + im] / 6.0;
+        PY[i] = -G[G_C1Y * np + i] / 3.0 + 0.5 * G[G_C2Y * np + i] - G[G_C3Y * np + i] / 6.0
+                - G[G_C1Y * np + im] / 6.0 + G[G_C3Y * np + im] / 6.0;
+        H[i] = 1.0;
+    }
+    __syncthreads();
+    closed_spline(sv, np, n, nullptr, nullptr, nullptr, true);      // MX, MY = 6 D2 A^-1 gm
+    const double *MX = sv + 6 * np, *MY = sv + 7 * np;
+    const double *nv = a.normvec + row * 2, *al = a.alpha + row;
+    for (int i = threadIdx.x; i < n; i += blockDim.x) {
+        const int im = (i == 0) ? n - 1 : i - 1;
+        const double gpx = G[G_C0X * np + i] - G[G_C1X * np + i] + G[G_C1X * np + im] + MX[i];
+        const double gpy = G[G_C0Y * np + i] - G[G_C1Y * np + i] + G[G_C1Y * np + im] + MY[i];
+        const double2 nn = *reinterpret_cast<const double2 *>(nv + (size_t)i * 2);
+        a.g_alpha[row + i] = nn.x * gpx + nn.y * gpy;               // P = p + alpha n
+        if (a.g_refline) { a.g_refline[2 * (row + i)] = gpx; a.g_refline[2 * (row + i) + 1] = gpy; }
+        if (a.g_normvec) { a.g_normvec[2 * (row + i)] = al[i] * gpx; a.g_normvec[2 * (row + i) + 1] = al[i] * gpy; }
+    }
+}
+
+void launch_create_raceline_adjoint(int B, int n_max, const int32_t *n_pts, const double *normvec, const double *alpha, int n_out_max, const double *cx,
+                                    const double *cy, const double *sl, const int32_t *n_out, const int32_t *si,
+                                    const double *tv, const double *g_raceline, const double *g_kappa, const double *g_el,
+                                    double *g_alpha, double *g_refline, double *g_normvec, double *ws, cudaStream_t stream) {
+    CraAdjArgs a;
+    a.n_max = n_max; a.n_out_max = n_out_max; a.n_pts = n_pts; a.n_out = n_out;
+    a.spline_inds = si; a.normvec = normvec; a.alpha = alpha; a.coeffs_x = cx; a.coeffs_y = cy;
+    a.spline_lengths = sl; a.t_values = tv; a.g_raceline = g_raceline; a.g_kappa = g_kappa; a.g_el = g_el;
+    a.g_alpha = g_alpha; a.g_refline = g_refline; a.g_normvec = g_normvec; a.ws = ws;
+    const size_t sm = spline_smem_bytes(n_max) <= SPL_SMEM_LIMIT ? spline_smem_bytes(n_max) : 0;
+    cudaFuncSetAttribute(create_raceline_adjoint_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SPL_SMEM_LIMIT);
+    create_raceline_adjoint_kernel<<<B, 256, sm, stream>>>(a);
+}
+
+// ---------------------------------------------------------------------------------------------
 void launch_calc_splines(int B, int n_max, const int32_t *n_pts, const double *xy, int xy_stride,
                          const double *el_lengths, int use_dist_scaling, double *cx, double *cy, double *nvec,
                          double *h_out, double *ws, cudaStream_t stream) {

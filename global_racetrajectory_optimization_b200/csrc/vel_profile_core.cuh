@@ -156,12 +156,31 @@ VP_HD double ax_poss(double vx, double radius, double mu, bool has_mu, bool acce
 // sqrt(v^2 + 2 a el)
 VP_HD double v_next(double v, double a, double el) { return sqrt(add(mul(v, v), mul(mul(2.0, a), el))); }
 
+// Tape policy of profile_thread that records nothing (the forward kernel); TapeRecorder below records what the adjoint
+// needs.  The hooks see the values of the forward statements and never change them.
+struct NoTape {
+    VP_HD void initial(int, int, double, double, double, double, const Tables &, double) const {}
+    VP_HD void fwd(int, double, int) const {}
+    VP_HD void bwd(int, double, int) const {}
+};
+
+// Branch codes of one step of the forward / backward pass (the low byte; the adjoint adds the table segments above it)
+constexpr int VP_BR_ACTIVE = 1;     // the step computed a reachable speed
+constexpr int VP_BR_TAKEN = 2;      // ... and it won the min against the initial profile
+constexpr int VP_BR_LEAVE = 4;      // ... and it exceeded v_max (the phase ends)
+constexpr int VP_BR_VTMP = 8;       // backward pass: the one-step correction vtmp won the min against vpn
+constexpr int VP_BR_CLAMP = 16;     // set by the adjoint: the radicand of an ax_poss call was clamped to 0
+constexpr int VP_BR_MACH = 32;      // set by the adjoint: the machine limit won against the tyre limit
+constexpr int VP_BR_CLAMP2 = 64;    // set by the adjoint: the radicand of the correction step's ax_poss was clamped
+
 // One closed-track profile.  kappa/el/mu: this profile's track rows (contiguous, n entries; mu may be null).
 // R, EL, MU, V, W: scratch vectors of n entries each (MU unused without mu, W unused without filter).
 // vx_out/ax_out [n], t_out [n + 1] may each be null; *laptime always written.  Returns the status code.
+// tp: the tape policy (NoTape: the forward alone).
+template <class Tape = NoTape>
 VP_HD int profile_thread(int n, const double *kappa, const double *el, const double *mu, double scale, double v_max,
                          const Tables &tb, const Params &pr, Strided R, Strided EL, Strided MU, Strided V, Strided W,
-                         double *vx_out, double *ax_out, double *t_out, double *laptime) {
+                         double *vx_out, double *ax_out, double *t_out, double *laptime, const Tape &tp = Tape()) {
     const bool has_mu = (mu != nullptr);
     // radii = |1 / kappa| (inf where kappa == 0); private coalesced copies of the track rows.
     // All streaming loops below are blocked by VP_UNROLL with the loads of a block issued before its arithmetic
@@ -217,6 +236,7 @@ VP_HD int profile_thread(int n, const double *kappa, const double *el, const dou
                     if (has_mu) ay = mul(m[u], ay);
                     const double vn = sqrt(mul(ay, r[u]));
                     V[i + u] = vn;
+                    tp.initial(it, i + u, r[u], vp[u], ay, vn, tb, scale);
                     const double d = fabs(sub(vn / vp[u], 1.0));
                     if (d != d) any_nan = true;
                     else if (d > dmax) dmax = d;
@@ -252,12 +272,15 @@ VP_HD int profile_thread(int n, const double *kappa, const double *el, const dou
             const double dj = sub(nxt0, prev0);
             if (dj > 0.0 && (j == 0 || !(dprev > 0.0))) active = true;
             double nxt = nxt0;
+            int code = 0;
             if (active) {
                 const double a = ax_poss(cur, r, m, has_mu, true, tb, scale, pr, hints);
                 const double vpn = v_next(cur, a, e);
                 if (vpn < nxt0) nxt = vpn;
                 if (vpn > v_max) active = false;
+                code = VP_BR_ACTIVE | (vpn < nxt0 ? VP_BR_TAKEN : 0) | (vpn > v_max ? VP_BR_LEAVE : 0);
             }
+            tp.fwd(j, cur, code);
             if (j + 1 >= n) V[i1] = nxt;
             cur = nxt;
             prev0 = nxt0;
@@ -291,16 +314,20 @@ VP_HD int profile_thread(int n, const double *kappa, const double *el, const dou
             const double dj = sub(nxt0, prev0);
             if (dj > 0.0 && (j == 0 || !(dprev > 0.0))) active = true;
             double nxt = nxt0;
+            int code = 0;
             if (active) {
                 const double a = ax_poss(cur, r0, m0, has_mu, false, tb, scale, pr, hints);
                 double vpn = v_next(cur, a, e0);
                 // the acceleration found at this point need not be feasible at the next one: one correction step
                 const double a2 = ax_poss(vpn, r1, m1, has_mu, false, tb, scale, pr, hints);
                 const double vtmp = v_next(cur, a2, e0);
+                code = VP_BR_ACTIVE | (vtmp < vpn ? VP_BR_VTMP : 0);
                 if (vtmp < vpn) vpn = vtmp;
                 if (vpn < nxt0) nxt = vpn;
                 if (vpn > v_max) active = false;
+                code |= (vpn < nxt0 ? VP_BR_TAKEN : 0) | (vpn > v_max ? VP_BR_LEAVE : 0);
             }
+            tp.bwd(j, cur, code);
             if (slice_upper || j + 1 >= n) V[i1] = nxt;
             cur = nxt;
             prev0 = nxt0;
@@ -348,6 +375,238 @@ VP_HD int profile_thread(int n, const double *kappa, const double *el, const dou
     }
     *laptime = t;
     return (t == t && fabs(t) < (double)INFINITY) ? VP_STATUS_OK : VP_STATUS_NONFINITE;
+}
+
+// ================================================================================================================
+// K5d -- vector-Jacobian product of profile_thread (mu == nullptr) with respect to kappa and el (DESIGN.md section 3.12).
+// The function differentiated is the one the forward evaluates with every discrete decision frozen as it took it: the
+// active flags, the winner of every min, the radicand clamp, the table segments, the v_max clip and the number of
+// fixed-point iterations of the initial profile.
+// ================================================================================================================
+
+// d/dx of numpy.interp(x, xp, fp * s) on the segment interp takes (the right-hand one at a knot), 0 where interp clamps.
+// *seg: that segment, -1 where clamped.
+VP_HD double interp_slope(double x, const double *xp, const double *fp, int n, double s, int *seg) {
+    if (!(x >= xp[0]) || x >= xp[n - 1]) {
+        *seg = -1;
+        return 0.0;
+    }
+    int h = 0;
+    const int lo = find_segment(x, xp, n, h);
+    *seg = lo;
+    return sub(mul(fp[lo + 1], s), mul(fp[lo], s)) / sub(xp[lo + 1], xp[lo]);
+}
+
+// What profile_thread<TapeRecorder> leaves for the reverse walk, interleaved like the forward's scratch vectors:
+//   V0 [n]      the initial profile (before the v_max clip)
+//   D  [n]      dV0/dr, carried in forward mode through the fixed-point iterations (pointwise: one scalar per point)
+//   CF, CB [2n] the carried speed `cur` before every step of the forward / backward pass
+//   KF, KB [2n] the branch code of every step (VP_BR_*; the reverse walk adds the table segments in bits 8..23)
+//   iters [1]   index of the last fixed-point iteration
+// keep_codes: the reverse walk writes the codes with the table segments back into KF / KB (for tests that compare the
+// decisions at +-delta; the kernel does not)
+struct TapeRecorder {
+    Strided V0, D, CF, CB, KF, KB, iters;
+    bool keep_codes;
+    VP_HD void initial(int it, int i, double r, double vp, double ay, double vn, const Tables &tb, double scale) const {
+        V0[i] = vn;
+        if (i == 0) iters[0] = it;
+        if (!(r < (double)INFINITY)) {           // kappa == 0: V0 = inf is clipped, nothing flows back
+            D[i] = 0.0;
+            return;
+        }
+        const double dvp = (it == 0) ? vp / (2.0 * r) : (double)D[i];     // it == 0: vp = sqrt(ay_global r)
+        int seg;
+        const double say = interp_slope(vp, tb.gv, tb.gay, tb.n_ggv, scale, &seg);
+        D[i] = (say * dvp * r + ay) / (2.0 * vn);                          // vn = sqrt(ay(vp) r)
+    }
+    VP_HD void fwd(int j, double cur, int code) const { CF[j] = cur; KF[j] = code; }
+    VP_HD void bwd(int j, double cur, int code) const { CB[j] = cur; KB[j] = code; }
+};
+
+// Partial derivatives of ax_poss (no mu) at (vx, radius): da/dvx, da/dradius.  Returns the frozen decisions of the call
+// as a code: VP_BR_CLAMP, VP_BR_MACH, the ggv segment + 1 in bits 8..15 and (accel_forw) the machine segment + 1 in
+// bits 16..23.
+VP_HD int ax_poss_lin(double vx, double radius, bool accel_forw, const Tables &tb, double s, const Params &pr,
+                      double &da_dv, double &da_dr) {
+    int hint = 0, seg_g, seg_m = -1;
+    double ax_t, ay_t;
+    interp2(vx, tb.gv, tb.gax, tb.gay, tb.n_ggv, s, ax_t, ay_t, hint);
+    const double sax = interp_slope(vx, tb.gv, tb.gax, tb.n_ggv, s, &seg_g);
+    const double say = interp_slope(vx, tb.gv, tb.gay, tb.n_ggv, s, &seg_g);
+    const double q = mul(vx, vx) / radius / ay_t;
+    const double dq_dv = (2.0 * vx / radius - q * say) / ay_t, dq_dr = -q / radius;
+    const double p = pr.dyn_model_exp;
+    const bool lin = (p == 1.0);
+    const double radicand = sub(1.0, lin ? q : pow(q, p));
+    int code = 0;
+    double avail = 0.0, dav_dv = 0.0, dav_dr = 0.0;
+    if (radicand > 0.0) {
+        if (lin) {
+            avail = mul(ax_t, radicand);
+            dav_dv = sax * radicand - ax_t * dq_dv;
+            dav_dr = -ax_t * dq_dr;
+        } else {
+            const double rp = pow(radicand, 1.0 / p);
+            avail = mul(ax_t, rp);
+            // d rp = rp / (p radicand) d radicand,  d radicand = -p q^(p - 1) dq
+            const double drp_dq = (q > 0.0) ? -rp / radicand * pow(q, p - 1.0) : 0.0;
+            dav_dv = sax * rp + ax_t * drp_dq * dq_dv;
+            dav_dr = ax_t * drp_dq * dq_dr;
+        }
+    } else {
+        code |= VP_BR_CLAMP;
+    }
+    if (accel_forw) {
+        int hm = 0;
+        const double ax_mach = interp(vx, tb.mv, tb.ma, tb.n_mach, 1.0, hm);
+        const double sm = interp_slope(vx, tb.mv, tb.ma, tb.n_mach, 1.0, &seg_m);
+        if (ax_mach < avail) {
+            code |= VP_BR_MACH;
+            dav_dv = sm;
+            dav_dr = 0.0;
+        }
+    }
+    const double ddrag = 2.0 * vx * pr.drag_coeff / pr.m_veh;        // |d ax_drag / dvx|
+    da_dv = accel_forw ? dav_dv - ddrag : dav_dv + ddrag;
+    da_dr = dav_dr;
+    return code | ((seg_g + 1) & 0xff) << 8 | ((seg_m + 1) & 0xff) << 16;
+}
+
+// Reverse walk of profile_thread<TapeRecorder> (mu == nullptr, so MU is not touched).  Runs the forward again with the
+// recorder, then walks its stages backwards: t / ax, filter, backward pass, forward pass, initial profile, r = |1 / kappa|.
+// Upstream: g_lap (d L / d laptime) and g_vx [n] (d L / d vx, may be null).  Writes g_kappa [n] and g_el [n] (either may
+// be null).  GV, GR, GE: scratch vectors of n entries (adjoints of the speeds, the radii and the lengths).
+// Returns the forward's status, or VP_STATUS_NONFINITE for a non-finite gradient; the gradients are zero unless it is 0.
+VP_HD int profile_adjoint_thread(int n, const double *kappa, const double *el, double scale, double v_max, const Tables &tb,
+                                 const Params &pr, Strided R, Strided EL, Strided V, Strided W, const TapeRecorder &tp,
+                                 Strided GV, Strided GR, Strided GE, double g_lap, const double *g_vx, double *g_kappa,
+                                 double *g_el, double *laptime) {
+    int st = profile_thread(n, kappa, el, nullptr, scale, v_max, tb, pr, R, EL, GR, V, W, nullptr, nullptr, nullptr,
+                            laptime, tp);
+    const bool filt = pr.filt_window > 1;
+    const Strided F = filt ? W : V;
+    if (st == VP_STATUS_OK) {
+        // ---- t / ax: laptime = sum_i 2 e_i / (v_i + v_i+1), the closed form of calc_t_profile's step times --------
+        for (int i = 0; i < n; ++i) {
+            GV[i] = g_vx ? g_vx[i] : 0.0;
+            GR[i] = 0.0;
+            GE[i] = 0.0;
+        }
+        for (int i = 0; i < n; ++i) {
+            const int i1 = (i + 1 < n) ? i + 1 : 0;
+            const double s = F[i] + F[i1];
+            const double dv = -2.0 * EL[i] / (s * s) * g_lap;
+            GV[i] += dv;
+            GV[i1] += dv;
+            GE[i] += 2.0 / s * g_lap;
+        }
+        // ---- the cyclic moving average is symmetric: its transpose is itself ------------------------------------
+        if (filt) {
+            const int h = (pr.filt_window - 1) / 2;
+            const double wgt = 1.0 / (double)pr.filt_window;
+            for (int i = 0; i < n; ++i) W[i] = GV[i];
+            for (int i = 0; i < n; ++i) {
+                double acc = 0.0;
+                for (int k = -h; k <= h; ++k) {
+                    int m = (i + k) % n;
+                    if (m < 0) m += n;
+                    acc += W[m] * wgt;
+                }
+                GV[i] = acc;
+            }
+        }
+        // ---- backward pass, steps in reverse.  GV holds the adjoint of the stored speeds (seeds); a step that stored
+        // consumes its seed on the first visit, every step passes what the initial speed nxt0 receives into GV[i1].
+        {
+            const bool slice_upper = pr.decel_slice_upper != 0;
+            const int j_end = slice_upper ? n - 1 : 2 * n - 1;
+            double gc = 0.0;                                  // adjoint of cur after step j
+            for (int j = j_end - 1; j >= 0; --j) {
+                const int i1 = (j + 1 < n) ? n - 2 - j : 2 * n - 2 - j;
+                const int i0 = (j < n) ? n - 1 - j : 2 * n - 1 - j;
+                const bool stored = slice_upper || j + 1 >= n;
+                const double g = gc + (stored ? (double)GV[i1] : 0.0);
+                int code = (int)tp.KB[j];
+                if ((code & VP_BR_ACTIVE) && (code & VP_BR_TAKEN)) {
+                    const double cur = tp.CB[j], r0 = R[i0], e0 = EL[i0];
+                    Hints hh{0, 0};
+                    double da_dv, da_dr;
+                    code |= ax_poss_lin(cur, r0, false, tb, scale, pr, da_dv, da_dr) & 0xff3f;
+                    const double a = ax_poss(cur, r0, 1.0, false, false, tb, scale, pr, hh);
+                    const double vpn = v_next(cur, a, e0);
+                    double dc = (cur + e0 * da_dv) / vpn, dr0 = e0 * da_dr / vpn, de0 = a / vpn, dr1 = 0.0;
+                    if (code & VP_BR_VTMP) {                     // vtmp = v_next(cur, ax_poss(vpn, r1), e0)
+                        const double r1 = R[i1];
+                        double db_dv, db_dr;
+                        const int c2 = ax_poss_lin(vpn, r1, false, tb, scale, pr, db_dv, db_dr);
+                        code |= ((c2 & VP_BR_CLAMP) ? VP_BR_CLAMP2 : 0) | (c2 & 0xff00) << 8;
+                        const double a2 = ax_poss(vpn, r1, 1.0, false, false, tb, scale, pr, hh);
+                        const double vt = v_next(cur, a2, e0);
+                        dc = (cur + e0 * db_dv * dc) / vt;
+                        dr0 = e0 * db_dv * dr0 / vt;
+                        de0 = (a2 + e0 * db_dv * de0) / vt;
+                        dr1 = e0 * db_dr / vt;
+                        GR[i1] += g * dr1;
+                    }
+                    gc = g * dc;
+                    GR[i0] += g * dr0;
+                    GE[i0] += g * de0;
+                    if (stored) GV[i1] = 0.0;
+                } else {
+                    gc = 0.0;
+                    if (stored) GV[i1] = g; else GV[i1] += g;
+                }
+                if (tp.keep_codes) tp.KB[j] = code;
+            }
+            GV[n - 1] += gc;                                  // cur of step 0 is V[n - 1]
+        }
+        // ---- forward pass, steps in reverse (the same bookkeeping; GV becomes the adjoint of the clipped V0) ------
+        {
+            double gc = 0.0;
+            for (int j = 2 * n - 2; j >= 0; --j) {
+                const int i1 = (j + 1 < n) ? j + 1 : j + 1 - n;
+                const int i0 = (j < n) ? j : j - n;
+                const bool stored = j + 1 >= n;
+                const double g = gc + (stored ? (double)GV[i1] : 0.0);
+                int code = (int)tp.KF[j];
+                if ((code & VP_BR_ACTIVE) && (code & VP_BR_TAKEN)) {
+                    const double cur = tp.CF[j], r = R[i0], e = EL[i0];
+                    Hints hh{0, 0};
+                    double da_dv, da_dr;
+                    code |= ax_poss_lin(cur, r, true, tb, scale, pr, da_dv, da_dr);
+                    const double a = ax_poss(cur, r, 1.0, false, true, tb, scale, pr, hh);
+                    const double vpn = v_next(cur, a, e);
+                    gc = g * (cur + e * da_dv) / vpn;
+                    GR[i0] += g * e * da_dr / vpn;
+                    GE[i0] += g * a / vpn;
+                    if (stored) GV[i1] = 0.0;
+                } else {
+                    gc = 0.0;
+                    if (stored) GV[i1] = g; else GV[i1] += g;
+                }
+                if (tp.keep_codes) tp.KF[j] = code;
+            }
+            GV[0] += gc;                                      // cur of step 0 is the clipped V0[0]
+        }
+        // ---- initial profile (V0 > v_max was clipped: no dependence), then r = |1 / kappa| ------------------------
+        bool finite = true;
+        for (int i = 0; i < n; ++i) {
+            const double k = kappa[i];
+            const double v0 = tp.V0[i];
+            const double gr = GR[i] + ((v0 > v_max) ? 0.0 : GV[i] * tp.D[i]);
+            const double gk = (k != 0.0) ? gr * (k > 0.0 ? -1.0 : 1.0) / (k * k) : 0.0;
+            const double ge = GE[i];
+            if (!(fabs(gk) < (double)INFINITY && fabs(ge) < (double)INFINITY)) finite = false;
+            GR[i] = gk;
+        }
+        if (!finite) st = VP_STATUS_NONFINITE;
+    }
+    for (int i = 0; i < n; ++i) {
+        if (g_kappa) g_kappa[i] = (st == VP_STATUS_OK) ? (double)GR[i] : 0.0;
+        if (g_el) g_el[i] = (st == VP_STATUS_OK) ? (double)GE[i] : 0.0;
+    }
+    return st;
 }
 
 // tph.calc_ax_profile / tph.calc_t_profile on given profiles (stand-alone forms of the two stages above).
