@@ -66,11 +66,6 @@ def _ptr(t: Optional[torch.Tensor]):
     return ctypes.c_void_p(t.data_ptr()) if t is not None else None
 
 
-def _rows_ptr(t: Optional[torch.Tensor], s: int, e: int):
-    """Pointer to rows s:e of t (the instances of one chunked launch); NULL for an absent tensor."""
-    return _ptr(t[s:e]) if t is not None else None
-
-
 def _stream():
     return ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
 
@@ -166,6 +161,24 @@ def _chunk(B: int, per_item_bytes: int, device) -> int:
     return max(1, min(B, budget // max(per_item_bytes, 1)))
 
 
+def _rows(t: Optional[torch.Tensor]):
+    """A per-instance argument of _launch_chunks: rows s:e of t for the chunk of instances s:e (None stays NULL)."""
+    return lambda s, e: None if t is None else t[s:e]
+
+
+def _launch_chunks(entry: str, B: int, chunk: int, ws: torch.Tensor, *args) -> None:
+    """Runs the C-ABI entry on chunks of at most chunk of the B instances, with the chunk's size as B.  args are the
+    entry's arguments between B and the workspace: a callable of (s, e) such as _rows gives the argument of the chunk of
+    instances s:e, a tensor is passed as its pointer, None as NULL and anything else as it is.  The workspace, its size
+    and the stream follow."""
+    fn = getattr(_lib.load(), entry)
+    for s in range(0, B, chunk):
+        e = min(B, s + chunk)
+        chunk_args = [a(s, e) if callable(a) else a for a in args]       # (holds what the callables made until the call)
+        rc = fn(e - s, *(_ptr(a) if isinstance(a, torch.Tensor) else a for a in chunk_args), _ptr(ws), ws.numel(), _stream())
+        _lib.check(rc, entry)
+
+
 def _mincurv_inputs(tracks: dict, shape_error: str, n_pts, w_veh, centre_id, max_chunk, f_scale) -> SimpleNamespace:
     """The checked and normalised inputs of opt_min_curv_batch and opt_min_curv_diff.  tracks: name -> (tensor, cols), every
     tensor [B, n_max, cols] ([B, n_max] for cols None; the first fixes B and n_max).  Returns a namespace of the tracks as
@@ -229,11 +242,10 @@ def shared_centre_ids(group: torch.Tensor) -> torch.Tensor:
     return first[inv].to(torch.int32)
 
 
-def _chunk_centre_ids(centre_id, s, e, B):
-    # owners are addressed inside the chunk: the first instance of the chunk with the same owner takes the role
-    if centre_id is None:
-        return None
-    return centre_id if (s == 0 and e == B) else shared_centre_ids(centre_id[s:e])
+def _chunk_centre_ids(centre_id, B):
+    """centre_id as a per-instance argument of _launch_chunks: owners are addressed inside the chunk, the first instance of
+    the chunk with the same owner takes the role."""
+    return lambda s, e: centre_id if centre_id is None or (s == 0 and e == B) else shared_centre_ids(centre_id[s:e])
 
 
 def _mincurv_launch(entry: str, chunk: int, n_pts, reftrack, normvec, h, kappa_bound, w_scalar, w_batch, f_scale, centre_id,
@@ -241,17 +253,22 @@ def _mincurv_launch(entry: str, chunk: int, n_pts, reftrack, normvec, h, kappa_b
     """Runs the C-ABI entry mc_mincurv_solve_batch_shared, mc_mincurv_solve_batch_sens or mc_mincurv_adjoint_batch on
     chunks of at most chunk instances.  The arguments are the entry's own in its order, outputs the per-instance tensors
     after centre_id; kappa_bound is None for the adjoint, which takes none."""
-    lib = _lib.load()
     B, n_max = h.shape
-    ws = _workspace("mincurv", lib.mc_mincurv_workspace_bytes(chunk, n_max), h.device)
+    ws = _workspace("mincurv", _lib.load().mc_mincurv_workspace_bytes(chunk, n_max), h.device)
     kb = () if kappa_bound is None else (kappa_bound,)
-    for s in range(0, B, chunk):
-        e = min(B, s + chunk)
-        cid = _chunk_centre_ids(centre_id, s, e, B)
-        rc = getattr(lib, entry)(e - s, n_max, _rows_ptr(n_pts, s, e), _ptr(reftrack[s:e]), _ptr(normvec[s:e]), _ptr(h[s:e]),
-                                 *kb, w_scalar, _rows_ptr(w_batch, s, e), f_scale, _ptr(cid),
-                                 *(_ptr(t[s:e]) for t in outputs), _ptr(ws), ws.numel(), _stream())
-        _lib.check(rc, entry)
+    _launch_chunks(entry, B, chunk, ws, n_max, *map(_rows, (n_pts, reftrack, normvec, h)), *kb, w_scalar, _rows(w_batch),
+                   f_scale, _chunk_centre_ids(centre_id, B), *map(_rows, outputs))
+
+
+def _wanted(B: int, *grads, device=None) -> torch.Tensor:
+    """bool [B]: the instances with a nonzero upstream gradient in any of grads (each [B, ...] or None, which counts as
+    zero).  device: where the mask lives when every gradient is None (autograd passes None for an output it has no
+    gradient for when the function does not materialise them)."""
+    wanted = torch.zeros((B,), dtype=torch.bool, device=next((g.device for g in grads if g is not None), device))
+    for g in grads:
+        if g is not None:
+            wanted |= (g != 0).flatten(1).any(dim=1) if g.ndim > 1 else g != 0
+    return wanted
 
 
 def _refuse(strict: bool, wanted: torch.Tensor, gs: torch.Tensor, who: str, what: str) -> None:
@@ -287,7 +304,7 @@ class _MinCurvDiff(torch.autograd.Function):
         B, n_max, _ = centre.shape
         dev = centre.device
         grad_alpha = grad_alpha.to(dtype=torch.float64).contiguous()
-        wanted = (grad_alpha != 0).any(dim=1)
+        wanted = _wanted(B, grad_alpha)
         who = "opt_min_curv_diff: no width gradient"
         _refuse(ctx.strict, wanted, grad_status, who, "with a nonzero upstream gradient")
         gs = grad_status.clone()            # (the adjoint sets 3 where its factorisation breaks down)
@@ -389,7 +406,7 @@ class _ShortestPathDiff(torch.autograd.Function):
         B, n_max, _ = reftrack.shape
         f64 = dict(dtype=torch.float64, device=reftrack.device)
         grad_alpha = grad_alpha.to(dtype=torch.float64).contiguous()
-        wanted = (grad_alpha != 0).any(dim=1)
+        wanted = _wanted(B, grad_alpha)
         who = "opt_shortest_path_diff: no gradient"
         _refuse(ctx.strict, wanted, grad_status, who, "with a nonzero upstream gradient")
         gs = grad_status.clone()            # (the adjoint sets 3 where its solution is not finite)
@@ -523,10 +540,7 @@ class _CreateRacelineDiff(torch.autograd.Function):
         B, n_max = alpha.shape
         f64 = dict(dtype=torch.float64, device=alpha.device)
         g_ri, g_kappa, g_el = (None if g is None else g.to(**f64).contiguous() for g in (g_ri, g_kappa, g_el))
-        wanted = torch.zeros((B,), dtype=torch.bool, device=alpha.device)
-        for g in (g_ri, g_kappa, g_el):
-            if g is not None:
-                wanted |= (g.reshape(B, -1) != 0).any(dim=1)
+        wanted = _wanted(B, g_ri, g_kappa, g_el, device=alpha.device)
         # n_out <= 0: an overflow of an explicit n_out_max (-points needed) or an inactive track: nothing to differentiate
         _refuse(ctx.strict, wanted, (n_out <= 0).to(torch.int32), "create_raceline_diff: no gradient",
                 "with n_out <= 0 (overflow of n_out_max or an inactive track)")
@@ -536,16 +550,8 @@ class _CreateRacelineDiff(torch.autograd.Function):
         g_nv = torch.empty((B, n_max, 2), **f64) if need_nv else None
         chunk = _chunk(B, lib.mc_create_raceline_adjoint_workspace_bytes(1, n_max), alpha.device)
         ws = _workspace("raceline_adjoint", lib.mc_create_raceline_adjoint_workspace_bytes(chunk, n_max), alpha.device)
-        n_out_max = si.shape[1]
-        for s in range(0, B, chunk):
-            e = min(B, s + chunk)
-            rc = lib.mc_create_raceline_adjoint_batch(e - s, n_max, _rows_ptr(n_pts, s, e), _ptr(normvec[s:e]),
-                                                      _ptr(alpha[s:e]), n_out_max, _ptr(cx[s:e]), _ptr(cy[s:e]),
-                                                      _ptr(sl[s:e]), _ptr(n_out[s:e]), _ptr(si[s:e]), _ptr(tv[s:e]),
-                                                      _rows_ptr(g_ri, s, e), _rows_ptr(g_kappa, s, e),
-                                                      _rows_ptr(g_el, s, e), _ptr(g_alpha[s:e]), _rows_ptr(g_ref, s, e),
-                                                      _rows_ptr(g_nv, s, e), _ptr(ws), ws.numel(), _stream())
-            _lib.check(rc, "mc_create_raceline_adjoint_batch")
+        _launch_chunks("mc_create_raceline_adjoint_batch", B, chunk, ws, n_max, *map(_rows, (n_pts, normvec, alpha)),
+                       si.shape[1], *map(_rows, (cx, cy, sl, n_out, si, tv, g_ri, g_kappa, g_el, g_alpha, g_ref, g_nv)))
         if g_ref is not None and ctx.ref_cols != 2:               # the width columns of a reftrack: no influence
             g_ref = torch.cat((g_ref, torch.zeros((B, n_max, ctx.ref_cols - 2), **f64)), dim=2)
         return g_ref, g_nv, g_alpha if ctx.needs_input_grad[2] else None, None, None, None, None
@@ -807,16 +813,11 @@ def vel_profile_batch(kappa: torch.Tensor, el_lengths: torch.Tensor, ggv, ax_max
     chunk = _chunk(B, per_track, dev) if max_chunk is None else min(B, int(max_chunk))
     chunk = max(1, min(chunk, (2 ** 31 - 1024) // V))
     ws = _workspace("velprofile", lib.mc_vel_profile_workspace_bytes(chunk, V, n_max), dev)
-    for s in range(0, B, chunk):
-        e = min(B, s + chunk)
-        rc = lib.mc_vel_profile_batch_ex(e - s, n_max, _rows_ptr(n_pts, s, e), _ptr(kappa[s:e]), _ptr(el_lengths[s:e]),
-                                         _rows_ptr(mu, s, e), V, _ptr(scale_t), _ptr(vmax_t), v_scalar, int(ggv_t.shape[0]),
-                                         _ptr(ggv_t), int(mach_t.shape[0]), _ptr(mach_t), float(dyn_model_exp),
-                                         float(drag_coeff), float(m_veh), fw,
-                                         int(VP_DECEL_SLICE_UPPER if decel_slice_upper is None else decel_slice_upper),
-                                         _rows_ptr(vx, s, e), _rows_ptr(ax, s, e), _rows_ptr(t, s, e), _ptr(laptime[s:e]),
-                                         _ptr(status[s:e]), _ptr(ws), ws.numel(), _stream())
-        _lib.check(rc, "mc_vel_profile_batch_ex")
+    _launch_chunks("mc_vel_profile_batch_ex", B, chunk, ws, n_max, *map(_rows, (n_pts, kappa, el_lengths, mu)), V, scale_t,
+                   vmax_t, v_scalar, int(ggv_t.shape[0]), ggv_t, int(mach_t.shape[0]), mach_t, float(dyn_model_exp),
+                   float(drag_coeff), float(m_veh), fw,
+                   int(VP_DECEL_SLICE_UPPER if decel_slice_upper is None else decel_slice_upper),
+                   *map(_rows, (vx, ax, t, laptime, status)))
     out = dict(laptime=laptime, status=status)
     if want_profiles:
         out.update(vx=vx, ax=ax, t=t)
@@ -850,11 +851,7 @@ class _VelProfileDiff(torch.autograd.Function):
         f64 = dict(dtype=torch.float64, device=kappa.device)
         grad_laptime = None if grad_laptime is None else grad_laptime.to(**f64).contiguous()
         grad_vx = None if grad_vx is None else grad_vx.to(**f64).contiguous()
-        wanted = torch.zeros((B,), dtype=torch.bool, device=kappa.device)
-        if grad_laptime is not None:
-            wanted |= grad_laptime != 0
-        if grad_vx is not None:
-            wanted |= (grad_vx != 0).any(dim=1)
+        wanted = _wanted(B, grad_laptime, grad_vx, device=kappa.device)
         who = "vel_profile_diff: no gradient"
         _refuse(ctx.strict, wanted, grad_status, who, "with a nonzero upstream gradient")
         need_k, need_e = ctx.needs_input_grad[:2]
@@ -863,15 +860,9 @@ class _VelProfileDiff(torch.autograd.Function):
         gs = torch.empty((B,), dtype=torch.int32, device=kappa.device)
         chunk = _chunk(B, lib.mc_vel_profile_adjoint_workspace_bytes(1, n_max), kappa.device)
         ws = _workspace("velprofile_adjoint", lib.mc_vel_profile_adjoint_workspace_bytes(chunk, n_max), kappa.device)
-        for s in range(0, B, chunk):
-            e = min(B, s + chunk)
-            rc = lib.mc_vel_profile_adjoint_batch(e - s, n_max, _rows_ptr(n_pts, s, e), _ptr(kappa[s:e]),
-                                                  _ptr(el_lengths[s:e]), v_max, int(ggv_t.shape[0]), _ptr(ggv_t),
-                                                  int(mach_t.shape[0]), _ptr(mach_t), dyn_model_exp, drag_coeff, m_veh, fw,
-                                                  dsu, _rows_ptr(grad_laptime, s, e), _rows_ptr(grad_vx, s, e),
-                                                  _rows_ptr(gk, s, e), _rows_ptr(ge, s, e), _ptr(gs[s:e]), _ptr(ws),
-                                                  ws.numel(), _stream())
-            _lib.check(rc, "mc_vel_profile_adjoint_batch")
+        _launch_chunks("mc_vel_profile_adjoint_batch", B, chunk, ws, n_max, *map(_rows, (n_pts, kappa, el_lengths)), v_max,
+                       int(ggv_t.shape[0]), ggv_t, int(mach_t.shape[0]), mach_t, dyn_model_exp, drag_coeff, m_veh, fw, dsu,
+                       *map(_rows, (grad_laptime, grad_vx, gk, ge, gs)))
         _refuse(ctx.strict, wanted, gs, who, "whose gradient is not finite")
         return (gk, ge) + (None,) * 10
 

@@ -11,12 +11,9 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(_HERE, "csrc")
 INCLUDE = os.path.join(os.path.dirname(_HERE), "include")
 HEADER = os.path.join(INCLUDE, "mincurv_b200.h")      # the C-ABI; _lib derives its ctypes signatures from it
-SP_SENS_HEADER = os.path.join(CSRC, "shortest_path_sens.h")     # the shortest path's sensitivity entries, bound the same way
-LAP_SENS_HEADER = os.path.join(CSRC, "lap_time_sens.h")         # the lap time's sensitivity entries, bound the same way
 LIB_PATH = os.path.join(_HERE, "libmincurv_b200.so")
 SOURCES = sorted(glob.glob(os.path.join(CSRC, "*.cu")))
-HEADERS = sorted(glob.glob(os.path.join(CSRC, "*.cuh")) + glob.glob(os.path.join(CSRC, "*.h")) +
-                 glob.glob(os.path.join(INCLUDE, "*.h")))
+HEADERS = sorted(glob.glob(os.path.join(CSRC, "*.cuh")) + glob.glob(os.path.join(INCLUDE, "*.h")))
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "-Xcompiler", "-fPIC", "-shared"]
 

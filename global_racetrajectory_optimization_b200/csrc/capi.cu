@@ -7,8 +7,6 @@
 
 #include "../../include/mincurv_b200.h"
 #include "mincurv_ws.cuh"
-#include "shortest_path_sens.h"
-#include "lap_time_sens.h"
 
 namespace mc {
 size_t spline_ws_doubles(int n_max);

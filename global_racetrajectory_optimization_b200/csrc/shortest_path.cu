@@ -202,7 +202,7 @@ int launch_shortest_path(int B, int n_max, const int32_t *n_pts, const double *r
     return 0;
 }
 
-// ---- sensitivities (csrc/shortest_path_sens.h, DESIGN.md section 3.11) ----
+// ---- sensitivities (include/mincurv_b200.h, DESIGN.md section 3.11) ----
 // Run right after shortest_path_kernel on the same workspace: the final iterate's lu / su and ll / sl, the diagonal D of
 // M = H + D that the backward pass factorises, and grad_status = status.
 __global__ void __launch_bounds__(128)

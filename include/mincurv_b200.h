@@ -196,6 +196,42 @@ int mc_shortest_path_solve_batch(int B, int n_max, const int32_t *n_pts,
                                  double *alpha, int32_t *status, int32_t *iters,
                                  void *workspace, size_t workspace_bytes, void *stream);
 
+/* Sensitivities of this QP (batch.opt_shortest_path_diff; DESIGN.md section 3.11 has the derivation).  H and f are
+ * explicit in the centre line and the normals, so alpha is differentiated with respect to all of them: x, y, w_tr_right,
+ * w_tr_left, the normal vectors and w_veh.  grad_status[b] (int32):
+ *   0  the solve converged (status 0): gradients are computed
+ *   2, 3, -1  the solve's status (iteration cap, breakdown, unsupported size)
+ *   3  also: a non-finite adjoint solution
+ * Every unsupported instance gets zero gradients.  A bound clamped to 0.001 m (tph's clamp of w - w_veh / 2) does not
+ * move with the widths: its width gradients are zero.
+ *
+ * mc_shortest_path_solve_batch_sens: mc_shortest_path_solve_batch (same arguments, bit-identical alpha, status, iters)
+ * that also exports what the backward pass needs, 16 bytes per point:
+ *   sens        [B][2][n_max] : lu / su and ll / sl, the final multiplier-to-slack ratios of the upper and lower bounds
+ *                               (zero beyond n_pts[b] and for grad_status != 0)
+ *   grad_status [B]           : see above
+ *
+ * mc_shortest_path_adjoint_batch: vector-Jacobian product of alpha: for an upstream gradient grad_alpha [B][n_max] of a
+ * loss L,
+ *   grad_reftrack [B][n_max][4]        = dL / d(x, y, w_tr_right, w_tr_left)   (x, y at fixed normals)
+ *   grad_normvec  [B][n_max][2] or NULL = dL / dnormvec
+ *   grad_w_veh    [B] or NULL           = dL / dw_veh per instance (the scalar w_veh's gradient is their sum)
+ * reftrack, normvec, w_veh / w_veh_batch, alpha, sens and grad_status are those of the mc_shortest_path_solve_batch_sens
+ * call.  One cyclic tridiagonal factorisation of H + diag(sens[0] + sens[1]) and one solve per instance in a workspace of
+ * mc_shortest_path_workspace_bytes(B, n_max); nothing has to survive in it between the two calls.  grad_status is read,
+ * and set to 3 where the adjoint solution is not finite. */
+int mc_shortest_path_solve_batch_sens(int B, int n_max, const int32_t *n_pts,
+                                      const double *reftrack, const double *normvec,
+                                      double w_veh, const double *w_veh_batch,
+                                      double *alpha, int32_t *status, int32_t *iters, double *sens, int32_t *grad_status,
+                                      void *workspace, size_t workspace_bytes, void *stream);
+int mc_shortest_path_adjoint_batch(int B, int n_max, const int32_t *n_pts,
+                                   const double *reftrack, const double *normvec,
+                                   double w_veh, const double *w_veh_batch,
+                                   const double *alpha, const double *sens, int32_t *grad_status, const double *grad_alpha,
+                                   double *grad_reftrack, double *grad_normvec, double *grad_w_veh,
+                                   void *workspace, size_t workspace_bytes, void *stream);
+
 /* -------------------------------------------------------------------------------------------------
  * tph.create_raceline.create_raceline(refline, normvectors, alpha, stepsize_interp)
  * -- call site main_globaltraj.py:371-376 (9-tuple; the dense A_raceline is replaced
@@ -216,6 +252,27 @@ int mc_create_raceline_batch(int B, int n_max, const int32_t *n_pts,
                              int32_t *n_out, double *raceline_interp, int32_t *spline_inds, double *t_values,
                              double *s_interp, double *el_lengths_interp, double *psi, double *kappa,
                              void *workspace, size_t workspace_bytes, void *stream);
+
+/* Sensitivities of create_raceline (batch.create_raceline_diff; DESIGN.md section 3.12 has the derivation).
+ *
+ * mc_create_raceline_adjoint_workspace_bytes: 25 (n_max rounded up to 32, + 32) doubles per track.
+ *
+ * mc_create_raceline_adjoint_batch: vector-Jacobian product of mc_create_raceline_batch (unit parameter scales, the
+ * raceline refline + alpha normvec): for upstream gradients grad_raceline [B][n_out_max][2], grad_kappa [B][n_out_max]
+ * and grad_el_lengths [B][n_out_max] (each may be NULL: zero) of a loss L,
+ *   grad_alpha   [B][n_max]          = dL / dalpha
+ *   grad_refline [B][n_max][2] or NULL = dL / d(x, y) of the reference line
+ *   grad_normvec [B][n_max][2] or NULL = dL / dnormvec
+ * all zero beyond n_pts[b], and zero for a track with n_out[b] <= 0 (overflow or inactive) or n_pts[b] < 3.  n_out and the
+ * segment of every station are held: coeffs_x / coeffs_y, spline_lengths, n_out, spline_inds and t_values are the
+ * forward call's outputs (n_out_max its capacity); normvec and alpha its inputs. */
+size_t mc_create_raceline_adjoint_workspace_bytes(int B, int n_max);
+int mc_create_raceline_adjoint_batch(int B, int n_max, const int32_t *n_pts, const double *normvec, const double *alpha,
+                                     int n_out_max, const double *coeffs_x, const double *coeffs_y,
+                                     const double *spline_lengths, const int32_t *n_out, const int32_t *spline_inds,
+                                     const double *t_values, const double *grad_raceline, const double *grad_kappa,
+                                     const double *grad_el_lengths, double *grad_alpha, double *grad_refline,
+                                     double *grad_normvec, void *workspace, size_t workspace_bytes, void *stream);
 
 /* tph.calc_head_curv_an.calc_head_curv_an stand-alone (any (spline index, t) pairs), call site
  * main_globaltraj.py:383-387.  dkappa may be NULL (calc_dcurv=False). */
@@ -274,6 +331,32 @@ int mc_vel_profile_batch_ex(int B, int n_max, const int32_t *n_pts, const double
                             double dyn_model_exp, double drag_coeff, double m_veh, int filt_window, int decel_slice_upper,
                             double *vx, double *ax, double *t, double *laptime, int32_t *status,
                             void *workspace, size_t workspace_bytes, void *stream);
+
+/* Sensitivities of the lap time (batch.vel_profile_diff; DESIGN.md section 3.12 has the derivation).  The velocity
+ * profile (closed track, ggv branch, one profile per track, no mu) is differentiated with respect to kappa and el_lengths
+ * as the forward evaluates it, with every discrete decision frozen as the forward took it.  grad_status[b] (int32):
+ *   0  the gradient is computed
+ *   3  non-finite lap time (the forward's status) or a non-finite gradient
+ *   for n_pts[b] < 2 (an inactive slot) the forward's status (0 for n_pts 0, 3 otherwise)
+ * Every such instance gets zero gradients.
+ *
+ * mc_vel_profile_adjoint_workspace_bytes: 17 n_max + 1 doubles per track (the forward's scratch vectors, its tape and
+ * the adjoint vectors).
+ *
+ * mc_vel_profile_adjoint_batch: vector-Jacobian product of mc_vel_profile_batch_ex with V = 1 (no ggv scales, no
+ * per-variant top speed, no mu): for upstream gradients grad_laptime [B] and grad_vx [B][n_max] (either may be NULL:
+ * zero) of a loss L,
+ *   grad_kappa      [B][n_max] or NULL = dL / dkappa
+ *   grad_el_lengths [B][n_max] or NULL = dL / del_lengths
+ * both zero beyond n_pts[b].  The other arguments are those of the forward call; the forward is run again inside (its
+ * outputs are not inputs here). */
+size_t mc_vel_profile_adjoint_workspace_bytes(int B, int n_max);
+int mc_vel_profile_adjoint_batch(int B, int n_max, const int32_t *n_pts, const double *kappa, const double *el_lengths,
+                                 double v_max, int n_ggv, const double *ggv, int n_mach, const double *ax_max_machines,
+                                 double dyn_model_exp, double drag_coeff, double m_veh, int filt_window,
+                                 int decel_slice_upper, const double *grad_laptime, const double *grad_vx,
+                                 double *grad_kappa, double *grad_el_lengths, int32_t *grad_status,
+                                 void *workspace, size_t workspace_bytes, void *stream);
 
 /* tph.calc_ax_profile.calc_ax_profile(vx_profile, el_lengths, eq_length_output=False) and
  * tph.calc_t_profile.calc_t_profile(vx_profile, el_lengths, t_start, ax_profile) stand-alone

@@ -26,7 +26,14 @@ def test_every_wrapper_matches_the_signature_table(fake):
     assert widths.grad.shape == (B, n, 2)
     alpha = torch.zeros((B, n), dtype=torch.float64)      # (the stand-in library writes nothing: outputs are uninitialised)
     B_.opt_shortest_path_batch(rt, nv, 2.0, n_pts=npts)
+    rt_g = rt.clone().requires_grad_()
+    B_.opt_shortest_path_diff(rt_g, nv, 2.0, n_pts=npts)["alpha"].sum().backward()
+    assert rt_g.grad.shape == (B, n, 4)
     rl = B_.create_raceline_batch(rt, nv, alpha, 2.0, n_pts=npts)
+    alpha_g = alpha.clone().requires_grad_()
+    # (the stand-in writes nothing: n_out stays 0, so only strict=False lets the gradient through -- as zeros)
+    B_.create_raceline_diff(rt, nv, alpha_g, 2.0, n_pts=npts, n_out_max=300, strict=False)["kappa"].sum().backward()
+    assert alpha_g.grad.shape == (B, n)
     B_.calc_head_curv_batch(rl["coeffs_x"], rl["coeffs_y"], rl["spline_inds"], rl["t_values"], n_eval=rl["n_out"])
     B_.iqp_relinearise_batch(rt, nv, alpha, 3.0, n_pts=npts)
     B_.scale_alpha_batch(alpha, 0.5)
@@ -39,6 +46,9 @@ def test_every_wrapper_matches_the_signature_table(fake):
     assert ltm.shape == (B, 3, 2)
     last = [c for c in fake.calls if c[0] == "mc_vel_profile_batch_ex"][-1][1]
     assert last[6] == 6                                                              # V = 3 top speeds x 2 ggv scales
+    kap_g = kap.clone().requires_grad_()
+    B_.vel_profile_diff(kap_g, el, ggv, mach, 70.0, 0.75, 1200.0)["laptime"].sum().backward()
+    assert kap_g.grad.shape == (B, 200)
     B_.calc_ax_t_profile_batch(torch.rand((B, 201), dtype=torch.float64), el)
     out, n_out = B_.interp_track_batch(rt, 1.0, n_pts=npts)
     assert out.shape[0] == B and out.shape[2] == 4

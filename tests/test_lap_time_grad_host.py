@@ -11,9 +11,8 @@ import numpy as np
 import pytest
 import torch
 
-import fake_lib
 from fake_lib import fake  # noqa: F401  (the fixture)
-from global_racetrajectory_optimization_b200 import _lib, batch as B_, build
+from global_racetrajectory_optimization_b200 import _lib, batch as B_
 from vp_adj_ref import Harness
 
 # (relative perturbation of every kappa / el, bound on |central difference - adjoint| / |directional derivative|): the
@@ -154,13 +153,12 @@ def test_host_adjoint_is_linear_in_the_upstream_gradient_and_independent_of_the_
 # ------------------------------------------------------------------------------------------------
 def test_lap_time_entries_are_exported_and_bound():
     lib = _lib.load()
-    assert set(_lib.LAP_SENS_SYMBOLS) == {"mc_vel_profile_adjoint_workspace_bytes", "mc_vel_profile_adjoint_batch",
-                                          "mc_create_raceline_adjoint_workspace_bytes", "mc_create_raceline_adjoint_batch"}
-    assert not set(_lib.LAP_SENS_SYMBOLS) & set(_lib._SIGS)
-    assert build.LAP_SENS_HEADER in build.HEADERS
-    for name, (res, args) in _lib.LAP_SENS_SIGS.items():
+    assert {"mc_vel_profile_adjoint_workspace_bytes", "mc_vel_profile_adjoint_batch",
+            "mc_create_raceline_adjoint_workspace_bytes", "mc_create_raceline_adjoint_batch"} <= set(_lib.EXPORTED_SYMBOLS)
+    assert set(_lib._SIGS) == set(_lib.EXPORTED_SYMBOLS)
+    for name, (res, args) in _lib._SIGS.items():
         fn = getattr(lib, name)
-        assert fn.restype == res and list(fn.argtypes) == args
+        assert fn.restype == res and list(fn.argtypes) == args, name
 
 
 def test_vel_profile_adjoint_validates_its_arguments_without_gpu():
@@ -183,29 +181,7 @@ def test_vel_profile_adjoint_validates_its_arguments_without_gpu():
 
 
 # ------------------------------------------------------------------------------------------------
-class LapFakeLib(fake_lib.FakeLib):
-    """The recording stand-in, knowing the lap-time entries as well."""
-
-    def __getattr__(self, name):
-        if name in _lib.LAP_SENS_SIGS:
-            _, args = _lib.LAP_SENS_SIGS[name]
-
-            def fn(*a):
-                assert len(a) == len(args), f"{name}: {len(a)} arguments passed, {len(args)} declared"
-                self.calls.append((name, a))
-                return 4096 if name.endswith("_workspace_bytes") else 0
-            return fn
-        return super().__getattr__(name)
-
-
-@pytest.fixture()
-def lapfake(fake, monkeypatch):
-    lib = LapFakeLib()
-    monkeypatch.setattr(_lib, "load", lambda build_if_missing=True: lib)
-    return lib
-
-
-def test_vel_profile_diff_calls_forward_and_adjoint_with_their_declared_arity(lapfake):
+def test_vel_profile_diff_calls_forward_and_adjoint_with_their_declared_arity(fake):
     B, n = 5, 200
     ggv = np.array([[0.0, 12.0, 12.0], [80.0, 12.0, 12.0]])
     mach = np.array([[0.0, 5.0], [80.0, 5.0]])
@@ -217,27 +193,27 @@ def test_vel_profile_diff_calls_forward_and_adjoint_with_their_declared_arity(la
     assert res["laptime"].shape == (B,) and res["vx"].shape == (B, n) and res["t"].shape == (B, n + 1)
     assert res["laptime"].requires_grad and res["vx"].requires_grad
     assert not res["ax"].requires_grad and not res["status"].requires_grad and not res["grad_status"].requires_grad
-    fwd = [a for name, a in lapfake.calls if name == "mc_vel_profile_batch_ex"]
+    fwd = [a for name, a in fake.calls if name == "mc_vel_profile_batch_ex"]
     assert len(fwd) == 3 and fwd[0][6] == 1                           # V = 1, chunks of 2
     res["laptime"].sum().backward()
     assert kap.grad.shape == (B, n) and el.grad.shape == (B, n)
-    bwd = [a for name, a in lapfake.calls if name == "mc_vel_profile_adjoint_batch"]
+    bwd = [a for name, a in fake.calls if name == "mc_vel_profile_adjoint_batch"]
     assert [a[0] for a in bwd] == [2, 2, 1]                           # chunked like the forward
     a = bwd[0]
     assert a[5] == 70.0 and a[13] == 5 and a[14] == 0                 # v_max, filt_window, decel_slice_upper
     assert a[15] is not None and a[16] is None                        # grad_laptime only: vx received no gradient
     assert a[17] is not None and a[18] is not None
     # a constant el_lengths: its gradient is not asked for
-    lapfake.calls.clear()
+    fake.calls.clear()
     k2 = kap.detach().clone().requires_grad_()
     r2 = B_.vel_profile_diff(k2, el.detach(), ggv, mach, 70.0, 0.75, 1200.0, n_pts=npts)
     (r2["vx"] * 2.0).sum().backward()
-    a = [a for name, a in lapfake.calls if name == "mc_vel_profile_adjoint_batch"][0]
+    a = [a for name, a in fake.calls if name == "mc_vel_profile_adjoint_batch"][0]
     assert a[15] is None and a[16] is not None and a[17] is not None and a[18] is None and a[13] == 0
     assert k2.grad.shape == (B, n)
 
 
-def test_vel_profile_diff_checks_its_arguments(lapfake):
+def test_vel_profile_diff_checks_its_arguments(fake):
     kap, el = torch.zeros((2, 50), dtype=torch.float64), torch.ones((2, 50), dtype=torch.float64)
     ggv = np.array([[0.0, 12.0, 12.0], [80.0, 12.0, 12.0]])
     mach = np.array([[0.0, 5.0], [80.0, 5.0]])
@@ -251,7 +227,7 @@ def test_vel_profile_diff_checks_its_arguments(lapfake):
         B_.vel_profile_diff(kap, el, ggv[:, :2], mach, 70.0, 0.75, 1200.0)
 
 
-def test_create_raceline_diff_calls_forward_and_adjoint_with_their_declared_arity(lapfake):
+def test_create_raceline_diff_calls_forward_and_adjoint_with_their_declared_arity(fake):
     B, n = 5, 120
     rt = (torch.rand((B, n, 4), dtype=torch.float64) + 3.0).requires_grad_()
     nv = torch.rand((B, n, 2), dtype=torch.float64).requires_grad_()
@@ -265,18 +241,18 @@ def test_create_raceline_diff_calls_forward_and_adjoint_with_their_declared_arit
     # (the stand-in writes nothing: n_out stays 0, so only strict=False lets the gradient through -- as zeros)
     with pytest.raises(_lib.MinCurvLibError, match="n_out <= 0"):
         rl["kappa"].sum().backward()
-    lapfake.calls.clear()
+    fake.calls.clear()
     rl = B_.create_raceline_diff(rt, nv, al, 2.0, n_pts=npts, n_out_max=300, strict=False)
     (rl["kappa"].sum() + rl["el_lengths_interp"].sum()).backward()
     assert rt.grad.shape == (B, n, 4) and not rt.grad[:, :, 2:].any() and nv.grad.shape == (B, n, 2) and al.grad.shape == (B, n)
-    bwd = [a for name, a in lapfake.calls if name == "mc_create_raceline_adjoint_batch"]
+    bwd = [a for name, a in fake.calls if name == "mc_create_raceline_adjoint_batch"]
     assert [a[0] for a in bwd] == [2, 2, 1] and bwd[0][5] == 300                # chunks of 2, n_out_max
     assert bwd[0][12] is None and bwd[0][13] is not None and bwd[0][14] is not None   # no raceline gradient
     assert all(x is not None for x in bwd[0][15:18])
-    lapfake.calls.clear()
+    fake.calls.clear()
     al2 = al.detach().clone().requires_grad_()
     B_.create_raceline_diff(rt.detach(), nv.detach(), al2, 2.0, n_out_max=300, strict=False)["raceline_interp"].sum().backward()
-    a = [a for name, a in lapfake.calls if name == "mc_create_raceline_adjoint_batch"][0]
+    a = [a for name, a in fake.calls if name == "mc_create_raceline_adjoint_batch"][0]
     assert a[12] is not None and a[16] is None and a[17] is None and al2.grad.shape == (B, n)
 
 

@@ -3,6 +3,9 @@ central finite differences of the oracle's own Goldfarb-Idnani solves, the argum
 without a GPU, and the host logic of batch.opt_shortest_path_diff against the recording stand-in of the library
 (fake_lib.py)."""
 import ctypes
+import glob
+import os
+import re
 
 import numpy as np
 import pytest
@@ -114,8 +117,9 @@ def test_opt_shortest_path_diff_calls_both_entries_with_their_declared_arity(fak
     (res["alpha"] * 2.0).sum().backward()
     assert rt.grad.shape == (B, n, 4) and nv.grad.shape == (B, n, 2) and wv.grad.shape == (B,)
     calls = {name: a for name, a in fake.calls}
-    assert set(_lib.SP_SENS_SYMBOLS) == {"mc_shortest_path_solve_batch_sens", "mc_shortest_path_adjoint_batch"}
-    assert set(_lib.SP_SENS_SYMBOLS) <= set(calls)
+    sens_entries = {"mc_shortest_path_solve_batch_sens", "mc_shortest_path_adjoint_batch"}
+    assert sens_entries <= set(_lib.EXPORTED_SYMBOLS)
+    assert sens_entries <= set(calls)
     fwd, bwd = calls["mc_shortest_path_solve_batch_sens"], calls["mc_shortest_path_adjoint_batch"]
     assert fwd[0] == bwd[0] == B                                       # one unchunked call each way
     assert bwd[12] is not None and bwd[13] is not None                 # grad_normvec, grad_w_veh
@@ -135,8 +139,12 @@ def test_opt_shortest_path_diff_calls_both_entries_with_their_declared_arity(fak
 
 
 def test_the_public_header_keeps_its_symbol_set():
-    public = _lib.header_signatures(build.HEADER)
-    assert _lib.EXPORTED_SYMBOLS == tuple(public)
-    assert not set(_lib.SP_SENS_SYMBOLS) & set(public)
-    assert _lib._SIGS == {**public, **_lib.header_signatures(build.SP_SENS_HEADER)}
-    assert build.SP_SENS_HEADER in build.HEADERS
+    """Every entry point capi.cu defines is declared in the public header (the table load() binds), and no header of the
+    kernels declares one."""
+    block = _lib._c_source(os.path.join(build.CSRC, "capi.cu")).split('extern "C" {', 1)[1]
+    defined = re.findall(r"^\w[\w \t*]*?\b(mc_\w+)\s*\([^)]*\)\s*\{", block, flags=re.M)
+    assert sorted(defined) == sorted(_lib.EXPORTED_SYMBOLS)
+    kernel_headers = glob.glob(os.path.join(build.CSRC, "*.h")) + glob.glob(os.path.join(build.CSRC, "*.cuh"))
+    assert kernel_headers
+    for path in kernel_headers:
+        assert not re.findall(r"\bmc_\w+\s*\(", _lib._c_source(path)), path
