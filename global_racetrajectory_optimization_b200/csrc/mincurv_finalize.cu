@@ -2,6 +2,7 @@
 // main_globaltraj.py:264-271): the linearised curvature k_ref + E alpha (checked
 // against kappa_bound) and the linearisation error curv_error_max, both through the O(N) operator
 // form E a = S_y Z (n_y a) - S_x Z (n_x a) (one periodic tridiagonal solve with two right-hand sides).
+#include "capi.cuh"
 #include "mincurv_ws.cuh"
 
 namespace mc {
@@ -86,16 +87,83 @@ mincurv_sens_export_kernel(int n_max, const int32_t *__restrict__ n_pts, double 
     if (threadIdx.x == 0) grad_status[b] = st;
 }
 
-void launch_mincurv_sens_export(int B, int n_max, const int32_t *n_pts, double *ws, const Layout &L, const int32_t *status,
-                                double *sens, int32_t *grad_status, cudaStream_t stream) {
-    mincurv_sens_export_kernel<<<B, 256, 0, stream>>>(n_max, n_pts, ws, L, status, sens, grad_status);
-}
-
-void launch_mincurv_finalize(int B, int n_max, const int32_t *n_pts, double *ws, const Layout &L, const double *alpha,
-                             double kappa_bound, double *curv_error_max, double *kappa_lin_max, int32_t *status,
-                             cudaStream_t stream) {
-    mincurv_finalize_kernel<<<B, 256, 0, stream>>>(n_max, n_pts, ws, L, alpha, kappa_bound, curv_error_max,
-                                                    kappa_lin_max, status);
-}
-
 }  // namespace mc
+
+extern "C" {
+
+int mc_mincurv_finalize_batch(int B, int n_max, const int32_t *n_pts, const double *alpha, double kappa_bound,
+                              double *curv_error_max, double *kappa_lin_max, int32_t *status, void *workspace,
+                              size_t workspace_bytes, void *stream) {
+    if (!alpha || !curv_error_max || !status) return bad("mc_mincurv_finalize_batch: NULL argument");
+    int rc = mc::mincurv_args("mc_mincurv_finalize_batch", B, n_max, workspace, workspace_bytes);
+    if (rc) return rc;
+    mc::mincurv_finalize_kernel<<<B, 256, 0, (cudaStream_t)stream>>>(n_max, n_pts, (double *)workspace, mc::make_layout(n_max),
+                                                                     alpha, kappa_bound, curv_error_max, kappa_lin_max, status);
+    return check_cuda("mincurv_finalize_kernel");
+}
+
+int mc_mincurv_solve_batch(int B, int n_max, const int32_t *n_pts, const double *reftrack, const double *normvec,
+                           const double *h, double kappa_bound, double w_veh, const double *w_veh_batch, double *alpha,
+                           double *curv_error_max, double *kappa_lin_max, int32_t *status, int32_t *iters,
+                           void *workspace, size_t workspace_bytes, void *stream) {
+    return mc_mincurv_solve_batch_ex(B, n_max, n_pts, reftrack, normvec, h, kappa_bound, w_veh, w_veh_batch, MC_F_SCALE_DEFAULT,
+                                     alpha, curv_error_max, kappa_lin_max, status, iters, workspace, workspace_bytes, stream);
+}
+
+int mc_mincurv_solve_batch_ex(int B, int n_max, const int32_t *n_pts, const double *reftrack, const double *normvec,
+                              const double *h, double kappa_bound, double w_veh, const double *w_veh_batch, double f_scale,
+                              double *alpha, double *curv_error_max, double *kappa_lin_max, int32_t *status, int32_t *iters,
+                              void *workspace, size_t workspace_bytes, void *stream) {
+    return mc_mincurv_solve_batch_shared(B, n_max, n_pts, reftrack, normvec, h, kappa_bound, w_veh, w_veh_batch, f_scale, nullptr,
+                                         alpha, curv_error_max, kappa_lin_max, status, iters, workspace, workspace_bytes, stream);
+}
+
+// setup -> pdip -> finalize -> (export of the sensitivity data) -> kappa -> finalize; sens == NULL: no export.  Every
+// argument is checked before the first launch: the pointers here, f_scale and the sizes by the setup stage.
+static int mincurv_solve(int B, int n_max, const int32_t *n_pts, const double *reftrack, const double *normvec, const double *h,
+                         double kappa_bound, double w_veh, const double *w_veh_batch, double f_scale, const int32_t *centre_id,
+                         double *alpha, double *curv_error_max, double *kappa_lin_max, int32_t *status, int32_t *iters,
+                         double *sens, int32_t *grad_status, void *workspace, size_t workspace_bytes, void *stream) {
+    if (!reftrack || !normvec || !h || !alpha || !curv_error_max || !status)
+        return bad("mc_mincurv_solve_batch: NULL argument");
+    int rc = mc_mincurv_setup_batch_shared(B, n_max, n_pts, reftrack, normvec, h, w_veh, w_veh_batch, f_scale, centre_id, status,
+                                           workspace, workspace_bytes, stream);
+    if (rc) return rc;
+    rc = mc_mincurv_pdip_batch(B, n_max, n_pts, alpha, status, iters, workspace, workspace_bytes, stream);
+    if (rc) return rc;
+    rc = mc_mincurv_finalize_batch(B, n_max, n_pts, alpha, kappa_bound, curv_error_max, kappa_lin_max, status, workspace,
+                                   workspace_bytes, stream);
+    if (rc) return rc;
+    if (sens) {
+        // the box phase's final iterate, before the curvature-row phase takes over the status-4 slabs
+        mc::mincurv_sens_export_kernel<<<B, 256, 0, (cudaStream_t)stream>>>(n_max, n_pts, (double *)workspace,
+                                                                            mc::make_layout(n_max), status, sens, grad_status);
+        rc = check_cuda("mincurv_sens_export_kernel");
+        if (rc) return rc;
+    }
+    // instances whose box-only optimum violates the curvature rows (status 4) are re-solved with the rows
+    rc = mc_mincurv_kappa_batch(B, n_max, n_pts, kappa_bound, alpha, status, iters, workspace, workspace_bytes, stream);
+    if (rc) return rc;
+    return mc_mincurv_finalize_batch(B, n_max, n_pts, alpha, kappa_bound, curv_error_max, kappa_lin_max, status, workspace,
+                                     workspace_bytes, stream);
+}
+
+int mc_mincurv_solve_batch_shared(int B, int n_max, const int32_t *n_pts, const double *reftrack, const double *normvec,
+                                  const double *h, double kappa_bound, double w_veh, const double *w_veh_batch, double f_scale,
+                                  const int32_t *centre_id, double *alpha, double *curv_error_max, double *kappa_lin_max,
+                                  int32_t *status, int32_t *iters, void *workspace, size_t workspace_bytes, void *stream) {
+    return mincurv_solve(B, n_max, n_pts, reftrack, normvec, h, kappa_bound, w_veh, w_veh_batch, f_scale, centre_id, alpha,
+                         curv_error_max, kappa_lin_max, status, iters, nullptr, nullptr, workspace, workspace_bytes, stream);
+}
+
+int mc_mincurv_solve_batch_sens(int B, int n_max, const int32_t *n_pts, const double *reftrack, const double *normvec,
+                                const double *h, double kappa_bound, double w_veh, const double *w_veh_batch, double f_scale,
+                                const int32_t *centre_id, double *alpha, double *curv_error_max, double *kappa_lin_max,
+                                int32_t *status, int32_t *iters, double *sens, int32_t *grad_status, void *workspace,
+                                size_t workspace_bytes, void *stream) {
+    if (!sens || !grad_status) return bad("mc_mincurv_solve_batch_sens: NULL argument");
+    return mincurv_solve(B, n_max, n_pts, reftrack, normvec, h, kappa_bound, w_veh, w_veh_batch, f_scale, centre_id, alpha,
+                         curv_error_max, kappa_lin_max, status, iters, sens, grad_status, workspace, workspace_bytes, stream);
+}
+
+}  // extern "C"

@@ -26,6 +26,7 @@
 // three times (the predictor's forward sweep is fused into the factorisation).
 #include <cstdio>
 #include <cstdlib>
+#include "capi.cuh"
 #include "mincurv_ops.cuh"
 
 namespace mc {
@@ -1351,36 +1352,27 @@ mincurv_pdip_kernel(int B, int n_max, const int32_t *__restrict__ n_pts, double 
     }
 }
 
-int debug_read_profile(unsigned long long *host_out, int reset) {
-#ifdef MC_PROFILE
-    if (cudaMemcpyFromSymbol(host_out, g_prof, sizeof(unsigned long long) * PROF_SLOTS) != cudaSuccess) return -1;
-    if (getenv("MC_PROFILE_SEGMENTS")) {       // tools/prof_run.py: sub-phase counters of one panel
-        unsigned long long seg[32];
-        if (cudaMemcpyFromSymbol(seg, g_seg, sizeof(seg)) == cudaSuccess) {
-            fprintf(stderr, "segments:");
-            for (int i = 0; i < 32; ++i) fprintf(stderr, " %d:%llu", i, seg[i]);
-            fprintf(stderr, "\n");
-        }
-    }
-    if (reset) {
-        unsigned long long z[32] = {0};
-        if (cudaMemcpyToSymbol(g_prof, z, sizeof(unsigned long long) * PROF_SLOTS) != cudaSuccess) return -1;
-        cudaMemcpyToSymbol(g_seg, z, sizeof(z));
-    }
-    return 0;
-#else
-    (void)reset;
-    for (int i = 0; i < PROF_SLOTS; ++i) host_out[i] = 0ull;
-    return 0;
-#endif
-}
-
 // resident CTAs per SM of a solver kernel on the current device (registers and shared memory both count)
 template <typename K>
 static int ctas_per_sm(K kernel) {
     int nb = 0;
     if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, kernel, IP_THREADS, sizeof(IpShared)) != cudaSuccess) return 1;
     return nb > 0 ? nb : 1;
+}
+
+// launch shape of a persistent solver kernel: per_sm resident CTAs on every SM, but no more CTAs than instances; the counter
+// that hands out the instances sits behind the slabs
+struct SolverGrid {
+    int grid;
+    int *counter;
+};
+static SolverGrid solver_grid(int B, int n_max, void *workspace, int per_sm) {
+    int dev = 0, sms = 132;
+    cudaGetDevice(&dev);
+    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+    int grid = sms * (per_sm > 0 ? per_sm : 1);
+    if (grid > B) grid = B;
+    return {grid, (int *)((char *)workspace + mincurv_slabs_bytes(B, n_max))};
 }
 
 // launches a solver kernel (CTA state in dynamic shared memory); its work counter, if it has one, starts from zero
@@ -1392,18 +1384,6 @@ static int launch_solver(void (*kernel)(P...), int grid, int *work_counter, cuda
     if (work_counter) cudaMemsetAsync(work_counter, 0, sizeof(int), stream);
     kernel<<<grid, IP_THREADS, sizeof(IpShared), stream>>>(args...);
     return 0;
-}
-
-int pdip_ctas_per_sm() { return ctas_per_sm(mincurv_pdip_kernel); }
-
-// slice > 0 and more instances than CTAs: the sliced schedule (one launch, no grid-wide wait: the CTAs need not all be resident)
-int launch_mincurv_pdip(int B, int n_max, const int32_t *n_pts, double *ws, const Layout &L, const PdipParams &prm, int slice,
-                        double *alpha, int32_t *status, int32_t *iters, int grid, int *sched, cudaStream_t stream) {
-    if (B <= grid) slice = 0;
-    cudaMemsetAsync(sched, 0, SCHED_INTS * sizeof(int), stream);
-    if (slice > 0)      // the PARK_LIST entries of every slab
-        cudaMemset2DAsync(ws + (size_t)V_PARK * L.np + PARK_LIST, L.stride * sizeof(double), 0, PARK_BUCKETS * sizeof(int), B, stream);
-    return launch_solver(mincurv_pdip_kernel, grid, nullptr, stream, B, n_max, n_pts, ws, L, prm, slice, alpha, status, iters, sched);
 }
 
 // ================================================================================================
@@ -1580,15 +1560,6 @@ mincurv_pdip_kappa_kernel(int B, int n_max, const int32_t *__restrict__ n_pts, d
     }
 }
 
-int launch_mincurv_pdip_kappa(int B, int n_max, const int32_t *n_pts, double *ws, const Layout &L, const PdipParams &prm,
-                              double kappa_bound, double *alpha, int32_t *status, int32_t *iters, int grid, int *work_counter,
-                              cudaStream_t stream) {
-    return launch_solver(mincurv_pdip_kappa_kernel, grid, work_counter, stream, B, n_max, n_pts, ws, L, prm, kappa_bound, alpha, status,
-                         iters, work_counter);
-}
-
-int pdip_kappa_ctas_per_sm() { return ctas_per_sm(mincurv_pdip_kappa_kernel); }
-
 // ================================================================================================
 // debug aid (tests/test_gpu_factor.py): factorise M = H + D of every instance with the fused forward substitution of
 // V_RHS, solve into V_DX; then solve M x = V_T0 with the full sweeps into V_T1.  HB, V_DD, V_RHS, V_T0 are inputs.
@@ -1614,12 +1585,6 @@ debug_factor_solve_kernel(int B, int n_max, const int32_t *__restrict__ n_pts, d
         if (threadIdx.x == 0) status[b] = (ok && ok2) ? 0 : 3;
         __syncthreads();
     }
-}
-
-int debug_factor_solve_ctas_per_sm() { return ctas_per_sm(debug_factor_solve_kernel); }
-
-int launch_debug_factor_solve(int B, int n_max, const int32_t *n_pts, double *ws, const Layout &L, int32_t *status, int grid, cudaStream_t stream) {
-    return launch_solver(debug_factor_solve_kernel, grid, nullptr, stream, B, n_max, n_pts, ws, L, status);
 }
 
 // ================================================================================================
@@ -1691,14 +1656,136 @@ mincurv_adjoint_kernel(int B, int n_max, const int32_t *__restrict__ n_pts, cons
     }
 }
 
-int adjoint_ctas_per_sm() { return ctas_per_sm(mincurv_adjoint_kernel); }
+}  // namespace mc
 
-int launch_mincurv_adjoint(int B, int n_max, const int32_t *n_pts, const double *reftrack, double w_veh, const double *w_veh_batch,
-                           double *ws, const Layout &L, const double *sens, const double *grad_alpha, int32_t *grad_status,
-                           double *grad_w_right, double *grad_w_left, double *grad_w_veh, int grid, int *work_counter,
-                           cudaStream_t stream) {
-    return launch_solver(mincurv_adjoint_kernel, grid, work_counter, stream, B, n_max, n_pts, reftrack, w_veh, w_veh_batch, ws, L, sens,
-                         grad_alpha, grad_status, grad_w_right, grad_w_left, grad_w_veh, work_counter);
+static constexpr int PDIP_SLICE_DEFAULT = 8;      // DESIGN.md section 3.3: the predictor of the remaining iterations is
+                                                  // no better than chance after 4 iterations, within one iteration after 8
+
+extern "C" {
+
+int mc_mincurv_pdip_batch(int B, int n_max, const int32_t *n_pts, double *alpha, int32_t *status, int32_t *iters,
+                          void *workspace, size_t workspace_bytes, void *stream) {
+    if (!alpha || !status) return bad("mc_mincurv_pdip_batch: NULL argument");
+    int rc = mc::mincurv_args("mc_mincurv_pdip_batch", B, n_max, workspace, workspace_bytes);
+    if (rc) return rc;
+    mc::PdipParams prm;
+    prm.max_iter = 40;
+    prm.mu_rel = 1e-10;
+    prm.rd_rel = 1e-8;
+    prm.eta = 0.995;
+    prm.dx_rel = 1e-5;
+    prm.lam0_rel = 1e-2;
+    if (const char *e = getenv("MC_DEBUG_PDIP_LAM0")) { const double v = atof(e); if (v > 0.0) prm.lam0_rel = v; }   // start-point experiments only
+    if (const char *e = getenv("MC_DEBUG_PDIP_ETA")) { const double v = atof(e); if (v > 0.5 && v < 1.0) prm.eta = v; }
+    if (const char *e = getenv("MC_DEBUG_PDIP_DX_REL")) { const double v = atof(e); if (v >= 0.0) prm.dx_rel = v; }
+    if (const char *e = getenv("MC_DEBUG_PDIP_MU_REL")) { const double v = atof(e); if (v > 0.0) prm.mu_rel = v; }   // tolerance experiments only
+    int per_sm = mc::ctas_per_sm(mc::mincurv_pdip_kernel);
+    if (const char *e = getenv("MC_DEBUG_PDIP_CTAS_PER_SM")) {      // occupancy experiments only (tools/prof_run.py)
+        const int v = atoi(e);
+        if (v > 0 && v < per_sm) per_sm = v;
+    }
+    // iterations before an instance is parked in the sliced schedule (DESIGN.md section 3.3); 0: every instance to the end
+    int slice = PDIP_SLICE_DEFAULT;
+    if (const char *e = getenv("MC_DEBUG_PDIP_SLICE")) { const int v = atoi(e); if (v >= 0) slice = v; }   // A/B runs and tests
+    const mc::SolverGrid g = mc::solver_grid(B, n_max, workspace, per_sm);
+    const mc::Layout L = mc::make_layout(n_max);
+    double *ws = (double *)workspace;
+    cudaStream_t s = (cudaStream_t)stream;
+    // slice > 0 and more instances than CTAs: the sliced schedule (one launch, no grid-wide wait: the CTAs need not all be
+    // resident); the schedule's ints sit behind the slabs
+    if (B <= g.grid) slice = 0;
+    cudaMemsetAsync(g.counter, 0, mc::SCHED_INTS * sizeof(int), s);
+    if (slice > 0)      // the PARK_LIST entries of every slab
+        cudaMemset2DAsync(ws + (size_t)mc::V_PARK * L.np + mc::PARK_LIST, L.stride * sizeof(double), 0,
+                          mc::PARK_BUCKETS * sizeof(int), B, s);
+    if (mc::launch_solver(mc::mincurv_pdip_kernel, g.grid, nullptr, s, B, n_max, n_pts, ws, L, prm, slice, alpha, status, iters,
+                          g.counter) != 0) {
+        snprintf(mc::g_err, sizeof(mc::g_err), "mincurv_pdip_kernel: cudaFuncSetAttribute failed");
+        return MC_ECUDA;
+    }
+    return check_cuda("mincurv_pdip_kernel");
 }
 
-}  // namespace mc
+int mc_mincurv_kappa_batch(int B, int n_max, const int32_t *n_pts, double kappa_bound, double *alpha, int32_t *status,
+                           int32_t *iters, void *workspace, size_t workspace_bytes, void *stream) {
+    if (!alpha || !status) return bad("mc_mincurv_kappa_batch: NULL argument");
+    int rc = mc::mincurv_args("mc_mincurv_kappa_batch", B, n_max, workspace, workspace_bytes);
+    if (rc) return rc;
+    mc::PdipParams prm;
+    prm.max_iter = 40;
+    prm.mu_rel = 1e-11;
+    prm.rd_rel = 1e-8;
+    prm.eta = 0.995;
+    prm.dx_rel = 0.0;
+    prm.lam0_rel = 1e-2;
+    const mc::SolverGrid g = mc::solver_grid(B, n_max, workspace, mc::ctas_per_sm(mc::mincurv_pdip_kappa_kernel));
+    if (mc::launch_solver(mc::mincurv_pdip_kappa_kernel, g.grid, g.counter, (cudaStream_t)stream, B, n_max, n_pts,
+                          (double *)workspace, mc::make_layout(n_max), prm, kappa_bound, alpha, status, iters, g.counter) != 0) {
+        snprintf(mc::g_err, sizeof(mc::g_err), "mincurv_pdip_kappa_kernel: cudaFuncSetAttribute failed");
+        return MC_ECUDA;
+    }
+    return check_cuda("mincurv_pdip_kappa_kernel");
+}
+
+int mc_mincurv_adjoint_batch(int B, int n_max, const int32_t *n_pts, const double *reftrack, const double *normvec,
+                             const double *h, double w_veh, const double *w_veh_batch, double f_scale, const int32_t *centre_id,
+                             const double *sens, int32_t *grad_status, const double *grad_alpha, double *grad_w_right,
+                             double *grad_w_left, double *grad_w_veh, void *workspace, size_t workspace_bytes, void *stream) {
+    if (!sens || !grad_status || !grad_alpha || !grad_w_right || !grad_w_left || !grad_w_veh)
+        return bad("mc_mincurv_adjoint_batch: NULL argument");
+    // the band of H and the bounds are rebuilt in the slabs; the assembly's status words (the forward pass's, recorded in
+    // grad_status) go to grad_w_right, which the adjoint kernel overwrites
+    int rc = mc_mincurv_setup_batch_shared(B, n_max, n_pts, reftrack, normvec, h, w_veh, w_veh_batch, f_scale, centre_id,
+                                           reinterpret_cast<int32_t *>(grad_w_right), workspace, workspace_bytes, stream);
+    if (rc) return rc;
+    const mc::SolverGrid g = mc::solver_grid(B, n_max, workspace, mc::ctas_per_sm(mc::mincurv_adjoint_kernel));
+    if (mc::launch_solver(mc::mincurv_adjoint_kernel, g.grid, g.counter, (cudaStream_t)stream, B, n_max, n_pts, reftrack, w_veh,
+                          w_veh_batch, (double *)workspace, mc::make_layout(n_max), sens, grad_alpha, grad_status, grad_w_right,
+                          grad_w_left, grad_w_veh, g.counter) != 0) {
+        snprintf(mc::g_err, sizeof(mc::g_err), "mincurv_adjoint_kernel: cudaFuncSetAttribute failed");
+        return MC_ECUDA;
+    }
+    return check_cuda("mincurv_adjoint_kernel");
+}
+
+/* debug aid (tests/test_gpu_factor.py): one factorisation + the two kinds of solve of the interior-point kernel on slabs
+ * whose H band, V_DD, V_RHS and V_T0 the caller has filled in; results in V_DX, V_T1, V_T2 */
+int mc_debug_factor_solve(int B, int n_max, const int32_t *n_pts, int32_t *status, void *workspace, size_t workspace_bytes,
+                          void *stream) {
+    if (!status) return bad("mc_debug_factor_solve: NULL argument");
+    int rc = mc::mincurv_args("mc_debug_factor_solve", B, n_max, workspace, workspace_bytes);
+    if (rc) return rc;
+    const mc::SolverGrid g = mc::solver_grid(B, n_max, workspace, mc::ctas_per_sm(mc::debug_factor_solve_kernel));
+    if (mc::launch_solver(mc::debug_factor_solve_kernel, g.grid, nullptr, (cudaStream_t)stream, B, n_max, n_pts,
+                          (double *)workspace, mc::make_layout(n_max), status) != 0)
+        return bad("mc_debug_factor_solve: cudaFuncSetAttribute failed");
+    return check_cuda("debug_factor_solve_kernel");
+}
+
+// debug aid: the cycle counters of CTA 0 of mincurv_pdip_kernel, slots as in enum ProfSlot; zeros unless built with
+// -DMC_PROFILE
+int mc_debug_read_profile(unsigned long long *host_out24, int reset) {
+#ifdef MC_PROFILE
+    if (cudaMemcpyFromSymbol(host_out24, mc::g_prof, sizeof(unsigned long long) * mc::PROF_SLOTS) != cudaSuccess) return MC_ECUDA;
+    if (getenv("MC_PROFILE_SEGMENTS")) {       // tools/prof_run.py: sub-phase counters of one panel
+        unsigned long long seg[32];
+        if (cudaMemcpyFromSymbol(seg, mc::g_seg, sizeof(seg)) == cudaSuccess) {
+            fprintf(stderr, "segments:");
+            for (int i = 0; i < 32; ++i) fprintf(stderr, " %d:%llu", i, seg[i]);
+            fprintf(stderr, "\n");
+        }
+    }
+    if (reset) {
+        unsigned long long z[32] = {0};
+        if (cudaMemcpyToSymbol(mc::g_prof, z, sizeof(unsigned long long) * mc::PROF_SLOTS) != cudaSuccess) return MC_ECUDA;
+        cudaMemcpyToSymbol(mc::g_seg, z, sizeof(z));
+    }
+    return MC_OK;
+#else
+    (void)reset;
+    for (int i = 0; i < mc::PROF_SLOTS; ++i) host_out24[i] = 0ull;
+    return MC_OK;
+#endif
+}
+
+}  // extern "C"

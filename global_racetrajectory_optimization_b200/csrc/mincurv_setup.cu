@@ -17,6 +17,7 @@
 //   Mid_t(c, c'+1) = rho+_{c'+1} (Mid_t(c, c') + w_t[c'] Ti[c'][c] Ti[c'][c'])
 // (exact sums over all m -- no truncation of E -- verified against the explicit E^T E in tools/).
 // One CTA per QP instance; O(N) vectors and the B / H bands live in the instance's HBM slab.
+#include "capi.cuh"
 #include "mincurv_ops.cuh"
 
 namespace mc {
@@ -159,15 +160,47 @@ mincurv_share_kernel(int B, int n_max, const int32_t *__restrict__ n_pts, const 
     if (threadIdx.x == 0) *band_owner(dst, L) = o;
 }
 
-void launch_mincurv_setup(int B, int n_max, const int32_t *n_pts, const double *reftrack, const double *normvec,
-                          const double *h, double w_veh, const double *w_veh_batch, double f_scale, const int32_t *centre_id,
-                          double *ws, const Layout &L, int32_t *status, cudaStream_t stream) {
-    constexpr int smem = hband_win_doubles(256) * (int)sizeof(double);      // 49 KB: above the static limit
-    // (per launch: the attribute is per device and a process may drive several)
-    cudaFuncSetAttribute(mincurv_setup_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-    mincurv_setup_kernel<<<B, 256, smem, stream>>>(n_max, n_pts, reftrack, normvec, h, w_veh, w_veh_batch, f_scale, centre_id, ws, L,
-                                                   status);
-    if (centre_id) mincurv_share_kernel<<<B, 256, 0, stream>>>(B, n_max, n_pts, centre_id, ws, L, status);
+}  // namespace mc
+
+extern "C" {
+
+size_t mc_mincurv_workspace_bytes(int B, int n_max) {
+    if (B <= 0 || n_max < mc::N_MIN) return 0;
+    return mc::mincurv_slabs_bytes(B, n_max) + 256;      // + the work counters of the persistent solver kernels (SCHED_INTS)
 }
 
-}  // namespace mc
+int mc_mincurv_setup_batch_shared(int B, int n_max, const int32_t *n_pts, const double *reftrack, const double *normvec,
+                                  const double *h, double w_veh, const double *w_veh_batch, double f_scale,
+                                  const int32_t *centre_id, int32_t *status, void *workspace, size_t workspace_bytes,
+                                  void *stream) {
+    if (!reftrack || !normvec || !h || !status) return bad("mc_mincurv_setup_batch: NULL argument");
+    if (!(f_scale > 0.0)) return bad("mc_mincurv_setup_batch: f_scale must be positive");
+    int rc = mc::mincurv_args("mc_mincurv_setup_batch", B, n_max, workspace, workspace_bytes);
+    if (rc) return rc;
+    const mc::Layout L = mc::make_layout(n_max);
+    double *ws = (double *)workspace;
+    cudaStream_t s = (cudaStream_t)stream;
+    constexpr int smem = mc::hband_win_doubles(256) * (int)sizeof(double);      // 49 KB: above the static limit
+    // (per launch: the attribute is per device and a process may drive several)
+    cudaFuncSetAttribute(mc::mincurv_setup_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    mc::mincurv_setup_kernel<<<B, 256, smem, s>>>(n_max, n_pts, reftrack, normvec, h, w_veh, w_veh_batch, f_scale, centre_id,
+                                                  ws, L, status);
+    if (centre_id) mc::mincurv_share_kernel<<<B, 256, 0, s>>>(B, n_max, n_pts, centre_id, ws, L, status);
+    return check_cuda("mincurv_setup_kernel");
+}
+
+int mc_mincurv_setup_batch_ex(int B, int n_max, const int32_t *n_pts, const double *reftrack, const double *normvec,
+                              const double *h, double w_veh, const double *w_veh_batch, double f_scale, int32_t *status,
+                              void *workspace, size_t workspace_bytes, void *stream) {
+    return mc_mincurv_setup_batch_shared(B, n_max, n_pts, reftrack, normvec, h, w_veh, w_veh_batch, f_scale, nullptr, status,
+                                         workspace, workspace_bytes, stream);
+}
+
+int mc_mincurv_setup_batch(int B, int n_max, const int32_t *n_pts, const double *reftrack, const double *normvec,
+                           const double *h, double w_veh, const double *w_veh_batch, int32_t *status, void *workspace,
+                           size_t workspace_bytes, void *stream) {
+    return mc_mincurv_setup_batch_ex(B, n_max, n_pts, reftrack, normvec, h, w_veh, w_veh_batch, MC_F_SCALE_DEFAULT, status,
+                                     workspace, workspace_bytes, stream);
+}
+
+}  // extern "C"

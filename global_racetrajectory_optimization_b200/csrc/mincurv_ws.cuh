@@ -8,6 +8,7 @@
 //                        columns, fill rows [G | w], and z = w y of the last forward substitution (mincurv_ipm.cu)
 // With shared centre lines a follower's band stays in its owner's slab: V_HBSRC says whose band an instance uses.
 #pragma once
+#include "capi.cuh"
 #include "common.cuh"
 
 namespace mc {
@@ -48,6 +49,18 @@ __host__ __device__ inline Layout make_layout(int n_max) {
 // ints behind the slabs (within the 256 bytes there): the work counter of the persistent solver kernels and the schedule
 // of the box phase's two launches (mincurv_ipm.cu)
 constexpr int SCHED_INTS = 64;
+static_assert(SCHED_INTS * sizeof(int) <= 256, "the counters behind the slabs");
+
+// the slabs of B instances; the workspace is these and the 256 bytes of counters behind them (mc_mincurv_workspace_bytes)
+static inline size_t mincurv_slabs_bytes(int B, int n_max) { return align256((size_t)B * make_layout(n_max).stride * sizeof(double)); }
+
+// the argument checks every stage of the minimum-curvature path starts with
+static inline int mincurv_args(const char *who, int B, int n_max, void *workspace, size_t workspace_bytes) {
+    if (B <= 0) return bad("mincurv: B <= 0");
+    if (n_max < N_MIN) return bad("mincurv: n_max below the supported minimum (%d points)", N_MIN);
+    if (!workspace || workspace_bytes < mincurv_slabs_bytes(B, n_max) + 256) return small_workspace(who);
+    return MC_OK;
+}
 
 struct PdipParams {
     int max_iter;

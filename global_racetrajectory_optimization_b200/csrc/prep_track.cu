@@ -10,13 +10,12 @@
 // point a knot: (R + lam Q^T Q) gamma = Q^T p, f = p - lam Q gamma, a cyclic pentadiagonal SPD system solved in O(n) per
 // trial lam.  oracle/tph_prep.py states the same algorithm in dense numpy (checked to 1e-8 in tests/test_gpu_prep.py, which
 // also reports the distance to the scipy/FITPACK route: decimetres at sharp corners, centimetres on the real circuits).
+#include "capi.cuh"
 #include "common.cuh"
 
 namespace mc {
 
-constexpr int PT_VECS = 22;       // per-track scratch vectors of n_int_max doubles
-
-size_t prep_track_ws_doubles(int n_raw_max, int n_int_max) { return (size_t)PT_VECS * n_int_max + (size_t)6 * (n_raw_max + 1); }
+constexpr int PT_VECS = 22;       // per-track scratch vectors of n_int_max doubles (and six of n_raw_max + 1)
 
 struct PtSpline {                 // the fitted curve: knots u (period 1), values f, second derivatives g
     const double *u, *fx, *fy, *gx, *gy;
@@ -317,11 +316,29 @@ prep_track_kernel(int n_raw_max, const int32_t *__restrict__ n_raw_b, const doub
     if (tid == 0) n_out[b] = n_reg;
 }
 
-void launch_prep_track(int B, int n_raw_max, const int32_t *n_raw, const double *raw, double s_reg, double stepsize_prep,
-                       double stepsize_reg, double min_width, int n_int_max, int n_out_max, double *out, int32_t *n_out,
-                       double *lam_out, double *ws, cudaStream_t stream) {
-    prep_track_kernel<<<B, 256, 0, stream>>>(n_raw_max, n_raw, raw, s_reg, stepsize_prep, stepsize_reg, min_width, n_int_max,
-                                             n_out_max, out, n_out, lam_out, ws);
+}  // namespace mc
+
+extern "C" {
+
+size_t mc_prep_track_workspace_bytes(int B, int n_raw_max, int n_int_max) {
+    if (B <= 0 || n_raw_max < 5 || n_int_max < 6) return 0;
+    return align256((size_t)B * ((size_t)mc::PT_VECS * n_int_max + (size_t)6 * (n_raw_max + 1)) * sizeof(double));
 }
 
-}  // namespace mc
+int mc_prep_track_batch(int B, int n_raw_max, const int32_t *n_raw, const double *track, int k_reg, double s_reg,
+                        double stepsize_prep, double stepsize_reg, double min_width, int n_int_max, int n_out_max,
+                        double *reftrack_interp, int32_t *n_out, double *smoothing_lambda, void *workspace,
+                        size_t workspace_bytes, void *stream) {
+    if (B <= 0 || n_raw_max < 5 || !track || !(s_reg > 0.0) || !(stepsize_prep > 0.0) || !(stepsize_reg > 0.0) || n_int_max < 6 ||
+        n_out_max < 4 || !reftrack_interp || !n_out)
+        return bad("mc_prep_track_batch: bad argument");
+    if (k_reg != 3) return bad("mc_prep_track_batch: only cubic splines (k_reg = 3, the reference's setting) are implemented");
+    if (!workspace || workspace_bytes < mc_prep_track_workspace_bytes(B, n_raw_max, n_int_max))
+        return small_workspace("mc_prep_track_batch");
+    mc::prep_track_kernel<<<B, 256, 0, (cudaStream_t)stream>>>(n_raw_max, n_raw, track, s_reg, stepsize_prep, stepsize_reg,
+                                                               min_width, n_int_max, n_out_max, reftrack_interp, n_out,
+                                                               smoothing_lambda, (double *)workspace);
+    return check_cuda("prep_track_kernel");
+}
+
+}  // extern "C"

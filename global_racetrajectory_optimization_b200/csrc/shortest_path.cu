@@ -7,14 +7,12 @@
 // (element i of instance b at [i * B + b]) so that every pass is a fully coalesced stream; the cyclic
 // system is solved by the Thomas recurrences + Sherman-Morrison (gamma = -diag_0, T = M + |gamma| w w^T
 // stays SPD).  Large batches (BASELINE config 5: 32k instances) fill the machine.
+#include "capi.cuh"
 #include "common.cuh"
-#include "../../include/mincurv_b200.h"
 
 namespace mc {
 
 enum SpVec : int { SP_LB = 0, SP_UB, SP_F, SP_OFF, SP_DG, SP_AL, SP_LU, SP_LL, SP_RD, SP_X, SP_CP, SP_MI, SP_Q, SP_TU, SP_TL, SP_DD, SP_RHS, SP_SU, SP_SL, SP_NUM };
-
-size_t shortest_path_ws_doubles(int n_max) { return (size_t)SP_NUM * n_max; }
 
 struct SpView {
     double *base; size_t B; size_t nB;   // nB = n_max * B
@@ -193,15 +191,6 @@ shortest_path_kernel(int B, int n_max, const int32_t *__restrict__ n_pts, const 
     if (iters) iters[b] = it;
 }
 
-int launch_shortest_path(int B, int n_max, const int32_t *n_pts, const double *reftrack, const double *normvec,
-                         double w_veh, const double *w_veh_batch, double *alpha, int32_t *status, int32_t *iters,
-                         double *ws, cudaStream_t stream) {
-    const int threads = 128;
-    shortest_path_kernel<<<(B + threads - 1) / threads, threads, 0, stream>>>(B, n_max, n_pts, reftrack, normvec, w_veh,
-                                                                             w_veh_batch, alpha, status, iters, ws);
-    return 0;
-}
-
 // ---- sensitivities (include/mincurv_b200.h, DESIGN.md section 3.11) ----
 // Run right after shortest_path_kernel on the same workspace: the final iterate's lu / su and ll / sl, the diagonal D of
 // M = H + D that the backward pass factorises, and grad_status = status.
@@ -292,21 +281,56 @@ shortest_path_adjoint_kernel(int B, int n_max, const int32_t *__restrict__ n_pts
     if (grad_w_veh) grad_w_veh[b] = ok ? gwv : 0.0;
 }
 
-void launch_shortest_path_sens_export(int B, int n_max, const int32_t *n_pts, const int32_t *status, const double *ws,
-                                      double *sens, int32_t *grad_status, cudaStream_t stream) {
-    const int threads = 128;
-    shortest_path_sens_export_kernel<<<(B + threads - 1) / threads, threads, 0, stream>>>(B, n_max, n_pts, status, ws, sens,
-                                                                                         grad_status);
-}
-
-void launch_shortest_path_adjoint(int B, int n_max, const int32_t *n_pts, const double *reftrack, const double *normvec,
-                                  double w_veh, const double *w_veh_batch, const double *alpha, const double *sens,
-                                  int32_t *grad_status, const double *grad_alpha, double *grad_reftrack, double *grad_normvec,
-                                  double *grad_w_veh, double *ws, cudaStream_t stream) {
-    const int threads = 128;
-    shortest_path_adjoint_kernel<<<(B + threads - 1) / threads, threads, 0, stream>>>(
-        B, n_max, n_pts, reftrack, normvec, w_veh, w_veh_batch, alpha, sens, grad_status, grad_alpha, grad_reftrack,
-        grad_normvec, grad_w_veh, ws);
-}
-
 }  // namespace mc
+
+extern "C" {
+
+size_t mc_shortest_path_workspace_bytes(int B, int n_max) {
+    if (B <= 0 || n_max < 3) return 0;
+    return align256((size_t)B * mc::SP_NUM * n_max * sizeof(double));
+}
+
+int mc_shortest_path_solve_batch(int B, int n_max, const int32_t *n_pts, const double *reftrack, const double *normvec,
+                                 double w_veh, const double *w_veh_batch, double *alpha, int32_t *status, int32_t *iters,
+                                 void *workspace, size_t workspace_bytes, void *stream) {
+    if (B <= 0 || n_max < 3 || !reftrack || !normvec || !alpha || !status)
+        return bad("mc_shortest_path_solve_batch: bad argument");
+    if (!workspace || workspace_bytes < mc_shortest_path_workspace_bytes(B, n_max))
+        return small_workspace("mc_shortest_path_solve_batch");
+    const int threads = 128;
+    mc::shortest_path_kernel<<<(B + threads - 1) / threads, threads, 0, (cudaStream_t)stream>>>(
+        B, n_max, n_pts, reftrack, normvec, w_veh, w_veh_batch, alpha, status, iters, (double *)workspace);
+    return check_cuda("shortest_path_kernel");
+}
+
+int mc_shortest_path_solve_batch_sens(int B, int n_max, const int32_t *n_pts, const double *reftrack, const double *normvec,
+                                      double w_veh, const double *w_veh_batch, double *alpha, int32_t *status, int32_t *iters,
+                                      double *sens, int32_t *grad_status, void *workspace, size_t workspace_bytes,
+                                      void *stream) {
+    if (!sens || !grad_status) return bad("mc_shortest_path_solve_batch_sens: NULL argument");
+    int rc = mc_shortest_path_solve_batch(B, n_max, n_pts, reftrack, normvec, w_veh, w_veh_batch, alpha, status, iters,
+                                          workspace, workspace_bytes, stream);
+    if (rc) return rc;
+    // the workspace still holds the final iterate
+    const int threads = 128;
+    mc::shortest_path_sens_export_kernel<<<(B + threads - 1) / threads, threads, 0, (cudaStream_t)stream>>>(
+        B, n_max, n_pts, status, (const double *)workspace, sens, grad_status);
+    return check_cuda("shortest_path_sens_export_kernel");
+}
+
+int mc_shortest_path_adjoint_batch(int B, int n_max, const int32_t *n_pts, const double *reftrack, const double *normvec,
+                                   double w_veh, const double *w_veh_batch, const double *alpha, const double *sens,
+                                   int32_t *grad_status, const double *grad_alpha, double *grad_reftrack, double *grad_normvec,
+                                   double *grad_w_veh, void *workspace, size_t workspace_bytes, void *stream) {
+    if (B <= 0 || n_max < 3 || !reftrack || !normvec || !alpha || !sens || !grad_status || !grad_alpha || !grad_reftrack)
+        return bad("mc_shortest_path_adjoint_batch: bad argument");
+    if (!workspace || workspace_bytes < mc_shortest_path_workspace_bytes(B, n_max))
+        return small_workspace("mc_shortest_path_adjoint_batch");
+    const int threads = 128;
+    mc::shortest_path_adjoint_kernel<<<(B + threads - 1) / threads, threads, 0, (cudaStream_t)stream>>>(
+        B, n_max, n_pts, reftrack, normvec, w_veh, w_veh_batch, alpha, sens, grad_status, grad_alpha, grad_reftrack,
+        grad_normvec, grad_w_veh, (double *)workspace);
+    return check_cuda("shortest_path_adjoint_kernel");
+}
+
+}  // extern "C"

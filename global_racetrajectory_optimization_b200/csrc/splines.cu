@@ -8,6 +8,7 @@
 //                            main_globaltraj.py:273-284)                     SURVEY.md A.5
 // The dense 4N x 4N solve of the reference is the periodic tridiagonal moment system of common.cuh.
 // One CTA per track; O(N) scratch vectors live in the caller-provided workspace (HBM, L2-resident).
+#include "capi.cuh"
 #include "common.cuh"
 
 namespace mc {
@@ -15,7 +16,6 @@ namespace mc {
 enum SVec : int { S_H = 0, S_DG, S_DFW, S_DBW, S_LFW, S_INVD, S_R0, S_R1, S_Y0, S_Y1, S_MX, S_MY, S_PX, S_PY, S_CUM, S_NUM };
 
 __host__ __device__ inline int spl_np(int n_max) { return ((n_max + 31) / 32) * 32 + 32; }
-size_t spline_ws_doubles(int n_max) { return (size_t)S_NUM * spl_np(n_max); }
 
 // ---------------------------------------------------------------------------------------------
 // Closed spline through (PX, PY) with parameter scales H on EIGHT vectors that live in shared memory whenever the track
@@ -419,8 +419,6 @@ __global__ void scale_alpha_kernel(int n_max, double *__restrict__ alpha, const 
 // ---------------------------------------------------------------------------------------------
 enum CraVec : int { G_SL = 0, G_CUM, G_C0X, G_C1X, G_C2X, G_C3X, G_C0Y, G_C1Y, G_C2Y, G_C3Y, G_NUM };
 
-size_t create_raceline_adjoint_ws_doubles(int n_max) { return (size_t)(S_NUM + G_NUM) * spl_np(n_max); }
-
 struct CraAdjArgs {
     int n_max, n_out_max;
     const int32_t *n_pts, *n_out, *spline_inds;
@@ -568,55 +566,6 @@ __global__ void __launch_bounds__(256) create_raceline_adjoint_kernel(const CraA
     }
 }
 
-void launch_create_raceline_adjoint(int B, int n_max, const int32_t *n_pts, const double *normvec, const double *alpha, int n_out_max, const double *cx,
-                                    const double *cy, const double *sl, const int32_t *n_out, const int32_t *si,
-                                    const double *tv, const double *g_raceline, const double *g_kappa, const double *g_el,
-                                    double *g_alpha, double *g_refline, double *g_normvec, double *ws, cudaStream_t stream) {
-    CraAdjArgs a;
-    a.n_max = n_max; a.n_out_max = n_out_max; a.n_pts = n_pts; a.n_out = n_out;
-    a.spline_inds = si; a.normvec = normvec; a.alpha = alpha; a.coeffs_x = cx; a.coeffs_y = cy;
-    a.spline_lengths = sl; a.t_values = tv; a.g_raceline = g_raceline; a.g_kappa = g_kappa; a.g_el = g_el;
-    a.g_alpha = g_alpha; a.g_refline = g_refline; a.g_normvec = g_normvec; a.ws = ws;
-    const size_t sm = spline_smem_bytes(n_max) <= SPL_SMEM_LIMIT ? spline_smem_bytes(n_max) : 0;
-    cudaFuncSetAttribute(create_raceline_adjoint_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SPL_SMEM_LIMIT);
-    create_raceline_adjoint_kernel<<<B, 256, sm, stream>>>(a);
-}
-
-// ---------------------------------------------------------------------------------------------
-void launch_calc_splines(int B, int n_max, const int32_t *n_pts, const double *xy, int xy_stride,
-                         const double *el_lengths, int use_dist_scaling, double *cx, double *cy, double *nvec,
-                         double *h_out, double *ws, cudaStream_t stream) {
-    const size_t sm = spline_smem_bytes(n_max) <= SPL_SMEM_LIMIT ? spline_smem_bytes(n_max) : 0;
-    cudaFuncSetAttribute(calc_splines_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SPL_SMEM_LIMIT);
-    calc_splines_kernel<<<B, 256, sm, stream>>>(n_max, n_pts, xy, xy_stride, el_lengths, use_dist_scaling, cx, cy, nvec,
-                                                h_out, ws);
-}
-void launch_create_raceline(int B, int n_max, const int32_t *n_pts, const double *refline, int ref_stride,
-                            const double *normvec, const double *alpha, double stepsize, int n_out_max, double *cx,
-                            double *cy, double *sl, int32_t *n_out, double *ri, int32_t *si, double *tv, double *ss,
-                            double *el, double *psi, double *kappa, double *ws, cudaStream_t stream) {
-    const size_t sm = spline_smem_bytes(n_max) <= SPL_SMEM_LIMIT ? spline_smem_bytes(n_max) : 0;
-    cudaFuncSetAttribute(create_raceline_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SPL_SMEM_LIMIT);
-    create_raceline_kernel<<<B, 256, sm, stream>>>(n_max, n_pts, refline, ref_stride, normvec, alpha, stepsize, n_out_max,
-                                                   cx, cy, sl, n_out, ri, si, tv, ss, el, psi, kappa, ws);
-}
-void launch_head_curv(int B, int n_max, const double *cx, const double *cy, int n_eval_max, const int32_t *n_eval,
-                      const int32_t *ind, const double *t, double *psi, double *kappa, double *dkappa,
-                      cudaStream_t stream) {
-    for_grid_y_chunks(B, [&](int b0, int nb) {
-        const size_t oe = (size_t)b0 * n_eval_max, oc = (size_t)b0 * n_max * 4;
-        dim3 grid((n_eval_max + 255) / 256, nb);
-        head_curv_kernel<<<grid, 256, 0, stream>>>(n_max, cx + oc, cy + oc, n_eval_max, n_eval ? n_eval + b0 : nullptr, ind + oe,
-                                                   t + oe, psi + oe, kappa ? kappa + oe : nullptr, dkappa ? dkappa + oe : nullptr);
-    });
-}
-void launch_iqp_new_reftrack(int B, int n_max, const int32_t *n_pts, const int32_t *active, const double *reftrack,
-                             const double *normvec, const double *alpha, int n_max_new, const int32_t *n_new,
-                             const double *race_xy, const int32_t *inds, const double *tvals, double *reftrack_new,
-                             double *normvec_new, int32_t *n_pts_new, cudaStream_t stream) {
-    iqp_new_reftrack_kernel<<<B, 256, 0, stream>>>(n_max, n_pts, active, reftrack, normvec, alpha, n_max_new, n_new,
-                                                   race_xy, inds, tvals, reftrack_new, normvec_new, n_pts_new);
-}
 // ---------------------------------------------------------------------------------------------
 // tph.iqp_handler's per-track termination (SURVEY.md A.5) on the device: a track leaves the loop once
 // iter >= iters_min and curv_error_max <= curv_error_allowed (or its QP failed, or the iteration cap is reached: status 2);
@@ -660,22 +609,182 @@ iqp_finish_kernel(int n_max, int n_cap, int it, int iters_min, double curv_error
         atomicAdd(&counters[1], 1);
     }
 }
-void launch_iqp_finish(int B, int n_max, int n_cap, int it, int iters_min, double curv_error_allowed, int fixed_iters, int limit,
-                       int32_t *active, const int32_t *status, const double *curv_err, const int32_t *n_pts, const double *alpha,
-                       const double *reftrack, const double *normvec, double *fin_alpha, double *fin_reftrack,
-                       double *fin_normvec, int32_t *fin_n_pts, int32_t *fin_iters, int32_t *fin_status, double *fin_curv_err,
-                       int32_t *counters, cudaStream_t stream) {
-    cudaMemsetAsync(counters, 0, 2 * sizeof(int32_t), stream);
-    iqp_finish_kernel<<<B, 256, 0, stream>>>(n_max, n_cap, it, iters_min, curv_error_allowed, fixed_iters, limit, active, status,
-                                             curv_err, n_pts, alpha, reftrack, normvec, fin_alpha, fin_reftrack, fin_normvec,
-                                             fin_n_pts, fin_iters, fin_status, fin_curv_err, counters);
-}
 
-void launch_scale_alpha(int B, int n_max, double *alpha, const double *scale_batch, double scale, cudaStream_t stream) {
-    for_grid_y_chunks(B, [&](int b0, int nb) {
-        dim3 grid((n_max + 255) / 256, nb);
-        scale_alpha_kernel<<<grid, 256, 0, stream>>>(n_max, alpha + (size_t)b0 * n_max, scale_batch ? scale_batch + b0 : nullptr, scale);
-    });
+// dynamic shared memory of a closed-spline kernel's launch: its eight vectors when they fit, else none (global scratch)
+template <typename K>
+static size_t spline_smem(K kernel, int n_max) {
+    cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)SPL_SMEM_LIMIT);
+    return spline_smem_bytes(n_max) <= SPL_SMEM_LIMIT ? spline_smem_bytes(n_max) : 0;
 }
 
 }  // namespace mc
+
+extern "C" {
+
+size_t mc_calc_splines_workspace_bytes(int B, int n_max) {
+    if (B <= 0 || n_max <= 0) return 0;
+    return align256((size_t)B * mc::S_NUM * mc::spl_np(n_max) * sizeof(double));
+}
+
+int mc_calc_splines_batch(int B, int n_max, const int32_t *n_pts, const double *xy, int xy_stride,
+                          const double *el_lengths, int use_dist_scaling, double *coeffs_x, double *coeffs_y,
+                          double *normvec, double *h_out, void *workspace, size_t workspace_bytes, void *stream) {
+    if (B <= 0 || n_max < 3 || !xy || (xy_stride != 2 && xy_stride != 4)) return bad("mc_calc_splines_batch: bad argument");
+    if ((coeffs_x == nullptr) != (coeffs_y == nullptr)) return bad("mc_calc_splines_batch: coeffs_x/coeffs_y must both be given or both NULL");
+    if (!workspace || workspace_bytes < mc_calc_splines_workspace_bytes(B, n_max))
+        return small_workspace("mc_calc_splines_batch");
+    mc::calc_splines_kernel<<<B, 256, mc::spline_smem(mc::calc_splines_kernel, n_max), (cudaStream_t)stream>>>(
+        n_max, n_pts, xy, xy_stride, el_lengths, use_dist_scaling, coeffs_x, coeffs_y, normvec, h_out, (double *)workspace);
+    return check_cuda("mc_calc_splines_batch");
+}
+
+size_t mc_create_raceline_workspace_bytes(int B, int n_max) { return mc_calc_splines_workspace_bytes(B, n_max); }
+
+int mc_create_raceline_batch(int B, int n_max, const int32_t *n_pts, const double *refline, int ref_stride,
+                             const double *normvec, const double *alpha, double stepsize_interp, int n_out_max,
+                             double *coeffs_x, double *coeffs_y, double *spline_lengths, int32_t *n_out,
+                             double *raceline_interp, int32_t *spline_inds, double *t_values, double *s_interp,
+                             double *el_lengths_interp, double *psi, double *kappa, void *workspace,
+                             size_t workspace_bytes, void *stream) {
+    if (B <= 0 || n_max < 3 || n_out_max <= 0 || !refline || (ref_stride != 2 && ref_stride != 4) || !normvec || !alpha ||
+        !(stepsize_interp > 0.0) || !coeffs_x || !coeffs_y || !spline_lengths || !n_out || !raceline_interp ||
+        !spline_inds || !t_values || !s_interp || !el_lengths_interp)
+        return bad("mc_create_raceline_batch: bad argument");
+    if (!workspace || workspace_bytes < mc_create_raceline_workspace_bytes(B, n_max))
+        return small_workspace("mc_create_raceline_batch");
+    mc::create_raceline_kernel<<<B, 256, mc::spline_smem(mc::create_raceline_kernel, n_max), (cudaStream_t)stream>>>(
+        n_max, n_pts, refline, ref_stride, normvec, alpha, stepsize_interp, n_out_max, coeffs_x, coeffs_y, spline_lengths,
+        n_out, raceline_interp, spline_inds, t_values, s_interp, el_lengths_interp, psi, kappa, (double *)workspace);
+    return check_cuda("create_raceline_kernel");
+}
+
+int mc_calc_head_curv_batch(int B, int n_max, const double *coeffs_x, const double *coeffs_y, int n_eval_max,
+                            const int32_t *n_eval, const int32_t *ind_spls, const double *t_spls, double *psi,
+                            double *kappa, double *dkappa, void *stream) {
+    if (B <= 0 || n_max <= 0 || n_eval_max <= 0 || !coeffs_x || !coeffs_y || !ind_spls || !t_spls || !psi)
+        return bad("mc_calc_head_curv_batch: bad argument");
+    if (dkappa && !kappa) return bad("dkappa cannot be calculated without kappa!");
+    mc::for_grid_y_chunks(B, [&](int b0, int nb) {
+        const size_t oe = (size_t)b0 * n_eval_max, oc = (size_t)b0 * n_max * 4;
+        dim3 grid((n_eval_max + 255) / 256, nb);
+        mc::head_curv_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(n_max, coeffs_x + oc, coeffs_y + oc, n_eval_max,
+                                                                     n_eval ? n_eval + b0 : nullptr, ind_spls + oe, t_spls + oe,
+                                                                     psi + oe, kappa ? kappa + oe : nullptr,
+                                                                     dkappa ? dkappa + oe : nullptr);
+    });
+    return check_cuda("head_curv_kernel");
+}
+
+// ------------------------------------------------------------------------------------------------
+// workspace of the IQP re-linearisation: spline scratch + the create_raceline outputs it discards
+static size_t iqp_ws_parts(int B, int n_max, int n_max_new, size_t off[10]) {
+    size_t o = 0;
+    const size_t spl = mc_calc_splines_workspace_bytes(B, n_max > n_max_new ? n_max : n_max_new);
+    off[0] = o; o += spl;                                                    // spline scratch
+    off[1] = o; o += align256((size_t)B * n_max * 4 * sizeof(double));       // coeffs_x
+    off[2] = o; o += align256((size_t)B * n_max * 4 * sizeof(double));       // coeffs_y
+    off[3] = o; o += align256((size_t)B * n_max * sizeof(double));           // spline_lengths
+    off[4] = o; o += align256((size_t)B * sizeof(int32_t));                  // n_out
+    off[5] = o; o += align256((size_t)B * n_max_new * 2 * sizeof(double));   // raceline_interp
+    off[6] = o; o += align256((size_t)B * n_max_new * sizeof(int32_t));      // spline_inds
+    off[7] = o; o += align256((size_t)B * n_max_new * sizeof(double));       // t_values
+    off[8] = o; o += align256((size_t)B * n_max_new * sizeof(double));       // s_interp
+    off[9] = o; o += align256((size_t)B * n_max_new * sizeof(double));       // el_lengths
+    return o;
+}
+
+size_t mc_iqp_relinearise_workspace_bytes(int B, int n_max, int n_max_new) {
+    if (B <= 0 || n_max < 3 || n_max_new < 3) return 0;
+    size_t off[10];
+    return iqp_ws_parts(B, n_max, n_max_new, off);
+}
+
+int mc_iqp_relinearise_batch(int B, int n_max, const int32_t *n_pts, const int32_t *active, const double *reftrack,
+                             const double *normvec, const double *alpha, double stepsize_interp, int n_max_new,
+                             double *reftrack_new, double *normvec_new, int32_t *n_pts_new, void *workspace,
+                             size_t workspace_bytes, void *stream) {
+    if (B <= 0 || n_max < 3 || n_max_new < 3 || !reftrack || !normvec || !alpha || !(stepsize_interp > 0.0) ||
+        !reftrack_new || !normvec_new || !n_pts_new)
+        return bad("mc_iqp_relinearise_batch: bad argument");
+    size_t off[10];
+    const size_t need = iqp_ws_parts(B, n_max, n_max_new, off);
+    if (!workspace || workspace_bytes < need) return small_workspace("mc_iqp_relinearise_batch");
+    char *w = (char *)workspace;
+    cudaStream_t s = (cudaStream_t)stream;
+    double *spl = (double *)(w + off[0]);
+    int32_t *n_out = (int32_t *)(w + off[4]);
+    mc::create_raceline_kernel<<<B, 256, mc::spline_smem(mc::create_raceline_kernel, n_max), s>>>(
+        n_max, n_pts, reftrack, 4, normvec, alpha, stepsize_interp, n_max_new, (double *)(w + off[1]), (double *)(w + off[2]),
+        (double *)(w + off[3]), n_out, (double *)(w + off[5]), (int32_t *)(w + off[6]), (double *)(w + off[7]),
+        (double *)(w + off[8]), (double *)(w + off[9]), nullptr, nullptr, spl);
+    int rc = check_cuda("create_raceline_kernel");
+    if (rc) return rc;
+    mc::iqp_new_reftrack_kernel<<<B, 256, 0, s>>>(n_max, n_pts, active, reftrack, normvec, alpha, n_max_new, n_out,
+                                                  (double *)(w + off[5]), (int32_t *)(w + off[6]), (double *)(w + off[7]),
+                                                  reftrack_new, normvec_new, n_pts_new);
+    rc = check_cuda("iqp_new_reftrack_kernel");
+    if (rc) return rc;
+    // splines of the new reference line without distance scaling -> new normal vectors
+    mc::calc_splines_kernel<<<B, 256, mc::spline_smem(mc::calc_splines_kernel, n_max_new), s>>>(
+        n_max_new, n_pts_new, reftrack_new, 4, nullptr, 0, nullptr, nullptr, normvec_new, nullptr, spl);
+    return check_cuda("calc_splines_kernel");
+}
+
+int mc_iqp_finish_batch(int B, int n_max, int n_cap, int iter, int iters_min, double curv_error_allowed, int fixed_iters,
+                        int iter_limit, int32_t *active, const int32_t *status, const double *curv_error_max,
+                        const int32_t *n_pts, const double *alpha, const double *reftrack, const double *normvec,
+                        double *fin_alpha, double *fin_reftrack, double *fin_normvec, int32_t *fin_n_pts,
+                        int32_t *fin_outer_iters, int32_t *fin_status, double *fin_curv_error_max, int32_t *counters,
+                        void *stream) {
+    if (B <= 0 || n_max <= 0 || n_cap < n_max || iter < 1 || !active || !status || !curv_error_max || !alpha || !reftrack ||
+        !normvec || !fin_alpha || !fin_reftrack || !fin_normvec || !fin_n_pts || !fin_outer_iters || !fin_status ||
+        !fin_curv_error_max || !counters)
+        return bad("mc_iqp_finish_batch: bad argument");
+    cudaMemsetAsync(counters, 0, 2 * sizeof(int32_t), (cudaStream_t)stream);
+    mc::iqp_finish_kernel<<<B, 256, 0, (cudaStream_t)stream>>>(n_max, n_cap, iter, iters_min, curv_error_allowed, fixed_iters,
+                                                               iter_limit, active, status, curv_error_max, n_pts, alpha, reftrack,
+                                                               normvec, fin_alpha, fin_reftrack, fin_normvec, fin_n_pts,
+                                                               fin_outer_iters, fin_status, fin_curv_error_max, counters);
+    return check_cuda("iqp_finish_kernel");
+}
+
+int mc_scale_alpha_batch(int B, int n_max, double *alpha, const double *scale_batch, double scale, void *stream) {
+    if (B <= 0 || n_max <= 0 || !alpha) return bad("mc_scale_alpha_batch: bad argument");
+    mc::for_grid_y_chunks(B, [&](int b0, int nb) {
+        dim3 grid((n_max + 255) / 256, nb);
+        mc::scale_alpha_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(n_max, alpha + (size_t)b0 * n_max,
+                                                                       scale_batch ? scale_batch + b0 : nullptr, scale);
+    });
+    return check_cuda("scale_alpha_kernel");
+}
+
+// ------------------------------------------------------------------------------------------------
+size_t mc_create_raceline_adjoint_workspace_bytes(int B, int n_max) {
+    if (B <= 0 || n_max < 3) return 0;
+    return align256((size_t)B * (mc::S_NUM + mc::G_NUM) * mc::spl_np(n_max) * sizeof(double));
+}
+
+int mc_create_raceline_adjoint_batch(int B, int n_max, const int32_t *n_pts, const double *normvec, const double *alpha,
+                                     int n_out_max, const double *coeffs_x, const double *coeffs_y,
+                                     const double *spline_lengths, const int32_t *n_out, const int32_t *spline_inds,
+                                     const double *t_values, const double *grad_raceline, const double *grad_kappa,
+                                     const double *grad_el_lengths, double *grad_alpha, double *grad_refline,
+                                     double *grad_normvec, void *workspace, size_t workspace_bytes, void *stream) {
+    if (B <= 0 || n_max < 3 || n_out_max < 1 || !normvec || !alpha || !coeffs_x || !coeffs_y || !spline_lengths ||
+        !n_out || !spline_inds || !t_values || !grad_alpha)
+        return bad("mc_create_raceline_adjoint_batch: bad argument");
+    if (B > 65535 * 1024) return bad("mc_create_raceline_adjoint_batch: too many tracks in one call");
+    if (!workspace || workspace_bytes < mc_create_raceline_adjoint_workspace_bytes(B, n_max))
+        return small_workspace("mc_create_raceline_adjoint_batch");
+    mc::CraAdjArgs a;
+    a.n_max = n_max; a.n_out_max = n_out_max; a.n_pts = n_pts; a.n_out = n_out;
+    a.spline_inds = spline_inds; a.normvec = normvec; a.alpha = alpha; a.coeffs_x = coeffs_x; a.coeffs_y = coeffs_y;
+    a.spline_lengths = spline_lengths; a.t_values = t_values; a.g_raceline = grad_raceline; a.g_kappa = grad_kappa;
+    a.g_el = grad_el_lengths; a.g_alpha = grad_alpha; a.g_refline = grad_refline; a.g_normvec = grad_normvec;
+    a.ws = (double *)workspace;
+    mc::create_raceline_adjoint_kernel<<<B, 256, mc::spline_smem(mc::create_raceline_adjoint_kernel, n_max),
+                                         (cudaStream_t)stream>>>(a);
+    return check_cuda("create_raceline_adjoint_kernel");
+}
+
+}  // extern "C"

@@ -8,6 +8,7 @@
 //   out[v][i][2+s]  = base[c][i][2+s] * (1 + rel * g_s(i / n)),   g_s(u) = (1/3) sum_{k=0..2} a_k cos(2 pi (k+1) u + p_k)
 // with a_k in [-1, 1), p_k in [0, 2 pi) drawn from splitmix64(seed[v], s, k): the same stateless hash is implemented in
 // numpy (synth.jitter_widths_hash), so the CPU baseline and the tests see the same variants (cos differs by an ulp).
+#include "capi.cuh"
 #include "common.cuh"
 
 namespace mc {
@@ -89,15 +90,28 @@ polygon_length_kernel(int n_max, const int32_t *__restrict__ n_pts, const double
     if (threadIdx.x == 0) length[b] = (n > 1) ? acc : 0.0;
 }
 
-void launch_polygon_length(int B, int n_max, const int32_t *n_pts, const double *pts, int stride, const double *normvec,
-                           const double *shift, int shift_stride, double sign, double *length, cudaStream_t stream) {
-    polygon_length_kernel<<<B, 256, 0, stream>>>(n_max, n_pts, pts, stride, normvec, shift, shift_stride, sign, length);
-}
-
-void launch_jitter_widths(int V, int n_max, const int32_t *n_pts_base, int n_base, const double *base,
-                          const int32_t *centre_id, const int64_t *seed, double rel, double *out, int32_t *n_pts_out,
-                          cudaStream_t stream) {
-    jitter_widths_kernel<<<V, 256, 0, stream>>>(V, n_max, n_pts_base, n_base, base, centre_id, seed, rel, out, n_pts_out);
-}
-
 }  // namespace mc
+
+extern "C" {
+
+int mc_polygon_length_batch(int B, int n_max, const int32_t *n_pts, const double *pts, int stride, const double *normvec,
+                            const double *shift, int shift_stride, double sign, double *length, void *stream) {
+    if (B <= 0 || n_max <= 0 || !pts || stride < 2 || !length || ((normvec == nullptr) != (shift == nullptr)) ||
+        (shift && shift_stride < 1))
+        return bad("mc_polygon_length_batch: bad argument");
+    mc::polygon_length_kernel<<<B, 256, 0, (cudaStream_t)stream>>>(n_max, n_pts, pts, stride, normvec, shift, shift_stride,
+                                                                   sign, length);
+    return check_cuda("polygon_length_kernel");
+}
+
+int mc_jitter_widths_batch(int V, int n_max, const int32_t *n_pts_base, int n_base, const double *base,
+                           const int32_t *centre_id, const int64_t *seed, double rel, double *out, int32_t *n_pts_out,
+                           void *stream) {
+    if (V <= 0 || n_max <= 0 || n_base <= 0 || !base || !seed || !out || !(rel >= 0.0) || rel >= 1.0)
+        return bad("mc_jitter_widths_batch: bad argument");
+    mc::jitter_widths_kernel<<<V, 256, 0, (cudaStream_t)stream>>>(V, n_max, n_pts_base, n_base, base, centre_id, seed, rel, out,
+                                                                  n_pts_out);
+    return check_cuda("jitter_widths_kernel");
+}
+
+}  // extern "C"

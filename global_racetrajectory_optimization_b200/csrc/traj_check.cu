@@ -9,17 +9,15 @@
 // brute-force minimum the reference runs as a Python loop over numpy rows.  One thread per trajectory point keeps its
 // four corners in registers; boundary points are staged through shared memory in tiles and read as broadcasts, so the
 // kernel is bound by the fp64 pipe (5 DADD/DMUL + 1 min per corner-point pair), not by memory.
+#include "capi.cuh"
 #include "common.cuh"
 #include "traj_check_core.cuh"
-#include "../../include/mincurv_b200.h"
 
 namespace mc {
 
 constexpr int IT_THREADS = 256;
 constexpr int MB_THREADS = 128;
 constexpr int MB_TILE = 512;
-
-size_t interp_track_ws_doubles(int n_max) { return (size_t)n_max + 1; }
 
 // ---- interp_track -------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(IT_THREADS) interp_track_kernel(int B, int n_max, const int32_t *n_pts, const double *pts,
@@ -67,13 +65,6 @@ __global__ void __launch_bounds__(IT_THREADS) interp_track_kernel(int B, int n_m
         orow[4 * (size_t)j + 2] = plain4 ? tc::interp_closed(d, dc, c2) : 0.0;
         orow[4 * (size_t)j + 3] = plain4 ? tc::interp_closed(d, dc, c3) : 0.0;
     }
-}
-
-void launch_interp_track(int B, int n_max, const int32_t *n_pts, const double *pts, int stride, const double *normvec,
-                         double sign, int width_col, double stepsize, int n_out_max, double *out, int32_t *n_out, double *ws,
-                         cudaStream_t stream) {
-    interp_track_kernel<<<B, IT_THREADS, 0, stream>>>(B, n_max, n_pts, pts, stride, normvec, sign, width_col, stepsize,
-                                                      n_out_max, out, n_out, ws);
 }
 
 // ---- calc_min_bound_dists -----------------------------------------------------------------------------------------
@@ -124,19 +115,6 @@ __global__ void __launch_bounds__(MB_THREADS) min_bound_dists_kernel(int n_traj_
     if (live) min_dists[(size_t)b * n_traj_max + i] = sqrt(best);
 }
 
-void launch_min_bound_dists(int B, int n_traj_max, const int32_t *n_traj, const double *xy, const double *psi, int nb_max1,
-                            const int32_t *nb1, const double *bound1, int nb_max2, const int32_t *nb2, const double *bound2,
-                            int bstride, double length_veh, double width_veh, double *min_dists, cudaStream_t stream) {
-    for_grid_y_chunks(B, [&](int b0, int nb) {
-        const size_t ot = (size_t)b0 * n_traj_max;
-        dim3 grid((n_traj_max + MB_THREADS - 1) / MB_THREADS, nb);
-        min_bound_dists_kernel<<<grid, MB_THREADS, 0, stream>>>(
-            n_traj_max, n_traj ? n_traj + b0 : nullptr, xy + 2 * ot, psi + ot, nb_max1, nb1 ? nb1 + b0 : nullptr,
-            bound1 + (size_t)b0 * nb_max1 * bstride, nb_max2, nb2 ? nb2 + b0 : nullptr, bound2 + (size_t)b0 * nb_max2 * bstride,
-            bstride, length_veh, width_veh, min_dists + ot);
-    });
-}
-
 // ---- extrema tested by check_traj ---------------------------------------------------------------------------------
 // extrema[b][0..7] = min(min_dists), max |kappa|, max ay, max ax_wo_drag, min ax_wo_drag, max a_tot, max vx, n points
 __global__ void __launch_bounds__(256) traj_extrema_kernel(int n_max, const int32_t *n_traj, const double *kappa,
@@ -171,11 +149,6 @@ __global__ void __launch_bounds__(256) traj_extrema_kernel(int n_max, const int3
     }
 }
 
-void launch_traj_extrema(int B, int n_max, const int32_t *n_traj, const double *kappa, const double *vx, const double *ax,
-                         const double *min_dists, double dragcoeff, double mass_veh, double *extrema, cudaStream_t stream) {
-    traj_extrema_kernel<<<B, 256, 0, stream>>>(n_max, n_traj, kappa, vx, ax, min_dists, dragcoeff, mass_veh, extrema);
-}
-
 // ---- trajectory_opt / traj_race_cl --------------------------------------------------------------------------------
 // traj[b][j][0..6] = s, x, y, psi, kappa, vx, ax for j < n; row n = row 0 with s = sum(spline_lengths) (closed race
 // trajectory); rows beyond stay untouched.
@@ -203,13 +176,6 @@ __global__ void __launch_bounds__(256) assemble_trajectory_kernel(int n_max, con
     }
 }
 
-void launch_assemble_trajectory(int B, int n_max, const int32_t *n_traj, const double *s, const double *xy, const double *psi,
-                                const double *kappa, const double *vx, const double *ax, int n_spl_max, const int32_t *n_spl,
-                                const double *spline_lengths, double *traj, cudaStream_t stream) {
-    assemble_trajectory_kernel<<<B, 256, 0, stream>>>(n_max, n_traj, s, xy, psi, kappa, vx, ax, n_spl_max, n_spl,
-                                                      spline_lengths, traj);
-}
-
 // ---- tph.check_normals_crossing (prep_track.py:57-59) -------------------------------------------------------------
 // crossing[b] = 1 if any two normals within `horizon` points of each other cross inside the track (0 otherwise)
 __global__ void __launch_bounds__(128) normals_crossing_kernel(int n_max, const int32_t *n_pts, const double *track,
@@ -222,14 +188,78 @@ __global__ void __launch_bounds__(128) normals_crossing_kernel(int n_max, const 
         atomicOr(crossing + b, 1);
 }
 
-void launch_normals_crossing(int B, int n_max, const int32_t *n_pts, const double *track, const double *normvec, int horizon,
-                             int32_t *crossing, cudaStream_t stream) {
-    cudaMemsetAsync(crossing, 0, (size_t)B * sizeof(int32_t), stream);
-    for_grid_y_chunks(B, [&](int b0, int nb) {
-        dim3 grid((n_max + 127) / 128, nb);
-        normals_crossing_kernel<<<grid, 128, 0, stream>>>(n_max, n_pts ? n_pts + b0 : nullptr, track + (size_t)b0 * n_max * 4,
-                                                          normvec + (size_t)b0 * n_max * 2, horizon, crossing + b0);
-    });
+}  // namespace mc
+
+extern "C" {
+
+size_t mc_interp_track_workspace_bytes(int B, int n_max) {
+    if (B <= 0 || n_max < 2) return 0;
+    return align256((size_t)B * ((size_t)n_max + 1) * sizeof(double));
 }
 
-}  // namespace mc
+int mc_interp_track_batch(int B, int n_max, const int32_t *n_pts, const double *pts, int stride, const double *normvec,
+                          double normal_sign, int width_col, double stepsize_approx, int n_out_max, double *out,
+                          int32_t *n_out, void *workspace, size_t workspace_bytes, void *stream) {
+    if (B <= 0 || n_max < 2 || !pts || (stride != 2 && stride != 4) || !(stepsize_approx > 0.0) || n_out_max <= 0 || !out ||
+        !n_out || (normvec && (stride != 4 || (width_col != 2 && width_col != 3))))
+        return bad("mc_interp_track_batch: bad argument");
+    if (!workspace || workspace_bytes < mc_interp_track_workspace_bytes(B, n_max))
+        return small_workspace("mc_interp_track_batch");
+    mc::interp_track_kernel<<<B, mc::IT_THREADS, 0, (cudaStream_t)stream>>>(B, n_max, n_pts, pts, stride, normvec, normal_sign,
+                                                                            normvec ? width_col : 2, stepsize_approx, n_out_max,
+                                                                            out, n_out, (double *)workspace);
+    return check_cuda("interp_track_kernel");
+}
+
+int mc_min_bound_dists_batch(int B, int n_traj_max, const int32_t *n_traj, const double *xy, const double *psi, int nb1_max,
+                             const int32_t *nb1, const double *bound1, int nb2_max, const int32_t *nb2, const double *bound2,
+                             int bound_stride, double length_veh, double width_veh, double *min_dists, void *stream) {
+    if (B <= 0 || n_traj_max <= 0 || !xy || !psi || !bound1 || !bound2 || nb1_max <= 0 || nb2_max <= 0 ||
+        bound_stride < 2 || !min_dists)
+        return bad("mc_min_bound_dists_batch: bad argument");
+    mc::for_grid_y_chunks(B, [&](int b0, int nb) {
+        const size_t ot = (size_t)b0 * n_traj_max;
+        dim3 grid((n_traj_max + mc::MB_THREADS - 1) / mc::MB_THREADS, nb);
+        mc::min_bound_dists_kernel<<<grid, mc::MB_THREADS, 0, (cudaStream_t)stream>>>(
+            n_traj_max, n_traj ? n_traj + b0 : nullptr, xy + 2 * ot, psi + ot, nb1_max, nb1 ? nb1 + b0 : nullptr,
+            bound1 + (size_t)b0 * nb1_max * bound_stride, nb2_max, nb2 ? nb2 + b0 : nullptr,
+            bound2 + (size_t)b0 * nb2_max * bound_stride, bound_stride, length_veh, width_veh, min_dists + ot);
+    });
+    return check_cuda("min_bound_dists_kernel");
+}
+
+int mc_traj_extrema_batch(int B, int n_max, const int32_t *n_traj, const double *kappa, const double *vx, const double *ax,
+                          const double *min_dists, double dragcoeff, double mass_veh, double *extrema, void *stream) {
+    if (B <= 0 || n_max <= 0 || !kappa || !vx || !ax || !extrema || !(mass_veh > 0.0))
+        return bad("mc_traj_extrema_batch: bad argument");
+    mc::traj_extrema_kernel<<<B, 256, 0, (cudaStream_t)stream>>>(n_max, n_traj, kappa, vx, ax, min_dists, dragcoeff, mass_veh,
+                                                                 extrema);
+    return check_cuda("traj_extrema_kernel");
+}
+
+int mc_assemble_trajectory_batch(int B, int n_max, const int32_t *n_traj, const double *s, const double *xy,
+                                 const double *psi, const double *kappa, const double *vx, const double *ax, int n_spl_max,
+                                 const int32_t *n_spl, const double *spline_lengths, double *traj, void *stream) {
+    if (B <= 0 || n_max <= 0 || !s || !xy || !psi || !kappa || !vx || !ax || n_spl_max <= 0 || !spline_lengths || !traj)
+        return bad("mc_assemble_trajectory_batch: bad argument");
+    mc::assemble_trajectory_kernel<<<B, 256, 0, (cudaStream_t)stream>>>(n_max, n_traj, s, xy, psi, kappa, vx, ax, n_spl_max,
+                                                                        n_spl, spline_lengths, traj);
+    return check_cuda("assemble_trajectory_kernel");
+}
+
+int mc_check_normals_crossing_batch(int B, int n_max, const int32_t *n_pts, const double *track, const double *normvec,
+                                    int horizon, int32_t *crossing, void *stream) {
+    if (B <= 0 || n_max < 3 || !track || !normvec || horizon < 1 || !crossing)
+        return bad("mc_check_normals_crossing_batch: bad argument");
+    cudaMemsetAsync(crossing, 0, (size_t)B * sizeof(int32_t), (cudaStream_t)stream);
+    mc::for_grid_y_chunks(B, [&](int b0, int nb) {
+        dim3 grid((n_max + 127) / 128, nb);
+        mc::normals_crossing_kernel<<<grid, 128, 0, (cudaStream_t)stream>>>(n_max, n_pts ? n_pts + b0 : nullptr,
+                                                                            track + (size_t)b0 * n_max * 4,
+                                                                            normvec + (size_t)b0 * n_max * 2, horizon,
+                                                                            crossing + b0);
+    });
+    return check_cuda("normals_crossing_kernel");
+}
+
+}  // extern "C"

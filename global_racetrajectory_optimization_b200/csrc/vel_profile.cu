@@ -8,16 +8,14 @@
 // The ggv / machine tables (a few dozen rows) are staged in shared memory once per CTA.
 // Bound: latency of the sequential fp64 recurrences (div/sqrt chains), hidden by P >> resident threads; the
 // streaming traffic is 5 workspace vectors x a handful of passes.
+#include "capi.cuh"
 #include "common.cuh"
 #include "vel_profile_core.cuh"
-#include "../../include/mincurv_b200.h"
 
 namespace mc {
 
 constexpr int VP_TAB_MAX = 256;      // rows of the ggv / ax_max_machines tables held in shared memory
 constexpr int VP_VECS = 5;           // R, EL, MU, V, W
-
-size_t vel_profile_ws_doubles(int n_max) { return (size_t)VP_VECS * n_max; }
 
 struct VpArgs {
     int B, V, n_max;
@@ -74,33 +72,12 @@ __global__ void __launch_bounds__(128, 5) vel_profile_kernel(const VpArgs a) {
     if (a.status) a.status[p] = st;
 }
 
-int launch_vel_profile(int B, int V, int n_max, const int32_t *n_pts, const double *kappa, const double *el,
-                       const double *mu, const double *ggv_scale, const double *v_max_batch, double v_max, int n_ggv,
-                       const double *ggv, int n_mach, const double *mach, double dyn_model_exp, double drag_coeff,
-                       double m_veh, int filt_window, int decel_slice_upper, double *vx, double *ax, double *t, double *laptime,
-                       int32_t *status, double *ws, cudaStream_t stream) {
-    if (n_ggv > VP_TAB_MAX || n_mach > VP_TAB_MAX) return -1;
-    VpArgs a;
-    a.B = B; a.V = V; a.n_max = n_max; a.n_pts = n_pts; a.kappa = kappa; a.el = el; a.mu = mu;
-    a.ggv_scale = ggv_scale; a.v_max_batch = v_max_batch; a.v_max = v_max; a.n_ggv = n_ggv; a.n_mach = n_mach;
-    a.ggv = ggv; a.mach = mach;
-    a.pr.dyn_model_exp = dyn_model_exp; a.pr.drag_coeff = drag_coeff; a.pr.m_veh = m_veh; a.pr.filt_window = filt_window;
-    a.pr.decel_slice_upper = decel_slice_upper;
-    a.vx = vx; a.ax = ax; a.t = t; a.laptime = laptime; a.status = status; a.ws = ws;
-    const size_t P = (size_t)B * V;
-    const int threads = 128;
-    vel_profile_kernel<<<(unsigned)((P + threads - 1) / threads), threads, 0, stream>>>(a);
-    return 0;
-}
-
 // ------------------------------------------------------------------------------------------------
 // K5d -- the adjoint of K5 for V = 1 (vel_profile_core.cuh: profile_adjoint_thread).  One thread per profile, like K5;
 // the forward is run again with the tape recorder, so the entry takes the forward's inputs only.  Workspace per profile:
 // the 9 vectors R, EL, V, W, V0, D, GV, GR, GE, the 4 step tapes CF, CB, KF, KB of 2 n_max entries and one scalar,
 // interleaved over the profiles ([vector][i][p]) like K5's.
 constexpr int VPA_VECS = 17;         // in units of n_max entries
-
-size_t vel_profile_adjoint_ws_doubles(int n_max) { return (size_t)VPA_VECS * n_max + 1; }
 
 struct VpAdjArgs {
     int B, n_max;
@@ -154,23 +131,6 @@ __global__ void __launch_bounds__(128) vel_profile_adjoint_kernel(const VpAdjArg
     a.grad_status[p] = st;
 }
 
-int launch_vel_profile_adjoint(int B, int n_max, const int32_t *n_pts, const double *kappa, const double *el, double v_max,
-                               int n_ggv, const double *ggv, int n_mach, const double *mach, double dyn_model_exp,
-                               double drag_coeff, double m_veh, int filt_window, int decel_slice_upper, const double *g_lap,
-                               const double *g_vx, double *g_kappa, double *g_el, int32_t *grad_status, double *ws,
-                               cudaStream_t stream) {
-    if (n_ggv > VP_TAB_MAX || n_mach > VP_TAB_MAX) return -1;
-    VpAdjArgs a;
-    a.B = B; a.n_max = n_max; a.n_pts = n_pts; a.kappa = kappa; a.el = el; a.v_max = v_max;
-    a.n_ggv = n_ggv; a.n_mach = n_mach; a.ggv = ggv; a.mach = mach;
-    a.pr.dyn_model_exp = dyn_model_exp; a.pr.drag_coeff = drag_coeff; a.pr.m_veh = m_veh; a.pr.filt_window = filt_window;
-    a.pr.decel_slice_upper = decel_slice_upper;
-    a.g_lap = g_lap; a.g_vx = g_vx; a.g_kappa = g_kappa; a.g_el = g_el; a.grad_status = grad_status; a.ws = ws;
-    const int threads = 128;
-    vel_profile_adjoint_kernel<<<(unsigned)((B + threads - 1) / threads), threads, 0, stream>>>(a);
-    return 0;
-}
-
 // stand-alone calc_ax_profile / calc_t_profile: one thread per profile, rows contiguous
 __global__ void __launch_bounds__(128) ax_t_profile_kernel(int P, int n_max, const int32_t *n_pts, const double *vx,
                                                            int vx_pitch, const double *el, const double *ax_in,
@@ -184,11 +144,97 @@ __global__ void __launch_bounds__(128) ax_t_profile_kernel(int P, int n_max, con
                     t_out ? t_out + (size_t)p * (n_max + 1) : nullptr);
 }
 
-void launch_ax_t_profile(int P, int n_max, const int32_t *n_pts, const double *vx, int vx_pitch, const double *el,
-                         const double *ax_in, double t_start, double *ax_out, double *t_out, cudaStream_t stream) {
-    const int threads = 128;
-    ax_t_profile_kernel<<<(P + threads - 1) / threads, threads, 0, stream>>>(P, n_max, n_pts, vx, vx_pitch, el, ax_in,
-                                                                            t_start, ax_out, t_out);
+}  // namespace mc
+
+extern "C" {
+
+size_t mc_vel_profile_workspace_bytes(int B, int V, int n_max) {
+    if (B <= 0 || V <= 0 || n_max < 2) return 0;
+    return align256((size_t)B * V * mc::VP_VECS * n_max * sizeof(double));
 }
 
-}  // namespace mc
+int mc_vel_profile_batch(int B, int n_max, const int32_t *n_pts, const double *kappa, const double *el_lengths,
+                         const double *mu, int V, const double *ggv_scale, const double *v_max_batch, double v_max,
+                         int n_ggv, const double *ggv, int n_mach, const double *ax_max_machines, double dyn_model_exp,
+                         double drag_coeff, double m_veh, int filt_window, double *vx, double *ax, double *t,
+                         double *laptime, int32_t *status, void *workspace, size_t workspace_bytes, void *stream) {
+    return mc_vel_profile_batch_ex(B, n_max, n_pts, kappa, el_lengths, mu, V, ggv_scale, v_max_batch, v_max, n_ggv, ggv, n_mach,
+                                   ax_max_machines, dyn_model_exp, drag_coeff, m_veh, filt_window, MC_VP_DECEL_SLICE_UPPER_DEFAULT,
+                                   vx, ax, t, laptime, status, workspace, workspace_bytes, stream);
+}
+
+int mc_vel_profile_batch_ex(int B, int n_max, const int32_t *n_pts, const double *kappa, const double *el_lengths,
+                            const double *mu, int V, const double *ggv_scale, const double *v_max_batch, double v_max,
+                            int n_ggv, const double *ggv, int n_mach, const double *ax_max_machines, double dyn_model_exp,
+                            double drag_coeff, double m_veh, int filt_window, int decel_slice_upper, double *vx, double *ax,
+                            double *t, double *laptime, int32_t *status, void *workspace, size_t workspace_bytes,
+                            void *stream) {
+    if (B <= 0 || V <= 0 || n_max < 2 || !kappa || !el_lengths || !ggv || !ax_max_machines || !laptime || n_ggv < 1 ||
+        n_mach < 1 || !(m_veh > 0.0) || !(dyn_model_exp > 0.0) || (!v_max_batch && !(v_max > 0.0)))
+        return bad("mc_vel_profile_batch: bad argument");
+    if (filt_window > 1 && (filt_window % 2 == 0 || filt_window >= n_max))
+        return bad("mc_vel_profile_batch: filt_window must be odd (tph: 'Window width of moving average filter must be odd!')");
+    if ((size_t)B * V > (size_t)0x7fffffff - 256) return bad("mc_vel_profile_batch: too many profiles in one call");
+    if (!workspace || workspace_bytes < mc_vel_profile_workspace_bytes(B, V, n_max))
+        return small_workspace("mc_vel_profile_batch");
+    if (n_ggv > mc::VP_TAB_MAX || n_mach > mc::VP_TAB_MAX)
+        return bad("mc_vel_profile_batch: ggv / ax_max_machines tables are limited to 256 rows");
+    mc::VpArgs a;
+    a.B = B; a.V = V; a.n_max = n_max; a.n_pts = n_pts; a.kappa = kappa; a.el = el_lengths; a.mu = mu;
+    a.ggv_scale = ggv_scale; a.v_max_batch = v_max_batch; a.v_max = v_max; a.n_ggv = n_ggv; a.n_mach = n_mach;
+    a.ggv = ggv; a.mach = ax_max_machines;
+    a.pr.dyn_model_exp = dyn_model_exp; a.pr.drag_coeff = drag_coeff; a.pr.m_veh = m_veh; a.pr.filt_window = filt_window;
+    a.pr.decel_slice_upper = decel_slice_upper != 0;
+    a.vx = vx; a.ax = ax; a.t = t; a.laptime = laptime; a.status = status; a.ws = (double *)workspace;
+    const size_t P = (size_t)B * V;
+    const int threads = 128;
+    mc::vel_profile_kernel<<<(unsigned)((P + threads - 1) / threads), threads, 0, (cudaStream_t)stream>>>(a);
+    return check_cuda("vel_profile_kernel");
+}
+
+size_t mc_vel_profile_adjoint_workspace_bytes(int B, int n_max) {
+    if (B <= 0 || n_max < 2) return 0;
+    return align256((size_t)B * ((size_t)mc::VPA_VECS * n_max + 1) * sizeof(double));
+}
+
+int mc_vel_profile_adjoint_batch(int B, int n_max, const int32_t *n_pts, const double *kappa, const double *el_lengths,
+                                 double v_max, int n_ggv, const double *ggv, int n_mach, const double *ax_max_machines,
+                                 double dyn_model_exp, double drag_coeff, double m_veh, int filt_window,
+                                 int decel_slice_upper, const double *grad_laptime, const double *grad_vx,
+                                 double *grad_kappa, double *grad_el_lengths, int32_t *grad_status,
+                                 void *workspace, size_t workspace_bytes, void *stream) {
+    if (B <= 0 || n_max < 2 || !kappa || !el_lengths || !ggv || !ax_max_machines || !grad_status || n_ggv < 1 ||
+        n_mach < 1 || !(m_veh > 0.0) || !(dyn_model_exp > 0.0) || !(v_max > 0.0))
+        return bad("mc_vel_profile_adjoint_batch: bad argument");
+    if (filt_window > 1 && (filt_window % 2 == 0 || filt_window >= n_max))
+        return bad("mc_vel_profile_adjoint_batch: filt_window must be odd and smaller than n_max");
+    if ((size_t)B > (size_t)0x7fffffff - 256) return bad("mc_vel_profile_adjoint_batch: too many profiles in one call");
+    if (!workspace || workspace_bytes < mc_vel_profile_adjoint_workspace_bytes(B, n_max))
+        return small_workspace("mc_vel_profile_adjoint_batch");
+    if (n_ggv > mc::VP_TAB_MAX || n_mach > mc::VP_TAB_MAX)
+        return bad("mc_vel_profile_adjoint_batch: ggv / ax_max_machines tables are limited to 256 rows");
+    mc::VpAdjArgs a;
+    a.B = B; a.n_max = n_max; a.n_pts = n_pts; a.kappa = kappa; a.el = el_lengths; a.v_max = v_max;
+    a.n_ggv = n_ggv; a.n_mach = n_mach; a.ggv = ggv; a.mach = ax_max_machines;
+    a.pr.dyn_model_exp = dyn_model_exp; a.pr.drag_coeff = drag_coeff; a.pr.m_veh = m_veh; a.pr.filt_window = filt_window;
+    a.pr.decel_slice_upper = decel_slice_upper != 0;
+    a.g_lap = grad_laptime; a.g_vx = grad_vx; a.g_kappa = grad_kappa; a.g_el = grad_el_lengths; a.grad_status = grad_status;
+    a.ws = (double *)workspace;
+    const int threads = 128;
+    mc::vel_profile_adjoint_kernel<<<(unsigned)((B + threads - 1) / threads), threads, 0, (cudaStream_t)stream>>>(a);
+    return check_cuda("vel_profile_adjoint_kernel");
+}
+
+int mc_calc_ax_t_profile_batch(int P, int n_max, const int32_t *n_pts, const double *vx, int vx_pitch,
+                               const double *el_lengths, const double *ax_in, double t_start, double *ax_out,
+                               double *t_out, void *stream) {
+    if (P <= 0 || n_max < 1 || !vx || !el_lengths || (!ax_out && !t_out) || vx_pitch < n_max + (ax_in ? 0 : 1))
+        return bad("mc_calc_ax_t_profile_batch: bad argument");
+    const int threads = 128;
+    mc::ax_t_profile_kernel<<<(P + threads - 1) / threads, threads, 0, (cudaStream_t)stream>>>(P, n_max, n_pts, vx, vx_pitch,
+                                                                                              el_lengths, ax_in, t_start,
+                                                                                              ax_out, t_out);
+    return check_cuda("ax_t_profile_kernel");
+}
+
+}  // extern "C"

@@ -41,8 +41,9 @@ ASM_TOL = dict(band=5e-12, f=1e-10, kref=1e-10, xp=4e-12)
 # (against mincurv_ref.periodic_spline); f = E^T k_ref carries it.  Measured: f 3.6e-10, k_ref 7.1e-11.
 ASM_TOL_1_20 = dict(f=2e-9, kref=5e-10)
 # KKT certificate of a device solution (mincurv_ref.kkt_certificate with the oracle's H, f, E, k_ref).  The solver stops
-# at mu <= 1e-10 mu0 (box phase) / 1e-11 mu0 (curvature-row phase) and |r_d| <= 1e-8 (|f| + |g0|) (capi.cu); the
-# multipliers of the constraints the certificate treats as inactive are ~mu / slack.  Measured on an H100 over B and C:
+# at mu <= 1e-10 mu0 (box phase) / 1e-11 mu0 (curvature-row phase) and |r_d| <= 1e-8 (|f| + |g0|)
+# (mincurv_ipm.cu); the multipliers of the constraints the certificate treats as inactive are ~mu / slack.  Measured on an
+# H100 over B and C:
 # stationarity 8.3e-7 (synth333_kappa), complementarity 4.0e-10 (the collapsed-box instance of C).
 CERT_STAT_TOL = 8e-6
 CERT_COMP_TOL = 4e-9

@@ -138,13 +138,36 @@ def test_opt_shortest_path_diff_calls_both_entries_with_their_declared_arity(fak
         B_.opt_shortest_path_diff(rt, nv[:, :-1], 2.0)
 
 
-def test_the_public_header_keeps_its_symbol_set():
-    """Every entry point capi.cu defines is declared in the public header (the table load() binds), and no header of the
-    kernels declares one."""
-    block = _lib._c_source(os.path.join(build.CSRC, "capi.cu")).split('extern "C" {', 1)[1]
-    defined = re.findall(r"^\w[\w \t*]*?\b(mc_\w+)\s*\([^)]*\)\s*\{", block, flags=re.M)
-    assert sorted(defined) == sorted(_lib.EXPORTED_SYMBOLS)
+def _kernel_sources():
+    return {os.path.basename(p): _lib._c_source(p) for p in sorted(glob.glob(os.path.join(build.CSRC, "*.cu")))}
+
+
+def test_the_kernel_files_define_each_header_entry_once():
+    """Every entry point is defined once, in the extern "C" block of the kernel file that launches its kernels, and the
+    defined set is the one the public header declares (the table load() binds); no header of the kernels declares one."""
+    where = {}
+    for name, src in _kernel_sources().items():
+        for block in src.split('extern "C" {')[1:]:
+            for sym in re.findall(r"^\w[\w \t*]*?\b(mc_\w+)\s*\([^)]*\)\s*\{", block, flags=re.M):
+                where.setdefault(sym, []).append(name)
+    assert {sym: files for sym, files in where.items() if len(files) != 1} == {}
+    assert sorted(where) == sorted(_lib.EXPORTED_SYMBOLS)
     kernel_headers = glob.glob(os.path.join(build.CSRC, "*.h")) + glob.glob(os.path.join(build.CSRC, "*.cuh"))
     assert kernel_headers
     for path in kernel_headers:
         assert not re.findall(r"\bmc_\w+\s*\(", _lib._c_source(path)), path
+
+
+def test_no_source_declares_a_function_it_does_not_define():
+    """A prototype in a .cu file of a function defined in another one is never compared with its definition by the
+    compiler (a drifted type shows only when the library is loaded, swapped arguments of one type never): calls between
+    the sources go through the mc_ entries of the public header."""
+    prototype = re.compile(r"^[A-Za-z_][\w \t*&:<>,]*?\b(\w+)\s*\([^;{}]*\)\s*;", re.M)
+    definition = re.compile(r"\b(\w+)\s*\([^;{}]*\)\s*(?:const\s*)?\{")
+    undefined = {}
+    for name, src in _kernel_sources().items():
+        declared = set(prototype.findall(src)) - {"static_assert"}
+        missing = sorted(declared - set(definition.findall(src)))
+        if missing:
+            undefined[name] = missing
+    assert undefined == {}
