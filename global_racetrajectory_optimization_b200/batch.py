@@ -817,7 +817,7 @@ def vel_profile_batch(kappa: torch.Tensor, el_lengths: torch.Tensor, ggv, ax_max
                    vmax_t, v_scalar, int(ggv_t.shape[0]), ggv_t, int(mach_t.shape[0]), mach_t, float(dyn_model_exp),
                    float(drag_coeff), float(m_veh), fw,
                    int(VP_DECEL_SLICE_UPPER if decel_slice_upper is None else decel_slice_upper),
-                   *map(_rows, (vx, ax, t, laptime, status)))
+                   *map(_rows, (vx, ax, t, laptime, status)), None, None, None, None)
     out = dict(laptime=laptime, status=status)
     if want_profiles:
         out.update(vx=vx, ax=ax, t=t)
@@ -899,21 +899,105 @@ def vel_profile_diff(kappa: torch.Tensor, el_lengths: torch.Tensor, ggv, ax_max_
     return dict(laptime=laptime, vx=vx, ax=ax, t=t, status=status, grad_status=grad_status)
 
 
+def _lap_time_variants(ggv_scales, top_speeds):
+    """(top speed [V], ggv scale [V], T, S): the V = T * S variants of the lap-time matrix in its order, variant
+    v = (top-speed index) * S + (scale index)."""
+    ts = torch.as_tensor(top_speeds, dtype=torch.float64).reshape(-1)
+    gs = torch.as_tensor(ggv_scales, dtype=torch.float64).reshape(-1)
+    return ts.repeat_interleave(gs.numel()), gs.repeat(ts.numel()), ts.numel(), gs.numel()
+
+
 def lap_time_matrix_batch(kappa: torch.Tensor, el_lengths: torch.Tensor, ggv, ax_max_machines, ggv_scales, top_speeds,
                           drag_coeff: float, m_veh: float, dyn_model_exp: float = 1.0,
                           filt_window: Optional[int] = None, n_pts: Optional[torch.Tensor] = None) -> torch.Tensor:
     """The lap-time matrix of main_globaltraj.py:442-496 for every track of the batch in one launch:
     returns [B, len(top_speeds), len(ggv_scales)] lap times (top speeds in m/s)."""
-    ts = torch.as_tensor(top_speeds, dtype=torch.float64).reshape(-1)
-    gs = torch.as_tensor(ggv_scales, dtype=torch.float64).reshape(-1)
-    vm = ts.repeat_interleave(gs.numel())
-    sc = gs.repeat(ts.numel())
+    vm, sc, T, S = _lap_time_variants(ggv_scales, top_speeds)
     res = vel_profile_batch(kappa, el_lengths, ggv, ax_max_machines, vm, drag_coeff, m_veh, dyn_model_exp, filt_window,
                             n_pts=n_pts, ggv_scales=sc, want_profiles=False)
     bad_ = res["status"] != 0
     if bool(bad_.any().item()):
         raise RuntimeError("lap_time_matrix_batch: non-finite lap time for %i profile(s)" % int(bad_.sum().item()))
-    return res["laptime"].reshape(kappa.shape[0], ts.numel(), gs.numel())
+    return res["laptime"].reshape(kappa.shape[0], T, S)
+
+
+class _LapTimeMatrixDiff(torch.autograd.Function):
+    """The lap times [B, V] of V (ggv scale, top speed) variants per track as functions of kappa and el_lengths; see
+    lap_time_matrix_diff."""
+
+    @staticmethod
+    def forward(ctx, kappa, el_lengths, n_pts, ggv_t, mach_t, vmax_t, scale_t, drag_coeff, m_veh, dyn_model_exp, fw, dsu,
+                strict):
+        res = vel_profile_batch(kappa, el_lengths, ggv_t, mach_t, vmax_t, drag_coeff, m_veh, dyn_model_exp,
+                                fw if fw > 1 else None, n_pts=n_pts, ggv_scales=scale_t, want_profiles=False,
+                                decel_slice_upper=dsu)
+        laptime, status = res["laptime"], res["status"]
+        grad_status = status.clone()
+        ctx.save_for_backward(kappa, el_lengths, n_pts, ggv_t, mach_t, vmax_t, scale_t, grad_status)
+        ctx.params = (dyn_model_exp, drag_coeff, m_veh, fw, dsu)
+        ctx.strict = strict
+        ctx.mark_non_differentiable(status, grad_status)
+        ctx.set_materialize_grads(False)
+        return laptime, status, grad_status
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, grad_laptime, *_unused):
+        kappa, el_lengths, n_pts, ggv_t, mach_t, vmax_t, scale_t, grad_status = ctx.saved_tensors
+        if grad_laptime is None:
+            return (None,) * 13
+        dyn_model_exp, drag_coeff, m_veh, fw, dsu = ctx.params
+        lib = _lib.load()
+        B, n_max = kappa.shape
+        V = int(scale_t.numel())
+        f64 = dict(dtype=torch.float64, device=kappa.device)
+        grad_laptime = grad_laptime.to(**f64).contiguous()
+        wanted = (grad_laptime != 0).flatten()                  # per profile b * V + v
+        who, cells = "lap_time_matrix_diff: no gradient", " (instance: the cell b * V + v)"
+        _refuse(ctx.strict, wanted, grad_status.flatten(), who, "with a nonzero upstream gradient" + cells)
+        need_k, need_e = ctx.needs_input_grad[:2]
+        gk = torch.empty((B, n_max), **f64) if need_k else None
+        ge = torch.empty((B, n_max), **f64) if need_e else None
+        gs = torch.empty((B, V), dtype=torch.int32, device=kappa.device)
+        chunk = _chunk(B, lib.mc_vel_profile_adjoint_workspace_bytes(V, n_max), kappa.device)
+        chunk = max(1, min(chunk, (2 ** 31 - 1024) // V))
+        ws = _workspace("velprofile_adjoint", lib.mc_vel_profile_adjoint_workspace_bytes(chunk * V, n_max), kappa.device)
+        _launch_chunks("mc_vel_profile_batch_ex", B, chunk, ws, n_max, *map(_rows, (n_pts, kappa, el_lengths)), None, V,
+                       scale_t, vmax_t, 0.0, int(ggv_t.shape[0]), ggv_t, int(mach_t.shape[0]), mach_t, dyn_model_exp,
+                       drag_coeff, m_veh, fw, dsu, None, None, None, None, None, *map(_rows, (grad_laptime, gk, ge, gs)))
+        _refuse(ctx.strict, wanted, gs.flatten(), who, "whose gradient is not finite" + cells)
+        return (gk, ge) + (None,) * 11
+
+
+@_device_guard
+def lap_time_matrix_diff(kappa: torch.Tensor, el_lengths: torch.Tensor, ggv, ax_max_machines, ggv_scales, top_speeds,
+                         drag_coeff: float, m_veh: float, dyn_model_exp: float = 1.0, filt_window: Optional[int] = None,
+                         n_pts: Optional[torch.Tensor] = None, decel_slice_upper: Optional[int] = None,
+                         strict: bool = True) -> dict:
+    """lap_time_matrix_batch with the lap-time matrix differentiable with respect to kappa and el_lengths (autograd).
+
+    Returns dict(laptime, status, grad_status), each [B, len(top_speeds), len(ggv_scales)]: laptime holds the values of
+    lap_time_matrix_batch bit for bit (a non-finite cell is reported in status, not raised) and carries a grad_fn;
+    backward() / torch.autograd.grad give dL/dkappa and dL/del_lengths [B, n_max] (zero beyond n_pts): for each track the
+    sum over its cells, in cell order, of what vel_profile_diff gives for one cell with the ggv scaled by that cell's
+    scale and that cell's top speed (DESIGN.md section 3.12).  The backward runs every profile of the matrix again with a
+    tape (17 n_max + 1 doubles per profile; tracks are chunked by free device memory).
+    grad_status per cell: 0 = the gradient is computed; 3 = a non-finite lap time or gradient; for an inactive slot
+    (n_pts < 2) the forward's status.  strict=True: backward raises if a cell with a nonzero upstream gradient has
+    grad_status != 0; strict=False: such cells add nothing to their track's gradient."""
+    _require_cuda()
+    dev = kappa.device
+    if filt_window is not None and int(filt_window) % 2 != 1:
+        raise RuntimeError("Window width of moving average filter must be odd!")
+    vm, sc, T, S = _lap_time_variants(ggv_scales, top_speeds)
+    kappa_t, el_t = _f64(kappa, "kappa"), _f64(el_lengths, "el_lengths")
+    B = kappa_t.shape[0]
+    laptime, status, grad_status = _LapTimeMatrixDiff.apply(
+        kappa_t, el_t, _npts(n_pts, B, dev), _table(ggv, 3, "ggv", dev), _table(ax_max_machines, 2, "ax_max_machines", dev),
+        vm.to(dev).contiguous(), sc.to(dev).contiguous(), float(drag_coeff), float(m_veh), float(dyn_model_exp),
+        0 if filt_window is None else int(filt_window),
+        int(VP_DECEL_SLICE_UPPER if decel_slice_upper is None else decel_slice_upper), bool(strict))
+    return dict(laptime=laptime.reshape(B, T, S), status=status.reshape(B, T, S), grad_status=grad_status.reshape(B, T, S))
 
 
 @_device_guard

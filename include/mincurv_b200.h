@@ -324,13 +324,27 @@ int mc_vel_profile_batch(int B, int n_max, const int32_t *n_pts, const double *k
                          double dyn_model_exp, double drag_coeff, double m_veh, int filt_window,
                          double *vx, double *ax, double *t, double *laptime, int32_t *status,
                          void *workspace, size_t workspace_bytes, void *stream);
-/* the same with an explicit decel_slice_upper (see MC_VP_DECEL_SLICE_UPPER_DEFAULT) */
+/* The same with an explicit decel_slice_upper (see MC_VP_DECEL_SLICE_UPPER_DEFAULT) and, optionally, the
+ * vector-Jacobian product of the lap times (the lap-time matrix for V > 1; batch.lap_time_matrix_diff, DESIGN.md
+ * section 3.12):
+ *   grad_laptime [B][V] or NULL : NULL => the forward above, nothing else is read or written.  Otherwise the upstream
+ *                                 gradient dL/dlaptime of a loss L, and the call writes only
+ *   grad_kappa [B][n_max] or NULL, grad_el_lengths [B][n_max] or NULL : dL/dkappa, dL/del_lengths, the sum of the V
+ *                                 profiles' gradients of a track in variant order (zero beyond n_pts[b]);
+ *   grad_status [B][V] (required) : per profile, the codes of mc_vel_profile_adjoint_batch below (a profile whose code
+ *                                 is not 0 adds nothing to its track's sum).
+ *   In this mode vx, ax, t, laptime and status are not written (they may be NULL), mu must be NULL (the adjoint has no
+ *   mu), and the forward is run again inside: the other arguments are those of the forward call.
+ * workspace: mc_vel_profile_workspace_bytes(B, V, n_max) for the forward,
+ *            mc_vel_profile_adjoint_workspace_bytes(B * V, n_max) with grad_laptime (the tape of every profile; the
+ *            sum over the variants reads it and needs nothing more) */
 int mc_vel_profile_batch_ex(int B, int n_max, const int32_t *n_pts, const double *kappa, const double *el_lengths,
                             const double *mu, int V, const double *ggv_scale, const double *v_max_batch, double v_max,
                             int n_ggv, const double *ggv, int n_mach, const double *ax_max_machines,
                             double dyn_model_exp, double drag_coeff, double m_veh, int filt_window, int decel_slice_upper,
                             double *vx, double *ax, double *t, double *laptime, int32_t *status,
-                            void *workspace, size_t workspace_bytes, void *stream);
+                            const double *grad_laptime, double *grad_kappa, double *grad_el_lengths,
+                            int32_t *grad_status, void *workspace, size_t workspace_bytes, void *stream);
 
 /* Sensitivities of the lap time (batch.vel_profile_diff; DESIGN.md section 3.12 has the derivation).  The velocity
  * profile (closed track, ggv branch, one profile per track, no mu) is differentiated with respect to kappa and el_lengths
@@ -340,8 +354,8 @@ int mc_vel_profile_batch_ex(int B, int n_max, const int32_t *n_pts, const double
  *   for n_pts[b] < 2 (an inactive slot) the forward's status (0 for n_pts 0, 3 otherwise)
  * Every such instance gets zero gradients.
  *
- * mc_vel_profile_adjoint_workspace_bytes: 17 n_max + 1 doubles per track (the forward's scratch vectors, its tape and
- * the adjoint vectors).
+ * mc_vel_profile_adjoint_workspace_bytes: 17 n_max + 1 doubles per profile (the forward's scratch vectors, its tape and
+ * the adjoint vectors); B here counts profiles (B * V for mc_vel_profile_batch_ex).
  *
  * mc_vel_profile_adjoint_batch: vector-Jacobian product of mc_vel_profile_batch_ex with V = 1 (no ggv scales, no
  * per-variant top speed, no mu): for upstream gradients grad_laptime [B] and grad_vx [B][n_max] (either may be NULL:
