@@ -1224,13 +1224,31 @@ def jitter_widths_batch(base: torch.Tensor, seeds: torch.Tensor, rel: float = 0.
 # ------------------------------------------------------------------------------------------------
 # prep_track front end (SURVEY.md section 8f-2): tph.spline_approximation + min-width inflation + splines + normals check
 # ------------------------------------------------------------------------------------------------
+# n_out[b] of mc_prep_track_batch (include/mincurv_b200.h): >= 0 points; -(points needed) above -PREP_REFUSED for a
+# capacity; -PREP_REFUSED - reason for a refused track
+PREP_REFUSED = 1 << 30
+PREP_REASONS = {
+    1: "n_raw is outside [0, n_raw_max]",
+    2: "fewer than 5 points (raw, or after the pre-interpolation)",
+    3: "a non-finite coordinate, width or length",
+    4: "a point count (length / step) too large to hold",
+    5: "the residual budget s_reg is not reached (s_reg >= the residual of the best constant fit, or the root search ran out)",
+    6: "fewer than 3 re-sampled points",
+}
+
+
+def _prep_refuse(b: int, why: str):
+    return ValueError(f"spline_approximation_batch: track {b} is refused: {why}")
+
+
 @_device_guard
 def spline_approximation_batch(track: torch.Tensor, k_reg: int = 3, s_reg: float = 10.0, stepsize_prep: float = 1.0,
                                stepsize_reg: float = 3.0, n_raw: Optional[torch.Tensor] = None,
                                min_width: Optional[float] = None):
     """Batched tph.spline_approximation (+ prep_track's min-width inflation) for imported tracks [B, n_raw_max, 4]
-    (unclosed; n_raw[b] points each).  Returns (reftrack_interp [B, n_out_max, 4], n_pts [B], smoothing_lambda [B]).
-    The smoothing spline is the Reinsch formulation with residual budget s_reg (csrc/prep_track.cu)."""
+    (unclosed; n_raw[b] points each, 0 for an unused slot).  Returns (reftrack_interp [B, n_out_max, 4], n_pts [B],
+    smoothing_lambda [B]).  The smoothing spline is the Reinsch formulation with residual budget s_reg
+    (csrc/prep_track.cu).  A track the kernel cannot smooth raises ValueError naming the track and the reason."""
     _require_cuda()
     lib = _lib.load()
     track = _f64(track, "track")
@@ -1239,7 +1257,23 @@ def spline_approximation_batch(track: torch.Tensor, k_reg: int = 3, s_reg: float
         raise ValueError("track must be [B, n_raw_max, 4]")
     dev = track.device
     n_raw = _npts(n_raw, B, dev)
-    length = float(_closed_polygon_length(track, n_raw).max().item())
+    counts = n_raw.cpu().tolist() if n_raw is not None else [n_raw_max] * B
+    for b, nr in enumerate(counts):            # (the polygon length below reads n_raw[b] rows: check them first)
+        if nr < 0 or nr > n_raw_max:
+            raise _prep_refuse(b, f"n_raw = {nr} is outside [0, {n_raw_max}]")
+        if 0 < nr < 5:
+            raise _prep_refuse(b, f"{nr} raw points, fewer than 5")
+    used = torch.arange(n_raw_max, device=dev)[None, :] < torch.tensor(counts, device=dev)[:, None]
+    nonfinite = ((~torch.isfinite(track)).any(dim=2) & used).any(dim=1)
+    lengths = _closed_polygon_length(track, n_raw)
+    nonfinite |= ~torch.isfinite(lengths)
+    if bool(nonfinite.any()):
+        raise _prep_refuse(int(nonfinite.nonzero()[0, 0]), PREP_REASONS[3])
+    lengths = lengths.cpu().tolist()
+    for b, length in enumerate(lengths):
+        if max(length / float(stepsize_prep), 1.05 * length / float(stepsize_reg), 4.0 * length) + 16 >= PREP_REFUSED:
+            raise _prep_refuse(b, f"{PREP_REASONS[4]} (closed length {length:.6g} m)")
+    length = max(lengths)
     n_int_max = int(math.ceil(length / float(stepsize_prep))) + 8
     n_out_max = int(math.ceil(1.05 * length / float(stepsize_reg))) + 16
     while True:
@@ -1251,12 +1285,13 @@ def spline_approximation_batch(track: torch.Tensor, k_reg: int = 3, s_reg: float
                                      float(stepsize_reg), float(min_width) if min_width is not None else 0.0, n_int_max,
                                      n_out_max, _ptr(out), _ptr(n_out), _ptr(lam), _ptr(ws), ws.numel(), _stream())
         _lib.check(rc, "mc_prep_track_batch")
-        need = int((-n_out).max().item())
+        codes = n_out.cpu().tolist()
+        for b, c in enumerate(codes):
+            if c <= -PREP_REFUSED:
+                raise _prep_refuse(b, PREP_REASONS.get(-PREP_REFUSED - c, f"unknown reason {-PREP_REFUSED - c}"))
+        need = max(-c for c in codes)
         if need <= 0:
             return out, n_out, lam
-        if need + 16 <= min(n_out_max, n_int_max):     # the kernel refused for another reason than capacity
-            raise ValueError("spline_approximation_batch: a track is too short to be smoothed (fewer than 5 points after "
-                             "pre-interpolation)")
         n_out_max = max(n_out_max, need + 16)          # (a curve longer than 1.05 x its polygon, or a tiny capacity)
         n_int_max = max(n_int_max, need + 16)
 

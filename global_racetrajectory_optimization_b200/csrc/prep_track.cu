@@ -128,27 +128,38 @@ prep_track_kernel(int n_raw_max, const int32_t *__restrict__ n_raw_b, const doub
     __shared__ double red[32];
     __shared__ double sh_val[4];
     __shared__ int sh_n[4];
-    if (tid == 0) n_out[b] = 0;
-    if (nr < 5) return;
+    // n_out[b] (include/mincurv_b200.h): >= 0 points, -(points needed) for a capacity, -MC_PREP_REFUSED - reason for a
+    // track refused.  Every refusal is decided from values all threads share, before anything is written to the row.
+    if (tid == 0) { n_out[b] = 0; if (lam_out) lam_out[b] = 0.0; }
+    if (nr == 0) return;                                    // an inactive slot
+    if (nr < 0 || nr > n_raw_max) { if (tid == 0) n_out[b] = -MC_PREP_REFUSED - MC_PREP_R_N_RAW; return; }
+    if (nr < 5) { if (tid == 0) n_out[b] = -MC_PREP_REFUSED - MC_PREP_R_TOO_FEW; return; }
     // ---- 1. cumulative chord length of the closed raw polygon (numpy.cumsum order) ----
     if (tid == 0) {
         double acc = 0.0;
+        bool finite = true;
         dist[0] = 0.0;
         for (int i = 0; i < nr; ++i) {
             const int j = (i + 1 == nr) ? 0 : i + 1;
             const double ex = tr[4 * j] - tr[4 * i], ey = tr[4 * j + 1] - tr[4 * i + 1];
             acc += sqrt(ex * ex + ey * ey);
             dist[i + 1] = acc;
+            finite = finite && isfinite(tr[4 * i + 2]) && isfinite(tr[4 * i + 3]);
         }
-        const int ni = (int)ceil(acc / stepsize_prep) + 1;      // points of the interpolated closed track
-        sh_n[0] = ni;
+        // (a non-finite coordinate makes the length inf or NaN; the counts are compared in double before the conversions)
+        if (!finite || !isfinite(acc)) sh_n[0] = -MC_PREP_REFUSED - MC_PREP_R_NONFINITE;
+        else if (!(ceil(acc / stepsize_prep) + 1.0 < (double)MC_PREP_REFUSED) || !(ceil(acc) * 4.0 < (double)MC_PREP_REFUSED))
+            sh_n[0] = -MC_PREP_REFUSED - MC_PREP_R_COUNT;
+        else sh_n[0] = (int)ceil(acc / stepsize_prep) + 1;     // points of the interpolated closed track
         sh_val[0] = acc;
     }
     __syncthreads();
     const int ni_cl = sh_n[0];
     const double Lraw = sh_val[0];
     const int n = ni_cl - 1;                                // periodic data points
-    if (ni_cl > n_int_max || n < 5) { if (tid == 0) n_out[b] = -ni_cl; return; }
+    if (ni_cl < 0) { if (tid == 0) n_out[b] = ni_cl; return; }
+    if (n < 5) { if (tid == 0) n_out[b] = -MC_PREP_REFUSED - MC_PREP_R_TOO_FEW; return; }
+    if (ni_cl > n_int_max) { if (tid == 0) n_out[b] = -ni_cl; return; }
     // ---- 2. linear pre-interpolation (numpy.linspace / numpy.interp statements) ----
     for (int i = tid; i < ni_cl; i += nt) {
         const double di = (i == ni_cl - 1) ? Lraw : i * (Lraw / (double)(ni_cl - 1));
@@ -192,8 +203,8 @@ prep_track_kernel(int n_raw_max, const int32_t *__restrict__ n_raw_b, const doub
     __syncthreads();
     // ---- 4. smoothing parameter: F(lam) = |lam Q gamma|^2 = s, F increasing; bracket by factors of 16, then the Illinois
     //         variant of regula falsi on log F over log lam ----
-    double lo_l = 1e-12, hi_l = 1.0, f_lo = 0.0, f_hi = 0.0, lam = 1.0;
-    bool have_lo = false, have_hi = false;
+    double lo_l = 1e-12, hi_l = 1.0, f_lo = 0.0, f_hi = 0.0, lam = 1.0, F_last = 0.0;
+    bool have_lo = false, have_hi = false, reached = false;  // reached: the loop ended on its tolerance with a finite F
     int side = 0;
     for (int iter = 0; iter < 200; ++iter) {
         if (!have_hi) lam = hi_l;
@@ -217,6 +228,7 @@ prep_track_kernel(int n_raw_max, const int32_t *__restrict__ n_raw_b, const doub
         }
         const double F = block_reduce<0>(acc, red);
         __syncthreads();
+        F_last = F;
         if (!have_hi) {
             if (F >= s_reg) { have_hi = true; f_hi = F; }
             else { lo_l = hi_l; f_lo = F; have_lo = true; hi_l *= 16.0; if (hi_l > 1e30) break; }
@@ -227,11 +239,16 @@ prep_track_kernel(int n_raw_max, const int32_t *__restrict__ n_raw_b, const doub
             else { hi_l = lo_l; f_hi = F; lo_l /= 16.0; if (lo_l < 1e-300) break; }
             continue;
         }
-        if (fabs(F - s_reg) <= 1e-13 * s_reg || hi_l / lo_l < 1.0 + 4e-16) break;
+        if (fabs(F - s_reg) <= 1e-13 * s_reg || hi_l / lo_l < 1.0 + 4e-16) { reached = isfinite(F); break; }
         if (F < s_reg) { lo_l = lam; f_lo = F; if (side == -1) f_hi = s_reg + 0.5 * (f_hi - s_reg); side = -1; }
         else { hi_l = lam; f_hi = F; if (side == 1) f_lo = s_reg - 0.5 * (s_reg - f_lo); side = 1; }
     }
     if (tid == 0 && lam_out) lam_out[b] = lam;
+    // s_reg >= F(inf) (the residual of the best constant) ends the bracket at lam > 1e30, and a bracket below 1e-300 ends
+    // it too: the budget is not reached and the curve would not be the one asked for.  At the iteration cap (rounding in
+    // F can keep the loop from its 1e-13 tolerance under heavy smoothing) the budget counts as reached within 1e-6 s_reg.
+    if (!reached && have_lo && have_hi && isfinite(F_last) && fabs(F_last - s_reg) <= 1e-6 * s_reg) reached = true;
+    if (!reached) { if (tid == 0) n_out[b] = -MC_PREP_REFUSED - MC_PREP_R_BUDGET; return; }
     // fitted values f = p - lam Q gamma (fy takes the place of bx)
     double *fy = bx;
     __syncthreads();
@@ -256,7 +273,10 @@ prep_track_kernel(int n_raw_max, const int32_t *__restrict__ n_raw_b, const doub
         acc += sqrt((x1 - x0) * (x1 - x0) + (y1 - y0) * (y1 - y0));
     }
     const double Lsm = block_reduce<0>(acc, red);
+    if (!isfinite(Lsm)) { if (tid == 0) n_out[b] = -MC_PREP_REFUSED - MC_PREP_R_NONFINITE; return; }
+    if (!(ceil(Lsm / stepsize_reg) < (double)MC_PREP_REFUSED)) { if (tid == 0) n_out[b] = -MC_PREP_REFUSED - MC_PREP_R_COUNT; return; }
     const int n_reg_cl = (int)ceil(Lsm / stepsize_reg) + 1, n_reg = n_reg_cl - 1;
+    if (n_reg < 3) { if (tid == 0) n_out[b] = -MC_PREP_REFUSED - MC_PREP_R_FEW_OUT; return; }
     if (n_reg > n_out_max) { if (tid == 0) n_out[b] = -n_reg; return; }
     // ---- 6. closest curve point of every point of the closed raw track (tph: fmin from the chord-length guess) ----
     for (int i = tid; i <= nr; i += nt) {

@@ -460,9 +460,21 @@ int mc_jitter_widths_batch(int V, int n_max, const int32_t *n_pts_base, int n_ba
  *   track [B][n_raw_max][4]       : imported tracks x, y, w_tr_right, w_tr_left (unclosed), n_raw[b] points each
  *   n_int_max                     : capacity for the pre-interpolated closed track (>= ceil(length / stepsize_prep) + 1)
  *   min_width                     : <= 0 => no inflation (prep_track's min_width=None)
- *   reftrack_interp [B][n_out_max][4], n_out [B]: the prepared tracks; n_out[b] = -(points needed) if a capacity is too small
- *   smoothing_lambda [B] or NULL  : the smoothing parameter found for every track
+ *   reftrack_interp [B][n_out_max][4], n_out [B]: the prepared tracks, with n_out[b] telling three outcomes apart:
+ *     n_out[b] >= 0                          points written (0: an inactive slot, n_raw[b] == 0)
+ *     -MC_PREP_REFUSED < n_out[b] < 0        a capacity is too small: -(points needed) for n_int_max or n_out_max
+ *     n_out[b] == -MC_PREP_REFUSED - reason  the track is refused (nothing is written to its row), reason one of
+ *                                            MC_PREP_R_*; every count the kernel needs is below MC_PREP_REFUSED
+ *   smoothing_lambda [B] or NULL  : the smoothing parameter found for every track (0 if refused before the fit)
  */
+#define MC_PREP_REFUSED (1 << 30)
+#define MC_PREP_R_N_RAW 1         /* n_raw[b] < 0 or n_raw[b] > n_raw_max */
+#define MC_PREP_R_TOO_FEW 2       /* 1 <= n_raw[b] < 5, or fewer than 5 points after the pre-interpolation */
+#define MC_PREP_R_NONFINITE 3     /* a coordinate or width is inf or NaN, or a length overflows */
+#define MC_PREP_R_COUNT 4         /* a point count (length / step) does not fit below MC_PREP_REFUSED */
+#define MC_PREP_R_BUDGET 5        /* the residual budget s_reg is not reached: s_reg >= F(inf), or the bracket or the
+                                     iteration cap of the root search runs out */
+#define MC_PREP_R_FEW_OUT 6       /* fewer than 3 re-sampled points */
 size_t mc_prep_track_workspace_bytes(int B, int n_raw_max, int n_int_max);
 int mc_prep_track_batch(int B, int n_raw_max, const int32_t *n_raw, const double *track, int k_reg, double s_reg,
                         double stepsize_prep, double stepsize_reg, double min_width, int n_int_max, int n_out_max,
