@@ -127,7 +127,6 @@ def calc_splines_batch(xy: torch.Tensor, n_pts: Optional[torch.Tensor] = None,
 
     xy: [B, n_max, 2] (or a reftrack [B, n_max, 4]); returns (coeffs_x, coeffs_y, normvec, h)."""
     _require_cuda()
-    lib = _lib.load()
     xy = _f64(xy, "xy")
     B, n_max, stride = xy.shape
     dev = xy.device
@@ -138,11 +137,9 @@ def calc_splines_batch(xy: torch.Tensor, n_pts: Optional[torch.Tensor] = None,
     h = torch.ones((B, n_max), dtype=torch.float64, device=dev)
     if el_lengths is not None:
         el_lengths = _f64(el_lengths, "el_lengths")
-    nbytes = lib.mc_calc_splines_workspace_bytes(B, n_max)
-    ws = _workspace("splines", nbytes, dev)
-    rc = lib.mc_calc_splines_batch(B, n_max, _ptr(n_pts), _ptr(xy), stride, _ptr(el_lengths), int(bool(use_dist_scaling)),
-                                   _ptr(cx), _ptr(cy), _ptr(nv), _ptr(h), _ptr(ws), ws.numel(), _stream())
-    _lib.check(rc, "mc_calc_splines_batch")
+    ws = _workspace("splines", _lib.load().mc_calc_splines_workspace_bytes(B, n_max), dev)
+    _call("mc_calc_splines_batch", B, n_max, n_pts, xy, stride, el_lengths, int(bool(use_dist_scaling)), cx, cy, nv, h,
+          ws=ws)
     return cx, cy, nv, h
 
 
@@ -166,17 +163,23 @@ def _rows(t: Optional[torch.Tensor]):
     return lambda s, e: None if t is None else t[s:e]
 
 
+def _call(entry: str, *args, ws: Optional[torch.Tensor] = None) -> None:
+    """Runs the C-ABI entry with args, a tensor passed as its pointer, None as NULL and anything else as it is, followed
+    by the workspace and its size (with ws) and the current stream.  A nonzero return raises MinCurvLibError naming the
+    entry."""
+    c_args = [_ptr(a) if isinstance(a, torch.Tensor) else a for a in args]      # (args holds the tensors until the call)
+    if ws is not None:
+        c_args += [_ptr(ws), ws.numel()]
+    _lib.check(getattr(_lib.load(), entry)(*c_args, _stream()), entry)
+
+
 def _launch_chunks(entry: str, B: int, chunk: int, ws: torch.Tensor, *args) -> None:
-    """Runs the C-ABI entry on chunks of at most chunk of the B instances, with the chunk's size as B.  args are the
-    entry's arguments between B and the workspace: a callable of (s, e) such as _rows gives the argument of the chunk of
-    instances s:e, a tensor is passed as its pointer, None as NULL and anything else as it is.  The workspace, its size
-    and the stream follow."""
-    fn = getattr(_lib.load(), entry)
+    """_call of the entry on chunks of at most chunk of the B instances, with the chunk's size as B.  args are the entry's
+    arguments between B and the workspace: a callable of (s, e) such as _rows gives the argument of the chunk of instances
+    s:e, anything else is passed as _call passes it."""
     for s in range(0, B, chunk):
         e = min(B, s + chunk)
-        chunk_args = [a(s, e) if callable(a) else a for a in args]       # (holds what the callables made until the call)
-        rc = fn(e - s, *(_ptr(a) if isinstance(a, torch.Tensor) else a for a in chunk_args), _ptr(ws), ws.numel(), _stream())
-        _lib.check(rc, entry)
+        _call(entry, e - s, *(a(s, e) if callable(a) else a for a in args), ws=ws)
 
 
 def _mincurv_inputs(tracks: dict, shape_error: str, n_pts, w_veh, centre_id, max_chunk, f_scale) -> SimpleNamespace:
@@ -353,17 +356,14 @@ def opt_shortest_path_batch(reftrack: torch.Tensor, normvec: torch.Tensor, w_veh
                             n_pts: Optional[torch.Tensor] = None) -> dict:
     """Batched tph.opt_shortest_path.  Returns dict(alpha, status, iters)."""
     _require_cuda()
-    lib = _lib.load()
     reftrack, normvec, n_pts, w_scalar, w_batch = _shortest_path_inputs(reftrack, normvec, w_veh, n_pts)
     B, n_max, _ = reftrack.shape
     dev = reftrack.device
     alpha = torch.empty((B, n_max), dtype=torch.float64, device=dev)
     status = torch.empty((B,), dtype=torch.int32, device=dev)
     iters = torch.empty((B,), dtype=torch.int32, device=dev)
-    ws = _workspace("shortest", lib.mc_shortest_path_workspace_bytes(B, n_max), dev)
-    rc = lib.mc_shortest_path_solve_batch(B, n_max, _ptr(n_pts), _ptr(reftrack), _ptr(normvec), w_scalar, _ptr(w_batch),
-                                          _ptr(alpha), _ptr(status), _ptr(iters), _ptr(ws), ws.numel(), _stream())
-    _lib.check(rc, "mc_shortest_path_solve_batch")
+    ws = _workspace("shortest", _lib.load().mc_shortest_path_workspace_bytes(B, n_max), dev)
+    _call("mc_shortest_path_solve_batch", B, n_max, n_pts, reftrack, normvec, w_scalar, w_batch, alpha, status, iters, ws=ws)
     return dict(alpha=alpha, status=status, iters=iters)
 
 
@@ -383,16 +383,13 @@ class _ShortestPathDiff(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, reftrack, normvec, w_veh_t, w_scalar, n_pts, strict):
-        lib = _lib.load()
         B, n_max, _ = reftrack.shape
         f64, i32 = dict(dtype=torch.float64, device=reftrack.device), dict(dtype=torch.int32, device=reftrack.device)
         alpha, status, iters = torch.empty((B, n_max), **f64), torch.empty((B,), **i32), torch.empty((B,), **i32)
         sens, grad_status = torch.empty((B, 2, n_max), **f64), torch.empty((B,), **i32)
-        ws = _workspace("shortest", lib.mc_shortest_path_workspace_bytes(B, n_max), reftrack.device)
-        rc = lib.mc_shortest_path_solve_batch_sens(B, n_max, _ptr(n_pts), _ptr(reftrack), _ptr(normvec), w_scalar,
-                                                   _ptr(w_veh_t), _ptr(alpha), _ptr(status), _ptr(iters), _ptr(sens),
-                                                   _ptr(grad_status), _ptr(ws), ws.numel(), _stream())
-        _lib.check(rc, "mc_shortest_path_solve_batch_sens")
+        ws = _workspace("shortest", _lib.load().mc_shortest_path_workspace_bytes(B, n_max), reftrack.device)
+        _call("mc_shortest_path_solve_batch_sens", B, n_max, n_pts, reftrack, normvec, w_scalar, w_veh_t, alpha, status, iters,
+              sens, grad_status, ws=ws)
         ctx.save_for_backward(reftrack, normvec, w_veh_t, n_pts, alpha, sens, grad_status)
         ctx.w_scalar, ctx.strict = w_scalar, strict
         ctx.mark_non_differentiable(status, iters, grad_status)
@@ -402,7 +399,6 @@ class _ShortestPathDiff(torch.autograd.Function):
     @torch.autograd.function.once_differentiable
     def backward(ctx, grad_alpha, *_unused):
         reftrack, normvec, w_veh_t, n_pts, alpha, sens, grad_status = ctx.saved_tensors
-        lib = _lib.load()
         B, n_max, _ = reftrack.shape
         f64 = dict(dtype=torch.float64, device=reftrack.device)
         grad_alpha = grad_alpha.to(dtype=torch.float64).contiguous()
@@ -414,11 +410,9 @@ class _ShortestPathDiff(torch.autograd.Function):
         grt = torch.empty((B, n_max, 4), **f64)
         gnv = torch.empty((B, n_max, 2), **f64) if need_nv else None
         gwv = torch.empty((B,), **f64) if need_wv else None
-        ws = _workspace("shortest", lib.mc_shortest_path_workspace_bytes(B, n_max), reftrack.device)
-        rc = lib.mc_shortest_path_adjoint_batch(B, n_max, _ptr(n_pts), _ptr(reftrack), _ptr(normvec), ctx.w_scalar,
-                                                _ptr(w_veh_t), _ptr(alpha), _ptr(sens), _ptr(gs), _ptr(grad_alpha), _ptr(grt),
-                                                _ptr(gnv), _ptr(gwv), _ptr(ws), ws.numel(), _stream())
-        _lib.check(rc, "mc_shortest_path_adjoint_batch")
+        ws = _workspace("shortest", _lib.load().mc_shortest_path_workspace_bytes(B, n_max), reftrack.device)
+        _call("mc_shortest_path_adjoint_batch", B, n_max, n_pts, reftrack, normvec, ctx.w_scalar, w_veh_t, alpha, sens, gs,
+              grad_alpha, grt, gnv, gwv, ws=ws)
         _refuse(ctx.strict, wanted, gs, who, "whose adjoint solution is not finite")
         return grt if need_rt else None, gnv, gwv, None, None, None
 
@@ -447,12 +441,9 @@ def _closed_polygon_length(pts: torch.Tensor, n_pts: Optional[torch.Tensor], nor
                            shift: Optional[torch.Tensor] = None, shift_stride: int = 1, sign: float = 1.0) -> torch.Tensor:
     """Length [B] of the closed polygon through the first n_pts[b] points p_i (+ sign * shift_i * n_i) of every row
     (mc_polygon_length_batch: a block reduction per track on the device)."""
-    lib = _lib.load()
     B, n_max, stride = pts.shape
     out = torch.zeros((B,), dtype=torch.float64, device=pts.device)
-    rc = lib.mc_polygon_length_batch(B, n_max, _ptr(n_pts), _ptr(pts), stride, _ptr(normvec), _ptr(shift), int(shift_stride),
-                                     float(sign), _ptr(out), _stream())
-    _lib.check(rc, "mc_polygon_length_batch")
+    _call("mc_polygon_length_batch", B, n_max, n_pts, pts, stride, normvec, shift, int(shift_stride), float(sign), out)
     return out
 
 
@@ -466,12 +457,12 @@ def create_raceline_batch(refline: torch.Tensor, normvec: torch.Tensor, alpha: t
     the polygon length of the shifted line (one small device->host read) and the call is repeated with a larger one if
     a track still does not fit; with an explicit n_out_max an overflow is reported as n_out[b] = -(points needed)."""
     _require_cuda()
-    lib = _lib.load()
     refline = _f64(refline, "refline")
     normvec = _f64(normvec, "normvec")
     alpha = _f64(alpha, "alpha")
     B, n_max, stride = refline.shape
     dev = refline.device
+    f64, i32 = dict(dtype=torch.float64, device=dev), dict(dtype=torch.int32, device=dev)
     n_pts = _npts(n_pts, B, dev)
     derived = n_out_max is None
     if derived:
@@ -479,38 +470,24 @@ def create_raceline_batch(refline: torch.Tensor, normvec: torch.Tensor, alpha: t
         n_out_max = int(math.ceil(float(poly.max().item()) * 1.1 / float(stepsize_interp))) + 16
     n_out_max = int(n_out_max)
     while True:
-        out = _create_raceline_once(lib, refline, normvec, alpha, stepsize_interp, n_pts, n_out_max, with_head_curv)
+        out = dict(       # (in the order of the C-ABI)
+            coeffs_x=torch.zeros((B, n_max, 4), **f64), coeffs_y=torch.zeros((B, n_max, 4), **f64),
+            spline_lengths=torch.zeros((B, n_max), **f64), n_out=torch.zeros((B,), **i32),
+            raceline_interp=torch.zeros((B, n_out_max, 2), **f64), spline_inds=torch.zeros((B, n_out_max), **i32),
+            t_values=torch.zeros((B, n_out_max), **f64), s_interp=torch.zeros((B, n_out_max), **f64),
+            el_lengths_interp=torch.zeros((B, n_out_max), **f64),
+            psi=torch.zeros((B, n_out_max), **f64) if with_head_curv else None,
+            kappa=torch.zeros((B, n_out_max), **f64) if with_head_curv else None,
+        )
+        ws = _workspace("splines", _lib.load().mc_create_raceline_workspace_bytes(B, n_max), dev)
+        _call("mc_create_raceline_batch", B, n_max, n_pts, refline, stride, normvec, alpha, float(stepsize_interp), n_out_max,
+              *out.values(), ws=ws)
         if not derived:           # the caller fixed the capacity: an overflow is reported as n_out[b] = -(points needed)
             return out
         need = int((-out["n_out"]).max().item())
         if need <= 0:
             return out
         n_out_max = need + 16     # (the spline is longer than 1.1 x its polygon: re-run with what the kernel asked for)
-
-
-def _create_raceline_once(lib, refline, normvec, alpha, stepsize_interp, n_pts, n_out_max, with_head_curv):
-    B, n_max, stride = refline.shape
-    dev = refline.device
-    f64 = dict(dtype=torch.float64, device=dev)
-    out = dict(
-        coeffs_x=torch.zeros((B, n_max, 4), **f64), coeffs_y=torch.zeros((B, n_max, 4), **f64),
-        spline_lengths=torch.zeros((B, n_max), **f64), n_out=torch.zeros((B,), dtype=torch.int32, device=dev),
-        raceline_interp=torch.zeros((B, n_out_max, 2), **f64),
-        spline_inds=torch.zeros((B, n_out_max), dtype=torch.int32, device=dev),
-        t_values=torch.zeros((B, n_out_max), **f64), s_interp=torch.zeros((B, n_out_max), **f64),
-        el_lengths_interp=torch.zeros((B, n_out_max), **f64),
-        psi=torch.zeros((B, n_out_max), **f64) if with_head_curv else None,
-        kappa=torch.zeros((B, n_out_max), **f64) if with_head_curv else None,
-    )
-    ws = _workspace("splines", lib.mc_create_raceline_workspace_bytes(B, n_max), dev)
-    rc = lib.mc_create_raceline_batch(B, n_max, _ptr(n_pts), _ptr(refline), stride, _ptr(normvec), _ptr(alpha),
-                                      float(stepsize_interp), n_out_max, _ptr(out["coeffs_x"]), _ptr(out["coeffs_y"]),
-                                      _ptr(out["spline_lengths"]), _ptr(out["n_out"]), _ptr(out["raceline_interp"]),
-                                      _ptr(out["spline_inds"]), _ptr(out["t_values"]), _ptr(out["s_interp"]),
-                                      _ptr(out["el_lengths_interp"]), _ptr(out["psi"]), _ptr(out["kappa"]),
-                                      _ptr(ws), ws.numel(), _stream())
-    _lib.check(rc, "mc_create_raceline_batch")
-    return out
 
 
 _RL_KEYS = ("raceline_interp", "kappa", "el_lengths_interp", "coeffs_x", "coeffs_y", "spline_lengths", "n_out",
@@ -582,7 +559,6 @@ def create_raceline_diff(refline: torch.Tensor, normvec: torch.Tensor, alpha: to
 def calc_head_curv_batch(coeffs_x: torch.Tensor, coeffs_y: torch.Tensor, ind_spls: torch.Tensor, t_spls: torch.Tensor,
                          n_eval: Optional[torch.Tensor] = None, calc_curv: bool = True, calc_dcurv: bool = False):
     _require_cuda()
-    lib = _lib.load()
     if not calc_curv and calc_dcurv:
         raise ValueError("dkappa cannot be calculated without kappa!")
     coeffs_x = _f64(coeffs_x, "coeffs_x")
@@ -595,10 +571,8 @@ def calc_head_curv_batch(coeffs_x: torch.Tensor, coeffs_y: torch.Tensor, ind_spl
     psi = torch.empty((B, n_eval_max), dtype=torch.float64, device=dev)
     kappa = torch.empty_like(psi) if calc_curv else None
     dkappa = torch.empty_like(psi) if calc_dcurv else None
-    rc = lib.mc_calc_head_curv_batch(B, n_max, _ptr(coeffs_x), _ptr(coeffs_y), n_eval_max,
-                                     _ptr(_npts(n_eval, B, dev)), _ptr(ind), _ptr(t_spls), _ptr(psi), _ptr(kappa),
-                                     _ptr(dkappa), _stream())
-    _lib.check(rc, "mc_calc_head_curv_batch")
+    _call("mc_calc_head_curv_batch", B, n_max, coeffs_x, coeffs_y, n_eval_max, _npts(n_eval, B, dev), ind, t_spls, psi, kappa,
+          dkappa)
     return psi, kappa, dkappa
 
 
@@ -607,7 +581,6 @@ def iqp_relinearise_batch(reftrack, normvec, alpha, stepsize_interp, n_pts=None,
     """One re-linearisation step of tph.iqp_handler for every (active) track: returns
     (reftrack_new [B, n_max_new, 4], normvec_new [B, n_max_new, 2], n_pts_new [B])."""
     _require_cuda()
-    lib = _lib.load()
     reftrack = _f64(reftrack, "reftrack")
     normvec = _f64(normvec, "normvec")
     alpha = _f64(alpha, "alpha")
@@ -621,21 +594,17 @@ def iqp_relinearise_batch(reftrack, normvec, alpha, stepsize_interp, n_pts=None,
     rnew = torch.zeros((B, n_max_new, 4), dtype=torch.float64, device=dev)
     nnew = torch.zeros((B, n_max_new, 2), dtype=torch.float64, device=dev)
     npn = torch.zeros((B,), dtype=torch.int32, device=dev)
-    ws = _workspace("iqp", lib.mc_iqp_relinearise_workspace_bytes(B, n_max, n_max_new), dev)
-    rc = lib.mc_iqp_relinearise_batch(B, n_max, _ptr(n_pts), _ptr(active), _ptr(reftrack), _ptr(normvec), _ptr(alpha),
-                                      float(stepsize_interp), int(n_max_new), _ptr(rnew), _ptr(nnew), _ptr(npn),
-                                      _ptr(ws), ws.numel(), _stream())
-    _lib.check(rc, "mc_iqp_relinearise_batch")
+    ws = _workspace("iqp", _lib.load().mc_iqp_relinearise_workspace_bytes(B, n_max, n_max_new), dev)
+    _call("mc_iqp_relinearise_batch", B, n_max, n_pts, active, reftrack, normvec, alpha, float(stepsize_interp), int(n_max_new),
+          rnew, nnew, npn, ws=ws)
     return rnew, nnew, npn
 
 
 @_device_guard
 def scale_alpha_batch(alpha: torch.Tensor, scale: Union[float, torch.Tensor]) -> None:
-    lib = _lib.load()
     B, n_max = alpha.shape
     sb = scale.to(device=alpha.device, dtype=torch.float64).contiguous() if isinstance(scale, torch.Tensor) else None
-    rc = lib.mc_scale_alpha_batch(B, n_max, _ptr(alpha), _ptr(sb), 1.0 if sb is not None else float(scale), _stream())
-    _lib.check(rc, "mc_scale_alpha_batch")
+    _call("mc_scale_alpha_batch", B, n_max, alpha, sb, 1.0 if sb is not None else float(scale))
 
 
 @_device_guard
@@ -674,7 +643,6 @@ def iqp_batch(reftrack: torch.Tensor, normvec: torch.Tensor, h: torch.Tensor, ka
                     reftrack=torch.zeros((B, cap, 4), dtype=torch.float64, device=dev),
                     normvec=torch.zeros((B, cap, 2), dtype=torch.float64, device=dev))
 
-    lib = _lib.load()
     fin = _alloc(n_cap)
     fin.update(n_pts=torch.zeros((B,), dtype=torch.int32, device=dev),
                outer_iters=torch.zeros((B,), dtype=torch.int32, device=dev),
@@ -696,13 +664,10 @@ def iqp_batch(reftrack: torch.Tensor, normvec: torch.Tensor, h: torch.Tensor, ka
         if it < iters_min:
             scale_alpha_batch(alpha, it * 1.0 / iters_min)
         # per-track termination and the copy of finished tracks into the result buffers: on the device
-        rc = lib.mc_iqp_finish_batch(B, n_cur_max, n_cap, it, int(iters_min), float(curv_error_allowed),
-                                     int(fixed_iters) if fixed_iters is not None else 0, int(limit), _ptr(active),
-                                     _ptr(res["status"]), _ptr(res["curv_error_max"]), _ptr(cur_n), _ptr(alpha), _ptr(reftrack),
-                                     _ptr(normvec), _ptr(fin["alpha"]), _ptr(fin["reftrack"]), _ptr(fin["normvec"]),
-                                     _ptr(fin["n_pts"]), _ptr(fin["outer_iters"]), _ptr(fin["status"]),
-                                     _ptr(fin["curv_error_max"]), _ptr(counters), _stream())
-        _lib.check(rc, "mc_iqp_finish_batch")
+        _call("mc_iqp_finish_batch", B, n_cur_max, n_cap, it, int(iters_min), float(curv_error_allowed),
+              int(fixed_iters) if fixed_iters is not None else 0, int(limit), active, res["status"], res["curv_error_max"],
+              cur_n, alpha, reftrack, normvec,
+              *(fin[k] for k in ("alpha", "reftrack", "normvec", "n_pts", "outer_iters", "status", "curv_error_max")), counters)
         if it >= limit:                       # every track was finished by this call (fixed count or cap): nothing to read back
             break
         if fixed_iters is not None:
@@ -752,22 +717,13 @@ def _table(t, cols: int, name: str, dev) -> torch.Tensor:
     return t
 
 
-@_device_guard
-def vel_profile_batch(kappa: torch.Tensor, el_lengths: torch.Tensor, ggv, ax_max_machines, v_max,
-                      drag_coeff: float, m_veh: float, dyn_model_exp: float = 1.0, filt_window: Optional[int] = None,
-                      mu: Optional[torch.Tensor] = None, n_pts: Optional[torch.Tensor] = None,
-                      ggv_scales=None, want_profiles: bool = True, max_chunk: Optional[int] = None,
-                      decel_slice_upper: Optional[int] = None) -> dict:
-    """Batched tph.calc_vel_profile (closed, ggv branch) + calc_ax_profile + calc_t_profile.
-
-    kappa, el_lengths: [B, n_max] device tensors (n_pts[b] valid entries), e.g. the ``kappa`` /
-    ``el_lengths_interp`` / ``n_out`` results of create_raceline_batch.  ``v_max`` is a float, or -- together with
-    ``ggv_scales`` -- a sequence of V per-variant values: variant v of every track runs with
-    ggv[:, 1:] * ggv_scales[v] and top speed v_max[v] (one cell of the reference's lap-time matrix,
-    main_globaltraj.py:442-496).  Returns dict(laptime [B, V], status [B, V] and, if want_profiles,
-    vx [B, V, n_max], ax [B, V, n_max], t [B, V, n_max + 1])."""
-    _require_cuda()
-    lib = _lib.load()
+def _vp_inputs(kappa, el_lengths, ggv, ax_max_machines, v_max, ggv_scales, drag_coeff, m_veh, dyn_model_exp, filt_window,
+               n_pts, decel_slice_upper, mu=None, max_chunk=None):
+    """The checked and normalised inputs of vel_profile_batch, vel_profile_diff and lap_time_matrix_diff: kappa and
+    el_lengths as contiguous float64 CUDA tensors [B, n_max], and a namespace of the rest as the C-ABI takes it: B, n_max,
+    dev, mu, n_pts, V variants per track with their top speeds vmax_t and ggv scales scale_t ([V] on the device; both None
+    for one profile per track at top speed v_scalar), common: the arguments from n_ggv to decel_slice_upper, which
+    mc_vel_profile_batch_ex and mc_vel_profile_adjoint_batch take alike, and max_chunk (see _vp_chunk)."""
     kappa = _f64(kappa, "kappa")
     el_lengths = _f64(el_lengths, "el_lengths")
     B, n_max = kappa.shape
@@ -783,10 +739,8 @@ def vel_profile_batch(kappa: torch.Tensor, el_lengths: torch.Tensor, ggv, ax_max
     mach_t = _table(ax_max_machines, 2, "ax_max_machines", dev)
     if filt_window is not None and int(filt_window) % 2 != 1:
         raise RuntimeError("Window width of moving average filter must be odd!")
-    fw = 0 if filt_window is None else int(filt_window)
     vmax_t = scale_t = None
-    per_variant = ggv_scales is not None or isinstance(v_max, torch.Tensor) or hasattr(v_max, "__len__")
-    if per_variant:
+    if ggv_scales is not None or isinstance(v_max, torch.Tensor) or hasattr(v_max, "__len__"):
         vm = torch.as_tensor(v_max, dtype=torch.float64).reshape(-1)
         sc = torch.ones_like(vm) if ggv_scales is None else torch.as_tensor(ggv_scales, dtype=torch.float64).reshape(-1)
         if vm.numel() == 1 and sc.numel() > 1:
@@ -803,40 +757,75 @@ def vel_profile_batch(kappa: torch.Tensor, el_lengths: torch.Tensor, ggv, ax_max
         raise RuntimeError("ax_max_machines has to cover the entire velocity range of the car (i.e. >= v_max)!")
     if float(ggv_t[-1, 0].item()) < v_hi:
         raise RuntimeError("ggv has to cover the entire velocity range of the car (i.e. >= v_max)!")
-    f64 = dict(dtype=torch.float64, device=dev)
+    common = (int(ggv_t.shape[0]), ggv_t, int(mach_t.shape[0]), mach_t, float(dyn_model_exp), float(drag_coeff), float(m_veh),
+              0 if filt_window is None else int(filt_window),
+              int(VP_DECEL_SLICE_UPPER if decel_slice_upper is None else decel_slice_upper))
+    return kappa, el_lengths, SimpleNamespace(B=B, n_max=n_max, dev=dev, mu=mu, n_pts=n_pts, V=V, vmax_t=vmax_t,
+                                              scale_t=scale_t, v_scalar=v_scalar, common=common, max_chunk=max_chunk)
+
+
+def _vp_chunk(p: SimpleNamespace, per_track: int) -> int:
+    """Tracks per launch of a velocity-profile entry whose workspace takes per_track bytes per track: as many as free
+    device memory holds (or p.max_chunk), and at most (2 ** 31 - 1024) // V, so that one launch's B * V profiles stay
+    within what the entry accepts."""
+    chunk = _chunk(p.B, per_track, p.dev) if p.max_chunk is None else min(p.B, int(p.max_chunk))
+    return max(1, min(chunk, (2 ** 31 - 1024) // p.V))
+
+
+def _vel_profile_launch(kappa: torch.Tensor, el_lengths: torch.Tensor, p: SimpleNamespace, want_profiles: bool) -> dict:
+    """The velocity profiles of the inputs of _vp_inputs: dict(laptime [B, V], status [B, V] and, if want_profiles,
+    vx [B, V, n_max], ax [B, V, n_max], t [B, V, n_max + 1])."""
+    lib = _lib.load()
+    B, V, n_max = p.B, p.V, p.n_max
+    f64 = dict(dtype=torch.float64, device=p.dev)
     laptime = torch.zeros((B, V), **f64)
-    status = torch.zeros((B, V), dtype=torch.int32, device=dev)
+    status = torch.zeros((B, V), dtype=torch.int32, device=p.dev)
     vx = torch.zeros((B, V, n_max), **f64) if want_profiles else None
     ax = torch.zeros((B, V, n_max), **f64) if want_profiles else None
     t = torch.zeros((B, V, n_max + 1), **f64) if want_profiles else None
-    per_track = lib.mc_vel_profile_workspace_bytes(1, V, n_max)
-    chunk = _chunk(B, per_track, dev) if max_chunk is None else min(B, int(max_chunk))
-    chunk = max(1, min(chunk, (2 ** 31 - 1024) // V))
-    ws = _workspace("velprofile", lib.mc_vel_profile_workspace_bytes(chunk, V, n_max), dev)
-    _launch_chunks("mc_vel_profile_batch_ex", B, chunk, ws, n_max, *map(_rows, (n_pts, kappa, el_lengths, mu)), V, scale_t,
-                   vmax_t, v_scalar, int(ggv_t.shape[0]), ggv_t, int(mach_t.shape[0]), mach_t, float(dyn_model_exp),
-                   float(drag_coeff), float(m_veh), fw,
-                   int(VP_DECEL_SLICE_UPPER if decel_slice_upper is None else decel_slice_upper),
-                   *map(_rows, (vx, ax, t, laptime, status)), None, None, None, None)
+    chunk = _vp_chunk(p, lib.mc_vel_profile_workspace_bytes(1, V, n_max))
+    ws = _workspace("velprofile", lib.mc_vel_profile_workspace_bytes(chunk, V, n_max), p.dev)
+    _launch_chunks("mc_vel_profile_batch_ex", B, chunk, ws, n_max, *map(_rows, (p.n_pts, kappa, el_lengths, p.mu)), V,
+                   p.scale_t, p.vmax_t, p.v_scalar, *p.common, *map(_rows, (vx, ax, t, laptime, status)), None, None, None,
+                   None)
     out = dict(laptime=laptime, status=status)
     if want_profiles:
         out.update(vx=vx, ax=ax, t=t)
     return out
 
 
+@_device_guard
+def vel_profile_batch(kappa: torch.Tensor, el_lengths: torch.Tensor, ggv, ax_max_machines, v_max,
+                      drag_coeff: float, m_veh: float, dyn_model_exp: float = 1.0, filt_window: Optional[int] = None,
+                      mu: Optional[torch.Tensor] = None, n_pts: Optional[torch.Tensor] = None,
+                      ggv_scales=None, want_profiles: bool = True, max_chunk: Optional[int] = None,
+                      decel_slice_upper: Optional[int] = None) -> dict:
+    """Batched tph.calc_vel_profile (closed, ggv branch) + calc_ax_profile + calc_t_profile.
+
+    kappa, el_lengths: [B, n_max] device tensors (n_pts[b] valid entries), e.g. the ``kappa`` /
+    ``el_lengths_interp`` / ``n_out`` results of create_raceline_batch.  ``v_max`` is a float, or -- together with
+    ``ggv_scales`` -- a sequence of V per-variant values: variant v of every track runs with
+    ggv[:, 1:] * ggv_scales[v] and top speed v_max[v] (one cell of the reference's lap-time matrix,
+    main_globaltraj.py:442-496).  Returns dict(laptime [B, V], status [B, V] and, if want_profiles,
+    vx [B, V, n_max], ax [B, V, n_max], t [B, V, n_max + 1])."""
+    _require_cuda()
+    kappa, el_lengths, p = _vp_inputs(kappa, el_lengths, ggv, ax_max_machines, v_max, ggv_scales, drag_coeff, m_veh,
+                                      dyn_model_exp, filt_window, n_pts, decel_slice_upper, mu=mu, max_chunk=max_chunk)
+    return _vel_profile_launch(kappa, el_lengths, p, want_profiles)
+
+
 class _VelProfileDiff(torch.autograd.Function):
-    """laptime and vx of the velocity profile as functions of kappa and el_lengths; see vel_profile_diff."""
+    """laptime and vx of the velocity profile as functions of kappa and el_lengths; see vel_profile_diff.  p: the
+    namespace of _vp_inputs (V = 1) and strict."""
 
     @staticmethod
-    def forward(ctx, kappa, el_lengths, n_pts, ggv_t, mach_t, v_max, drag_coeff, m_veh, dyn_model_exp, fw, dsu, strict):
-        res = vel_profile_batch(kappa, el_lengths, ggv_t, mach_t, v_max, drag_coeff, m_veh, dyn_model_exp,
-                                fw if fw > 1 else None, n_pts=n_pts, decel_slice_upper=dsu)
+    def forward(ctx, kappa, el_lengths, p):
+        res = _vel_profile_launch(kappa, el_lengths, p, want_profiles=True)
         laptime, status = res["laptime"][:, 0], res["status"][:, 0]
         vx, ax, t = res["vx"][:, 0], res["ax"][:, 0], res["t"][:, 0]
         grad_status = status.clone()
-        ctx.save_for_backward(kappa, el_lengths, n_pts, ggv_t, mach_t, grad_status)
-        ctx.params = (v_max, dyn_model_exp, drag_coeff, m_veh, fw, dsu)
-        ctx.strict = strict
+        ctx.save_for_backward(kappa, el_lengths, grad_status)
+        ctx.p = p
         ctx.mark_non_differentiable(ax, t, status, grad_status)
         ctx.set_materialize_grads(False)
         return laptime, vx, ax, t, status, grad_status
@@ -844,8 +833,8 @@ class _VelProfileDiff(torch.autograd.Function):
     @staticmethod
     @torch.autograd.function.once_differentiable
     def backward(ctx, grad_laptime, grad_vx, *_unused):
-        kappa, el_lengths, n_pts, ggv_t, mach_t, grad_status = ctx.saved_tensors
-        v_max, dyn_model_exp, drag_coeff, m_veh, fw, dsu = ctx.params
+        kappa, el_lengths, grad_status = ctx.saved_tensors
+        p = ctx.p
         lib = _lib.load()
         B, n_max = kappa.shape
         f64 = dict(dtype=torch.float64, device=kappa.device)
@@ -853,18 +842,17 @@ class _VelProfileDiff(torch.autograd.Function):
         grad_vx = None if grad_vx is None else grad_vx.to(**f64).contiguous()
         wanted = _wanted(B, grad_laptime, grad_vx, device=kappa.device)
         who = "vel_profile_diff: no gradient"
-        _refuse(ctx.strict, wanted, grad_status, who, "with a nonzero upstream gradient")
+        _refuse(p.strict, wanted, grad_status, who, "with a nonzero upstream gradient")
         need_k, need_e = ctx.needs_input_grad[:2]
         gk = torch.empty((B, n_max), **f64) if need_k else None
         ge = torch.empty((B, n_max), **f64) if need_e else None
         gs = torch.empty((B,), dtype=torch.int32, device=kappa.device)
-        chunk = _chunk(B, lib.mc_vel_profile_adjoint_workspace_bytes(1, n_max), kappa.device)
+        chunk = _vp_chunk(p, lib.mc_vel_profile_adjoint_workspace_bytes(1, n_max))
         ws = _workspace("velprofile_adjoint", lib.mc_vel_profile_adjoint_workspace_bytes(chunk, n_max), kappa.device)
-        _launch_chunks("mc_vel_profile_adjoint_batch", B, chunk, ws, n_max, *map(_rows, (n_pts, kappa, el_lengths)), v_max,
-                       int(ggv_t.shape[0]), ggv_t, int(mach_t.shape[0]), mach_t, dyn_model_exp, drag_coeff, m_veh, fw, dsu,
-                       *map(_rows, (grad_laptime, grad_vx, gk, ge, gs)))
-        _refuse(ctx.strict, wanted, gs, who, "whose gradient is not finite")
-        return (gk, ge) + (None,) * 10
+        _launch_chunks("mc_vel_profile_adjoint_batch", B, chunk, ws, n_max, *map(_rows, (p.n_pts, kappa, el_lengths)),
+                       p.v_scalar, *p.common, *map(_rows, (grad_laptime, grad_vx, gk, ge, gs)))
+        _refuse(p.strict, wanted, gs, who, "whose gradient is not finite")
+        return gk, ge, None
 
 
 @_device_guard
@@ -885,17 +873,12 @@ def vel_profile_diff(kappa: torch.Tensor, el_lengths: torch.Tensor, ggv, ax_max_
     the forward's status.  strict=True: backward raises if an instance with a nonzero upstream gradient has
     grad_status != 0; strict=False: such instances get zero gradients."""
     _require_cuda()
-    dev = kappa.device
     if isinstance(v_max, torch.Tensor) or hasattr(v_max, "__len__"):
         raise ValueError("vel_profile_diff: v_max must be one number (no per-variant top speeds)")
-    if filt_window is not None and int(filt_window) % 2 != 1:
-        raise RuntimeError("Window width of moving average filter must be odd!")
-    kappa_t, el_t = _f64(kappa, "kappa"), _f64(el_lengths, "el_lengths")
-    laptime, vx, ax, t, status, grad_status = _VelProfileDiff.apply(
-        kappa_t, el_t, _npts(n_pts, kappa_t.shape[0], dev), _table(ggv, 3, "ggv", dev),
-        _table(ax_max_machines, 2, "ax_max_machines", dev), float(v_max), float(drag_coeff), float(m_veh),
-        float(dyn_model_exp), 0 if filt_window is None else int(filt_window),
-        int(VP_DECEL_SLICE_UPPER if decel_slice_upper is None else decel_slice_upper), bool(strict))
+    kappa, el_lengths, p = _vp_inputs(kappa, el_lengths, ggv, ax_max_machines, v_max, None, drag_coeff, m_veh, dyn_model_exp,
+                                      filt_window, n_pts, decel_slice_upper)
+    p.strict = bool(strict)
+    laptime, vx, ax, t, status, grad_status = _VelProfileDiff.apply(kappa, el_lengths, p)
     return dict(laptime=laptime, vx=vx, ax=ax, t=t, status=status, grad_status=grad_status)
 
 
@@ -923,19 +906,15 @@ def lap_time_matrix_batch(kappa: torch.Tensor, el_lengths: torch.Tensor, ggv, ax
 
 class _LapTimeMatrixDiff(torch.autograd.Function):
     """The lap times [B, V] of V (ggv scale, top speed) variants per track as functions of kappa and el_lengths; see
-    lap_time_matrix_diff."""
+    lap_time_matrix_diff.  p: the namespace of _vp_inputs and strict."""
 
     @staticmethod
-    def forward(ctx, kappa, el_lengths, n_pts, ggv_t, mach_t, vmax_t, scale_t, drag_coeff, m_veh, dyn_model_exp, fw, dsu,
-                strict):
-        res = vel_profile_batch(kappa, el_lengths, ggv_t, mach_t, vmax_t, drag_coeff, m_veh, dyn_model_exp,
-                                fw if fw > 1 else None, n_pts=n_pts, ggv_scales=scale_t, want_profiles=False,
-                                decel_slice_upper=dsu)
+    def forward(ctx, kappa, el_lengths, p):
+        res = _vel_profile_launch(kappa, el_lengths, p, want_profiles=False)
         laptime, status = res["laptime"], res["status"]
         grad_status = status.clone()
-        ctx.save_for_backward(kappa, el_lengths, n_pts, ggv_t, mach_t, vmax_t, scale_t, grad_status)
-        ctx.params = (dyn_model_exp, drag_coeff, m_veh, fw, dsu)
-        ctx.strict = strict
+        ctx.save_for_backward(kappa, el_lengths, grad_status)
+        ctx.p = p
         ctx.mark_non_differentiable(status, grad_status)
         ctx.set_materialize_grads(False)
         return laptime, status, grad_status
@@ -943,30 +922,28 @@ class _LapTimeMatrixDiff(torch.autograd.Function):
     @staticmethod
     @torch.autograd.function.once_differentiable
     def backward(ctx, grad_laptime, *_unused):
-        kappa, el_lengths, n_pts, ggv_t, mach_t, vmax_t, scale_t, grad_status = ctx.saved_tensors
+        kappa, el_lengths, grad_status = ctx.saved_tensors
         if grad_laptime is None:
-            return (None,) * 13
-        dyn_model_exp, drag_coeff, m_veh, fw, dsu = ctx.params
+            return None, None, None
+        p = ctx.p
         lib = _lib.load()
-        B, n_max = kappa.shape
-        V = int(scale_t.numel())
+        B, n_max, V = p.B, p.n_max, p.V
         f64 = dict(dtype=torch.float64, device=kappa.device)
         grad_laptime = grad_laptime.to(**f64).contiguous()
         wanted = (grad_laptime != 0).flatten()                  # per profile b * V + v
         who, cells = "lap_time_matrix_diff: no gradient", " (instance: the cell b * V + v)"
-        _refuse(ctx.strict, wanted, grad_status.flatten(), who, "with a nonzero upstream gradient" + cells)
+        _refuse(p.strict, wanted, grad_status.flatten(), who, "with a nonzero upstream gradient" + cells)
         need_k, need_e = ctx.needs_input_grad[:2]
         gk = torch.empty((B, n_max), **f64) if need_k else None
         ge = torch.empty((B, n_max), **f64) if need_e else None
         gs = torch.empty((B, V), dtype=torch.int32, device=kappa.device)
-        chunk = _chunk(B, lib.mc_vel_profile_adjoint_workspace_bytes(V, n_max), kappa.device)
-        chunk = max(1, min(chunk, (2 ** 31 - 1024) // V))
+        chunk = _vp_chunk(p, lib.mc_vel_profile_adjoint_workspace_bytes(V, n_max))
         ws = _workspace("velprofile_adjoint", lib.mc_vel_profile_adjoint_workspace_bytes(chunk * V, n_max), kappa.device)
-        _launch_chunks("mc_vel_profile_batch_ex", B, chunk, ws, n_max, *map(_rows, (n_pts, kappa, el_lengths)), None, V,
-                       scale_t, vmax_t, 0.0, int(ggv_t.shape[0]), ggv_t, int(mach_t.shape[0]), mach_t, dyn_model_exp,
-                       drag_coeff, m_veh, fw, dsu, None, None, None, None, None, *map(_rows, (grad_laptime, gk, ge, gs)))
-        _refuse(ctx.strict, wanted, gs.flatten(), who, "whose gradient is not finite" + cells)
-        return (gk, ge) + (None,) * 11
+        _launch_chunks("mc_vel_profile_batch_ex", B, chunk, ws, n_max, *map(_rows, (p.n_pts, kappa, el_lengths)), None, V,
+                       p.scale_t, p.vmax_t, p.v_scalar, *p.common, None, None, None, None, None,
+                       *map(_rows, (grad_laptime, gk, ge, gs)))
+        _refuse(p.strict, wanted, gs.flatten(), who, "whose gradient is not finite" + cells)
+        return gk, ge, None
 
 
 @_device_guard
@@ -986,17 +963,12 @@ def lap_time_matrix_diff(kappa: torch.Tensor, el_lengths: torch.Tensor, ggv, ax_
     (n_pts < 2) the forward's status.  strict=True: backward raises if a cell with a nonzero upstream gradient has
     grad_status != 0; strict=False: such cells add nothing to their track's gradient."""
     _require_cuda()
-    dev = kappa.device
-    if filt_window is not None and int(filt_window) % 2 != 1:
-        raise RuntimeError("Window width of moving average filter must be odd!")
     vm, sc, T, S = _lap_time_variants(ggv_scales, top_speeds)
-    kappa_t, el_t = _f64(kappa, "kappa"), _f64(el_lengths, "el_lengths")
-    B = kappa_t.shape[0]
-    laptime, status, grad_status = _LapTimeMatrixDiff.apply(
-        kappa_t, el_t, _npts(n_pts, B, dev), _table(ggv, 3, "ggv", dev), _table(ax_max_machines, 2, "ax_max_machines", dev),
-        vm.to(dev).contiguous(), sc.to(dev).contiguous(), float(drag_coeff), float(m_veh), float(dyn_model_exp),
-        0 if filt_window is None else int(filt_window),
-        int(VP_DECEL_SLICE_UPPER if decel_slice_upper is None else decel_slice_upper), bool(strict))
+    kappa, el_lengths, p = _vp_inputs(kappa, el_lengths, ggv, ax_max_machines, vm, sc, drag_coeff, m_veh, dyn_model_exp,
+                                      filt_window, n_pts, decel_slice_upper)
+    p.strict = bool(strict)
+    laptime, status, grad_status = _LapTimeMatrixDiff.apply(kappa, el_lengths, p)
+    B = p.B
     return dict(laptime=laptime.reshape(B, T, S), status=status.reshape(B, T, S), grad_status=grad_status.reshape(B, T, S))
 
 
@@ -1006,7 +978,6 @@ def calc_ax_t_profile_batch(vx: torch.Tensor, el_lengths: torch.Tensor, ax_in: O
     """Stand-alone tph.calc_ax_profile (ax_in None: vx holds n + 1 values per row) / tph.calc_t_profile.
     Returns (ax [P, n_max], t [P, n_max + 1] or None)."""
     _require_cuda()
-    lib = _lib.load()
     vx = _f64(vx, "vx")
     el_lengths = _f64(el_lengths, "el_lengths")
     P, n_max = el_lengths.shape
@@ -1015,9 +986,8 @@ def calc_ax_t_profile_batch(vx: torch.Tensor, el_lengths: torch.Tensor, ax_in: O
         ax_in = _f64(ax_in, "ax_in")
     ax_out = torch.zeros((P, n_max), dtype=torch.float64, device=dev)
     t_out = torch.zeros((P, n_max + 1), dtype=torch.float64, device=dev) if want_t else None
-    rc = lib.mc_calc_ax_t_profile_batch(P, n_max, _ptr(_npts(n_pts, P, dev)), _ptr(vx), int(vx.shape[1]), _ptr(el_lengths),
-                                        _ptr(ax_in), float(t_start), _ptr(ax_out), _ptr(t_out), _stream())
-    _lib.check(rc, "mc_calc_ax_t_profile_batch")
+    _call("mc_calc_ax_t_profile_batch", P, n_max, _npts(n_pts, P, dev), vx, int(vx.shape[1]), el_lengths, ax_in, float(t_start),
+          ax_out, t_out)
     return ax_out, t_out
 
 
@@ -1034,7 +1004,6 @@ def interp_track_batch(pts: torch.Tensor, stepsize_approx: float = 1.0, n_pts: O
     pts: [B, n_max, 2 or 4].  With ``normvec`` the re-sampled polyline is pts.xy + normal_sign * normvec * pts[..., width_col]
     (the track boundaries of check_traj.py:50-61).  Returns (out [B, n_out_max, 4], n_out [B])."""
     _require_cuda()
-    lib = _lib.load()
     pts = _f64(pts, "pts")
     B, n_max, stride = pts.shape
     dev = pts.device
@@ -1050,14 +1019,12 @@ def interp_track_batch(pts: torch.Tensor, stepsize_approx: float = 1.0, n_pts: O
             poly = _closed_polygon_length(pts, n_pts, normvec=normvec, shift=pts.reshape(-1)[int(width_col):].view(-1),
                                           shift_stride=4, sign=float(normal_sign))
         n_out_max = int(math.ceil(float(poly.max().item()) / float(stepsize_approx))) + 8
-    ws = _workspace("interp_track", lib.mc_interp_track_workspace_bytes(B, n_max), dev)
+    ws = _workspace("interp_track", _lib.load().mc_interp_track_workspace_bytes(B, n_max), dev)
     while True:
         out = torch.zeros((B, int(n_out_max), 4), dtype=torch.float64, device=dev)
         n_out = torch.zeros((B,), dtype=torch.int32, device=dev)
-        rc = lib.mc_interp_track_batch(B, n_max, _ptr(n_pts), _ptr(pts), stride, _ptr(normvec), float(normal_sign),
-                                       int(width_col), float(stepsize_approx), int(n_out_max), _ptr(out), _ptr(n_out),
-                                       _ptr(ws), ws.numel(), _stream())
-        _lib.check(rc, "mc_interp_track_batch")
+        _call("mc_interp_track_batch", B, n_max, n_pts, pts, stride, normvec, float(normal_sign), int(width_col),
+              float(stepsize_approx), int(n_out_max), out, n_out, ws=ws)
         need = int((-n_out).max().item())
         if need <= 0:
             return out, n_out
@@ -1071,7 +1038,6 @@ def min_bound_dists_batch(xy: torch.Tensor, psi: torch.Tensor, bound1: torch.Ten
     """Batched helper_funcs_glob.src.calc_min_bound_dists.calc_min_bound_dists: [B, n_traj_max] minimum distances of
     the vehicle corners to the boundary points (bound1/bound2: [B, nb_max, >= 2], x and y first)."""
     _require_cuda()
-    lib = _lib.load()
     xy, psi, bound1, bound2 = _f64(xy, "xy"), _f64(psi, "psi"), _f64(bound1, "bound1"), _f64(bound2, "bound2")
     B, n_traj_max, _ = xy.shape
     if bound1.shape[2] != bound2.shape[2]:
@@ -1079,10 +1045,8 @@ def min_bound_dists_batch(xy: torch.Tensor, psi: torch.Tensor, bound1: torch.Ten
     dev = xy.device
     out = torch.zeros((B, n_traj_max), dtype=torch.float64, device=dev)
     n_traj, nb1, nb2 = _npts(n_traj, B, dev), _npts(nb1, B, dev), _npts(nb2, B, dev)
-    rc = lib.mc_min_bound_dists_batch(B, n_traj_max, _ptr(n_traj), _ptr(xy), _ptr(psi), int(bound1.shape[1]), _ptr(nb1),
-                                      _ptr(bound1), int(bound2.shape[1]), _ptr(nb2), _ptr(bound2), int(bound1.shape[2]),
-                                      float(length_veh), float(width_veh), _ptr(out), _stream())
-    _lib.check(rc, "mc_min_bound_dists_batch")
+    _call("mc_min_bound_dists_batch", B, n_traj_max, n_traj, xy, psi, int(bound1.shape[1]), nb1, bound1, int(bound2.shape[1]),
+          nb2, bound2, int(bound1.shape[2]), float(length_veh), float(width_veh), out)
     return out
 
 
@@ -1094,16 +1058,14 @@ def traj_extrema_batch(kappa: torch.Tensor, vx: torch.Tensor, ax: torch.Tensor, 
                        min_dists: Optional[torch.Tensor] = None, n_traj: Optional[torch.Tensor] = None) -> torch.Tensor:
     """[B, 8] extrema per trajectory, columns as in EXTREMA (min_dist = inf without min_dists)."""
     _require_cuda()
-    lib = _lib.load()
     kappa, vx, ax = _f64(kappa, "kappa"), _f64(vx, "vx"), _f64(ax, "ax")
     B, n_max = kappa.shape
     dev = kappa.device
     if min_dists is not None:
         min_dists = _f64(min_dists, "min_dists")
     ext = torch.zeros((B, 8), dtype=torch.float64, device=dev)
-    rc = lib.mc_traj_extrema_batch(B, n_max, _ptr(_npts(n_traj, B, dev)), _ptr(kappa), _ptr(vx), _ptr(ax), _ptr(min_dists),
-                                   float(dragcoeff), float(mass_veh), _ptr(ext), _stream())
-    _lib.check(rc, "mc_traj_extrema_batch")
+    _call("mc_traj_extrema_batch", B, n_max, _npts(n_traj, B, dev), kappa, vx, ax, min_dists, float(dragcoeff), float(mass_veh),
+          ext)
     return ext
 
 
@@ -1153,17 +1115,14 @@ def assemble_trajectory_batch(s: torch.Tensor, xy: torch.Tensor, psi: torch.Tens
     """trajectory_opt / traj_race_cl of main_globaltraj.py:501-512 for a batch: [B, n_max + 1, 7] rows
     [s, x, y, psi, kappa, vx, ax]; row n_traj[b] closes the lap with s = sum(spline_lengths[b])."""
     _require_cuda()
-    lib = _lib.load()
     s, xy, psi, kappa, vx, ax = (_f64(t, nm) for t, nm in ((s, "s"), (xy, "xy"), (psi, "psi"), (kappa, "kappa"), (vx, "vx"),
                                                           (ax, "ax")))
     spline_lengths = _f64(spline_lengths, "spline_lengths")
     B, n_max = s.shape
     dev = s.device
     traj = torch.zeros((B, n_max + 1, 7), dtype=torch.float64, device=dev)
-    rc = lib.mc_assemble_trajectory_batch(B, n_max, _ptr(_npts(n_traj, B, dev)), _ptr(s), _ptr(xy), _ptr(psi), _ptr(kappa),
-                                          _ptr(vx), _ptr(ax), int(spline_lengths.shape[1]), _ptr(_npts(n_spl, B, dev)),
-                                          _ptr(spline_lengths), _ptr(traj), _stream())
-    _lib.check(rc, "mc_assemble_trajectory_batch")
+    _call("mc_assemble_trajectory_batch", B, n_max, _npts(n_traj, B, dev), s, xy, psi, kappa, vx, ax, int(spline_lengths.shape[1]),
+          _npts(n_spl, B, dev), spline_lengths, traj)
     return traj
 
 
@@ -1173,7 +1132,6 @@ def check_normals_crossing_batch(track: torch.Tensor, normvec: torch.Tensor, hor
     """Batched tph.check_normals_crossing (helper_funcs_glob/src/prep_track.py:57-59): bool [B], True where
     two normals at most ``horizon`` points apart cross inside the track."""
     _require_cuda()
-    lib = _lib.load()
     track, normvec = _f64(track, "track"), _f64(normvec, "normvec")
     B, n_max, four = track.shape
     if four != 4 or normvec.shape != (B, n_max, 2):
@@ -1184,9 +1142,7 @@ def check_normals_crossing_batch(track: torch.Tensor, normvec: torch.Tensor, hor
     if horizon >= smallest:
         raise RuntimeError("Horizon of %i points is too large for a track with %i points, reduce horizon!" % (horizon, smallest))
     crossing = torch.zeros((B,), dtype=torch.int32, device=dev)
-    rc = lib.mc_check_normals_crossing_batch(B, n_max, _ptr(n_pts), _ptr(track), _ptr(normvec), int(horizon), _ptr(crossing),
-                                             _stream())
-    _lib.check(rc, "mc_check_normals_crossing_batch")
+    _call("mc_check_normals_crossing_batch", B, n_max, n_pts, track, normvec, int(horizon), crossing)
     return crossing != 0
 
 
@@ -1200,7 +1156,6 @@ def jitter_widths_batch(base: torch.Tensor, seeds: torch.Tensor, rel: float = 0.
     centre_id[v], default v % n_base): w <- w (1 + rel g(s)), g smooth with |g| <= 1 drawn from seeds[v] (int64) by the
     stateless hash that synth.jitter_widths_hash mirrors on the host.  Returns (tracks [V, n_max, 4], n_pts [V])."""
     _require_cuda()
-    lib = _lib.load()
     base = _f64(base, "base")
     n_base, n_max, four = base.shape
     if four != 4:
@@ -1215,9 +1170,8 @@ def jitter_widths_batch(base: torch.Tensor, seeds: torch.Tensor, rel: float = 0.
     if out is None:
         out = torch.empty((V, n_max, 4), dtype=torch.float64, device=dev)
     n_out = torch.empty((V,), dtype=torch.int32, device=dev)
-    rc = lib.mc_jitter_widths_batch(V, n_max, _ptr(_npts(n_pts_base, n_base, dev)), n_base, _ptr(base), _ptr(centre_id),
-                                    _ptr(seeds), float(rel), _ptr(out), _ptr(n_out), _stream())
-    _lib.check(rc, "mc_jitter_widths_batch")
+    _call("mc_jitter_widths_batch", V, n_max, _npts(n_pts_base, n_base, dev), n_base, base, centre_id, seeds, float(rel), out,
+          n_out)
     return out, n_out
 
 
@@ -1250,7 +1204,6 @@ def spline_approximation_batch(track: torch.Tensor, k_reg: int = 3, s_reg: float
     smoothing_lambda [B]).  The smoothing spline is the Reinsch formulation with residual budget s_reg
     (csrc/prep_track.cu).  A track the kernel cannot smooth raises ValueError naming the track and the reason."""
     _require_cuda()
-    lib = _lib.load()
     track = _f64(track, "track")
     B, n_raw_max, four = track.shape
     if four != 4:
@@ -1280,11 +1233,10 @@ def spline_approximation_batch(track: torch.Tensor, k_reg: int = 3, s_reg: float
         out = torch.zeros((B, n_out_max, 4), dtype=torch.float64, device=dev)
         n_out = torch.zeros((B,), dtype=torch.int32, device=dev)
         lam = torch.zeros((B,), dtype=torch.float64, device=dev)
-        ws = _workspace("prep_track", lib.mc_prep_track_workspace_bytes(B, n_raw_max, n_int_max), dev)
-        rc = lib.mc_prep_track_batch(B, n_raw_max, _ptr(n_raw), _ptr(track), int(k_reg), float(s_reg), float(stepsize_prep),
-                                     float(stepsize_reg), float(min_width) if min_width is not None else 0.0, n_int_max,
-                                     n_out_max, _ptr(out), _ptr(n_out), _ptr(lam), _ptr(ws), ws.numel(), _stream())
-        _lib.check(rc, "mc_prep_track_batch")
+        ws = _workspace("prep_track", _lib.load().mc_prep_track_workspace_bytes(B, n_raw_max, n_int_max), dev)
+        _call("mc_prep_track_batch", B, n_raw_max, n_raw, track, int(k_reg), float(s_reg), float(stepsize_prep),
+              float(stepsize_reg), float(min_width) if min_width is not None else 0.0, n_int_max, n_out_max, out, n_out, lam,
+              ws=ws)
         codes = n_out.cpu().tolist()
         for b, c in enumerate(codes):
             if c <= -PREP_REFUSED:

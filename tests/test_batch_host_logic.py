@@ -73,6 +73,107 @@ def test_every_wrapper_matches_the_signature_table(fake):
                                                  "mc_mincurv_kappa_batch", "mc_iqp_finish_batch", "mc_jitter_widths_batch"}
 
 
+_CHECK = _lib.check          # (the fake fixture replaces it with a no-op)
+
+
+class _FailingLib(FakeLib):
+    """The recording stand-in whose compute call number fail_at (from 0; workspace queries and mc_last_error aside) returns
+    -1, the code of an invalid argument."""
+
+    def __init__(self, fail_at):
+        super().__init__()
+        self.fail_at, self.computed = fail_at, 0
+
+    def __getattr__(self, name):
+        fn = super().__getattr__(name)
+        if not _computes(name):
+            return fn
+
+        def call(*a):
+            rc = fn(*a)
+            self.computed += 1
+            return -1 if self.computed == self.fail_at + 1 else rc
+        return call
+
+
+def _computes(name):
+    return not name.endswith("_workspace_bytes") and name != "mc_last_error"
+
+
+def _inputs():
+    B, n = 3, 120
+    f64 = dict(dtype=torch.float64)
+    return dict(rt=torch.rand((B, n, 4), **f64) + 3.0, nv=torch.rand((B, n, 2), **f64), h=torch.ones((B, n), **f64),
+                a=torch.zeros((B, n), **f64), kap=torch.rand((B, 200), **f64), el=torch.ones((B, 200), **f64),
+                ggv=np.array([[0.0, 12.0, 12.0], [80.0, 12.0, 12.0]]), mach=np.array([[0.0, 5.0], [80.0, 5.0]]))
+
+
+def _grad(t):
+    return t.clone().requires_grad_()
+
+
+# one call of every public wrapper that reaches the library; the differentiable ones run forward and backward
+WRAPPER_CALLS = {
+    "calc_splines_batch": lambda t: B_.calc_splines_batch(t["rt"]),
+    "opt_min_curv_batch": lambda t: B_.opt_min_curv_batch(t["rt"], t["nv"], t["h"], 0.12, 2.0),
+    "opt_min_curv_diff": lambda t: B_.opt_min_curv_diff(t["rt"][:, :, :2], _grad(t["rt"][:, :, 2:]), t["nv"], t["h"], 0.12,
+                                                        2.0)["alpha"].sum().backward(),
+    "opt_shortest_path_batch": lambda t: B_.opt_shortest_path_batch(t["rt"], t["nv"], 2.0),
+    "opt_shortest_path_diff": lambda t: B_.opt_shortest_path_diff(_grad(t["rt"]), t["nv"], 2.0)["alpha"].sum().backward(),
+    "create_raceline_batch": lambda t: B_.create_raceline_batch(t["rt"], t["nv"], t["a"], 2.0),
+    "create_raceline_diff": lambda t: B_.create_raceline_diff(t["rt"], t["nv"], _grad(t["a"]), 2.0, n_out_max=300,
+                                                              strict=False)["kappa"].sum().backward(),
+    "calc_head_curv_batch": lambda t: B_.calc_head_curv_batch(t["rt"], t["rt"], t["kap"].int(), t["kap"]),
+    "iqp_relinearise_batch": lambda t: B_.iqp_relinearise_batch(t["rt"], t["nv"], t["a"], 3.0),
+    "scale_alpha_batch": lambda t: B_.scale_alpha_batch(t["a"], 0.5),
+    "iqp_batch": lambda t: B_.iqp_batch(t["rt"], t["nv"], t["h"], 0.12, 2.0, 3.0),
+    "vel_profile_batch": lambda t: B_.vel_profile_batch(t["kap"], t["el"], t["ggv"], t["mach"], 70.0, 0.75, 1200.0),
+    "vel_profile_diff": lambda t: B_.vel_profile_diff(_grad(t["kap"]), t["el"], t["ggv"], t["mach"], 70.0, 0.75,
+                                                      1200.0)["laptime"].sum().backward(),
+    "lap_time_matrix_batch": lambda t: B_.lap_time_matrix_batch(t["kap"], t["el"], t["ggv"], t["mach"], [0.5, 1.0],
+                                                                [30.0, 40.0], 0.75, 1200.0),
+    "lap_time_matrix_diff": lambda t: B_.lap_time_matrix_diff(_grad(t["kap"]), t["el"], t["ggv"], t["mach"], [0.5, 1.0],
+                                                              [30.0, 40.0], 0.75, 1200.0)["laptime"].sum().backward(),
+    "calc_ax_t_profile_batch": lambda t: B_.calc_ax_t_profile_batch(torch.cat((t["el"], t["el"][:, :1]), dim=1), t["el"]),
+    "interp_track_batch": lambda t: B_.interp_track_batch(t["rt"], 1.0),
+    "min_bound_dists_batch": lambda t: B_.min_bound_dists_batch(t["nv"], t["a"], t["rt"], t["rt"], 4.7, 2.0),
+    "traj_extrema_batch": lambda t: B_.traj_extrema_batch(t["kap"], t["kap"], t["kap"], 0.75, 1200.0),
+    "check_traj_batch": lambda t: B_.check_traj_batch(t["rt"], t["nv"], t["nv"], t["a"], t["a"], t["a"], t["a"], 4.7, 2.0,
+                                                      0.75, 1200.0),
+    "assemble_trajectory_batch": lambda t: B_.assemble_trajectory_batch(t["a"], t["nv"], t["a"], t["a"], t["a"], t["a"],
+                                                                        t["a"]),
+    "check_normals_crossing_batch": lambda t: B_.check_normals_crossing_batch(t["rt"], t["nv"], 10),
+    "jitter_widths_batch": lambda t: B_.jitter_widths_batch(t["rt"], torch.arange(4)),
+    "spline_approximation_batch": lambda t: B_.spline_approximation_batch(t["rt"]),
+    "prep_track_batch": lambda t: B_.prep_track_batch(t["rt"], dict(k_reg=3, s_reg=10.0),
+                                                      dict(stepsize_prep=1.0, stepsize_reg=3.0), check_normals=False),
+}
+
+
+def test_every_public_wrapper_has_a_failure_case():
+    host_only = {"mincurv_slab_layout", "release_workspaces", "shared_centre_ids", "check_traj_flags"}
+    public = {nm for nm, f in vars(B_).items() if callable(f) and not nm.startswith("_") and not isinstance(f, type)
+              and getattr(f, "__module__", None) == B_.__name__}
+    assert public - host_only == set(WRAPPER_CALLS)
+
+
+@pytest.mark.parametrize("wrapper", sorted(WRAPPER_CALLS))
+def test_a_failing_entry_raises_naming_that_entry(fake, monkeypatch, wrapper):
+    """Each compute call a wrapper makes, failed in turn: the wrapper raises MinCurvLibError naming the entry of that call
+    and makes no call after it."""
+    t = _inputs()
+    WRAPPER_CALLS[wrapper](t)
+    entries = [name for name, _ in fake.calls if _computes(name)]
+    assert entries
+    monkeypatch.setattr(_lib, "check", _CHECK)
+    for k, entry in enumerate(entries):
+        lib = _FailingLib(k)
+        monkeypatch.setattr(_lib, "load", lambda build_if_missing=True: lib)
+        with pytest.raises(_lib.MinCurvLibError, match=f"^{entry} failed with code -1"):
+            WRAPPER_CALLS[wrapper](t)
+        assert [name for name, _ in lib.calls if _computes(name)] == entries[:k + 1]
+
+
 def test_shared_centre_ids_and_their_chunking(fake, monkeypatch):
     """centre_id: owners are the first instance of every group; inside a chunk the first instance of the chunk with the
     same owner takes the role (the owner itself may live in another chunk)."""
