@@ -707,14 +707,24 @@ def iqp_batch(reftrack: torch.Tensor, normvec: torch.Tensor, h: torch.Tensor, ka
 # ------------------------------------------------------------------------------------------------
 # velocity-profile stage (SURVEY.md 8f-1): tph.calc_vel_profile + calc_ax_profile + calc_t_profile
 # ------------------------------------------------------------------------------------------------
-def _table(t, cols: int, name: str, dev) -> torch.Tensor:
-    t = torch.as_tensor(t, dtype=torch.float64).to(dev).contiguous()
+def _table(t, cols: int, name: str) -> torch.Tensor:
+    """The checked table t as a float64 tensor where t lives (a host table stays on the host, so that the range checks
+    of _vp_inputs read no device memory)."""
+    t = torch.as_tensor(t, dtype=torch.float64)
     if t.ndim != 2 or t.shape[1] != cols:
         raise RuntimeError({3: "ggv diagram must consist of the three columns [vx, ax_max, ay_max]!",
                             2: "ax_max_machines must consist of the two columns [vx, ax_max_machines]!"}[cols])
     if t.shape[0] > 256:
         raise ValueError(f"{name}: at most 256 rows are supported")
     return t
+
+
+def _to_device(t: torch.Tensor, dev) -> torch.Tensor:
+    """t on dev.  A host table goes through pinned memory with a non-blocking copy: a copy from pageable memory would
+    synchronise the stream on every call."""
+    if t.device.type == "cpu" and torch.device(dev).type == "cuda":
+        return t.contiguous().pin_memory().to(dev, non_blocking=True)
+    return t.to(dev).contiguous()
 
 
 def _vp_inputs(kappa, el_lengths, ggv, ax_max_machines, v_max, ggv_scales, drag_coeff, m_veh, dyn_model_exp, filt_window,
@@ -735,8 +745,8 @@ def _vp_inputs(kappa, el_lengths, ggv, ax_max_machines, v_max, ggv_scales, drag_
         if mu.shape != (B, n_max):
             raise RuntimeError("kappa and mu must have the same length!")
     n_pts = _npts(n_pts, B, dev)
-    ggv_t = _table(ggv, 3, "ggv", dev)
-    mach_t = _table(ax_max_machines, 2, "ax_max_machines", dev)
+    ggv_h = _table(ggv, 3, "ggv")
+    mach_h = _table(ax_max_machines, 2, "ax_max_machines")
     if filt_window is not None and int(filt_window) % 2 != 1:
         raise RuntimeError("Window width of moving average filter must be odd!")
     vmax_t = scale_t = None
@@ -753,10 +763,11 @@ def _vp_inputs(kappa, el_lengths, ggv, ax_max_machines, v_max, ggv_scales, drag_
     else:
         V, v_hi, v_scalar = 1, float(v_max), float(v_max)
     # tph's range checks (the tables must cover the whole velocity range of the car)
-    if float(mach_t[-1, 0].item()) < v_hi:
+    if float(mach_h[-1, 0].item()) < v_hi:
         raise RuntimeError("ax_max_machines has to cover the entire velocity range of the car (i.e. >= v_max)!")
-    if float(ggv_t[-1, 0].item()) < v_hi:
+    if float(ggv_h[-1, 0].item()) < v_hi:
         raise RuntimeError("ggv has to cover the entire velocity range of the car (i.e. >= v_max)!")
+    ggv_t, mach_t = _to_device(ggv_h, dev), _to_device(mach_h, dev)
     common = (int(ggv_t.shape[0]), ggv_t, int(mach_t.shape[0]), mach_t, float(dyn_model_exp), float(drag_coeff), float(m_veh),
               0 if filt_window is None else int(filt_window),
               int(VP_DECEL_SLICE_UPPER if decel_slice_upper is None else decel_slice_upper))

@@ -1,0 +1,323 @@
+"""Quasi-steady-state lap-time refinement of the raceline: batched projected-gradient descent on alpha.
+
+The minimum-curvature raceline is not lap-time optimal (the ggv, the machine limit and drag make the fastest line differ
+from the least-curved one).  refine_raceline_batch starts from an alpha inside the box of the QP, normally the
+opt_min_curv_batch result, and lowers the lap time that create_raceline_batch followed by vel_profile_batch computes for
+it, with the gradient from the device adjoints create_raceline_diff and vel_profile_diff (DESIGN.md section 3.13).  This
+is not the reference's 'mintime' problem: the curvature limit is not enforced and the vehicle model is the QSS one of
+the velocity profile.
+
+The method is the spectral projected gradient (SPG2) of Birgin, Martinez and Raydan (2000), run per track and in
+lockstep over the batch by spg(), which takes the objective as a batched (value, gradient) callable.  Every operation of
+spg() is elementwise or a row reduction in a fixed order, so a track's iterates do not depend on the other tracks.
+"""
+from __future__ import annotations
+
+import contextlib
+import math
+import os
+import re
+from typing import Callable, Optional, Union
+
+import torch
+
+from . import _lib, batch as _b
+from . import build as _build
+
+# status of a track
+CONVERGED = 0          # ||P(x - g) - x||_inf <= pg_tol
+ITER_CAP = 1           # max_iters accepted steps without convergence
+LINE_SEARCH = 2        # max_halvings halvings found no acceptable step: the last accepted point is kept
+NO_GRADIENT = 3        # a non-finite lap time or gradient at the last accepted point, which is kept
+EMPTY_BOX = 4          # lb > ub at some point (the track is narrower than w_veh): alpha0 is returned as it is
+INACTIVE = -1          # n_pts[b] == 0
+STATUS_TEXT = {CONVERGED: "converged", ITER_CAP: "iteration cap reached", LINE_SEARCH: "line search exhausted",
+               NO_GRADIENT: "no usable gradient", EMPTY_BOX: "empty box (track narrower than w_veh)",
+               INACTIVE: "inactive slot"}
+
+# defaults of the method (Birgin, Martinez and Raydan 2000 use M = 10 and gamma = 1e-4 as well)
+MAX_ITERS = 100        # accepted steps per track
+PG_TOL = 1e-6          # on ||P(x - g) - x||_inf, x in m and g in s/m
+MEMORY = 10            # M: the Armijo test is against the largest of the last M accepted lap times
+GAMMA = 1e-4           # sufficient-decrease factor of the Armijo test
+LAM_MIN, LAM_MAX = 1e-6, 1e4      # clamp of the Barzilai-Borwein step length [m^2/s]; LAM_MAX where s^T y <= 0
+MAX_HALVINGS = 30      # trials per line search (the step goes down to 2^-29 of the spectral one)
+
+
+def _fix_eps() -> float:
+    """FIX_EPS of csrc/common.cuh: the half-width the QP setup gives a collapsed box."""
+    src = _lib._c_source(os.path.join(_build.CSRC, "common.cuh"))
+    return float(re.search(r"constexpr\s+double\s+FIX_EPS\s*=\s*([0-9.eE+-]+)\s*;", src).group(1))
+
+
+FIX_EPS = _fix_eps()
+
+
+def row_sum(v: torch.Tensor) -> torch.Tensor:
+    """Sums over the last dimension by pairwise halving (zero-padded to a power of two): elementwise additions only, so
+    a row's sum has the same bits whatever the other rows are (a library reduction may pick its order by the shape)."""
+    n = v.shape[-1]
+    p = 1 << max(0, (n - 1).bit_length())
+    if p != n:
+        v = torch.nn.functional.pad(v, (0, p - n))
+    while v.shape[-1] > 1:
+        h = v.shape[-1] // 2
+        v = v[..., :h] + v[..., h:]
+    return v[..., 0]
+
+
+def box(reftrack: torch.Tensor, w_veh: Union[float, torch.Tensor], n_pts: Optional[torch.Tensor] = None):
+    """(lb, ub, empty) of opt_min_curv's box for every track: ub = w_right - w_veh / 2, lb = -(w_left - w_veh / 2), a
+    collapsed box (ub - lb < 2 FIX_EPS) replaced by mid -+ FIX_EPS as in mincurv_setup.cu; empty [B] bool marks the
+    tracks with lb > ub at some point.  Beyond n_pts[b] both bounds are 0."""
+    B, n_max, _ = reftrack.shape
+    wv = w_veh.to(reftrack).reshape(B, 1) if isinstance(w_veh, torch.Tensor) else float(w_veh)
+    ub = reftrack[:, :, 2] - 0.5 * wv
+    lb = -(reftrack[:, :, 3] - 0.5 * wv)
+    valid = _valid(n_pts, B, n_max, reftrack.device)
+    empty = ((lb > ub) & valid).any(dim=1)
+    mid = 0.5 * (lb + ub)
+    collapsed = ub - lb < 2.0 * FIX_EPS
+    lb = torch.where(collapsed, mid - FIX_EPS, lb)
+    ub = torch.where(collapsed, mid + FIX_EPS, ub)
+    zero = torch.zeros_like(lb)
+    return torch.where(valid, lb, zero), torch.where(valid, ub, zero), empty
+
+
+def _valid(n_pts, B, n_max, dev) -> torch.Tensor:
+    """bool [B, n_max]: the points below n_pts[b]."""
+    if n_pts is None:
+        return torch.ones((B, n_max), dtype=torch.bool, device=dev)
+    return torch.arange(n_max, device=dev)[None, :] < n_pts.to(device=dev, dtype=torch.int64)[:, None]
+
+
+def spg(fun: Callable, x0: torch.Tensor, lb: torch.Tensor, ub: torch.Tensor, active: torch.Tensor,
+        max_iters: int = MAX_ITERS, pg_tol: float = PG_TOL, memory: int = MEMORY, gamma: float = GAMMA,
+        lam_min: float = LAM_MIN, lam_max: float = LAM_MAX, max_halvings: int = MAX_HALVINGS,
+        callback: Optional[Callable] = None) -> dict:
+    """Spectral projected gradient (SPG2 of Birgin, Martinez and Raydan 2000) on the box lb <= x <= ub [B, n] for the
+    tracks in active [B] (bool), in lockstep: per iteration and track
+
+      d = P(x - lam g) - x;  t = 1, 1/2, 1/4 ... until f(x + t d) <= max(last `memory` accepted f) + gamma t g^T d;
+      s = t d, y = g(x + t d) - g;  lam = clamp(s^T s / s^T y, lam_min, lam_max), lam_max where s^T y <= 0.
+
+    The first lam is 1 / ||P(x0 - g0) - x0||_inf, clamped.  A track converges when ||P(x - g) - x||_inf <= pg_tol.
+
+    fun(x, mask, need_grad) -> (f [B], g [B, n] or None, redo): the objective and, with need_grad, its gradient at
+    the rows of x in mask (other rows: anything, they are not read).  redo is None or a bool [B] mask of tracks fun could
+    not evaluate at this x for want of buffer space; spg then calls fun.grow() and repeats their trial at the same step
+    (such a trial counts neither as one of the track's max_halvings trials nor in evals).  A non-finite f of a trial
+    rejects the trial; a non-finite f or g at an accepted point ends the track (NO_GRADIENT).
+
+    One device-to-host read per trial and per iteration (whether any track is still searching / running).  callback(it,
+    x, f, status), if given, runs after every iteration (it = 0 after the first evaluation).  Returns dict(x, f, f0,
+    status, iters, evals, pg_norm) with the module's status codes (INACTIVE for rows outside active)."""
+    if max_iters < 0 or memory < 1 or max_halvings < 1:
+        raise ValueError("spg: max_iters >= 0, memory >= 1 and max_halvings >= 1 are required")
+    if not (pg_tol >= 0.0 and 0.0 < gamma < 1.0 and 0.0 < lam_min <= lam_max):
+        raise ValueError("spg: pg_tol >= 0, 0 < gamma < 1 and 0 < lam_min <= lam_max are required")
+    B = x0.shape[0]
+    dev = x0.device
+    proj = lambda v: torch.minimum(torch.maximum(v, lb), ub)      # noqa: E731
+    x = proj(x0)
+    f, g, _ = fun(x, active, True)
+    evals = active.to(torch.int32)
+    usable = active & torch.isfinite(f) & torch.isfinite(g).all(dim=1)
+    status = torch.full((B,), INACTIVE, dtype=torch.int32, device=dev)
+    status = torch.where(active, torch.where(usable, ITER_CAP, NO_GRADIENT), status).to(torch.int32)
+    running = usable.clone()
+    f0 = f.clone()
+    hist = f[:, None].repeat(1, int(memory))
+    iters = torch.zeros((B,), dtype=torch.int32, device=dev)
+
+    def pg_norm(x, g):
+        return (proj(x - g) - x).abs().amax(dim=1)
+
+    pgn = pg_norm(x, g)
+    lam = torch.clamp(1.0 / pgn, lam_min, lam_max)          # (pgn = 0: inf, clamped; such a track converges at once)
+    if callback is not None:
+        callback(0, x, f, status)
+    for it in range(1, int(max_iters) + 1):
+        conv = running & (pgn <= pg_tol)
+        status = torch.where(conv, CONVERGED, status).to(torch.int32)
+        running &= ~conv
+        if not bool(running.any()):                                         # the iteration's one read
+            break
+        run2 = running[:, None]
+        d = torch.where(run2, proj(x - lam[:, None] * g) - x, torch.zeros_like(x))
+        gd = row_sum(g * d)
+        f_ref = hist.amax(dim=1)
+        t = torch.ones((B,), dtype=x.dtype, device=dev)
+        searching = running.clone()
+        exhausted = torch.zeros_like(running)
+        n_tried = torch.zeros((B,), dtype=torch.int32, device=dev)      # per track: a redo does not use up a trial
+        x_new, f_new = x.clone(), f.clone()
+        while True:
+            xt = proj(x + t[:, None] * d)                                   # (rounding may leave the box by an ulp)
+            ft, _, redo = fun(xt, searching, False)
+            tried = searching if redo is None else searching & ~redo
+            evals += tried.to(torch.int32)
+            n_tried += tried.to(torch.int32)
+            ok = tried & (ft <= f_ref + gamma * t * gd)
+            x_new = torch.where(ok[:, None], xt, x_new)
+            f_new = torch.where(ok, ft, f_new)
+            searching &= ~ok
+            out = searching & (n_tried >= int(max_halvings))
+            exhausted |= out
+            searching &= ~out
+            t = torch.where(tried & ~ok, 0.5 * t, t)
+            flags = torch.stack((searching.any(), torch.zeros((), dtype=torch.bool, device=dev) if redo is None
+                                 else redo.any())).tolist()                   # the trial's one read
+            if flags[1]:
+                fun.grow()
+            if not flags[0]:
+                break
+        status = torch.where(exhausted, LINE_SEARCH, status).to(torch.int32)
+        acc = running & ~exhausted
+        _, g_new, _ = fun(x_new, acc, True)
+        evals += acc.to(torch.int32)
+        good = acc & torch.isfinite(f_new) & torch.isfinite(g_new).all(dim=1)
+        status = torch.where(acc & ~good, NO_GRADIENT, status).to(torch.int32)
+        running = good
+        s = x_new - x
+        sums = row_sum(torch.stack((s * s, s * (g_new - g))))
+        lam_bb = torch.where(sums[1] > 0.0, torch.clamp(sums[0] / sums[1], lam_min, lam_max),
+                             torch.full_like(lam, lam_max))
+        acc2 = acc[:, None]
+        x = torch.where(acc2, x_new, x)
+        f = torch.where(acc, f_new, f)
+        g = torch.where(good[:, None], g_new, g)
+        lam = torch.where(good, lam_bb, lam)
+        hist = torch.where(acc2, torch.cat((hist[:, 1:], f_new[:, None]), dim=1), hist)
+        iters += acc.to(torch.int32)
+        pgn = torch.where(good, pg_norm(x, g), pgn)
+        if callback is not None:
+            callback(it, x, f, status)
+    else:
+        conv = running & (pgn <= pg_tol)
+        status = torch.where(conv, CONVERGED, status).to(torch.int32)
+    ok_pg = (status == CONVERGED) | (status == ITER_CAP) | (status == LINE_SEARCH)
+    return dict(x=x, f=f, f0=f0, status=status, iters=iters, evals=evals,
+                pg_norm=torch.where(ok_pg, pgn, torch.full_like(pgn, math.nan)))
+
+
+class LapTime:
+    """The objective of refine_raceline_batch: the lap time of create_raceline_batch -> vel_profile_batch at alpha, for
+    the tracks of a mask (the others get n_pts = 0 for the launch, which every kernel skips), and its gradient from
+    create_raceline_diff -> vel_profile_diff (strict=False: n_out and every discrete decision of the forward held).
+
+    No usable gradient (g = NaN for the track) where vel_profile_diff reports grad_status != 0, where the station count
+    overflowed (n_out <= 0; f is NaN there too), and where g is exactly zero on every point: with strict=False the two
+    adjoints hand on zeros for a track they could not differentiate (the velocity-profile adjoint's own non-finite
+    status is not returned), and the lap time of a real raceline never has a zero gradient in every alpha.
+
+    n_out_max is derived as create_raceline_batch derives it, from the start point (unless it was set before); a trial
+    that overflows it is reported in redo and grow() enlarges it to what the kernel asked for.  The ggv and machine
+    tables are kept on the host (pinned), so that the checks of vel_profile_batch read no device memory and their copy
+    does not synchronise the stream.  timer(name), a context manager, brackets the launches of each part ('trial',
+    'forward', 'backward'); tools/refine_time.py times them."""
+
+    def __init__(self, reftrack, normvec, n_pts, stepsize_interp, vp_args: dict):
+        self.reftrack, self.normvec, self.step = reftrack, normvec, float(stepsize_interp)
+        host = lambda t: torch.as_tensor(t, dtype=torch.float64).cpu().contiguous()     # noqa: E731
+        pin = (lambda t: t.pin_memory()) if reftrack.is_cuda else (lambda t: t)          # noqa: E731
+        self.vp = dict(vp_args, ggv=pin(host(vp_args["ggv"])), ax_max_machines=pin(host(vp_args["ax_max_machines"])))
+        B, n_max, _ = reftrack.shape
+        self.n_pts = n_pts if n_pts is not None else torch.full((B,), n_max, dtype=torch.int32, device=reftrack.device)
+        self.n_out_max = None
+        self._need = None
+        self.timer = lambda name: contextlib.nullcontext()
+
+    def start(self, alpha: torch.Tensor, mask: torch.Tensor) -> None:
+        """Derives n_out_max at alpha as create_raceline_batch does (if it is not set yet)."""
+        if self.n_out_max is None:
+            rl = _b.create_raceline_batch(self.reftrack, self.normvec, alpha, self.step, n_pts=self._masked(mask),
+                                          with_head_curv=False)
+            self.n_out_max = int(rl["t_values"].shape[1])
+
+    def _masked(self, mask):
+        return torch.where(mask, self.n_pts, torch.zeros_like(self.n_pts))
+
+    def _laptime(self, rl):
+        return _b.vel_profile_batch(rl["kappa"], rl["el_lengths_interp"], n_pts=rl["n_out"], want_profiles=False,
+                                    **self.vp)["laptime"][:, 0]
+
+    def __call__(self, x, mask, need_grad):
+        if not need_grad:
+            with self.timer("trial"):
+                rl = _b.create_raceline_batch(self.reftrack, self.normvec, x, self.step, n_pts=self._masked(mask),
+                                              n_out_max=self.n_out_max)
+                f = self._laptime(rl)
+                redo = mask & (rl["n_out"] < 0)
+                self._need = (-rl["n_out"]).max()
+            return f, None, redo
+        with self.timer("forward"):
+            xg = x.detach().clone().requires_grad_()
+            rl = _b.create_raceline_diff(self.reftrack, self.normvec, xg, self.step, n_pts=self._masked(mask),
+                                         n_out_max=self.n_out_max, strict=False)
+            vp = _b.vel_profile_diff(rl["kappa"], rl["el_lengths_interp"], n_pts=rl["n_out"], strict=False, **self.vp)
+        with self.timer("backward"):
+            g, = torch.autograd.grad(vp["laptime"].sum(), xg)
+        bad = (vp["grad_status"] != 0) | (rl["n_out"] <= 0) | (g == 0.0).all(dim=1)
+        f = torch.where(rl["n_out"] > 0, vp["laptime"].detach(), torch.full_like(g[:, 0], math.nan))
+        return f, torch.where(bad[:, None], torch.full_like(g, math.nan), g), None
+
+    def grow(self):
+        """Enlarges n_out_max to what the last trial's overflowing track asked for (+16, as create_raceline_batch)."""
+        self.n_out_max = max(self.n_out_max, int(self._need.item()) + 16)
+
+
+def refine_raceline_batch(reftrack: torch.Tensor, normvec: torch.Tensor, alpha0: torch.Tensor,
+                          w_veh: Union[float, torch.Tensor], ggv, ax_max_machines, v_max: float, drag_coeff: float,
+                          m_veh: float, stepsize_interp: float = 2.0, n_pts: Optional[torch.Tensor] = None,
+                          dyn_model_exp: float = 1.0, filt_window: Optional[int] = None, max_iters: int = MAX_ITERS,
+                          pg_tol: float = PG_TOL, memory: int = MEMORY, gamma: float = GAMMA, lam_min: float = LAM_MIN,
+                          lam_max: float = LAM_MAX, max_halvings: int = MAX_HALVINGS,
+                          callback: Optional[Callable] = None, objective: Optional[LapTime] = None) -> dict:
+    """Lowers the quasi-steady-state lap time of every track's raceline by moving alpha inside opt_min_curv's box.
+
+    reftrack [B, n_max, 4], normvec [B, n_max, 2] and alpha0 [B, n_max] (normally the opt_min_curv_batch result) as for
+    create_raceline_batch; w_veh a float or [B]; the vehicle arguments as for vel_profile_diff (one top speed).  The box
+    is ub = w_right - w_veh / 2, lb = -(w_left - w_veh / 2) (collapsed boxes as in the QP); alpha0 is projected onto it.
+    The lap time is that of create_raceline_batch(stepsize_interp) followed by vel_profile_batch, each trial with its own
+    n_out; the gradient holds n_out and the profile's decisions, and the line search tests the real lap time.  The
+    curvature limit is not enforced (check_traj_batch reports it).  Method and defaults: spg() and the module constants.
+
+    Returns dict(alpha [B, n_max], laptime [B], laptime_start [B] (at the projected alpha0), iters [B] (accepted steps),
+    evals [B] (lap-time evaluations), status [B] int32 (CONVERGED 0, ITER_CAP 1, LINE_SEARCH 2, NO_GRADIENT 3,
+    EMPTY_BOX 4, INACTIVE -1), pg_norm [B] (||P(alpha - g) - alpha||_inf at the result; NaN for statuses 3, 4, -1)).
+    Statuses 4 and -1, and status 3 for a track with a non-finite reftrack, normal or alpha0 entry, return alpha0
+    unchanged; their laptime is NaN.  objective: a LapTime built for these inputs (its
+    timer is used), or None."""
+    _b._require_cuda()
+    reftrack, normvec, alpha0 = _b._f64(reftrack, "reftrack"), _b._f64(normvec, "normvec"), _b._f64(alpha0, "alpha0")
+    B, n_max, four = reftrack.shape
+    if four != 4 or normvec.shape != (B, n_max, 2) or alpha0.shape != (B, n_max):
+        raise RuntimeError("refine_raceline_batch: reftrack must be [B, n_max, 4], normvec [B, n_max, 2], alpha0 [B, n_max]")
+    if isinstance(v_max, torch.Tensor) or hasattr(v_max, "__len__"):
+        raise ValueError("refine_raceline_batch: v_max must be one number")
+    if not float(stepsize_interp) > 0.0:
+        raise ValueError("refine_raceline_batch: stepsize_interp must be positive")
+    dev = reftrack.device
+    n_pts = _b._npts(n_pts, B, dev)
+    if isinstance(w_veh, torch.Tensor) and w_veh.numel() != B:
+        raise ValueError("w_veh tensor must have one entry per track")
+    lb, ub, empty = box(reftrack, w_veh, n_pts)
+    valid = _valid(n_pts, B, n_max, dev)
+    lb, ub = torch.where(valid, lb, alpha0), torch.where(valid, ub, alpha0)        # padding stays as it is
+    finite = torch.isfinite(reftrack).all(dim=2) & torch.isfinite(normvec).all(dim=2) & torch.isfinite(alpha0)
+    broken = (~finite & valid).any(dim=1)
+    active = (n_pts > 0 if n_pts is not None else torch.ones((B,), dtype=torch.bool, device=dev)) & ~empty & ~broken
+    vp = dict(ggv=ggv, ax_max_machines=ax_max_machines, v_max=float(v_max), drag_coeff=float(drag_coeff),
+              m_veh=float(m_veh), dyn_model_exp=float(dyn_model_exp), filt_window=filt_window)
+    fun = objective if objective is not None else LapTime(reftrack, normvec, n_pts, stepsize_interp, vp)
+    x0 = torch.minimum(torch.maximum(alpha0, lb), ub)
+    fun.start(x0, active)
+    res = spg(fun, x0, lb, ub, active, max_iters=max_iters, pg_tol=pg_tol, memory=memory, gamma=gamma,
+              lam_min=lam_min, lam_max=lam_max, max_halvings=max_halvings, callback=callback)
+    status = torch.where(empty, EMPTY_BOX, torch.where(broken, NO_GRADIENT, res["status"])).to(torch.int32)
+    kept = ~active
+    nan = torch.full_like(res["f"], math.nan)
+    return dict(alpha=torch.where(kept[:, None], alpha0, res["x"]), laptime=torch.where(kept, nan, res["f"]),
+                laptime_start=torch.where(kept, nan, res["f0"]), iters=res["iters"], evals=res["evals"], status=status,
+                pg_norm=res["pg_norm"])
