@@ -3,9 +3,10 @@ closed track and a few width variants of it, refined for the quasi-steady-state 
 
     widths -> opt_min_curv_batch -> alpha -> refine_raceline_batch -> alpha' (lower lap time, same box)
 
-prints, per variant, the lap time of both lines, the iterations and the status.
+prints, per variant, the lap time of both lines, the iterations and the status, once with steps in the identity metric
+(the default) and once in the curvature metric I + l^4 H of the QP (metric_length, DESIGN.md section 3.13).
 
-    python examples/refine_raceline.py [--n 600] [--variants 4] [--max-iters 100]
+    python examples/refine_raceline.py [--n 600] [--variants 4] [--max-iters 100] [--metric-length 10]
 """
 import argparse
 import os
@@ -26,6 +27,7 @@ def main():
     ap.add_argument("--n", type=int, default=600)
     ap.add_argument("--variants", type=int, default=4)
     ap.add_argument("--max-iters", type=int, default=raceline_refine.MAX_ITERS)
+    ap.add_argument("--metric-length", type=float, default=10.0)
     args = ap.parse_args()
     dev = torch.device("cuda")
     base = torch.tensor(synth.make_track(7, args.n), device=dev)
@@ -33,15 +35,18 @@ def main():
     rt[:, :, 2:] *= torch.linspace(0.8, 1.2, args.variants, device=dev, dtype=torch.float64)[:, None, None]
     _, _, nv, h = B_.calc_splines_batch(rt, want_coeffs=False)
     alpha = B_.opt_min_curv_batch(rt, nv, h, 0.12, 2.0)["alpha"]
-    res = raceline_refine.refine_raceline_batch(rt, nv, alpha, 2.0, GGV, MACH, 70.0, drag_coeff=0.75, m_veh=1200.0,
-                                                stepsize_interp=2.0, max_iters=args.max_iters)
-    for b in range(args.variants):
-        t0, t1 = float(res["laptime_start"][b]), float(res["laptime"][b])
-        st = int(res["status"][b])
-        print(f"variant {b}: width scale {float(rt[b, 0, 2] / base[0, 2]):.2f}, minimum curvature {t0:.3f} s, "
-              f"refined {t1:.3f} s ({100.0 * (t0 - t1) / t0:.2f} % faster), {int(res['iters'][b])} iterations, "
-              f"status {st} ({raceline_refine.STATUS_TEXT[st]}), "
-              f"largest move {1000.0 * float((res['alpha'][b] - alpha[b]).abs().max()):.1f} mm")
+    for ell in (None, args.metric_length):
+        res = raceline_refine.refine_raceline_batch(rt, nv, alpha, 2.0, GGV, MACH, 70.0, drag_coeff=0.75, m_veh=1200.0,
+                                                    stepsize_interp=2.0, max_iters=args.max_iters, metric_length=ell)
+        print("identity metric" if ell is None else f"curvature metric, l = {ell:g} m")
+        for b in range(args.variants):
+            t0, t1 = float(res["laptime_start"][b]), float(res["laptime"][b])
+            st = int(res["status"][b])
+            fb = "" if ell is None else f", {int(res['metric_fallbacks'][b])} identity steps"
+            print(f"  variant {b}: width scale {float(rt[b, 0, 2] / base[0, 2]):.2f}, minimum curvature {t0:.3f} s, "
+                  f"refined {t1:.3f} s ({100.0 * (t0 - t1) / t0:.2f} % faster), {int(res['iters'][b])} iterations, "
+                  f"status {st} ({raceline_refine.STATUS_TEXT[st]}){fb}, "
+                  f"largest move {1000.0 * float((res['alpha'][b] - alpha[b]).abs().max()):.1f} mm")
 
 
 if __name__ == "__main__":

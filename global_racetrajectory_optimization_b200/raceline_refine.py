@@ -10,6 +10,10 @@ the velocity profile.
 The method is the spectral projected gradient (SPG2) of Birgin, Martinez and Raydan (2000), run per track and in
 lockstep over the batch by spg(), which takes the objective as a batched (value, gradient) callable.  Every operation of
 spg() is elementwise or a row reduction in a fixed order, so a track's iterates do not depend on the other tracks.
+
+With metric_length = l, the steps are taken in the curvature metric M = I + l^4 H (H = E^T E, the Hessian of the
+minimum-curvature QP), applied by CurvatureMetric through the minimum-curvature adjoint's banded solve: the lap-time
+gradient is dominated by short wavelengths, which M damps like 1 / (1 + l^4 k^4) while longer ones keep the identity.
 """
 from __future__ import annotations
 
@@ -42,6 +46,9 @@ MEMORY = 10            # M: the Armijo test is against the largest of the last M
 GAMMA = 1e-4           # sufficient-decrease factor of the Armijo test
 LAM_MIN, LAM_MAX = 1e-6, 1e4      # clamp of the Barzilai-Borwein step length [m^2/s]; LAM_MAX where s^T y <= 0
 MAX_HALVINGS = 30      # trials per line search (the step goes down to 2^-29 of the spectral one)
+ACTIVE_EPS = 1e-2      # [m] the two-metric projection pins the points within min(ACTIVE_EPS, ||P(x - g) - x||_inf) of a
+                       # bound that g pushes them against (Bertsekas 1982)
+PIN_FACTOR = 1e6       # CurvatureMetric's pin: PIN_FACTOR (mu + 6 / h_min^4), 6 / h^4 the diagonal of E^T E on a straight
 
 
 def _fix_eps() -> float:
@@ -94,7 +101,7 @@ def _valid(n_pts, B, n_max, dev) -> torch.Tensor:
 def spg(fun: Callable, x0: torch.Tensor, lb: torch.Tensor, ub: torch.Tensor, active: torch.Tensor,
         max_iters: int = MAX_ITERS, pg_tol: float = PG_TOL, memory: int = MEMORY, gamma: float = GAMMA,
         lam_min: float = LAM_MIN, lam_max: float = LAM_MAX, max_halvings: int = MAX_HALVINGS,
-        callback: Optional[Callable] = None) -> dict:
+        callback: Optional[Callable] = None, metric: Optional[Callable] = None) -> dict:
     """Spectral projected gradient (SPG2 of Birgin, Martinez and Raydan 2000) on the box lb <= x <= ub [B, n] for the
     tracks in active [B] (bool), in lockstep: per iteration and track
 
@@ -102,6 +109,15 @@ def spg(fun: Callable, x0: torch.Tensor, lb: torch.Tensor, ub: torch.Tensor, act
       s = t d, y = g(x + t d) - g;  lam = clamp(s^T s / s^T y, lam_min, lam_max), lam_max where s^T y <= 0.
 
     The first lam is 1 / ||P(x0 - g0) - x0||_inf, clamped.  A track converges when ||P(x - g) - x||_inf <= pg_tol.
+
+    metric (None: the above): the steps in a metric M, two-metric projection (Bertsekas 1982).  After every gradient
+    evaluation u = M^-1 g on the free points and u = g on the pinned ones, A = {x <= lb + eps, g > 0} u {x >= ub - eps,
+    g < 0} with eps = min(ACTIVE_EPS, ||P(x - g) - x||_inf); then d = P(x - lam u) - x, with lam = clamp(s^T y / y^T w)
+    (BB2 in M, w = M^-1 y without pins; lam_max where s^T y <= 0 or y^T w <= 0; the first 1 / ||P(x0 - u0) - x0||_inf).
+    The line search, the statuses and the stopping rule are the above.  A track takes the above step (u = g and its lam)
+    in an iteration whose metric solve failed or whose d has g^T d >= 0, counted in metric_fallbacks [B].
+    metric(g, pin, y, mask) -> (u, w, ok): u = M_FF^-1 g_F on the free points of every track in mask (pin [B, n] bool;
+    u on the pins is not read), w = M^-1 y (None for y None), ok [B] bool: both are usable.
 
     fun(x, mask, need_grad) -> (f [B], g [B, n] or None, redo): the objective and, with need_grad, its gradient at
     the rows of x in mask (other rows: anything, they are not read).  redo is None or a bool [B] mask of tracks fun could
@@ -133,8 +149,19 @@ def spg(fun: Callable, x0: torch.Tensor, lb: torch.Tensor, ub: torch.Tensor, act
     def pg_norm(x, g):
         return (proj(x - g) - x).abs().amax(dim=1)
 
+    def metric_step(x, g, pgn, y, mask):
+        """(u, w, ok) of metric at (x, g): u = g on the pins and wherever the solve is not usable."""
+        eps = torch.clamp(pgn, max=ACTIVE_EPS)[:, None]
+        pin = ((x <= lb + eps) & (g > 0.0)) | ((x >= ub - eps) & (g < 0.0))
+        u, w, ok = metric(g, pin, y, mask)
+        return torch.where(pin | ~ok[:, None], g, u), w, ok
+
     pgn = pg_norm(x, g)
     lam = torch.clamp(1.0 / pgn, lam_min, lam_max)          # (pgn = 0: inf, clamped; such a track converges at once)
+    if metric is not None:
+        u, _, m_ok = metric_step(x, g, pgn, None, running)
+        lam_m = torch.clamp(1.0 / pg_norm(x, u), lam_min, lam_max)
+        fallbacks = torch.zeros((B,), dtype=torch.int32, device=dev)
     if callback is not None:
         callback(0, x, f, status)
     for it in range(1, int(max_iters) + 1):
@@ -145,6 +172,11 @@ def spg(fun: Callable, x0: torch.Tensor, lb: torch.Tensor, ub: torch.Tensor, act
             break
         run2 = running[:, None]
         d = torch.where(run2, proj(x - lam[:, None] * g) - x, torch.zeros_like(x))
+        if metric is not None:
+            d_m = torch.where(run2, proj(x - lam_m[:, None] * u) - x, torch.zeros_like(x))
+            use_m = m_ok & (row_sum(g * d_m) < 0.0)
+            fallbacks += (running & ~use_m).to(torch.int32)
+            d = torch.where(use_m[:, None], d_m, d)
         gd = row_sum(g * d)
         f_ref = hist.amax(dim=1)
         t = torch.ones((B,), dtype=x.dtype, device=dev)
@@ -184,6 +216,7 @@ def spg(fun: Callable, x0: torch.Tensor, lb: torch.Tensor, ub: torch.Tensor, act
         lam_bb = torch.where(sums[1] > 0.0, torch.clamp(sums[0] / sums[1], lam_min, lam_max),
                              torch.full_like(lam, lam_max))
         acc2 = acc[:, None]
+        y = g_new - g if metric is not None else None
         x = torch.where(acc2, x_new, x)
         f = torch.where(acc, f_new, f)
         g = torch.where(good[:, None], g_new, g)
@@ -191,14 +224,25 @@ def spg(fun: Callable, x0: torch.Tensor, lb: torch.Tensor, ub: torch.Tensor, act
         hist = torch.where(acc2, torch.cat((hist[:, 1:], f_new[:, None]), dim=1), hist)
         iters += acc.to(torch.int32)
         pgn = torch.where(good, pg_norm(x, g), pgn)
+        if metric is not None:                      # the next direction and the metric's BB2 step in one solve
+            u_new, w, ok_new = metric_step(x, g, pgn, y, good)
+            yw = row_sum(y * w)
+            lam_m2 = torch.where((sums[1] > 0.0) & (yw > 0.0), torch.clamp(sums[1] / yw, lam_min, lam_max),
+                                 torch.full_like(lam, lam_max))
+            u = torch.where(good[:, None], u_new, u)
+            m_ok = torch.where(good, ok_new, m_ok)
+            lam_m = torch.where(good, lam_m2, lam_m)
         if callback is not None:
             callback(it, x, f, status)
     else:
         conv = running & (pgn <= pg_tol)
         status = torch.where(conv, CONVERGED, status).to(torch.int32)
     ok_pg = (status == CONVERGED) | (status == ITER_CAP) | (status == LINE_SEARCH)
-    return dict(x=x, f=f, f0=f0, status=status, iters=iters, evals=evals,
-                pg_norm=torch.where(ok_pg, pgn, torch.full_like(pgn, math.nan)))
+    out = dict(x=x, f=f, f0=f0, status=status, iters=iters, evals=evals,
+               pg_norm=torch.where(ok_pg, pgn, torch.full_like(pgn, math.nan)))
+    if metric is not None:
+        out["metric_fallbacks"] = fallbacks
+    return out
 
 
 class LapTime:
@@ -267,13 +311,80 @@ class LapTime:
         self.n_out_max = max(self.n_out_max, int(self._need.item()) + 16)
 
 
+class CurvatureMetric:
+    """The metric of refine_raceline_batch(metric_length=l): M = I + l^4 H, H = E^T E the Hessian of the minimum-curvature
+    QP for the track's centre line (DESIGN.md section 3.2), applied through mc_mincurv_adjoint_batch, which assembles H,
+    factors H + diag(sens[0] + sens[1]) and returns grad_w_right = sens[0] v, v = (H + diag(sens[0] + sens[1]))^-1 rhs.
+    With sens[0] = mu = l^-4 on a point and sens[1] = 0 that is mu v = M^-1 rhs there; a pinned point gets sens[0] = P =
+    PIN_FACTOR (mu + 6 / h_min^4), which decouples it (v = rhs / P there), so the free points get M_FF^-1 rhs_F.  The
+    widths are replaced by 1 m on each side and w_veh by 0 (H does not depend on them, and no box collapses).
+
+    A call is one launch of 2 B instances: row 2b solves for g with the pins, row 2b + 1 for y without (owned by row 2b
+    through centre_id, so it costs a factorisation and no assembly).  Tracks outside the mask, and those with fewer than
+    N_MIN points, are not launched (n_pts 0, grad_status -1: not ok); with n_max < N_MIN nothing is.  h, the chunk size
+    and the chunk-local centre ids are computed once here, so a call does not synchronise the stream.  timer(name) as
+    LapTime's ('metric')."""
+
+    def __init__(self, reftrack, normvec, n_pts, length: float):
+        B, n_max, _ = reftrack.shape
+        dev = reftrack.device
+        self.mu = float(length) ** -4
+        self.n_pts = n_pts if n_pts is not None else torch.full((B,), n_max, dtype=torch.int32, device=dev)
+        self.launchable = self.n_pts >= _b.N_MIN
+        self.timer = lambda name: contextlib.nullcontext()
+        self.chunk = None
+        if n_max < _b.N_MIN:
+            return
+        _, _, _, h = _b.calc_splines_batch(reftrack, n_pts=n_pts, want_coeffs=False)
+        valid = _valid(n_pts, B, n_max, dev)
+        h_min = torch.where(valid, h, torch.full_like(h, math.inf)).amin(dim=1)
+        self.pin = PIN_FACTOR * (self.mu + 6.0 / h_min ** 4)
+        two = lambda t: t.repeat_interleave(2, dim=0).contiguous()      # noqa: E731
+        self.reftrack = two(torch.cat((reftrack[:, :, :2], torch.ones_like(reftrack[:, :, 2:])), dim=2))
+        self.normvec, self.h = two(normvec), two(h)
+        chunk = _b._chunk(2 * B, _lib.load().mc_mincurv_workspace_bytes(1, n_max), dev)
+        self.chunk = max(2, chunk - chunk % 2)                           # (a track's two rows share a launch)
+        r = torch.arange(2 * B, dtype=torch.int32, device=dev)
+        self.centre_id = r % self.chunk - r % 2                          # row 2b + 1 owned by row 2b, chunk-local
+
+    def __call__(self, g, pin, y, mask):
+        B, n_max = g.shape
+        if self.chunk is None:
+            return g, y, torch.zeros_like(mask)
+        with self.timer("metric"):
+            go = mask & self.launchable
+            n_dir = torch.where(go, self.n_pts, torch.zeros_like(self.n_pts))
+            n_pts = torch.stack((n_dir, n_dir if y is not None else torch.zeros_like(n_dir)), dim=1).reshape(2 * B)
+            gs = torch.where(n_pts > 0, 0, -1).to(torch.int32)
+            sens = torch.zeros((B, 2, 2, n_max), dtype=torch.float64, device=g.device)
+            sens[:, 0, 0] = torch.where(pin, self.pin[:, None], self.mu)
+            sens[:, 1, 0] = self.mu
+            sens = sens.reshape(2 * B, 2, n_max)
+            rhs = torch.stack((g, y if y is not None else torch.zeros_like(g)), dim=1).reshape(2 * B, n_max)
+            out = torch.empty((2 * B, n_max), dtype=torch.float64, device=g.device)
+            gwl = torch.empty_like(out)
+            gwv = torch.empty((2 * B,), dtype=torch.float64, device=g.device)
+            for s in range(0, 2 * B, self.chunk):
+                e = min(2 * B, s + self.chunk)
+                _b._mincurv_launch("mc_mincurv_adjoint_batch", e - s, n_pts[s:e], self.reftrack[s:e], self.normvec[s:e],
+                                   self.h[s:e], None, 0.0, None, _b.F_SCALE, self.centre_id[s:e], sens[s:e], gs[s:e],
+                                   rhs[s:e], out[s:e], gwl[s:e], gwv[s:e])
+            out, gs = out.reshape(B, 2, n_max), gs.reshape(B, 2)
+            u, w = out[:, 0], (out[:, 1] if y is not None else None)
+            ok = go & (gs[:, 0] == 0) & torch.isfinite(u).all(dim=1)
+            if y is not None:
+                ok &= (gs[:, 1] == 0) & torch.isfinite(w).all(dim=1)
+            return u, w, ok
+
+
 def refine_raceline_batch(reftrack: torch.Tensor, normvec: torch.Tensor, alpha0: torch.Tensor,
                           w_veh: Union[float, torch.Tensor], ggv, ax_max_machines, v_max: float, drag_coeff: float,
                           m_veh: float, stepsize_interp: float = 2.0, n_pts: Optional[torch.Tensor] = None,
                           dyn_model_exp: float = 1.0, filt_window: Optional[int] = None, max_iters: int = MAX_ITERS,
                           pg_tol: float = PG_TOL, memory: int = MEMORY, gamma: float = GAMMA, lam_min: float = LAM_MIN,
                           lam_max: float = LAM_MAX, max_halvings: int = MAX_HALVINGS,
-                          callback: Optional[Callable] = None, objective: Optional[LapTime] = None) -> dict:
+                          callback: Optional[Callable] = None, objective: Optional[LapTime] = None,
+                          metric_length: Optional[float] = None) -> dict:
     """Lowers the quasi-steady-state lap time of every track's raceline by moving alpha inside opt_min_curv's box.
 
     reftrack [B, n_max, 4], normvec [B, n_max, 2] and alpha0 [B, n_max] (normally the opt_min_curv_batch result) as for
@@ -288,7 +399,13 @@ def refine_raceline_batch(reftrack: torch.Tensor, normvec: torch.Tensor, alpha0:
     EMPTY_BOX 4, INACTIVE -1), pg_norm [B] (||P(alpha - g) - alpha||_inf at the result; NaN for statuses 3, 4, -1)).
     Statuses 4 and -1, and status 3 for a track with a non-finite reftrack, normal or alpha0 entry, return alpha0
     unchanged; their laptime is NaN.  objective: a LapTime built for these inputs (its
-    timer is used), or None."""
+    timer is used, by the metric too), or None.
+
+    metric_length: None (steps in the identity metric), or l > 0 [m]: steps in the curvature metric I + l^4 H
+    (CurvatureMetric, spg's metric): wavelengths much longer than l move as with the identity, shorter ones are damped.
+    The result then also holds metric_fallbacks [B] int32, the iterations in which the track took the identity step."""
+    if metric_length is not None and not (math.isfinite(float(metric_length)) and float(metric_length) > 0.0):
+        raise ValueError("refine_raceline_batch: metric_length must be None or a finite length > 0 [m]")
     _b._require_cuda()
     reftrack, normvec, alpha0 = _b._f64(reftrack, "reftrack"), _b._f64(normvec, "normvec"), _b._f64(alpha0, "alpha0")
     B, n_max, four = reftrack.shape
@@ -313,11 +430,18 @@ def refine_raceline_batch(reftrack: torch.Tensor, normvec: torch.Tensor, alpha0:
     fun = objective if objective is not None else LapTime(reftrack, normvec, n_pts, stepsize_interp, vp)
     x0 = torch.minimum(torch.maximum(alpha0, lb), ub)
     fun.start(x0, active)
+    metric = None
+    if metric_length is not None:
+        metric = CurvatureMetric(reftrack, normvec, n_pts, float(metric_length))
+        metric.timer = fun.timer
     res = spg(fun, x0, lb, ub, active, max_iters=max_iters, pg_tol=pg_tol, memory=memory, gamma=gamma,
-              lam_min=lam_min, lam_max=lam_max, max_halvings=max_halvings, callback=callback)
+              lam_min=lam_min, lam_max=lam_max, max_halvings=max_halvings, callback=callback, metric=metric)
     status = torch.where(empty, EMPTY_BOX, torch.where(broken, NO_GRADIENT, res["status"])).to(torch.int32)
     kept = ~active
     nan = torch.full_like(res["f"], math.nan)
-    return dict(alpha=torch.where(kept[:, None], alpha0, res["x"]), laptime=torch.where(kept, nan, res["f"]),
-                laptime_start=torch.where(kept, nan, res["f0"]), iters=res["iters"], evals=res["evals"], status=status,
-                pg_norm=res["pg_norm"])
+    out = dict(alpha=torch.where(kept[:, None], alpha0, res["x"]), laptime=torch.where(kept, nan, res["f"]),
+               laptime_start=torch.where(kept, nan, res["f0"]), iters=res["iters"], evals=res["evals"], status=status,
+               pg_norm=res["pg_norm"])
+    if metric is not None:
+        out["metric_fallbacks"] = res["metric_fallbacks"]
+    return out

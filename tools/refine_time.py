@@ -2,10 +2,12 @@
 closed tracks, N = 1000, started from their minimum-curvature alpha (kappa_bound 0.12, w_veh 2 m), racelines resampled
 every STEP m.  CUDA events bracket, per iteration, the line-search trials (create_raceline_batch -> vel_profile_batch),
 the forward of the gradient (create_raceline_diff -> vel_profile_diff) and its backward; the rest of the iteration is
-the optimizer's own step (elementwise work, row sums, the one host read).  Prints one JSON line with the card's name and
-power limit read in the same run, the per-iteration split, and the mean lap time and running tracks against iteration.
+the optimizer's own step (elementwise work, row sums, the one host read).  With --metric-length l the refinement runs
+in the curvature metric and a fourth part, 'metric', brackets its solve (CurvatureMetric).  Prints one JSON line with
+the card's name and power limit read in the same run, the per-iteration split, and the mean lap time and running tracks
+against iteration.
 
-    python tools/refine_time.py [--batch 2112] [--n 1000] [--max-iters 100] [--out FILE]
+    python tools/refine_time.py [--batch 2112] [--n 1000] [--max-iters 100] [--metric-length L] [--out FILE]
 """
 import argparse
 import contextlib
@@ -26,7 +28,7 @@ STEP = 2.0
 GGV = np.array([[0.0, 12.0, 12.0], [90.0, 12.0, 12.0]])
 MACH = np.array([[0.0, 5.3], [40.0, 5.1], [60.0, 2.7], [90.0, 1.5]])
 VEH = dict(v_max=70.0, drag_coeff=0.75, m_veh=1200.0)
-PARTS = ("trial", "forward", "backward")
+PARTS = ("trial", "forward", "backward", "metric")
 
 
 class Recorder:
@@ -71,6 +73,7 @@ def main():
     ap.add_argument("--batch", type=int, default=2112)
     ap.add_argument("--n", type=int, default=1000)
     ap.add_argument("--max-iters", type=int, default=R.MAX_ITERS)
+    ap.add_argument("--metric-length", type=float, default=None)
     ap.add_argument("--out", default=None)
     args = ap.parse_args()
     if not torch.cuda.is_available():
@@ -86,7 +89,8 @@ def main():
         if rec is not None:
             obj.timer = rec
         return R.refine_raceline_batch(rt, nv, alpha, 2.0, GGV, MACH, stepsize_interp=STEP, max_iters=max_iters,
-                                       objective=obj, callback=None if rec is None else rec.callback, **VEH)
+                                       objective=obj, callback=None if rec is None else rec.callback,
+                                       metric_length=args.metric_length, **VEH)
 
     run(2)                                                    # warm-up: every launch and allocation size once
     torch.cuda.synchronize()
@@ -99,13 +103,16 @@ def main():
     total = e0.elapsed_time(e1)
     sums = {p: float(sum(r[p] for r in rows)) for p in PARTS + ("step", "ms")}
     gain = 1.0 - res["laptime"] / res["laptime_start"]
-    out = dict(card=card(), batch=args.batch, n=args.n, max_iters=args.max_iters, total_ms=total,
+    out = dict(card=card(), batch=args.batch, n=args.n, max_iters=args.max_iters, metric_length=args.metric_length,
+               total_ms=total,
                iterations=len(rows), per_iteration_ms={k: v / max(len(rows), 1) for k, v in sums.items()},
                step_share=sums["step"] / max(sums["ms"], 1e-30),
                trials_per_iteration=sum(r["trials"] for r in rows) / max(len(rows), 1),
                status={int(k): int(c) for k, c in zip(*torch.unique(res["status"], return_counts=True))},
                iters_median=float(res["iters"].double().median()), evals_median=float(res["evals"].double().median()),
                laptime_start_mean=float(res["laptime_start"].mean()), laptime_mean=float(res["laptime"].mean()),
+               metric_fallbacks_median=(float(res["metric_fallbacks"].double().median())
+                                        if "metric_fallbacks" in res else None),
                gain_pct=dict(mean=100.0 * float(gain.mean()), min=100.0 * float(gain.min()), max=100.0 * float(gain.max())),
                per_iteration=rows)
     line = json.dumps(out)
