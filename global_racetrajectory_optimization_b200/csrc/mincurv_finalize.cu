@@ -3,7 +3,7 @@
 // against kappa_bound) and the linearisation error curv_error_max, both through the O(N) operator
 // form E a = S_y Z (n_y a) - S_x Z (n_x a) (one periodic tridiagonal solve with two right-hand sides).
 #include "capi.cuh"
-#include "mincurv_ws.cuh"
+#include "mincurv_ops.cuh"
 
 namespace mc {
 
@@ -87,6 +87,27 @@ mincurv_sens_export_kernel(int n_max, const int32_t *__restrict__ n_pts, double 
     if (threadIdx.x == 0) grad_status[b] = st;
 }
 
+// The projection QP of mc_mincurv_solve_batch_ex, run after the assembly: Hessian H + mu I and linear term
+// c = mu q - (H + mu I) x.  mu goes onto the diagonal of the instance's band of H, which the box phase reads, and c
+// replaces f in V_F; H x is formed in operator form (E^T (E x)).  Only instances the assembly left at status 0.
+__global__ void __launch_bounds__(256)
+mincurv_prox_kernel(int n_max, const int32_t *__restrict__ n_pts, double *__restrict__ ws, Layout L, double mu,
+                    const double *__restrict__ prox_x, const double *__restrict__ prox_q,
+                    const int32_t *__restrict__ status) {
+    const int b = blockIdx.x;
+    if (status[b] != 0) return;
+    const int n = n_pts ? n_pts[b] : n_max;
+    double *slab = ws + (size_t)b * L.stride;
+    const double *x = prox_x + (size_t)b * n_max, *q = prox_q + (size_t)b * n_max;
+    double *HB = slab + L.o_hb, *F = vec(slab, L, V_F), *EX = vec(slab, L, V_EDX), *HX = vec(slab, L, V_T3K);
+    double *t0 = vec(slab, L, V_T0), *t1 = vec(slab, L, V_T1), *t2 = vec(slab, L, V_T2), *t3 = vec(slab, L, V_T3);
+    double *t4 = vec(slab, L, V_T4), *t5 = vec(slab, L, V_T5);
+    for (int i = threadIdx.x; i < n; i += blockDim.x) HB[(size_t)i * HB_PITCH] += mu;
+    apply_E(slab, L, n, x, EX, t0, t1, t2, t3, t4, t5);
+    apply_Et(slab, L, n, EX, HX, t0, t1, t2, t3, t4, t5);
+    for (int i = threadIdx.x; i < n; i += blockDim.x) F[i] = mu * q[i] - (HX[i] + mu * x[i]);
+}
+
 }  // namespace mc
 
 extern "C" {
@@ -107,13 +128,46 @@ int mc_mincurv_solve_batch(int B, int n_max, const int32_t *n_pts, const double 
                            double *curv_error_max, double *kappa_lin_max, int32_t *status, int32_t *iters,
                            void *workspace, size_t workspace_bytes, void *stream) {
     return mc_mincurv_solve_batch_ex(B, n_max, n_pts, reftrack, normvec, h, kappa_bound, w_veh, w_veh_batch, MC_F_SCALE_DEFAULT,
-                                     alpha, curv_error_max, kappa_lin_max, status, iters, workspace, workspace_bytes, stream);
+                                     alpha, curv_error_max, kappa_lin_max, status, iters, 0.0, nullptr, nullptr, workspace,
+                                     workspace_bytes, stream);
+}
+
+// the projection QP: setup -> prox -> pdip -> finalize -> kappa (with prox_mu) -> finalize
+static int mincurv_prox_solve(int B, int n_max, const int32_t *n_pts, const double *reftrack, const double *normvec,
+                              const double *h, double kappa_bound, double w_veh, const double *w_veh_batch, double f_scale,
+                              double *alpha, double *curv_error_max, double *kappa_lin_max, int32_t *status, int32_t *iters,
+                              double prox_mu, const double *prox_x, const double *prox_q, void *workspace,
+                              size_t workspace_bytes, void *stream) {
+    if (!reftrack || !normvec || !h || !alpha || !curv_error_max || !status || !prox_q)
+        return bad("mc_mincurv_solve_batch_ex: NULL argument");
+    if (!(prox_mu > 0.0) || !(prox_mu < INFINITY)) return bad("mc_mincurv_solve_batch_ex: prox_mu must be finite and positive");
+    int rc = mc_mincurv_setup_batch_shared(B, n_max, n_pts, reftrack, normvec, h, w_veh, w_veh_batch, f_scale, nullptr, status,
+                                           workspace, workspace_bytes, stream);
+    if (rc) return rc;
+    mc::mincurv_prox_kernel<<<B, 256, 0, (cudaStream_t)stream>>>(n_max, n_pts, (double *)workspace, mc::make_layout(n_max),
+                                                                 prox_mu, prox_x, prox_q, status);
+    rc = check_cuda("mincurv_prox_kernel");
+    if (rc) return rc;
+    rc = mc_mincurv_pdip_batch(B, n_max, n_pts, alpha, status, iters, workspace, workspace_bytes, stream);
+    if (rc) return rc;
+    rc = mc_mincurv_finalize_batch(B, n_max, n_pts, alpha, kappa_bound, curv_error_max, kappa_lin_max, status, workspace,
+                                   workspace_bytes, stream);
+    if (rc) return rc;
+    rc = mc::mincurv_kappa_phase(B, n_max, n_pts, kappa_bound, prox_mu, alpha, status, iters, workspace, workspace_bytes, stream);
+    if (rc) return rc;
+    return mc_mincurv_finalize_batch(B, n_max, n_pts, alpha, kappa_bound, curv_error_max, kappa_lin_max, status, workspace,
+                                     workspace_bytes, stream);
 }
 
 int mc_mincurv_solve_batch_ex(int B, int n_max, const int32_t *n_pts, const double *reftrack, const double *normvec,
                               const double *h, double kappa_bound, double w_veh, const double *w_veh_batch, double f_scale,
                               double *alpha, double *curv_error_max, double *kappa_lin_max, int32_t *status, int32_t *iters,
-                              void *workspace, size_t workspace_bytes, void *stream) {
+                              double prox_mu, const double *prox_x, const double *prox_q, void *workspace,
+                              size_t workspace_bytes, void *stream) {
+    if (prox_x)
+        return mincurv_prox_solve(B, n_max, n_pts, reftrack, normvec, h, kappa_bound, w_veh, w_veh_batch, f_scale, alpha,
+                                  curv_error_max, kappa_lin_max, status, iters, prox_mu, prox_x, prox_q, workspace,
+                                  workspace_bytes, stream);
     return mc_mincurv_solve_batch_shared(B, n_max, n_pts, reftrack, normvec, h, kappa_bound, w_veh, w_veh_batch, f_scale, nullptr,
                                          alpha, curv_error_max, kappa_lin_max, status, iters, workspace, workspace_bytes, stream);
 }

@@ -1393,11 +1393,15 @@ static int launch_solver(void (*kernel)(P...), int grid, int *work_counter, cuda
 //   M = H + D_box + E^T W E = E^T (I + W) E + D_box,  W = l3/s3 + l4/s4      -> weighted band assembly per iteration
 //   rhs = -(f + lu - ll) - tu/su + tl/sl - E^T v,  v = (kl - k_ref) + l3 - l4 + (t3 + l3 rp3)/s3 - (t4 + l4 rp4)/s4
 // with kl = k_ref + E a carried incrementally and E, E^T applied in O(N) operator form (mincurv_ops.cuh).
+// PROX: the Hessian is H + prox_mu I (the projection QP of mc_mincurv_solve_batch_ex, whose prox stage put prox_mu on the
+// band's diagonal and its linear term in V_F for the box phase): + prox_mu a in the gradient and the residuals, + prox_mu
+// on the factored diagonal.  Without PROX prox_mu is not read.
 // ================================================================================================
+template <bool PROX>
 __global__ void __launch_bounds__(IP_THREADS, 8)
 mincurv_pdip_kappa_kernel(int B, int n_max, const int32_t *__restrict__ n_pts, double *__restrict__ ws, Layout L,
                           PdipParams prm, double kb, double *__restrict__ alpha_out, int32_t *__restrict__ status,
-                          int32_t *__restrict__ iters_out, int *__restrict__ work_counter) {
+                          int32_t *__restrict__ iters_out, int *__restrict__ work_counter, double prox_mu) {
     IpShared &sh = ip_init_shared();
     unsigned tick = 0;
     for (int b; (b = next_instance(sh, work_counter)) < B;) {
@@ -1424,6 +1428,9 @@ mincurv_pdip_kappa_kernel(int B, int n_max, const int32_t *__restrict__ n_pts, d
         apply_E(slab, L, n, AL, EDX, t0, t1, t2, t3, t4, t5);
         apply_Et(slab, L, n, EDX, ETV, t0, t1, t2, t3, t4, t5);
         double gmax = 0.0, fmaxv = 0.0;
+        if constexpr (PROX) {
+            for (int i = threadIdx.x; i < n; i += IP_THREADS) ETV[i] += prox_mu * AL[i];
+        }
         for (int i = threadIdx.x; i < n; i += IP_THREADS) {
             gmax = fmax(gmax, fabs(ETV[i] + F[i]));
             fmaxv = fmax(fmaxv, fabs(F[i]));
@@ -1454,14 +1461,19 @@ mincurv_pdip_kappa_kernel(int B, int n_max, const int32_t *__restrict__ n_pts, d
                 const double s3 = S3[i], s4 = S4[i], l3 = L3[i], l4 = L4[i], kl = KL[i];
                 const double rp3 = kl + s3 - kb, rp4 = -kl + s4 - kb;
                 WK[i] = l3 / s3 + l4 / s4;
-                DD[i] = LU[i] * ISU[i] + LL[i] * ISL[i];
+                if constexpr (PROX) DD[i] = LU[i] * ISU[i] + LL[i] * ISL[i] + prox_mu;
+                else DD[i] = LU[i] * ISU[i] + LL[i] * ISL[i];
                 VV[i] = (kl - KR[i]) + l3 * rp3 / s3 - l4 * rp4 / s4;       // affine: t3 = -s3 l3, t4 = -s4 l4
             }
             __syncthreads();
             assemble_hband(slab, L, n, WK, sh.u.win);     // the tile area is free between the sweeps and the next factorisation
             __syncthreads();
             apply_Et(slab, L, n, VV, ETV, t0, t1, t2, t3, t4, t5);
-            for (int i = threadIdx.x; i < n; i += IP_THREADS) RHS[i] = -F[i] - ETV[i];
+            if constexpr (PROX) {
+                for (int i = threadIdx.x; i < n; i += IP_THREADS) RHS[i] = -F[i] - ETV[i] - prox_mu * AL[i];
+            } else {
+                for (int i = threadIdx.x; i < n; i += IP_THREADS) RHS[i] = -F[i] - ETV[i];
+            }
             __syncthreads();
             const bool fok = factor(sh, slab, L, n, slab + L.o_hb, RHS, tick);      // (the band assembled above, own slab)
             tick += factor_units(n);
@@ -1510,7 +1522,11 @@ mincurv_pdip_kappa_kernel(int B, int n_max, const int32_t *__restrict__ n_pts, d
             }
             __syncthreads();
             apply_Et(slab, L, n, VV, ETV, t0, t1, t2, t3, t4, t5);
-            for (int i = threadIdx.x; i < n; i += IP_THREADS) RHS[i] -= ETV[i];
+            if constexpr (PROX) {
+                for (int i = threadIdx.x; i < n; i += IP_THREADS) RHS[i] -= ETV[i] + prox_mu * AL[i];
+            } else {
+                for (int i = threadIdx.x; i < n; i += IP_THREADS) RHS[i] -= ETV[i];
+            }
             __syncthreads();
             solve(sh, slab, L, n, RHS, DX, false);
             apply_E(slab, L, n, DX, EDX, t0, t1, t2, t3, t4, t5);
@@ -1551,7 +1567,12 @@ mincurv_pdip_kappa_kernel(int B, int n_max, const int32_t *__restrict__ n_pts, d
             // dual residual r_d = E^T (kl - k_ref + l3 - l4) + f + lu - ll   (exact every iteration, O(N))
             apply_Et(slab, L, n, VV, ETV, t0, t1, t2, t3, t4, t5);
             rdmax = 0.0;
-            for (int i = threadIdx.x; i < n; i += IP_THREADS) rdmax = fmax(rdmax, fabs(ETV[i] + F[i] + LU[i] - LL[i]));
+            if constexpr (PROX) {
+                for (int i = threadIdx.x; i < n; i += IP_THREADS)
+                    rdmax = fmax(rdmax, fabs(ETV[i] + prox_mu * AL[i] + F[i] + LU[i] - LL[i]));
+            } else {
+                for (int i = threadIdx.x; i < n; i += IP_THREADS) rdmax = fmax(rdmax, fabs(ETV[i] + F[i] + LU[i] - LL[i]));
+            }
             rdmax = block_reduce<1>(rdmax, sh.red);
             if (mu <= prm.mu_rel * mu0 && rdmax <= rd_tol && rpmax <= 1e-8 * kb) { result = 0; ++it; break; }
             if (mu <= 1e-2 * prm.mu_rel * mu0) { result = (rdmax <= 1e3 * rd_tol && rpmax <= 1e-6 * kb) ? 0 : 2; ++it; break; }
@@ -1656,6 +1677,30 @@ mincurv_adjoint_kernel(int B, int n_max, const int32_t *__restrict__ n_pts, cons
     }
 }
 
+// the curvature-row phase of mc_mincurv_kappa_batch (prox_mu 0) or of the projection QP of mc_mincurv_solve_batch_ex
+// (Hessian H + prox_mu I, prox_mu > 0)
+int mincurv_kappa_phase(int B, int n_max, const int32_t *n_pts, double kappa_bound, double prox_mu, double *alpha,
+                        int32_t *status, int32_t *iters, void *workspace, size_t workspace_bytes, void *stream) {
+    if (!alpha || !status) return bad("mc_mincurv_kappa_batch: NULL argument");
+    int rc = mincurv_args("mc_mincurv_kappa_batch", B, n_max, workspace, workspace_bytes);
+    if (rc) return rc;
+    PdipParams prm;
+    prm.max_iter = 40;
+    prm.mu_rel = 1e-11;
+    prm.rd_rel = 1e-8;
+    prm.eta = 0.995;
+    prm.dx_rel = 0.0;
+    prm.lam0_rel = 1e-2;
+    auto kernel = prox_mu > 0.0 ? mincurv_pdip_kappa_kernel<true> : mincurv_pdip_kappa_kernel<false>;
+    const SolverGrid g = solver_grid(B, n_max, workspace, ctas_per_sm(kernel));
+    if (launch_solver(kernel, g.grid, g.counter, (cudaStream_t)stream, B, n_max, n_pts, (double *)workspace,
+                      make_layout(n_max), prm, kappa_bound, alpha, status, iters, g.counter, prox_mu) != 0) {
+        snprintf(g_err, sizeof(g_err), "mincurv_pdip_kappa_kernel: cudaFuncSetAttribute failed");
+        return MC_ECUDA;
+    }
+    return check_cuda("mincurv_pdip_kappa_kernel");
+}
+
 }  // namespace mc
 
 static constexpr int PDIP_SLICE_DEFAULT = 8;      // DESIGN.md section 3.3: the predictor of the remaining iterations is
@@ -1708,23 +1753,7 @@ int mc_mincurv_pdip_batch(int B, int n_max, const int32_t *n_pts, double *alpha,
 
 int mc_mincurv_kappa_batch(int B, int n_max, const int32_t *n_pts, double kappa_bound, double *alpha, int32_t *status,
                            int32_t *iters, void *workspace, size_t workspace_bytes, void *stream) {
-    if (!alpha || !status) return bad("mc_mincurv_kappa_batch: NULL argument");
-    int rc = mc::mincurv_args("mc_mincurv_kappa_batch", B, n_max, workspace, workspace_bytes);
-    if (rc) return rc;
-    mc::PdipParams prm;
-    prm.max_iter = 40;
-    prm.mu_rel = 1e-11;
-    prm.rd_rel = 1e-8;
-    prm.eta = 0.995;
-    prm.dx_rel = 0.0;
-    prm.lam0_rel = 1e-2;
-    const mc::SolverGrid g = mc::solver_grid(B, n_max, workspace, mc::ctas_per_sm(mc::mincurv_pdip_kappa_kernel));
-    if (mc::launch_solver(mc::mincurv_pdip_kappa_kernel, g.grid, g.counter, (cudaStream_t)stream, B, n_max, n_pts,
-                          (double *)workspace, mc::make_layout(n_max), prm, kappa_bound, alpha, status, iters, g.counter) != 0) {
-        snprintf(mc::g_err, sizeof(mc::g_err), "mincurv_pdip_kappa_kernel: cudaFuncSetAttribute failed");
-        return MC_ECUDA;
-    }
-    return check_cuda("mincurv_pdip_kappa_kernel");
+    return mc::mincurv_kappa_phase(B, n_max, n_pts, kappa_bound, 0.0, alpha, status, iters, workspace, workspace_bytes, stream);
 }
 
 int mc_mincurv_adjoint_batch(int B, int n_max, const int32_t *n_pts, const double *reftrack, const double *normvec,

@@ -71,6 +71,12 @@ struct PdipParams {
     double lam0_rel;   // initial multipliers: max(-+g, 0) + lam0_rel * |g|_inf
 };
 
+// the curvature-row phase (mincurv_ipm.cu): mc_mincurv_kappa_batch with prox_mu = 0, the projection QP of
+// mc_mincurv_solve_batch_ex (Hessian H + prox_mu I) with prox_mu > 0.  Not exported.
+__attribute__((visibility("hidden")))
+int mincurv_kappa_phase(int B, int n_max, const int32_t *n_pts, double kappa_bound, double prox_mu, double *alpha,
+                        int32_t *status, int32_t *iters, void *workspace, size_t workspace_bytes, void *stream);
+
 __device__ __forceinline__ double *vec(double *slab, const Layout &L, int v) { return slab + (size_t)v * L.np; }
 
 // index of the instance whose slab holds this instance's band of H: its own, or with shared centre lines the owner's

@@ -4,8 +4,8 @@ The minimum-curvature raceline is not lap-time optimal (the ggv, the machine lim
 from the least-curved one).  refine_raceline_batch starts from an alpha inside the box of the QP, normally the
 opt_min_curv_batch result, and lowers the lap time that create_raceline_batch followed by vel_profile_batch computes for
 it, with the gradient from the device adjoints create_raceline_diff and vel_profile_diff (DESIGN.md section 3.13).  This
-is not the reference's 'mintime' problem: the curvature limit is not enforced and the vehicle model is the QSS one of
-the velocity profile.
+is not the reference's 'mintime' problem: the curvature limit is not enforced (unless kappa_bound, below) and the vehicle
+model is the QSS one of the velocity profile.
 
 The method is the spectral projected gradient (SPG2) of Birgin, Martinez and Raydan (2000), run per track and in
 lockstep over the batch by spg(), which takes the objective as a batched (value, gradient) callable.  Every operation of
@@ -14,6 +14,10 @@ spg() is elementwise or a row reduction in a fixed order, so a track's iterates 
 With metric_length = l, the steps are taken in the curvature metric M = I + l^4 H (H = E^T E, the Hessian of the
 minimum-curvature QP), applied by CurvatureMetric through the minimum-curvature adjoint's banded solve: the lap-time
 gradient is dominated by short wavelengths, which M damps like 1 / (1 + l^4 k^4) while longer ones keep the identity.
+
+With kappa_bound as well, every step is taken inside the minimum-curvature QP's feasible set P = {lb <= alpha <= ub,
+|k_ref + E alpha| <= kappa_bound} instead of the box alone: the direction is the scaled projected gradient in M, one
+projection QP per iteration on the device (CurvatureProjection, mc_mincurv_solve_batch_ex with prox arguments).
 """
 from __future__ import annotations
 
@@ -34,10 +38,13 @@ ITER_CAP = 1           # max_iters accepted steps without convergence
 LINE_SEARCH = 2        # max_halvings halvings found no acceptable step: the last accepted point is kept
 NO_GRADIENT = 3        # a non-finite lap time or gradient at the last accepted point, which is kept
 EMPTY_BOX = 4          # lb > ub at some point (the track is narrower than w_veh): alpha0 is returned as it is
+NO_PROJECTION = 5      # spg(project=...): a projection failed (QP status != 0, non-finite y, or a track the QP does not
+                       # take) or gave no descent direction (g^T d >= 0, d != 0): the last accepted point is kept (alpha0,
+                       # with NaN lap times, where the projection of alpha0 failed)
 INACTIVE = -1          # n_pts[b] == 0
 STATUS_TEXT = {CONVERGED: "converged", ITER_CAP: "iteration cap reached", LINE_SEARCH: "line search exhausted",
                NO_GRADIENT: "no usable gradient", EMPTY_BOX: "empty box (track narrower than w_veh)",
-               INACTIVE: "inactive slot"}
+               NO_PROJECTION: "projection onto the curvature-limited set failed", INACTIVE: "inactive slot"}
 
 # defaults of the method (Birgin, Martinez and Raydan 2000 use M = 10 and gamma = 1e-4 as well)
 MAX_ITERS = 100        # accepted steps per track
@@ -101,7 +108,8 @@ def _valid(n_pts, B, n_max, dev) -> torch.Tensor:
 def spg(fun: Callable, x0: torch.Tensor, lb: torch.Tensor, ub: torch.Tensor, active: torch.Tensor,
         max_iters: int = MAX_ITERS, pg_tol: float = PG_TOL, memory: int = MEMORY, gamma: float = GAMMA,
         lam_min: float = LAM_MIN, lam_max: float = LAM_MAX, max_halvings: int = MAX_HALVINGS,
-        callback: Optional[Callable] = None, metric: Optional[Callable] = None) -> dict:
+        callback: Optional[Callable] = None, metric: Optional[Callable] = None,
+        project: Optional[Callable] = None) -> dict:
     """Spectral projected gradient (SPG2 of Birgin, Martinez and Raydan 2000) on the box lb <= x <= ub [B, n] for the
     tracks in active [B] (bool), in lockstep: per iteration and track
 
@@ -118,6 +126,17 @@ def spg(fun: Callable, x0: torch.Tensor, lb: torch.Tensor, ub: torch.Tensor, act
     in an iteration whose metric solve failed or whose d has g^T d >= 0, counted in metric_fallbacks [B].
     metric(g, pin, y, mask) -> (u, w, ok): u = M_FF^-1 g_F on the free points of every track in mask (pin [B, n] bool;
     u on the pins is not read), w = M^-1 y (None for y None), ok [B] bool: both are usable.
+
+    project (None: the above): steps inside a convex set P within the box, in the metric project works in.  x0 is first
+    replaced by its projection y(x0, 0); then after every gradient evaluation d = y(x, lam g) - x, where
+    project(x, q, mask) -> (y, ok) returns y = argmin_{a in P} 1/2 |a - x|^2_M + q^T (a - x) for the tracks in mask and
+    ok [B] bool.  lam is BB2 in metric (lam = s^T y / y^T w, w from metric(y, no pins, None, mask); lam_max where that is
+    not positive or not usable) or, without metric, the identity BB step above; the first lam is the identity one.  The
+    trials x + t d stay in P (convex) up to the box clamp, the pins are not used, the stopping rule is on
+    pg_norm = ||d||_inf / lam (the above at lam = 1 with the identity metric and P the box).  A track whose projection fails
+    (ok false or a non-finite y) or whose d has g^T d >= 0, d != 0, stops with NO_PROJECTION and keeps its last accepted
+    point; where the projection of x0 fails it keeps x0 (box-clamped), is never evaluated and f is NaN.  The result also
+    holds projection_failures [B] int32, the failed projections (0 or 1: a failure ends the track).
 
     fun(x, mask, need_grad) -> (f [B], g [B, n] or None, redo): the objective and, with need_grad, its gradient at
     the rows of x in mask (other rows: anything, they are not read).  redo is None or a bool [B] mask of tracks fun could
@@ -136,11 +155,20 @@ def spg(fun: Callable, x0: torch.Tensor, lb: torch.Tensor, ub: torch.Tensor, act
     dev = x0.device
     proj = lambda v: torch.minimum(torch.maximum(v, lb), ub)      # noqa: E731
     x = proj(x0)
-    f, g, _ = fun(x, active, True)
-    evals = active.to(torch.int32)
-    usable = active & torch.isfinite(f) & torch.isfinite(g).all(dim=1)
+    started = active
+    if project is not None:
+        y0, ok0 = project(x, torch.zeros_like(x), active)
+        started = active & ok0 & torch.isfinite(y0).all(dim=1)
+        x = torch.where(started[:, None], proj(y0), x)
+        p_fail = (active & ~started).to(torch.int32)
+    f, g, _ = fun(x, started, True)
+    evals = started.to(torch.int32)
+    usable = started & torch.isfinite(f) & torch.isfinite(g).all(dim=1)
     status = torch.full((B,), INACTIVE, dtype=torch.int32, device=dev)
     status = torch.where(active, torch.where(usable, ITER_CAP, NO_GRADIENT), status).to(torch.int32)
+    if project is not None:
+        status = torch.where(active & ~started, NO_PROJECTION, status).to(torch.int32)
+        f = torch.where(started, f, torch.full_like(f, math.nan))
     running = usable.clone()
     f0 = f.clone()
     hist = f[:, None].repeat(1, int(memory))
@@ -156,9 +184,22 @@ def spg(fun: Callable, x0: torch.Tensor, lb: torch.Tensor, ub: torch.Tensor, act
         u, w, ok = metric(g, pin, y, mask)
         return torch.where(pin | ~ok[:, None], g, u), w, ok
 
+    def projected_step(x, g, lam, mask):
+        """(d, pgn, stop, failed) of project at (x, lam g) for the tracks in mask: d = y - x (0 elsewhere and where the
+        projection failed), pgn = ||d||_inf / lam (NaN where it failed), stop: failed or g^T d >= 0 with d != 0."""
+        y, ok = project(x, lam[:, None] * g, mask)
+        failed = mask & ~(ok & torch.isfinite(y).all(dim=1))
+        d = torch.where((mask & ~failed)[:, None], y - x, torch.zeros_like(x))
+        pgn = torch.where(failed, torch.full_like(lam, math.nan), d.abs().amax(dim=1) / lam)
+        stop = failed | (mask & (row_sum(g * d) >= 0.0) & (d != 0.0).any(dim=1))
+        return d, pgn, stop, failed
+
     pgn = pg_norm(x, g)
     lam = torch.clamp(1.0 / pgn, lam_min, lam_max)          # (pgn = 0: inf, clamped; such a track converges at once)
-    if metric is not None:
+    if project is not None:
+        d_p, pgn, p_stop, failed = projected_step(x, g, lam, running)
+        p_fail += failed.to(torch.int32)
+    elif metric is not None:
         u, _, m_ok = metric_step(x, g, pgn, None, running)
         lam_m = torch.clamp(1.0 / pg_norm(x, u), lam_min, lam_max)
         fallbacks = torch.zeros((B,), dtype=torch.int32, device=dev)
@@ -168,11 +209,18 @@ def spg(fun: Callable, x0: torch.Tensor, lb: torch.Tensor, ub: torch.Tensor, act
         conv = running & (pgn <= pg_tol)
         status = torch.where(conv, CONVERGED, status).to(torch.int32)
         running &= ~conv
+        if project is not None:
+            stop = running & p_stop
+            status = torch.where(stop, NO_PROJECTION, status).to(torch.int32)
+            running &= ~stop
         if not bool(running.any()):                                         # the iteration's one read
             break
         run2 = running[:, None]
-        d = torch.where(run2, proj(x - lam[:, None] * g) - x, torch.zeros_like(x))
-        if metric is not None:
+        if project is not None:
+            d = torch.where(run2, d_p, torch.zeros_like(x))
+        else:
+            d = torch.where(run2, proj(x - lam[:, None] * g) - x, torch.zeros_like(x))
+        if metric is not None and project is None:
             d_m = torch.where(run2, proj(x - lam_m[:, None] * u) - x, torch.zeros_like(x))
             use_m = m_ok & (row_sum(g * d_m) < 0.0)
             fallbacks += (running & ~use_m).to(torch.int32)
@@ -224,7 +272,19 @@ def spg(fun: Callable, x0: torch.Tensor, lb: torch.Tensor, ub: torch.Tensor, act
         hist = torch.where(acc2, torch.cat((hist[:, 1:], f_new[:, None]), dim=1), hist)
         iters += acc.to(torch.int32)
         pgn = torch.where(good, pg_norm(x, g), pgn)
-        if metric is not None:                      # the next direction and the metric's BB2 step in one solve
+        if project is not None:                     # BB2 in the metric (its row without pins), then the next direction
+            if metric is not None:
+                w, _, ok_w = metric(y, torch.zeros_like(y, dtype=torch.bool), None, good)
+                yw = row_sum(y * w)
+                lam_p = torch.where(ok_w & (sums[1] > 0.0) & (yw > 0.0), torch.clamp(sums[1] / yw, lam_min, lam_max),
+                                    torch.full_like(lam, lam_max))
+                lam = torch.where(good, lam_p, lam)
+            d_new, pgn_new, stop_new, failed = projected_step(x, g, lam, good)
+            p_fail += failed.to(torch.int32)
+            d_p = torch.where(good[:, None], d_new, d_p)
+            pgn = torch.where(good, pgn_new, pgn)
+            p_stop = torch.where(good, stop_new, p_stop)
+        elif metric is not None:                    # the next direction and the metric's BB2 step in one solve
             u_new, w, ok_new = metric_step(x, g, pgn, y, good)
             yw = row_sum(y * w)
             lam_m2 = torch.where((sums[1] > 0.0) & (yw > 0.0), torch.clamp(sums[1] / yw, lam_min, lam_max),
@@ -240,7 +300,9 @@ def spg(fun: Callable, x0: torch.Tensor, lb: torch.Tensor, ub: torch.Tensor, act
     ok_pg = (status == CONVERGED) | (status == ITER_CAP) | (status == LINE_SEARCH)
     out = dict(x=x, f=f, f0=f0, status=status, iters=iters, evals=evals,
                pg_norm=torch.where(ok_pg, pgn, torch.full_like(pgn, math.nan)))
-    if metric is not None:
+    if project is not None:
+        out["projection_failures"] = p_fail
+    elif metric is not None:
         out["metric_fallbacks"] = fallbacks
     return out
 
@@ -287,6 +349,8 @@ class LapTime:
                                     **self.vp)["laptime"][:, 0]
 
     def __call__(self, x, mask, need_grad):
+        if self.n_out_max is None:                  # (refine_raceline_batch(kappa_bound=...): sized at the projected start)
+            self.start(x, mask)
         if not need_grad:
             with self.timer("trial"):
                 rl = _b.create_raceline_batch(self.reftrack, self.normvec, x, self.step, n_pts=self._masked(mask),
@@ -377,6 +441,73 @@ class CurvatureMetric:
             return u, w, ok
 
 
+class CurvatureProjection:
+    """The projection of refine_raceline_batch(kappa_bound=kb, metric_length=l) onto the minimum-curvature QP's feasible
+    set P = {lb <= alpha <= ub, |k_ref + E alpha| <= kb} (opt_min_curv's, for the same reftrack, w_veh and kb) in the
+    curvature metric M = I + l^4 H: spg's project(x, q, mask) -> (y, ok),
+
+      y = argmin_{a in P} 1/2 (a - x)^T M (a - x) + q^T (a - x),
+
+    which is, divided by l^4 with mu = l^-4, the minimum-curvature QP with Hessian H + mu I and linear term
+    c = mu q - (H + mu I) x: one mc_mincurv_solve_batch_ex call with prox arguments (the box phase and, where the rows
+    bind, the curvature-row phase).  ok: the QP's status is 0 and y is finite.  Tracks outside the mask get n_pts 0, those
+    with fewer than N_MIN points are never launched (not ok); with n_max < N_MIN nothing is.  h and the chunk size are
+    computed once here, so a call does not synchronise the stream.  kappa_lin(x, mask) -> kappa_lin_max [B], the QP's
+    max |k_ref + E x| at x (assembly and the finalize stage).  timer(name) as LapTime's ('projection')."""
+
+    def __init__(self, reftrack, normvec, n_pts, w_veh, kappa_bound: float, length: float):
+        B, n_max, _ = reftrack.shape
+        dev = reftrack.device
+        self.mu, self.kb = float(length) ** -4, float(kappa_bound)
+        self.n_pts = n_pts if n_pts is not None else torch.full((B,), n_max, dtype=torch.int32, device=dev)
+        self.launchable = self.n_pts >= _b.N_MIN
+        self.w_scalar, self.w_batch = _b._wveh(w_veh, B, dev)
+        self.timer = lambda name: contextlib.nullcontext()
+        self.chunk = None
+        if n_max < _b.N_MIN:
+            return
+        self.reftrack, self.normvec = reftrack.contiguous(), normvec.contiguous()
+        _, _, _, self.h = _b.calc_splines_batch(self.reftrack, n_pts=n_pts, want_coeffs=False)
+        self.chunk = _b._chunk(B, _lib.load().mc_mincurv_workspace_bytes(1, n_max), dev)
+
+    def _n(self, mask):
+        return torch.where(mask & self.launchable, self.n_pts, torch.zeros_like(self.n_pts))
+
+    def _ws(self):
+        return _b._workspace("mincurv", _lib.load().mc_mincurv_workspace_bytes(self.chunk, self.h.shape[1]), self.h.device)
+
+    def __call__(self, x, q, mask):
+        if self.chunk is None:
+            return x, torch.zeros_like(mask)
+        with self.timer("projection"):
+            B, n_max = x.shape
+            out = _b._mincurv_results(B, n_max, x.device)
+            _b._launch_chunks("mc_mincurv_solve_batch_ex", B, self.chunk, self._ws(), n_max,
+                              *map(_b._rows, (self._n(mask), self.reftrack, self.normvec, self.h)), self.kb, self.w_scalar,
+                              _b._rows(self.w_batch), _b.F_SCALE, *map(_b._rows, out.values()), self.mu,
+                              _b._rows(x.contiguous()), _b._rows(q.contiguous()))
+            ok = mask & self.launchable & (out["status"] == 0) & torch.isfinite(out["alpha"]).all(dim=1)
+            return out["alpha"], ok
+
+    def kappa_lin(self, x, mask):
+        B, n_max = x.shape
+        kmax = torch.full((B,), math.nan, dtype=torch.float64, device=x.device)
+        if self.chunk is None:
+            return kmax
+        out = _b._mincurv_results(B, n_max, x.device)
+        n = self._n(mask)
+        ws = self._ws()
+        x = x.contiguous()
+        for s in range(0, B, self.chunk):              # (assembly and finalize share the chunk's workspace)
+            e = min(B, s + self.chunk)
+            _b._call("mc_mincurv_setup_batch_ex", e - s, n_max, n[s:e], self.reftrack[s:e], self.normvec[s:e], self.h[s:e],
+                     self.w_scalar, None if self.w_batch is None else self.w_batch[s:e], _b.F_SCALE, out["status"][s:e],
+                     ws=ws)
+            _b._call("mc_mincurv_finalize_batch", e - s, n_max, n[s:e], x[s:e], self.kb, out["curv_error_max"][s:e],
+                     out["kappa_lin_max"][s:e], out["status"][s:e], ws=ws)
+        return torch.where(mask & self.launchable & (out["status"] != 1) & (out["status"] >= 0), out["kappa_lin_max"], kmax)
+
+
 def refine_raceline_batch(reftrack: torch.Tensor, normvec: torch.Tensor, alpha0: torch.Tensor,
                           w_veh: Union[float, torch.Tensor], ggv, ax_max_machines, v_max: float, drag_coeff: float,
                           m_veh: float, stepsize_interp: float = 2.0, n_pts: Optional[torch.Tensor] = None,
@@ -384,15 +515,15 @@ def refine_raceline_batch(reftrack: torch.Tensor, normvec: torch.Tensor, alpha0:
                           pg_tol: float = PG_TOL, memory: int = MEMORY, gamma: float = GAMMA, lam_min: float = LAM_MIN,
                           lam_max: float = LAM_MAX, max_halvings: int = MAX_HALVINGS,
                           callback: Optional[Callable] = None, objective: Optional[LapTime] = None,
-                          metric_length: Optional[float] = None) -> dict:
+                          metric_length: Optional[float] = None, kappa_bound: Optional[float] = None) -> dict:
     """Lowers the quasi-steady-state lap time of every track's raceline by moving alpha inside opt_min_curv's box.
 
     reftrack [B, n_max, 4], normvec [B, n_max, 2] and alpha0 [B, n_max] (normally the opt_min_curv_batch result) as for
     create_raceline_batch; w_veh a float or [B]; the vehicle arguments as for vel_profile_diff (one top speed).  The box
     is ub = w_right - w_veh / 2, lb = -(w_left - w_veh / 2) (collapsed boxes as in the QP); alpha0 is projected onto it.
     The lap time is that of create_raceline_batch(stepsize_interp) followed by vel_profile_batch, each trial with its own
-    n_out; the gradient holds n_out and the profile's decisions, and the line search tests the real lap time.  The
-    curvature limit is not enforced (check_traj_batch reports it).  Method and defaults: spg() and the module constants.
+    n_out; the gradient holds n_out and the profile's decisions, and the line search tests the real lap time.  Without
+    kappa_bound the curvature limit is not enforced (check_traj_batch reports it).  Method and defaults: spg() and the module constants.
 
     Returns dict(alpha [B, n_max], laptime [B], laptime_start [B] (at the projected alpha0), iters [B] (accepted steps),
     evals [B] (lap-time evaluations), status [B] int32 (CONVERGED 0, ITER_CAP 1, LINE_SEARCH 2, NO_GRADIENT 3,
@@ -403,9 +534,26 @@ def refine_raceline_batch(reftrack: torch.Tensor, normvec: torch.Tensor, alpha0:
 
     metric_length: None (steps in the identity metric), or l > 0 [m]: steps in the curvature metric I + l^4 H
     (CurvatureMetric, spg's metric): wavelengths much longer than l move as with the identity, shorter ones are damped.
-    The result then also holds metric_fallbacks [B] int32, the iterations in which the track took the identity step."""
+    The result then also holds metric_fallbacks [B] int32, the iterations in which the track took the identity step.
+
+    kappa_bound: None (alpha stays in the box only), or kb > 0 [1/m] (metric_length required): alpha stays in opt_min_curv's
+    feasible set for this kappa_bound, the box and the linearised curvature rows |k_ref + E alpha| <= kb about the centre
+    line.  alpha0 is projected onto it in the metric (replacing the clamp to the box), and every step is the projected
+    gradient step in the metric (CurvatureProjection, spg's project: one QP per iteration; no pins, no metric_fallbacks).
+    pg_norm is then ||d||_inf / lam of that step.  A track whose projection fails, or gives no descent direction, stops
+    with status NO_PROJECTION (5) at its last accepted point; where alpha0's projection fails (e.g. fewer than N_MIN
+    points) alpha0 is returned with NaN lap times.  The result also holds kappa_lin_max [B] (the QP's max |k_ref + E alpha|
+    at the result), kappa_max [B] (the raceline's max |kappa| from create_raceline_batch at the result; the rows are a
+    linearisation, so it may exceed kb by about curv_error_max) and projection_failures [B] int32; kappa_lin_max and
+    kappa_max are NaN where alpha0 is returned."""
     if metric_length is not None and not (math.isfinite(float(metric_length)) and float(metric_length) > 0.0):
         raise ValueError("refine_raceline_batch: metric_length must be None or a finite length > 0 [m]")
+    if kappa_bound is not None:
+        if not (math.isfinite(float(kappa_bound)) and float(kappa_bound) > 0.0):
+            raise ValueError("refine_raceline_batch: kappa_bound must be None or a finite curvature > 0 [1/m]")
+        if metric_length is None:
+            raise ValueError("refine_raceline_batch: kappa_bound needs metric_length (the projection runs in the "
+                             "curvature metric)")
     _b._require_cuda()
     reftrack, normvec, alpha0 = _b._f64(reftrack, "reftrack"), _b._f64(normvec, "normvec"), _b._f64(alpha0, "alpha0")
     B, n_max, four = reftrack.shape
@@ -429,19 +577,35 @@ def refine_raceline_batch(reftrack: torch.Tensor, normvec: torch.Tensor, alpha0:
               m_veh=float(m_veh), dyn_model_exp=float(dyn_model_exp), filt_window=filt_window)
     fun = objective if objective is not None else LapTime(reftrack, normvec, n_pts, stepsize_interp, vp)
     x0 = torch.minimum(torch.maximum(alpha0, lb), ub)
-    fun.start(x0, active)
-    metric = None
+    if kappa_bound is None:
+        fun.start(x0, active)                   # (with the projection: at the projected start, by fun's first call)
+    metric = project = None
     if metric_length is not None:
         metric = CurvatureMetric(reftrack, normvec, n_pts, float(metric_length))
         metric.timer = fun.timer
+    if kappa_bound is not None:
+        project = CurvatureProjection(reftrack, normvec, n_pts, w_veh, float(kappa_bound), float(metric_length))
+        project.timer = fun.timer
     res = spg(fun, x0, lb, ub, active, max_iters=max_iters, pg_tol=pg_tol, memory=memory, gamma=gamma,
-              lam_min=lam_min, lam_max=lam_max, max_halvings=max_halvings, callback=callback, metric=metric)
+              lam_min=lam_min, lam_max=lam_max, max_halvings=max_halvings, callback=callback, metric=metric,
+              project=project)
     status = torch.where(empty, EMPTY_BOX, torch.where(broken, NO_GRADIENT, res["status"])).to(torch.int32)
     kept = ~active
+    if project is not None:                     # alpha0 could not be projected: it is returned as it is
+        kept = kept | ((res["status"] == NO_PROJECTION) & (res["evals"] == 0))
     nan = torch.full_like(res["f"], math.nan)
     out = dict(alpha=torch.where(kept[:, None], alpha0, res["x"]), laptime=torch.where(kept, nan, res["f"]),
                laptime_start=torch.where(kept, nan, res["f0"]), iters=res["iters"], evals=res["evals"], status=status,
                pg_norm=res["pg_norm"])
-    if metric is not None:
+    if project is not None:
+        nan_b = torch.full_like(res["f"], math.nan)
+        out["kappa_lin_max"] = torch.where(kept, nan_b, project.kappa_lin(res["x"], ~kept))
+        rl = _b.create_raceline_batch(reftrack, normvec, out["alpha"], stepsize_interp,
+                                      n_pts=torch.where(kept, torch.zeros_like(project.n_pts), project.n_pts))
+        k = rl["kappa"].abs()
+        k = torch.where(torch.arange(k.shape[1], device=dev)[None, :] < rl["n_out"][:, None], k, torch.zeros_like(k))
+        out["kappa_max"] = torch.where(kept | (rl["n_out"] <= 0), nan_b, k.amax(dim=1))
+        out["projection_failures"] = res["projection_failures"]
+    elif metric is not None:
         out["metric_fallbacks"] = res["metric_fallbacks"]
     return out

@@ -97,12 +97,22 @@ int mc_mincurv_solve_batch(int B, int n_max, const int32_t *n_pts,
                            int32_t *status, int32_t *iters,
                            void *workspace, size_t workspace_bytes, void *stream);
 
-/* the same with an explicit f_scale (see MC_F_SCALE_DEFAULT) */
+/* the same with an explicit f_scale (see MC_F_SCALE_DEFAULT) and, with prox_x, the projection onto the QP's feasible set
+ * P = {lb <= alpha <= ub, |k_ref + E alpha| <= kappa_bound} in the metric H + prox_mu I (raceline_refine.CurvatureProjection,
+ * DESIGN.md section 3.13):
+ *   prox_x == NULL : the call above, bit for bit (prox_mu and prox_q are not read)
+ *   prox_x, prox_q [B][n_max] : solves  min 1/2 alpha^T (H + prox_mu I) alpha + c^T alpha  over P,
+ *                    c = prox_mu prox_q - (H + prox_mu I) prox_x,  i.e.  argmin_{alpha in P} 1/2 |alpha - x|^2_{I + H / prox_mu}
+ *                    + q^T (alpha - x);  prox_mu > 0 and finite, prox_q required.  f_scale is checked but does not enter
+ *                    the objective; the stages are those of mc_mincurv_solve_batch (assembly, box phase, finalize,
+ *                    curvature-row phase, finalize) on H + prox_mu I, without shared centre lines.  kappa_lin_max and
+ *                    curv_error_max are those of the result; status as above (4: the rows are still violated). */
 int mc_mincurv_solve_batch_ex(int B, int n_max, const int32_t *n_pts,
                               const double *reftrack, const double *normvec, const double *h,
                               double kappa_bound, double w_veh, const double *w_veh_batch, double f_scale,
                               double *alpha, double *curv_error_max, double *kappa_lin_max,
                               int32_t *status, int32_t *iters,
+                              double prox_mu, const double *prox_x, const double *prox_q,
                               void *workspace, size_t workspace_bytes, void *stream);
 
 /* the same for batches in which several instances share a centreline (x, y, normal vectors, h and n_pts identical, only

@@ -1,10 +1,12 @@
 """The metric length of the lap-time refinement (raceline_refine.refine_raceline_batch(metric_length=l)) swept on the
 golden tracks of tests/golden/ from their minimum-curvature alpha, with the fixtures' ggv and machine tables, against the
 identity metric.  Per run and track: lap time, status, ||P(alpha - g) - alpha||_inf, the largest move from the
-minimum-curvature alpha, the identity fallbacks, and max |kappa| of the raceline against curvlim (the refinement does not
-enforce it, so a violation shows here).  Prints one JSON line with the card's name and power limit read in the same run.
+minimum-curvature alpha, the identity fallbacks, and max |kappa| of the raceline against curvlim.  Every metric length runs
+without the curvature limit (kappa_bound None: a violation shows in max |kappa|) and with each --kappa-bounds kb, where
+the steps stay inside the QP's curvature-limited set (kappa_lin_max: the QP's linearised max |kappa| at the result).
+Prints one JSON line with the card's name and power limit read in the same run.
 
-    python tools/refine_sweep.py [--lengths 5 10 20 40 80] [--max-iters 100] [--out FILE]
+    python tools/refine_sweep.py [--lengths 5 10 20 40 80] [--kappa-bounds 0.12] [--max-iters 100] [--out FILE]
 """
 import argparse
 import json
@@ -32,6 +34,7 @@ def _golden(name):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--lengths", type=float, nargs="+", default=[5.0, 10.0, 20.0, 40.0, 80.0])
+    ap.add_argument("--kappa-bounds", type=float, nargs="*", default=[CURVLIM])
     ap.add_argument("--max-iters", type=int, default=R.MAX_ITERS)
     ap.add_argument("--out", default=None)
     args = ap.parse_args()
@@ -52,9 +55,9 @@ def main():
     wv = torch.tensor([float(g["w_veh"]) for g in gs], device=dev)
     _, _, nv, _ = B_.calc_splines_batch(rt, n_pts=npts, want_coeffs=False)
     runs = []
-    for ell in [None] + list(args.lengths):
+    for ell, kb in [(None, None)] + [(ell, kb) for ell in args.lengths for kb in [None] + list(args.kappa_bounds)]:
         res = R.refine_raceline_batch(rt, nv, al, wv, n_pts=npts, stepsize_interp=STEP, max_iters=args.max_iters,
-                                      metric_length=ell, **veh)
+                                      metric_length=ell, kappa_bound=kb, **veh)
         rl = B_.create_raceline_batch(rt, nv, res["alpha"], STEP, n_pts=npts)
         tracks = {}
         for b, nm in enumerate(NAMES):
@@ -63,9 +66,11 @@ def main():
                               status=int(res["status"][b]), iters=int(res["iters"][b]),
                               pg_norm=float(res["pg_norm"][b]),
                               max_move_m=float((res["alpha"][b, :n[b]] - al[b, :n[b]]).abs().max()),
-                              metric_fallbacks=None if ell is None else int(res["metric_fallbacks"][b]),
+                              metric_fallbacks=(int(res["metric_fallbacks"][b]) if "metric_fallbacks" in res
+                                                else None),
+                              kappa_lin_max=float(res["kappa_lin_max"][b]) if kb is not None else None,
                               max_abs_kappa=float(rl["kappa"][b, :no].abs().max()))
-        runs.append(dict(metric_length=ell, tracks=tracks))
+        runs.append(dict(metric_length=ell, kappa_bound=kb, tracks=tracks))
     line = json.dumps(dict(card=card(), max_iters=args.max_iters, curvlim=CURVLIM, runs=runs))
     print(line)
     if args.out:

@@ -3,11 +3,14 @@ closed tracks, N = 1000, started from their minimum-curvature alpha (kappa_bound
 every STEP m.  CUDA events bracket, per iteration, the line-search trials (create_raceline_batch -> vel_profile_batch),
 the forward of the gradient (create_raceline_diff -> vel_profile_diff) and its backward; the rest of the iteration is
 the optimizer's own step (elementwise work, row sums, the one host read).  With --metric-length l the refinement runs
-in the curvature metric and a fourth part, 'metric', brackets its solve (CurvatureMetric).  Prints one JSON line with
+in the curvature metric and a fourth part, 'metric', brackets its solve (CurvatureMetric); with --kappa-bound kb as well
+the steps stay inside the QP's curvature-limited set and a fifth part, 'projection', brackets the projection QP
+(CurvatureProjection, one per iteration).  Prints one JSON line with
 the card's name and power limit read in the same run, the per-iteration split, and the mean lap time and running tracks
 against iteration.
 
-    python tools/refine_time.py [--batch 2112] [--n 1000] [--max-iters 100] [--metric-length L] [--out FILE]
+    python tools/refine_time.py [--batch 2112] [--n 1000] [--max-iters 100] [--metric-length L] [--kappa-bound KB]
+                                [--out FILE]
 """
 import argparse
 import contextlib
@@ -28,7 +31,7 @@ STEP = 2.0
 GGV = np.array([[0.0, 12.0, 12.0], [90.0, 12.0, 12.0]])
 MACH = np.array([[0.0, 5.3], [40.0, 5.1], [60.0, 2.7], [90.0, 1.5]])
 VEH = dict(v_max=70.0, drag_coeff=0.75, m_veh=1200.0)
-PARTS = ("trial", "forward", "backward", "metric")
+PARTS = ("trial", "forward", "backward", "metric", "projection")
 
 
 class Recorder:
@@ -74,6 +77,7 @@ def main():
     ap.add_argument("--n", type=int, default=1000)
     ap.add_argument("--max-iters", type=int, default=R.MAX_ITERS)
     ap.add_argument("--metric-length", type=float, default=None)
+    ap.add_argument("--kappa-bound", type=float, default=None)
     ap.add_argument("--out", default=None)
     args = ap.parse_args()
     if not torch.cuda.is_available():
@@ -90,7 +94,7 @@ def main():
             obj.timer = rec
         return R.refine_raceline_batch(rt, nv, alpha, 2.0, GGV, MACH, stepsize_interp=STEP, max_iters=max_iters,
                                        objective=obj, callback=None if rec is None else rec.callback,
-                                       metric_length=args.metric_length, **VEH)
+                                       metric_length=args.metric_length, kappa_bound=args.kappa_bound, **VEH)
 
     run(2)                                                    # warm-up: every launch and allocation size once
     torch.cuda.synchronize()
@@ -103,17 +107,22 @@ def main():
     total = e0.elapsed_time(e1)
     sums = {p: float(sum(r[p] for r in rows)) for p in PARTS + ("step", "ms")}
     gain = 1.0 - res["laptime"] / res["laptime_start"]
+    kept = torch.isfinite(res["laptime"])
     out = dict(card=card(), batch=args.batch, n=args.n, max_iters=args.max_iters, metric_length=args.metric_length,
+               kappa_bound=args.kappa_bound,
                total_ms=total,
                iterations=len(rows), per_iteration_ms={k: v / max(len(rows), 1) for k, v in sums.items()},
                step_share=sums["step"] / max(sums["ms"], 1e-30),
                trials_per_iteration=sum(r["trials"] for r in rows) / max(len(rows), 1),
                status={int(k): int(c) for k, c in zip(*torch.unique(res["status"], return_counts=True))},
                iters_median=float(res["iters"].double().median()), evals_median=float(res["evals"].double().median()),
-               laptime_start_mean=float(res["laptime_start"].mean()), laptime_mean=float(res["laptime"].mean()),
+               laptime_start_mean=float(res["laptime_start"][kept].mean()), laptime_mean=float(res["laptime"][kept].mean()),
                metric_fallbacks_median=(float(res["metric_fallbacks"].double().median())
                                         if "metric_fallbacks" in res else None),
-               gain_pct=dict(mean=100.0 * float(gain.mean()), min=100.0 * float(gain.min()), max=100.0 * float(gain.max())),
+               kappa_lin_max=(float(res["kappa_lin_max"][kept].max()) if "kappa_lin_max" in res else None),
+               kappa_max=(float(res["kappa_max"][kept].max()) if "kappa_max" in res else None),
+               gain_pct=dict(mean=100.0 * float(gain[kept].mean()), min=100.0 * float(gain[kept].min()),
+                             max=100.0 * float(gain[kept].max())),
                per_iteration=rows)
     line = json.dumps(out)
     print(line)
