@@ -36,17 +36,49 @@ def _ctype(c: str, decl: str, ret: bool = False):
     return _SCALARS[c]
 
 
+def _declarations(path: str):
+    """(restype, name, [parameter types]) of every declaration `ret mc_name(type name, ...);` in the C header at path."""
+    for ret, name, args in re.findall(r"([\w\s*]+?)\b(mc_\w+)\s*\(([^)]*)\)\s*;", _c_source(path)):
+        yield ret, name, [] if args.strip() in ("", "void") else [re.sub(r"\w+\s*$", "", p) for p in args.split(",")]
+
+
 def header_signatures(path: str) -> dict:
     """name -> (restype, argtypes) of every declaration `ret mc_name(type name, ...);` in the C header at path."""
-    sigs = {}
-    for ret, name, args in re.findall(r"([\w\s*]+?)\b(mc_\w+)\s*\(([^)]*)\)\s*;", _c_source(path)):
-        params = [] if args.strip() in ("", "void") else [re.sub(r"\w+\s*$", "", p) for p in args.split(",")]
-        sigs[name] = (_ctype(ret, name, ret=True), [_ctype(p, name) for p in params])
-    return sigs
+    return {name: (_ctype(ret, name, ret=True), [_ctype(p.replace("MC_OPTIONAL", " "), name) for p in params])
+            for ret, name, params in _declarations(path)}
+
+
+def optional_parameters(path: str) -> dict:
+    """name -> (first, count) of the MC_OPTIONAL parameters of each declaration in the C header at path that has them
+    (one run of consecutive parameters)."""
+    out = {}
+    for _, name, params in _declarations(path):
+        k = [i for i, p in enumerate(params) if re.search(r"\bMC_OPTIONAL\b", p)]
+        if k:
+            if k != list(range(k[0], k[-1] + 1)):
+                raise MinCurvLibError(f"{name}: the MC_OPTIONAL parameters must be consecutive")
+            out[name] = (k[0], len(k))
+    return out
 
 
 _SIGS = header_signatures(_build.HEADER)
+_OPTIONAL = optional_parameters(_build.HEADER)
 EXPORTED_SYMBOLS = tuple(_SIGS)
+
+
+def _with_optional(fn, first: int, count: int):
+    """fn, which may also be called without its parameters [first, first + count): they are then NULL (0 for an int), as
+    the header documents for MC_OPTIONAL parameters, so that a call written for the entry before they were added still
+    binds its arguments to the right parameters."""
+    fill = tuple(0 if t is ctypes.c_int else None for t in fn.argtypes[first:first + count])
+    short = len(fn.argtypes) - count
+
+    def call(*args):
+        if len(args) == short:
+            args = args[:first] + fill + args[first:]
+        return fn(*args)
+    call.__name__, call.argtypes, call.restype = fn.__name__, fn.argtypes, fn.restype
+    return call
 
 
 def slab_mirror():
@@ -85,6 +117,8 @@ def load(build_if_missing: bool = True):
         fn = getattr(lib, name)
         fn.restype = res
         fn.argtypes = args
+        if name in _OPTIONAL:
+            setattr(lib, name, _with_optional(fn, *_OPTIONAL[name]))
     _LIB = lib
     return lib
 

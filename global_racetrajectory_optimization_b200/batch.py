@@ -159,8 +159,9 @@ def _chunk(B: int, per_item_bytes: int, device) -> int:
 
 
 def _rows(t: Optional[torch.Tensor]):
-    """A per-instance argument of _launch_chunks: rows s:e of t for the chunk of instances s:e (None stays NULL)."""
-    return lambda s, e: None if t is None else t[s:e]
+    """A per-instance argument of _launch_chunks: rows s:e of t for the chunk of instances s:e (anything but a tensor,
+    None for NULL among it, stays as it is)."""
+    return lambda s, e: t[s:e] if isinstance(t, torch.Tensor) else t
 
 
 def _call(entry: str, *args, ws: Optional[torch.Tensor] = None) -> None:
@@ -254,13 +255,14 @@ def _chunk_centre_ids(centre_id, B):
 def _mincurv_launch(entry: str, chunk: int, n_pts, reftrack, normvec, h, kappa_bound, w_scalar, w_batch, f_scale, centre_id,
                     *outputs) -> None:
     """Runs the C-ABI entry mc_mincurv_solve_batch_shared, mc_mincurv_solve_batch_sens or mc_mincurv_adjoint_batch on
-    chunks of at most chunk instances.  The arguments are the entry's own in its order, outputs the per-instance tensors
-    after centre_id; kappa_bound is None for the adjoint, which takes none."""
+    chunks of at most chunk instances.  The arguments are the entry's own in its order, outputs the arguments after
+    centre_id: a tensor is split by instances, a callable of (s, e) gives the argument of the chunk s:e, anything else
+    is passed as it is; kappa_bound is None for the adjoint, which takes none."""
     B, n_max = h.shape
     ws = _workspace("mincurv", _lib.load().mc_mincurv_workspace_bytes(chunk, n_max), h.device)
     kb = () if kappa_bound is None else (kappa_bound,)
     _launch_chunks(entry, B, chunk, ws, n_max, *map(_rows, (n_pts, reftrack, normvec, h)), *kb, w_scalar, _rows(w_batch),
-                   f_scale, _chunk_centre_ids(centre_id, B), *map(_rows, outputs))
+                   f_scale, _chunk_centre_ids(centre_id, B), *(o if callable(o) else _rows(o) for o in outputs))
 
 
 def _wanted(B: int, *grads, device=None) -> torch.Tensor:
@@ -287,15 +289,19 @@ class _MinCurvDiff(torch.autograd.Function):
     """alpha of the min-curvature QP as a function of the widths; see opt_min_curv_diff."""
 
     @staticmethod
-    def forward(ctx, widths, w_veh_t, centre, normvec, h, kappa_bound, w_scalar, n_pts, centre_id, chunk, f_scale, strict):
+    def forward(ctx, widths, w_veh_t, centre, normvec, h, kappa_bound, w_scalar, n_pts, centre_id, chunk, f_scale, strict,
+                curvature_rows):
         B, n_max, _ = centre.shape
+        dev = centre.device
         reftrack = torch.cat((centre, widths), dim=2).contiguous()
-        alpha, cerr, kmax, status, iters = _mincurv_results(B, n_max, centre.device).values()
-        sens = torch.empty((B, 2, n_max), dtype=torch.float64, device=centre.device)
-        grad_status = torch.empty((B,), dtype=torch.int32, device=centre.device)
+        alpha, cerr, kmax, status, iters = _mincurv_results(B, n_max, dev).values()
+        sens = torch.empty((B, 2, n_max), dtype=torch.float64, device=dev)
+        grad_status = torch.empty((B,), dtype=torch.int32, device=dev)
+        sens_rows = torch.empty((B, n_max), dtype=torch.float64, device=dev) if curvature_rows else None
+        n_rows = torch.empty((B,), dtype=torch.int32, device=dev) if curvature_rows else None
         _mincurv_launch("mc_mincurv_solve_batch_sens", chunk, n_pts, reftrack, normvec, h, kappa_bound, w_scalar, w_veh_t,
-                        f_scale, centre_id, alpha, cerr, kmax, status, iters, sens, grad_status)
-        ctx.save_for_backward(widths, centre, normvec, h, w_veh_t, n_pts, centre_id, sens, grad_status)
+                        f_scale, centre_id, alpha, cerr, kmax, status, iters, sens, grad_status, sens_rows, n_rows)
+        ctx.save_for_backward(widths, centre, normvec, h, w_veh_t, n_pts, centre_id, sens, grad_status, sens_rows, n_rows)
         ctx.w_scalar, ctx.chunk, ctx.f_scale, ctx.strict = w_scalar, chunk, f_scale, strict
         ctx.mark_non_differentiable(cerr, kmax, status, iters, grad_status)
         return alpha, cerr, kmax, status, iters, grad_status
@@ -303,7 +309,7 @@ class _MinCurvDiff(torch.autograd.Function):
     @staticmethod
     @torch.autograd.function.once_differentiable
     def backward(ctx, grad_alpha, *_unused):
-        widths, centre, normvec, h, w_veh_t, n_pts, centre_id, sens, grad_status = ctx.saved_tensors
+        widths, centre, normvec, h, w_veh_t, n_pts, centre_id, sens, grad_status, sens_rows, n_rows = ctx.saved_tensors
         B, n_max, _ = centre.shape
         dev = centre.device
         grad_alpha = grad_alpha.to(dtype=torch.float64).contiguous()
@@ -315,17 +321,25 @@ class _MinCurvDiff(torch.autograd.Function):
         gwr = torch.empty((B, n_max), dtype=torch.float64, device=dev)
         gwl = torch.empty((B, n_max), dtype=torch.float64, device=dev)
         gwv = torch.empty((B,), dtype=torch.float64, device=dev)
-        _mincurv_launch("mc_mincurv_adjoint_batch", ctx.chunk, n_pts, reftrack, normvec, h, None, ctx.w_scalar, w_veh_t,
-                        ctx.f_scale, centre_id, sens, gs, grad_alpha, gwr, gwl, gwv)
+        chunk, rows = ctx.chunk, (None, None, None, 0)
+        if sens_rows is not None:
+            # the Schur complement of the strong rows: cap^2 doubles per instance of a chunk, next to its slab
+            cap = int(n_rows.max())
+            per_item = _lib.load().mc_mincurv_workspace_bytes(1, n_max) + 8 * cap * cap
+            chunk = min(chunk, _chunk(B, per_item, dev))
+            schur = torch.empty((chunk, max(cap * cap, 1)), dtype=torch.float64, device=dev)
+            rows = (sens_rows, n_rows, lambda s, e: schur, cap)
+        _mincurv_launch("mc_mincurv_adjoint_batch", chunk, n_pts, reftrack, normvec, h, None, ctx.w_scalar, w_veh_t,
+                        ctx.f_scale, centre_id, sens, gs, grad_alpha, gwr, gwl, gwv, *rows)
         _refuse(ctx.strict, wanted, gs, who, "whose adjoint factorisation broke down")
-        return (torch.stack((gwr, gwl), dim=2), gwv if w_veh_t is not None else None) + (None,) * 10
+        return (torch.stack((gwr, gwl), dim=2), gwv if w_veh_t is not None else None) + (None,) * 11
 
 
 @_device_guard
 def opt_min_curv_diff(centre: torch.Tensor, widths: torch.Tensor, normvec: torch.Tensor, h: torch.Tensor, kappa_bound: float,
                       w_veh: Union[float, torch.Tensor], n_pts: Optional[torch.Tensor] = None,
                       centre_id: Optional[torch.Tensor] = None, max_chunk: Optional[int] = None,
-                      f_scale: Optional[float] = None, strict: bool = True) -> dict:
+                      f_scale: Optional[float] = None, strict: bool = True, curvature_rows: bool = False) -> dict:
     """opt_min_curv_batch with alpha differentiable with respect to the track widths and the vehicle width (autograd).
 
     centre [B, n_max, 2] (x, y) and widths [B, n_max, 2] (w_tr_right, w_tr_left) make up the reftrack of
@@ -337,7 +351,12 @@ def opt_min_curv_diff(centre: torch.Tensor, widths: torch.Tensor, normvec: torch
     grad_status: 0 = the gradient is computed; 4 = the curvature rows were active (solved by the curvature-row phase),
     not supported; otherwise the solve's status (1, 2, 3, -1).  strict=True: backward raises if an instance with a
     nonzero upstream gradient has grad_status != 0 (or its adjoint factorisation breaks down); strict=False: such
-    instances get zero gradients."""
+    instances get zero gradients.
+    curvature_rows=True: the instances the curvature-row phase solved are differentiated too, at that phase's final
+    iterate (DESIGN.md section 3.10, curvature rows): the forward exports 8 more bytes per point, grad_status is the final
+    solve status (4 only where the rows stay violated), and the backward reads the largest count of strongly active rows
+    once from the device to size their Schur complements.  The forward's values are those of curvature_rows=False bit
+    for bit, and so are the gradients of the instances the box phase solved."""
     _require_cuda()
     for t, name in ((centre, "centre"), (normvec, "normvec"), (h, "h")):
         if isinstance(t, torch.Tensor) and t.requires_grad:
@@ -347,7 +366,7 @@ def opt_min_curv_diff(centre: torch.Tensor, widths: torch.Tensor, normvec: torch
                         n_pts, w_veh, centre_id, max_chunk, f_scale)
     alpha, cerr, kmax, status, iters, grad_status = _MinCurvDiff.apply(
         a.widths, a.w_batch, a.centre, a.normvec, a.h, float(kappa_bound), a.w_scalar, a.n_pts, a.centre_id, a.chunk,
-        a.f_scale, bool(strict))
+        a.f_scale, bool(strict), bool(curvature_rows))
     return dict(alpha=alpha, curv_error_max=cerr, kappa_lin_max=kmax, status=status, iters=iters, grad_status=grad_status)
 
 

@@ -87,6 +87,41 @@ mincurv_sens_export_kernel(int n_max, const int32_t *__restrict__ n_pts, double 
     if (threadIdx.x == 0) grad_status[b] = st;
 }
 
+// Second export for the width sensitivities with the curvature rows (K2d', mincurv_ipm.cu), run after the curvature-row
+// phase and its finalize pass.  For the instances that phase re-solved (grad_status 4 from the first export) and solved
+// (status 0): its final box ratios into sens (over the first export's zeros), the row weights
+// sens_rows[b][i] = l3 / s3 + l4 / s4 and n_rows[b] = the count of strong rows (weight > 1).  grad_status[b] becomes
+// the final status.  Everything else keeps what the first export wrote, with zero row weights and n_rows 0.
+__global__ void __launch_bounds__(256)
+mincurv_sens_rows_export_kernel(int n_max, const int32_t *__restrict__ n_pts, double *__restrict__ ws, Layout L,
+                                const int32_t *__restrict__ status, double *__restrict__ sens, double *__restrict__ sens_rows,
+                                int32_t *__restrict__ n_rows, int32_t *__restrict__ grad_status) {
+    const int b = blockIdx.x;
+    __shared__ double red[32];
+    const int gs = grad_status[b], st = status[b];
+    const bool rows = gs == 4 && st == 0;
+    const int n = rows ? (n_pts ? n_pts[b] : n_max) : 0;
+    double *slab = ws + (size_t)b * L.stride;
+    const double *LU = vec(slab, L, V_LU), *LL = vec(slab, L, V_LL), *SU = vec(slab, L, V_SU), *SL = vec(slab, L, V_SL);
+    const double *S3 = vec(slab, L, V_S3), *S4 = vec(slab, L, V_S4), *L3 = vec(slab, L, V_L3), *L4 = vec(slab, L, V_L4);
+    double *du = sens + (size_t)b * 2 * n_max, *dl = du + n_max, *wr = sens_rows + (size_t)b * n_max;
+    double strong = 0.0;
+    for (int i = threadIdx.x; i < n_max; i += blockDim.x) {
+        const double w = (i < n) ? L3[i] / S3[i] + L4[i] / S4[i] : 0.0;
+        wr[i] = w;
+        strong += (w > 1.0) ? 1.0 : 0.0;
+        if (gs == 4) {
+            du[i] = (i < n) ? LU[i] / SU[i] : 0.0;
+            dl[i] = (i < n) ? LL[i] / SL[i] : 0.0;
+        }
+    }
+    strong = block_reduce<0>(strong, red);
+    if (threadIdx.x == 0) {
+        n_rows[b] = (int32_t)strong;
+        if (gs == 4) grad_status[b] = st;
+    }
+}
+
 // The projection QP of mc_mincurv_solve_batch_ex, run after the assembly: Hessian H + mu I and linear term
 // c = mu q - (H + mu I) x.  mu goes onto the diagonal of the instance's band of H, which the box phase reads, and c
 // replaces f in V_F; H x is formed in operator form (E^T (E x)).  Only instances the assembly left at status 0.
@@ -172,12 +207,14 @@ int mc_mincurv_solve_batch_ex(int B, int n_max, const int32_t *n_pts, const doub
                                          alpha, curv_error_max, kappa_lin_max, status, iters, workspace, workspace_bytes, stream);
 }
 
-// setup -> pdip -> finalize -> (export of the sensitivity data) -> kappa -> finalize; sens == NULL: no export.  Every
-// argument is checked before the first launch: the pointers here, f_scale and the sizes by the setup stage.
+// setup -> pdip -> finalize -> (export of the sensitivity data) -> kappa -> finalize -> (export of the curvature-row phase's
+// sensitivity data); sens == NULL: no export, sens_rows == NULL: no second export.  Every argument is checked before the
+// first launch: the pointers here, f_scale and the sizes by the setup stage.
 static int mincurv_solve(int B, int n_max, const int32_t *n_pts, const double *reftrack, const double *normvec, const double *h,
                          double kappa_bound, double w_veh, const double *w_veh_batch, double f_scale, const int32_t *centre_id,
                          double *alpha, double *curv_error_max, double *kappa_lin_max, int32_t *status, int32_t *iters,
-                         double *sens, int32_t *grad_status, void *workspace, size_t workspace_bytes, void *stream) {
+                         double *sens, int32_t *grad_status, double *sens_rows, int32_t *n_rows, void *workspace,
+                         size_t workspace_bytes, void *stream) {
     if (!reftrack || !normvec || !h || !alpha || !curv_error_max || !status)
         return bad("mc_mincurv_solve_batch: NULL argument");
     int rc = mc_mincurv_setup_batch_shared(B, n_max, n_pts, reftrack, normvec, h, w_veh, w_veh_batch, f_scale, centre_id, status,
@@ -198,8 +235,12 @@ static int mincurv_solve(int B, int n_max, const int32_t *n_pts, const double *r
     // instances whose box-only optimum violates the curvature rows (status 4) are re-solved with the rows
     rc = mc_mincurv_kappa_batch(B, n_max, n_pts, kappa_bound, alpha, status, iters, workspace, workspace_bytes, stream);
     if (rc) return rc;
-    return mc_mincurv_finalize_batch(B, n_max, n_pts, alpha, kappa_bound, curv_error_max, kappa_lin_max, status, workspace,
-                                     workspace_bytes, stream);
+    rc = mc_mincurv_finalize_batch(B, n_max, n_pts, alpha, kappa_bound, curv_error_max, kappa_lin_max, status, workspace,
+                                   workspace_bytes, stream);
+    if (rc || !sens_rows) return rc;
+    mc::mincurv_sens_rows_export_kernel<<<B, 256, 0, (cudaStream_t)stream>>>(n_max, n_pts, (double *)workspace, mc::make_layout(n_max),
+                                                                             status, sens, sens_rows, n_rows, grad_status);
+    return check_cuda("mincurv_sens_rows_export_kernel");
 }
 
 int mc_mincurv_solve_batch_shared(int B, int n_max, const int32_t *n_pts, const double *reftrack, const double *normvec,
@@ -207,17 +248,20 @@ int mc_mincurv_solve_batch_shared(int B, int n_max, const int32_t *n_pts, const 
                                   const int32_t *centre_id, double *alpha, double *curv_error_max, double *kappa_lin_max,
                                   int32_t *status, int32_t *iters, void *workspace, size_t workspace_bytes, void *stream) {
     return mincurv_solve(B, n_max, n_pts, reftrack, normvec, h, kappa_bound, w_veh, w_veh_batch, f_scale, centre_id, alpha,
-                         curv_error_max, kappa_lin_max, status, iters, nullptr, nullptr, workspace, workspace_bytes, stream);
+                         curv_error_max, kappa_lin_max, status, iters, nullptr, nullptr, nullptr, nullptr, workspace,
+                         workspace_bytes, stream);
 }
 
 int mc_mincurv_solve_batch_sens(int B, int n_max, const int32_t *n_pts, const double *reftrack, const double *normvec,
                                 const double *h, double kappa_bound, double w_veh, const double *w_veh_batch, double f_scale,
                                 const int32_t *centre_id, double *alpha, double *curv_error_max, double *kappa_lin_max,
-                                int32_t *status, int32_t *iters, double *sens, int32_t *grad_status, void *workspace,
-                                size_t workspace_bytes, void *stream) {
+                                int32_t *status, int32_t *iters, double *sens, int32_t *grad_status, double *sens_rows,
+                                int32_t *n_rows, void *workspace, size_t workspace_bytes, void *stream) {
     if (!sens || !grad_status) return bad("mc_mincurv_solve_batch_sens: NULL argument");
+    if (!sens_rows != !n_rows) return bad("mc_mincurv_solve_batch_sens: sens_rows and n_rows go together");
     return mincurv_solve(B, n_max, n_pts, reftrack, normvec, h, kappa_bound, w_veh, w_veh_batch, f_scale, centre_id, alpha,
-                         curv_error_max, kappa_lin_max, status, iters, sens, grad_status, workspace, workspace_bytes, stream);
+                         curv_error_max, kappa_lin_max, status, iters, sens, grad_status, sens_rows, n_rows, workspace,
+                         workspace_bytes, stream);
 }
 
 }  // extern "C"

@@ -1608,6 +1608,34 @@ debug_factor_solve_kernel(int B, int n_max, const int32_t *__restrict__ n_pts, d
     }
 }
 
+// the width gradients of one instance (K2d, K2d') from v = (H + D + ...)^-1 g (X) and its box ratios DU, DL
+__device__ __forceinline__ void width_grads(IpShared &sh, int n, int n_max, const double *__restrict__ rt, double wv,
+                                            const double *__restrict__ DU, const double *__restrict__ DL,
+                                            const double *__restrict__ X, double *__restrict__ gwr, double *__restrict__ gwl,
+                                            double *__restrict__ gwv) {
+    double gv = 0.0;
+    for (int i = threadIdx.x; i < n_max; i += IP_THREADS) {
+        double gr = 0.0, gl = 0.0;
+        if (i < n) {
+            const double v = X[i], gu = DU[i] * v, glb = DL[i] * v;
+            const double2 ww = *reinterpret_cast<const double2 *>(rt + (size_t)i * 4 + 2);
+            const double ub = ww.x - 0.5 * wv, lb = -(ww.y - 0.5 * wv);      // (the expressions of the setup)
+            if (ub - lb < 2.0 * FIX_EPS) {
+                gr = 0.5 * (gu + glb);
+                gl = -gr;
+            } else {
+                gr = gu;
+                gl = -glb;
+                gv += 0.5 * (glb - gu);
+            }
+        }
+        gwr[i] = gr;
+        gwl[i] = gl;
+    }
+    gv = block_reduce<0>(gv, sh.red);
+    if (threadIdx.x == 0) *gwv = gv;
+}
+
 // ================================================================================================
 // K2d -- width sensitivities of the box-only QP (DESIGN.md section 3.10): implicit differentiation of its KKT conditions
 // at the interior-point solution.  With the final ratios d_u = lu / su, d_l = ll / sl of the forward solve (`sens`,
@@ -1645,33 +1673,162 @@ mincurv_adjoint_kernel(int B, int n_max, const int32_t *__restrict__ n_pts, cons
             tick += factor_units(n);
             if (ok) {
                 solve(sh, slab, L, n, RHS, DX, true);
-                const double wv = w_veh_batch ? w_veh_batch[b] : w_veh;
-                const double *rt = reftrack + (size_t)b * n_max * 4;
-                double gv = 0.0;
-                for (int i = threadIdx.x; i < n_max; i += IP_THREADS) {
-                    double gr = 0.0, gl = 0.0;
-                    if (i < n) {
-                        const double v = DX[i], gu = DU[i] * v, glb = DL[i] * v;
-                        const double2 ww = *reinterpret_cast<const double2 *>(rt + (size_t)i * 4 + 2);
-                        const double ub = ww.x - 0.5 * wv, lb = -(ww.y - 0.5 * wv);      // (the expressions of the setup)
-                        if (ub - lb < 2.0 * FIX_EPS) {
-                            gr = 0.5 * (gu + glb);
-                            gl = -gr;
-                        } else {
-                            gr = gu;
-                            gl = -glb;
-                            gv += 0.5 * (glb - gu);
-                        }
-                    }
-                    gwr[i] = gr;
-                    gwl[i] = gl;
-                }
-                gv = block_reduce<0>(gv, sh.red);
-                if (threadIdx.x == 0) grad_w_veh[b] = gv;
+                width_grads(sh, n, n_max, reftrack + (size_t)b * n_max * 4, w_veh_batch ? w_veh_batch[b] : w_veh, DU, DL, DX,
+                            gwr, gwl, grad_w_veh + b);
                 continue;
             }
             if (threadIdx.x == 0) grad_status[b] = 3;
         }
+        for (int i = threadIdx.x; i < n_max; i += IP_THREADS) { gwr[i] = 0.0; gwl[i] = 0.0; }
+        if (threadIdx.x == 0) grad_w_veh[b] = 0.0;
+    }
+}
+
+// ================================================================================================
+// K2d' -- width sensitivities with the curvature rows (DESIGN.md section 3.10): the same iterate-based derivative at the
+// final iterate of the curvature-row phase, whose KKT linearisation adds E^T W E, W = l3 / s3 + l4 / s4 (`sens_rows`,
+// mincurv_sens_rows_export_kernel):
+//   (H + D + E^T W E) v = g,   dL/dub = d_u v,  dL/dlb = d_l v
+// W is split at 1, the weight of the objective's own rows in H = E^T I E.  The weak rows (W <= 1) stay in the band,
+// K = E^T (I + W_weak) E + D (assembled into the instance's own slab, as the row phase does); the m strong rows S
+// (W > 1: towards 1e12 at the row phase's end, where the band truncation is no longer SPD) are carried exactly by
+// Woodbury:
+//   Sigma = W_S^-1 + E_S K^-1 E_S^T (m x m, SPD, column j from one solve against E_S^T e_j; dense Cholesky in `schur`,
+//           n_rows_cap^2 doubles per instance),   v = K^-1 g - K^-1 E_S^T Sigma^-1 E_S K^-1 g
+// One factorisation, m + 2 solves, m + 1 applications each of E and E^T.  Instances with no row weight (solved by the
+// box phase, or not solved) take the arithmetic of mincurv_adjoint_kernel.  pass 0 runs those, pass 1 the others: a
+// row instance overwrites its own band of H, which followers of a shared centre line read in pass 0.  A non-positive
+// pivot in K or in Sigma, or more strong rows than n_rows_cap, set grad_status 3 (zero gradients).
+// ================================================================================================
+__global__ void __launch_bounds__(IP_THREADS, 8)
+mincurv_adjoint_rows_kernel(int B, int n_max, const int32_t *__restrict__ n_pts, const double *__restrict__ reftrack,
+                            double w_veh, const double *__restrict__ w_veh_batch, double *__restrict__ ws, Layout L,
+                            const double *__restrict__ sens, const double *__restrict__ sens_rows,
+                            const int32_t *__restrict__ n_rows, double *schur, int n_rows_cap, int pass,
+                            const double *__restrict__ grad_alpha, int32_t *__restrict__ grad_status,
+                            double *__restrict__ grad_w_right, double *__restrict__ grad_w_left, double *__restrict__ grad_w_veh,
+                            int *__restrict__ work_counter) {
+    IpShared &sh = ip_init_shared();
+    unsigned tick = 0;
+    for (int b; (b = next_instance(sh, work_counter)) < B;) {
+        const int n = n_pts ? n_pts[b] : n_max;
+        const double *__restrict__ WR = sens_rows + (size_t)b * n_max;
+        double wmax = 0.0;
+        for (int i = threadIdx.x; i < n_max; i += IP_THREADS) wmax = fmax(wmax, WR[i]);
+        if ((block_reduce<1>(wmax, sh.red) > 0.0) != (pass == 1)) continue;      // (every row weight is > 0 where the row phase ran)
+        double *gwr = grad_w_right + (size_t)b * n_max, *gwl = grad_w_left + (size_t)b * n_max;
+        const double *rt = reftrack + (size_t)b * n_max * 4;
+        const double wv = w_veh_batch ? w_veh_batch[b] : w_veh;
+        const int m = n_rows[b];
+        bool ok = grad_status[b] == 0 && m <= n_rows_cap;
+        if (ok) {
+            double *slab = ws + (size_t)b * L.stride;
+            const double *__restrict__ DU = sens + (size_t)b * 2 * n_max, *__restrict__ DL = DU + n_max;
+            const double *__restrict__ GA = grad_alpha + (size_t)b * n_max;
+            double *RHS = vec(slab, L, V_RHS), *X = vec(slab, L, V_DX), *DD = vec(slab, L, V_DD), *WK = vec(slab, L, V_WK);
+            if (threadIdx.x == 0) sh.flag = 0;
+            if (pass == 0) {
+                const double *HB = ws + (size_t)*band_owner(slab, L) * L.stride + L.o_hb;      // (shared centre lines: the owner's)
+                for (int i = threadIdx.x; i < L.np; i += IP_THREADS) {
+                    if (i < n) DD[i] = DU[i] + DL[i];
+                    RHS[i] = (i < n) ? GA[i] : 0.0;
+                }
+                ok = factor(sh, slab, L, n, HB, RHS, tick);
+                tick += factor_units(n);
+                if (ok) solve(sh, slab, L, n, RHS, X, true);
+            } else {
+                double *R = vec(slab, L, V_T4K), *Y = vec(slab, L, V_RD), *Z = vec(slab, L, V_T3K), *EZ = vec(slab, L, V_EDX);
+                double *U = vec(slab, L, V_VV);
+                int *S = reinterpret_cast<int *>(vec(slab, L, V_ISU));      // the strong rows, ascending
+                double *t0 = vec(slab, L, V_T0), *t1 = vec(slab, L, V_T1), *t2 = vec(slab, L, V_T2), *t3 = vec(slab, L, V_T3);
+                double *t4 = vec(slab, L, V_T4), *t5 = vec(slab, L, V_T5);
+                double *Sg = schur + (size_t)b * n_rows_cap * n_rows_cap;      // Sigma, row-major, lower triangle used
+                for (int i = threadIdx.x; i < L.np; i += IP_THREADS) {
+                    if (i < n) {
+                        DD[i] = DU[i] + DL[i];
+                        WK[i] = (WR[i] <= 1.0) ? WR[i] : 0.0;
+                    }
+                    RHS[i] = (i < n) ? GA[i] : 0.0;
+                    R[i] = 0.0;
+                }
+                if (threadIdx.x < 32) {
+                    const int lane = threadIdx.x;
+                    int cnt = 0;
+                    for (int base = 0; base < n; base += 32) {
+                        const bool st = base + lane < n && WR[base + lane] > 1.0;
+                        const unsigned bal = __ballot_sync(FULL, st);
+                        if (st) S[cnt + __popc(bal & ((1u << lane) - 1u))] = base + lane;
+                        cnt += __popc(bal);
+                    }
+                }
+                __syncthreads();
+                assemble_hband(slab, L, n, WK, sh.u.win);
+                __syncthreads();
+                ok = factor(sh, slab, L, n, slab + L.o_hb, RHS, tick);      // K, with the forward half of K^-1 g
+                tick += factor_units(n);
+                if (ok && m > 0) {
+                    solve(sh, slab, L, n, RHS, X, true);
+                    for (int j = 0; j < m; ++j) {      // column j of Sigma: E_S K^-1 E^T e_{S_j} + e_j / W_{S_j}
+                        if (threadIdx.x == 0) R[S[j]] = 1.0;
+                        __syncthreads();
+                        apply_Et(slab, L, n, R, Y, t0, t1, t2, t3, t4, t5);
+                        if (threadIdx.x == 0) R[S[j]] = 0.0;
+                        solve(sh, slab, L, n, Y, Z, false);
+                        apply_E(slab, L, n, Z, EZ, t0, t1, t2, t3, t4, t5);
+                        for (int k = j + threadIdx.x; k < m; k += IP_THREADS)
+                            Sg[(size_t)k * n_rows_cap + j] = EZ[S[k]] + ((k == j) ? 1.0 / WR[S[j]] : 0.0);
+                    }
+                    apply_E(slab, L, n, X, EZ, t0, t1, t2, t3, t4, t5);      // u = E_S K^-1 g
+                    for (int k = threadIdx.x; k < m; k += IP_THREADS) U[k] = EZ[S[k]];
+                    // Sigma = C C^T in place (right-looking, lower triangle)
+                    for (int k = 0; k < m && ok; ++k) {
+                        __syncthreads();
+                        const double d = Sg[(size_t)k * n_rows_cap + k];
+                        if (!(d > 0.0)) { ok = false; break; }
+                        const double c = sqrt(d), ic = 1.0 / c;
+                        __syncthreads();
+                        if (threadIdx.x == 0) Sg[(size_t)k * n_rows_cap + k] = c;
+                        for (int i = k + 1 + threadIdx.x; i < m; i += IP_THREADS) Sg[(size_t)i * n_rows_cap + k] *= ic;
+                        __syncthreads();
+                        const int r = m - k - 1;
+                        for (int e = threadIdx.x; e < r * r; e += IP_THREADS) {
+                            const int i = k + 1 + e / r, jj = k + 1 + e % r;
+                            if (jj <= i) Sg[(size_t)i * n_rows_cap + jj] -= Sg[(size_t)i * n_rows_cap + k] * Sg[(size_t)jj * n_rows_cap + k];
+                        }
+                    }
+                    if (ok) {
+                        for (int k = 0; k < m; ++k) {          // C y = u
+                            __syncthreads();
+                            if (threadIdx.x == 0) U[k] /= Sg[(size_t)k * n_rows_cap + k];
+                            __syncthreads();
+                            const double yk = U[k];
+                            for (int i = k + 1 + threadIdx.x; i < m; i += IP_THREADS) U[i] -= Sg[(size_t)i * n_rows_cap + k] * yk;
+                        }
+                        for (int k = m - 1; k >= 0; --k) {     // C^T z = y
+                            __syncthreads();
+                            if (threadIdx.x == 0) U[k] /= Sg[(size_t)k * n_rows_cap + k];
+                            __syncthreads();
+                            const double zk = U[k];
+                            for (int i = threadIdx.x; i < k; i += IP_THREADS) U[i] -= Sg[(size_t)k * n_rows_cap + i] * zk;
+                        }
+                        __syncthreads();
+                        for (int k = threadIdx.x; k < m; k += IP_THREADS) R[S[k]] = U[k];
+                        __syncthreads();
+                        apply_Et(slab, L, n, R, Y, t0, t1, t2, t3, t4, t5);      // v = K^-1 g - K^-1 E_S^T z
+                        solve(sh, slab, L, n, Y, Z, false);
+                        for (int i = threadIdx.x; i < n; i += IP_THREADS) X[i] -= Z[i];
+                        __syncthreads();
+                    }
+                } else if (ok) {
+                    solve(sh, slab, L, n, RHS, X, true);
+                }
+            }
+            if (ok) {
+                width_grads(sh, n, n_max, rt, wv, DU, DL, X, gwr, gwl, grad_w_veh + b);
+                continue;
+            }
+        }
+        if (threadIdx.x == 0 && grad_status[b] == 0) grad_status[b] = 3;
         for (int i = threadIdx.x; i < n_max; i += IP_THREADS) { gwr[i] = 0.0; gwl[i] = 0.0; }
         if (threadIdx.x == 0) grad_w_veh[b] = 0.0;
     }
@@ -1759,14 +1916,31 @@ int mc_mincurv_kappa_batch(int B, int n_max, const int32_t *n_pts, double kappa_
 int mc_mincurv_adjoint_batch(int B, int n_max, const int32_t *n_pts, const double *reftrack, const double *normvec,
                              const double *h, double w_veh, const double *w_veh_batch, double f_scale, const int32_t *centre_id,
                              const double *sens, int32_t *grad_status, const double *grad_alpha, double *grad_w_right,
-                             double *grad_w_left, double *grad_w_veh, void *workspace, size_t workspace_bytes, void *stream) {
+                             double *grad_w_left, double *grad_w_veh, const double *sens_rows, const int32_t *n_rows,
+                             double *schur, int n_rows_cap, void *workspace, size_t workspace_bytes, void *stream) {
     if (!sens || !grad_status || !grad_alpha || !grad_w_right || !grad_w_left || !grad_w_veh)
         return bad("mc_mincurv_adjoint_batch: NULL argument");
+    if (sens_rows && (!n_rows || !schur)) return bad("mc_mincurv_adjoint_batch: sens_rows needs n_rows and schur");
+    if (sens_rows && n_rows_cap < 0) return bad("mc_mincurv_adjoint_batch: n_rows_cap < 0");
     // the band of H and the bounds are rebuilt in the slabs; the assembly's status words (the forward pass's, recorded in
     // grad_status) go to grad_w_right, which the adjoint kernel overwrites
     int rc = mc_mincurv_setup_batch_shared(B, n_max, n_pts, reftrack, normvec, h, w_veh, w_veh_batch, f_scale, centre_id,
                                            reinterpret_cast<int32_t *>(grad_w_right), workspace, workspace_bytes, stream);
     if (rc) return rc;
+    if (sens_rows) {
+        // pass 0: the instances without row weights (reading their owner's band); pass 1: the curvature-row instances
+        const mc::SolverGrid g = mc::solver_grid(B, n_max, workspace, mc::ctas_per_sm(mc::mincurv_adjoint_rows_kernel));
+        for (int pass = 0; pass < 2; ++pass) {
+            if (mc::launch_solver(mc::mincurv_adjoint_rows_kernel, g.grid, g.counter, (cudaStream_t)stream, B, n_max, n_pts,
+                                  reftrack, w_veh, w_veh_batch, (double *)workspace, mc::make_layout(n_max), sens, sens_rows,
+                                  n_rows, schur, n_rows_cap, pass, grad_alpha, grad_status, grad_w_right, grad_w_left,
+                                  grad_w_veh, g.counter) != 0) {
+                snprintf(mc::g_err, sizeof(mc::g_err), "mincurv_adjoint_rows_kernel: cudaFuncSetAttribute failed");
+                return MC_ECUDA;
+            }
+        }
+        return check_cuda("mincurv_adjoint_rows_kernel");
+    }
     const mc::SolverGrid g = mc::solver_grid(B, n_max, workspace, mc::ctas_per_sm(mc::mincurv_adjoint_kernel));
     if (mc::launch_solver(mc::mincurv_adjoint_kernel, g.grid, g.counter, (cudaStream_t)stream, B, n_max, n_pts, reftrack, w_veh,
                           w_veh_batch, (double *)workspace, mc::make_layout(n_max), sens, grad_alpha, grad_status, grad_w_right,

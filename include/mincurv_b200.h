@@ -36,6 +36,11 @@ extern "C" {
 #define MC_ECUDA (-2)
 #define MC_EWORKSPACE (-3)
 
+/* MC_OPTIONAL marks parameters added to an entry point after its first release.  They are NULL-able (an int among them
+ * may be 0), and NULL gives the entry's earlier behaviour exactly.  The package's ctypes binding lets a call leave them
+ * out altogether, so code written for the earlier signature keeps working; C callers pass NULL / 0. */
+#define MC_OPTIONAL
+
 #define MC_STATUS_OK 0
 #define MC_STATUS_TOO_NARROW 1
 #define MC_STATUS_MAXITER 2
@@ -153,11 +158,15 @@ int mc_mincurv_finalize_batch(int B, int n_max, const int32_t *n_pts, const doub
 
 /* Width sensitivities of this QP: alpha differentiated with respect to w_tr_right, w_tr_left and w_veh by one more
  * factorisation per instance (batch.opt_min_curv_diff; DESIGN.md section 3.10 has the derivation).
- * Only instances solved by the box-only phase have a gradient.  grad_status[b] (int32):
- *   0  solved by the box-only phase (status 0): gradients are computed
- *   4  the box-only optimum violated the curvature rows and the curvature-row phase re-solved it: not supported
- *   1, 2, 3, -1  the forward solve's status (infeasible, iteration cap, breakdown, unsupported size)
- *   3  also: a non-positive pivot in the adjoint factorisation
+ * Without the curvature-row export (sens_rows NULL) only instances solved by the box-only phase have a gradient.
+ * grad_status[b] (int32):
+ *   0  solved by the box-only phase (status 0), or with sens_rows by the curvature-row phase: gradients are computed
+ *   4  without sens_rows: the box-only optimum violated the curvature rows and the curvature-row phase re-solved it:
+ *      not supported
+ *   1, 2, 3, -1  the forward solve's status (infeasible, iteration cap, breakdown, unsupported size; with sens_rows
+ *      also 4: rows still violated after the curvature-row phase)
+ *   3  also: a non-positive pivot in the adjoint factorisation (or in its Schur complement of the strong rows), or more
+ *      strong rows than n_rows_cap
  * Every unsupported instance gets zero gradients.  The widths are differentiated, the centre line, h, f_scale and
  * kappa_bound are constants.
  *
@@ -166,6 +175,12 @@ int mc_mincurv_finalize_batch(int B, int n_max, const int32_t *n_pts, const doub
  *   sens        [B][2][n_max] : lu / su and ll / sl, the box phase's final multiplier-to-slack ratios of the upper and
  *                               lower bounds (zero beyond n_pts[b] and for grad_status != 0)
  *   grad_status [B]           : see above; recorded after the box phase, before the curvature-row phase
+ * and with sens_rows and n_rows (both or neither; NULL: the call above), 8 more bytes per point, from the final
+ * iterate of the curvature-row phase for the instances it solved:
+ *   sens        [B][2][n_max] : that phase's final lu / su and ll / sl
+ *   sens_rows   [B][n_max]    : the row weights l3 / s3 + l4 / s4 (zero for the other instances and beyond n_pts[b])
+ *   n_rows      [B] (int32)   : the strong rows (weight > 1), the Schur complement size of the adjoint (0 elsewhere)
+ *   grad_status [B]           : the final solve status
  *
  * mc_mincurv_adjoint_batch: vector-Jacobian product of alpha with respect to the widths: for an upstream gradient
  * grad_alpha [B][n_max] of a loss L,
@@ -174,19 +189,27 @@ int mc_mincurv_finalize_batch(int B, int n_max, const int32_t *n_pts, const doub
  * must be those of the mc_mincurv_solve_batch_sens call that produced sens and grad_status.  The assembly is re-run in
  * the workspace, then one factorisation of H + diag(sens[0] + sens[1]) and one solve per instance; nothing has to
  * survive in the workspace between the two calls.  grad_status is read, and set to 3 where the factorisation breaks
- * down.  grad_w_right also serves as scratch of the assembly's status words before it is written. */
+ * down.  grad_w_right also serves as scratch of the assembly's status words before it is written.
+ * sens_rows, n_rows (NULL: the call above): those of the mc_mincurv_solve_batch_sens call.  An instance with row weights
+ * is differentiated at the curvature-row phase's iterate: one factorisation of H + diag(sens[0] + sens[1]) + E^T W E
+ * with the weak rows (W <= 1) in the band, and the n_rows[b] strong rows through their Schur complement, a dense
+ * n_rows[b]^2 matrix kept in schur [B][n_rows_cap][n_rows_cap] (required with sens_rows); an instance with
+ * n_rows[b] > n_rows_cap gets grad_status 3. */
 int mc_mincurv_solve_batch_sens(int B, int n_max, const int32_t *n_pts,
                                 const double *reftrack, const double *normvec, const double *h,
                                 double kappa_bound, double w_veh, const double *w_veh_batch, double f_scale,
                                 const int32_t *centre_id,
                                 double *alpha, double *curv_error_max, double *kappa_lin_max,
                                 int32_t *status, int32_t *iters, double *sens, int32_t *grad_status,
+                                MC_OPTIONAL double *sens_rows, MC_OPTIONAL int32_t *n_rows,
                                 void *workspace, size_t workspace_bytes, void *stream);
 int mc_mincurv_adjoint_batch(int B, int n_max, const int32_t *n_pts,
                              const double *reftrack, const double *normvec, const double *h,
                              double w_veh, const double *w_veh_batch, double f_scale, const int32_t *centre_id,
                              const double *sens, int32_t *grad_status, const double *grad_alpha,
                              double *grad_w_right, double *grad_w_left, double *grad_w_veh,
+                             MC_OPTIONAL const double *sens_rows, MC_OPTIONAL const int32_t *n_rows,
+                             MC_OPTIONAL double *schur, MC_OPTIONAL int n_rows_cap,
                              void *workspace, size_t workspace_bytes, void *stream);
 
 /* Fourth stage, run by mc_mincurv_solve_batch between two finalize passes: re-solves every instance flagged
