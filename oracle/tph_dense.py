@@ -452,9 +452,11 @@ def iqp_handler(reftrack, normvectors, A, kappa_bound, w_veh, print_debug, plot_
             alpha_mincurv_tmp = alpha_mincurv_tmp * (iter_cur * 1.0 / iters_min)
         if (iter_cur >= iters_min and curv_error_max_tmp <= curv_error_allowed) or iter_cur >= max_iters:
             break
-        refline_tmp, _, _, _, spline_inds_tmp, t_values_tmp = create_raceline(
+        refline_tmp, _, _, _, spline_inds_tmp, t_values_tmp, _, spline_lengths_tmp = create_raceline(
             refline=reftrack_tmp[:, :2], normvectors=normvectors_tmp, alpha=alpha_mincurv_tmp,
-            stepsize_interp=stepsize_interp)[:6]
+            stepsize_interp=stepsize_interp)[:8]
+        if history is not None:
+            history[-1]["s_total"] = float(np.sum(spline_lengths_tmp))      # (the lap length that sets the next point count)
         reftrack_tmp[:, 2] -= alpha_mincurv_tmp
         reftrack_tmp[:, 3] += alpha_mincurv_tmp
         ws_track_tmp = interp_track_widths(w_track=reftrack_tmp[:, 2:], spline_inds=spline_inds_tmp,
