@@ -24,6 +24,7 @@
 // is streamed back by the triangular sweeps through a shared-memory ring of 8-column units filled by cp.async.bulk
 // (TMA, 1-D) on mbarriers -- the band rows of H reach warp 0 the same way.  Per iteration: factor written once, read
 // three times (the predictor's forward sweep is fused into the factorisation).
+#include <cstddef>
 #include <cstdio>
 #include <cstdlib>
 #include "capi.cuh"
@@ -110,10 +111,8 @@ __device__ __forceinline__ void mbar_wait_relaxed(uint64_t *bar, unsigned parity
 #endif
 }
 // The factor is a stream (written once, read three times per iteration, 0.5 MB per instance, far beyond what L2 can
-// keep for the 1056 resident instances of an H100): its copies and stores carry an evict-first L2 policy so that they do not push the
-// O(N) iterate vectors of the interior-point loop out of L2.
-template <typename T>
-__device__ __forceinline__ void st_stream(T *p, T v) { __stcs(p, v); }      // factor rows: streaming (evict-first) stores
+// keep for the 1056 resident instances of an H100): its bulk stores and loads carry an evict-first L2 policy so that they
+// do not push the O(N) iterate vectors of the interior-point loop out of L2.
 __device__ __forceinline__ uint64_t l2_evict_first_policy() {
     uint64_t pol;
     asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(pol));
@@ -131,6 +130,18 @@ __device__ __forceinline__ void tma_load_1d(void *dst, const void *src, unsigned
                  ::"r"(smem_u32(dst)), "l"(src), "r"(bytes), "r"(smem_u32(bar)), "l"(policy) : "memory");
 }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async;" ::: "memory"); }
+// A factor unit is written into a shared-memory staging buffer and leaves it as one bulk store (bulk-group completion):
+// every sector of the unit reaches L2 whole and at once, instead of two or three partial writes per sector from
+// per-lane stores at different moments.  The writing lanes run fence_proxy_async_smem() and the warp __syncwarp() before
+// one lane issues the store; that lane runs bulk_wait_read() (then the warp __syncwarp()) before the buffer is written
+// again, and bulk_wait() before the units are read back.
+__device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+__device__ __forceinline__ void tma_store_1d(void *dst, const void *src, unsigned bytes, uint64_t policy) {
+    asm volatile("cp.async.bulk.global.shared::cta.bulk_group.L2::cache_hint [%0], [%1], %2, %3;\n"
+                 "cp.async.bulk.commit_group;" ::"l"(dst), "r"(smem_u32(src)), "r"(bytes), "l"(policy) : "memory");
+}
+__device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
+__device__ __forceinline__ void bulk_wait() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
 
 // cycle counters of the instrumented build (-DMC_PROFILE), accumulated by CTA 0 and read by mc_debug_read_profile; slots
 // 3, 4 and 16 are not written.  tools/prof_run.py names the slots in this order.
@@ -198,6 +209,7 @@ struct IpShared {
             double hb[HB_SLOTS][SUB * HB_PITCH];      // band rows of H staged for warp 0 (TMA)
             Handoff ho[HO_SLOTS];                     // warp 0 -> warp 1
             double gb[32 * VBP];                      // warp 1: the panel of the fill rows, row-major (DMMA fragments)
+            double gt[GT_UNIT_DOUBLES];               // warp 1: the panel's fill unit, staged for its bulk store
         } f;
         struct {
             double lt[LT_SLOTS][LT_UNIT_DOUBLES];     // sweeps: streamed chain units (warp 0)
@@ -208,7 +220,10 @@ struct IpShared {
     } u;
     union {
         double Ss[32 * 33];                           // separator block -> its L_S (strictly lower, in place)
-        double sfrag[20 * 32];                        // during the chain: S accumulators (DMMA C fragments, [block][lane][2])
+        struct {
+            double sfrag[20 * 32];                    // during the chain: S accumulators (DMMA C fragments, [block][lane][2])
+            double lt[LT_UNIT_DOUBLES];               // during the chain: warp 0's chain unit of the panel, staged for its bulk store
+        } c;
     } s;
     double wS[32], gs[32], part[2][32];
     double red[32];
@@ -219,6 +234,9 @@ struct IpShared {
     int next;                                         // next instance index (dynamic work distribution)
     int resumed;                                      // ... a parked one (sliced schedule of mincurv_pdip_kernel)
 };
+static_assert(offsetof(IpShared, s.c.lt) % 16 == 0 && offsetof(IpShared, u.f.gt) % 16 == 0,
+              "the sources of the factor's bulk stores must be 16-byte aligned");
+static_assert(sizeof(IpShared::s) == 32 * 33 * sizeof(double), "the chain unit's staging must fit beside the S accumulators");
 
 // pointers into the instance slab that the factorisation and the sweeps use.  Factor rows in HBM, one bulk copy per unit
 // of eight rows (every unit 16-byte aligned):
@@ -266,6 +284,7 @@ __device__ __noinline__ bool factor_chain(IpShared &sh, const double *__restrict
     const int gq = lane >> 2, q = lane & 3;
     const int nunits = (NA + SUB - 1) / SUB;
     const uint64_t pol = l2_evict_normal_policy();
+    double *lst = sh.s.c.lt;                           // the panel's unit, at its offsets in LT
     double W[10][2];
 #pragma unroll
     for (int b = 0; b < 10; ++b) { W[b][0] = 0.0; W[b][1] = 0.0; }
@@ -337,11 +356,11 @@ __device__ __noinline__ bool factor_chain(IpShared &sh, const double *__restrict
         }
         double gv2 = __shfl_sync(FULL, gcur, ((t & 3) << 3) + (lane & 7));
         if (lane >= 8) gv2 = 0.0;
+        if (lane == 0) bulk_wait_read();               // the previous panel's unit has left the staging buffer
         __syncwarp();                                  // every lane has read its row of block column 0: the slot can take L now
         SEG(10);
         // ---- (2) the panel ----
         double dsave = 1.0, wsave = 1.0, ysave = 0.0;
-        double *ltp = LTp + (size_t)k0 * LROW;
         const int wr = (lane >= 8) ? lane - 8 : 24 + lane;      // window row (after the slide) of the row this lane hands over
         // the eight slots lt_slot(j, 8 + wr) of this lane's L21 entries, recomputed in every panel: hoisted out of the loop
         // they took eight registers and made the loop spill
@@ -355,7 +374,7 @@ __device__ __noinline__ bool factor_chain(IpShared &sh, const double *__restrict
             const double w = fast_rcp(dj);
             const double lt = p[j] * w, lt2 = p2[j] * w;           // (lanes <= j: lt is not an entry of L; lanes > j: lt2 = 0)
             ho.vb[wr * VBP + j] = (lane >= 8) ? lt : lt2;
-            if (lane >= 8 || lane <= j) st_stream(ltp + lt_slot(j, 8 + wrs), (lane >= 8) ? lt : lt2);      // L21: the band of the 32 rows below the panel
+            if (lane >= 8 || lane <= j) lst[lt_slot(j, 8 + wrs)] = (lane >= 8) ? lt : lt2;      // L21: the band of the 32 rows below the panel
             if (lane < 8 && lane > j) ho.l11[lane * 8 + j] = lt;
             if (lane == j) { dsave = dj; wsave = w; ysave = yj; }
             gv = fma(-lt, yj, gv);                                 // (lanes <= j: gv is dead)
@@ -386,12 +405,13 @@ __device__ __noinline__ bool factor_chain(IpShared &sh, const double *__restrict
                 q8[m] = sacc;
             }
             if (lane < 8) {
-                double *ltq = ltp + 36 * lane - 1;     // + m = lt_slot(lane, m) for the rows m < 8 of Q (no wrap)
+                double *ltq = lst + 36 * lane - 1;     // + m = lt_slot(lane, m) for the rows m < 8 of Q (no wrap)
 #pragma unroll
                 for (int m = 1; m < 8; ++m)
-                    if (m > lane) st_stream(ltq + m, q8[m]);
-                st_stream(ltp + lane * LROW + 32, wsave);
+                    if (m > lane) ltq[m] = q8[m];
+                lst[lane * LROW + 32] = wsave;
             }
+            fence_proxy_async_smem();                  // the unit is complete: the bulk store after the next __syncwarp
         }
         // ---- (3) trailing update on the tensor cores; the window slides by one block ----
         double af[4][2], bf[4][2];
@@ -421,7 +441,14 @@ __device__ __noinline__ bool factor_chain(IpShared &sh, const double *__restrict
         }
         __syncwarp();
         SEG(12);
-        if (lane == 0) mbar_arrive(&sh.ho_full[ls]);
+        if (lane == 0) {
+            mbar_arrive(&sh.ho_full[ls]);
+            tma_store_1d(LTp + (size_t)k0 * LROW, lst, LT_UNIT_DOUBLES * sizeof(double), l2_evict_first_policy());
+        }
+    }
+    if (lane == 0) {            // every unit is in the slab before the sweeps read it back, and the staging is free for Ss
+        bulk_wait();
+        fence_proxy_async();
     }
     return ok;
 }
@@ -440,7 +467,7 @@ __device__ __noinline__ void factor_fill(IpShared &sh, const double *__restrict_
 #pragma unroll
         for (int J = 0; J < 4; ++J) { G[I][J][0] = 0.0; G[I][J][1] = 0.0; }
     double gsacc = 0.0;
-    double *gb = sh.u.f.gb;
+    double *gb = sh.u.f.gb, *gst = sh.u.f.gt;       // gst: the panel's unit, at its offsets in GT
     for (int t = 0; t < nunits; ++t) {
         const unsigned ht = tick + t, ls = ht % HO_SLOTS;
         const int k0 = t * SUB;
@@ -471,6 +498,7 @@ __device__ __noinline__ void factor_fill(IpShared &sh, const double *__restrict_
 #pragma unroll
             for (int j = 0; j < 8; ++j) gp[j] = -gp[j];
         }
+        if (lane == 0) bulk_wait_read();               // the previous panel's unit has left the staging buffer
         __syncwarp();
         PROF_T0(tw2);
         mbar_wait_relaxed(&sh.ho_full[ls], (ht / HO_SLOTS) & 1u);
@@ -481,20 +509,21 @@ __device__ __noinline__ void factor_fill(IpShared &sh, const double *__restrict_
         for (int m = 0; m < 7; ++m)                 // right-looking: gp[m] is final, the updates of one column are independent
 #pragma unroll
             for (int j = m + 1; j < 8; ++j) gp[j] = fma(-gp[m], ho.l11[j * 8 + m], gp[j]);
-        double *gtp = GTp + (size_t)k0 * FROW;
 #pragma unroll
         for (int j = 0; j < 8; ++j) {
-            st_stream(gtp + j * FROW + lane, gp[j]);
+            gst[j * FROW + lane] = gp[j];
             gsacc = fma(gp[j], ho.w[j] * ho.y[j], gsacc);
         }
         if (lane < 8) {
             const double w = ho.w[lane];
-            st_stream(gtp + lane * FROW + 32, w);
+            gst[lane * FROW + 32] = w;
             Zp[k0 + lane] = w * ho.y[lane];            // z of the predictor (the fused forward half)
         }
+        fence_proxy_async_smem();                      // the unit is complete: the bulk store after the next __syncwarp
 #pragma unroll
         for (int j = 0; j < 8; j += 2) *reinterpret_cast<double2 *>(&gb[lane * VBP + j]) = make_double2(gp[j], gp[j + 1]);
         __syncwarp();
+        if (lane == 0) tma_store_1d(GTp + (size_t)k0 * FROW, gst, GT_UNIT_DOUBLES * sizeof(double), l2_evict_first_policy());
         PROF_T0(tw3);
         // ---- trailing update: G'[I][J] = G[I][J+1] + G_panel[I] L[J]^T ----
         double af[4][2], bf[4][2], wq[2];
@@ -523,7 +552,7 @@ __device__ __noinline__ void factor_fill(IpShared &sh, const double *__restrict_
             double c2[4][2];
 #pragma unroll
             for (int J = 0; J <= I; ++J) {
-                const double2 cc = *reinterpret_cast<const double2 *>(&sh.s.sfrag[(blk(I, J) * 32 + lane) * 2]);
+                const double2 cc = *reinterpret_cast<const double2 *>(&sh.s.c.sfrag[(blk(I, J) * 32 + lane) * 2]);
                 c2[J][0] = cc.x; c2[J][1] = cc.y;
             }
 #pragma unroll
@@ -534,11 +563,15 @@ __device__ __noinline__ void factor_fill(IpShared &sh, const double *__restrict_
             }
 #pragma unroll
             for (int J = 0; J <= I; ++J)
-                *reinterpret_cast<double2 *>(&sh.s.sfrag[(blk(I, J) * 32 + lane) * 2]) = make_double2(c2[J][0], c2[J][1]);
+                *reinterpret_cast<double2 *>(&sh.s.c.sfrag[(blk(I, J) * 32 + lane) * 2]) = make_double2(c2[J][0], c2[J][1]);
         }
         __syncwarp();
         PROF_ADD1(PROF_W1_UPDATE, tw3);
         if (lane == 0) mbar_arrive(&sh.ho_empty[ls]);
+    }
+    if (lane == 0) {            // every unit is in the slab before the sweeps read it back, and the staging is free for their ring
+        bulk_wait();
+        fence_proxy_async();
     }
     sh.gs[lane] = g[NA + lane] - gsacc;
 }
@@ -551,7 +584,7 @@ __device__ __noinline__ bool factor(IpShared &sh, double *slab, const Layout &L,
     const Factor F = make_factor(slab, L, n, HB);
     const int NA = F.NA;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    for (int e = threadIdx.x; e < 20 * 32; e += IP_THREADS) sh.s.sfrag[e] = 0.0;
+    for (int e = threadIdx.x; e < 20 * 32; e += IP_THREADS) sh.s.c.sfrag[e] = 0.0;
     fence_proxy_async();        // the band may have been assembled by this kernel (K2b') and the band-row slots were last
     __syncthreads();            // used by the sweeps, both through the generic proxy; the bulk copies are the async proxy
     PROF_T0(tc0);
@@ -567,7 +600,7 @@ __device__ __noinline__ bool factor(IpShared &sh, double *slab, const Layout &L,
     double sf[20];
     if (warp == 1) {
 #pragma unroll
-        for (int e = 0; e < 20; ++e) sf[e] = sh.s.sfrag[((e >> 1) * 32 + lane) * 2 + (e & 1)];
+        for (int e = 0; e < 20; ++e) sf[e] = sh.s.c.sfrag[((e >> 1) * 32 + lane) * 2 + (e & 1)];
     }
     // (the separator block of M: 16 entries per thread, all loads in flight before the barrier)
     double sv[16];
