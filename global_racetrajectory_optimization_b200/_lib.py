@@ -44,37 +44,42 @@ def _declarations(path: str):
 
 def header_signatures(path: str) -> dict:
     """name -> (restype, argtypes) of every declaration `ret mc_name(type name, ...);` in the C header at path."""
-    return {name: (_ctype(ret, name, ret=True), [_ctype(p.replace("MC_OPTIONAL", " "), name) for p in params])
+    return {name: (_ctype(ret, name, ret=True), [_ctype(re.sub(r"\bMC_OPTIONAL2?\b", " ", p), name) for p in params])
             for ret, name, params in _declarations(path)}
 
 
-def optional_parameters(path: str) -> dict:
-    """name -> (first, count) of the MC_OPTIONAL parameters of each declaration in the C header at path that has them
-    (one run of consecutive parameters)."""
+def optional_parameters(path: str, marker: str = "MC_OPTIONAL") -> dict:
+    """name -> (first, count) of the MC_OPTIONAL parameters (or those of another marker, such as MC_OPTIONAL2) of each
+    declaration in the C header at path that has them (one run of consecutive parameters)."""
     out = {}
     for _, name, params in _declarations(path):
-        k = [i for i, p in enumerate(params) if re.search(r"\bMC_OPTIONAL\b", p)]
+        k = [i for i, p in enumerate(params) if re.search(rf"\b{marker}\b", p)]
         if k:
             if k != list(range(k[0], k[-1] + 1)):
-                raise MinCurvLibError(f"{name}: the MC_OPTIONAL parameters must be consecutive")
+                raise MinCurvLibError(f"{name}: the {marker} parameters must be consecutive")
             out[name] = (k[0], len(k))
     return out
 
 
 _SIGS = header_signatures(_build.HEADER)
 _OPTIONAL = optional_parameters(_build.HEADER)
+_OPTIONAL2 = optional_parameters(_build.HEADER, "MC_OPTIONAL2")
 EXPORTED_SYMBOLS = tuple(_SIGS)
 
 
-def _with_optional(fn, first: int, count: int):
-    """fn, which may also be called without its parameters [first, first + count): they are then NULL (0 for an int), as
-    the header documents for MC_OPTIONAL parameters, so that a call written for the entry before they were added still
-    binds its arguments to the right parameters."""
-    fill = tuple(0 if t is ctypes.c_int else None for t in fn.argtypes[first:first + count])
-    short = len(fn.argtypes) - count
+def _with_optional(fn, *groups):
+    """fn, which may also be called without its parameters [first, first + count) of the last of groups ((first, count)
+    each, in release order), or without those of the last two, and so on: they are then NULL (0 for an int), as the
+    header documents for MC_OPTIONAL and MC_OPTIONAL2 parameters, so that a call written for the entry before they were
+    added still binds its arguments to the right parameters."""
+    forms = {}
+    left_out = []
+    for first, count in sorted(groups, reverse=True):       # (the later groups come after the earlier ones)
+        left_out.append((first, tuple(0 if t is ctypes.c_int else None for t in fn.argtypes[first:first + count])))
+        forms[len(fn.argtypes) - sum(len(f) for _, f in left_out)] = list(reversed(left_out))
 
     def call(*args):
-        if len(args) == short:
+        for first, fill in forms.get(len(args), ()):
             args = args[:first] + fill + args[first:]
         return fn(*args)
     call.__name__, call.argtypes, call.restype = fn.__name__, fn.argtypes, fn.restype
@@ -117,8 +122,9 @@ def load(build_if_missing: bool = True):
         fn = getattr(lib, name)
         fn.restype = res
         fn.argtypes = args
-        if name in _OPTIONAL:
-            setattr(lib, name, _with_optional(fn, *_OPTIONAL[name]))
+        groups = [g[name] for g in (_OPTIONAL, _OPTIONAL2) if name in g]
+        if groups:
+            setattr(lib, name, _with_optional(fn, *groups))
     _LIB = lib
     return lib
 

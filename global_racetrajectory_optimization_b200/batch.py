@@ -219,18 +219,43 @@ def _mincurv_results(B: int, n_max: int, dev) -> dict:
 def opt_min_curv_batch(reftrack: torch.Tensor, normvec: torch.Tensor, h: torch.Tensor, kappa_bound: float,
                        w_veh: Union[float, torch.Tensor], n_pts: Optional[torch.Tensor] = None,
                        max_chunk: Optional[int] = None, f_scale: Optional[float] = None,
-                       centre_id: Optional[torch.Tensor] = None) -> dict:
+                       centre_id: Optional[torch.Tensor] = None, lin_alpha: Optional[torch.Tensor] = None) -> dict:
     """Batched tph.opt_min_curv (closed tracks).  Returns a dict of device tensors:
     alpha [B, n_max], curv_error_max [B], kappa_lin_max [B], status [B] (int32), iters [B] (int32).
     f_scale: None = the module default F_SCALE (see there).
     centre_id [B] (optional): for batches in which several instances share a centreline (x, y, normvec, h, n_pts identical;
     only the widths differ -- a width sweep of one track): centre_id[b] = index of the instance that owns b's centreline
     (owners: centre_id[b] == b).  H, f and k_ref are then assembled once per centreline (same results, less work);
-    shared_centre_ids() builds the tensor from group labels."""
+    shared_centre_ids() builds the tensor from group labels.
+    lin_alpha [B, n_max] (optional): the QP linearised about the line reftrack + lin_alpha * normvec on the same grid
+    instead of the centre line (the step of tph's iterative QP without re-sampling; DESIGN.md section 3.2): the curvature
+    rows, H and f use that line's first derivatives, and curv_error_max and kappa_lin_max refer to that linearisation.
+    alpha is still the shift from the centre line.  With centre_id a follower is linearised about its owner's row."""
     _require_cuda()
+    if lin_alpha is not None and (lin_alpha.shape != h.shape):
+        raise ValueError(f"opt_min_curv_batch: lin_alpha must be [B, n_max] like h, got {tuple(lin_alpha.shape)}")
     a = _mincurv_inputs(dict(reftrack=(reftrack, 4), normvec=(normvec, 2), h=(h, None)),
                         "Array size of reftrack should be the same as normvectors!", n_pts, w_veh, centre_id, max_chunk, f_scale)
     out = _mincurv_results(a.B, a.n_max, a.dev)
+    if lin_alpha is not None:
+        lin = _f64(lin_alpha, "lin_alpha")
+        invalid = None
+        if a.centre_id is not None:
+            # a follower is linearised about its owner's row, as the shared assembly does; the instances are solved one by
+            # one (bitwise what the shared solve gives), a follower without a valid owner gets status -1 as there
+            o = a.centre_id.long()
+            oc = o.clamp(0, a.B - 1)
+            invalid = (o < 0) | (o >= a.B) | (a.centre_id[oc] != oc.to(torch.int32))
+            if a.n_pts is not None:
+                invalid |= a.n_pts[oc] != a.n_pts
+            lin = lin[oc].contiguous()
+        ws = _workspace("mincurv", _lib.load().mc_mincurv_workspace_bytes(a.chunk, a.n_max), a.dev)
+        _launch_chunks("mc_mincurv_solve_batch_ex", a.B, a.chunk, ws, a.n_max, *map(_rows, (a.n_pts, a.reftrack, a.normvec,
+                       a.h)), float(kappa_bound), a.w_scalar, _rows(a.w_batch), a.f_scale, *map(_rows, out.values()), 0.0,
+                       None, None, _rows(lin))
+        if invalid is not None:
+            out["status"] = torch.where(invalid, -1, out["status"]).to(torch.int32)
+        return out
     _mincurv_launch("mc_mincurv_solve_batch_shared", a.chunk, a.n_pts, a.reftrack, a.normvec, a.h, float(kappa_bound),
                     a.w_scalar, a.w_batch, a.f_scale, a.centre_id, *out.values())
     return out
@@ -330,7 +355,7 @@ class _MinCurvDiff(torch.autograd.Function):
             schur = torch.empty((chunk, max(cap * cap, 1)), dtype=torch.float64, device=dev)
             rows = (sens_rows, n_rows, lambda s, e: schur, cap)
         _mincurv_launch("mc_mincurv_adjoint_batch", chunk, n_pts, reftrack, normvec, h, None, ctx.w_scalar, w_veh_t,
-                        ctx.f_scale, centre_id, sens, gs, grad_alpha, gwr, gwl, gwv, *rows)
+                        ctx.f_scale, centre_id, sens, gs, grad_alpha, gwr, gwl, gwv, *rows, None)
         _refuse(ctx.strict, wanted, gs, who, "whose adjoint factorisation broke down")
         return (torch.stack((gwr, gwl), dim=2), gwv if w_veh_t is not None else None) + (None,) * 11
 

@@ -2,11 +2,15 @@
 // main_globaltraj.py:264-271): the linearised curvature k_ref + E alpha (checked
 // against kappa_bound) and the linearisation error curv_error_max, both through the O(N) operator
 // form E a = S_y Z (n_y a) - S_x Z (n_x a) (one periodic tridiagonal solve with two right-hand sides).
+// LIN: the workspace was assembled about a linearisation point (mincurv_setup.cu): V_XP / V_YP hold its first
+// derivatives, which the linearised curvature uses, while the line P + alpha n takes those of the centre line, recomputed
+// here from its points and moments.
 #include "capi.cuh"
 #include "mincurv_ops.cuh"
 
 namespace mc {
 
+template <bool LIN>
 __global__ void __launch_bounds__(256)
 mincurv_finalize_kernel(int n_max, const int32_t *__restrict__ n_pts, double *__restrict__ ws, Layout L,
                         const double *__restrict__ alpha, double kappa_bound,
@@ -28,7 +32,7 @@ mincurv_finalize_kernel(int n_max, const int32_t *__restrict__ n_pts, double *__
     const double *H = vec(slab, L, V_H), *LFW = vec(slab, L, V_LFW), *INVD = vec(slab, L, V_INVD);
     const double *NX = vec(slab, L, V_NX), *NY = vec(slab, L, V_NY), *MX = vec(slab, L, V_MX), *MY = vec(slab, L, V_MY);
     const double *XP = vec(slab, L, V_XP), *YP = vec(slab, L, V_YP), *SX = vec(slab, L, V_SX), *SY = vec(slab, L, V_SY);
-    const double *KREF = vec(slab, L, V_KREF);
+    const double *KREF = vec(slab, L, V_KREF), *PX = vec(slab, L, V_PX), *PY = vec(slab, L, V_PY);
     double *T0 = vec(slab, L, V_T0), *T1 = vec(slab, L, V_T1), *T2 = vec(slab, L, V_T2), *T3 = vec(slab, L, V_T3);
     double *ZX = vec(slab, L, V_T4), *ZY = vec(slab, L, V_T5);
 
@@ -51,8 +55,13 @@ mincurv_finalize_kernel(int n_max, const int32_t *__restrict__ n_pts, double *__
         kmax = fmax(kmax, fabs(klin));
         const double ddx = h2 * (MX[i] + zx), ddy = h2 * (MY[i] + zy);
         const double xp = XP[i], yp = YP[i];
-        const double xpt = xp + (NX[ip1] * al[ip1] - NX[i] * al[i]) - h2 * (2.0 * zx + ZX[ip1]) * (1.0 / 6.0);
-        const double ypt = yp + (NY[ip1] * al[ip1] - NY[i] * al[i]) - h2 * (2.0 * zy + ZY[ip1]) * (1.0 / 6.0);
+        double xc = xp, yc = yp;                // first derivatives of the centre line
+        if (LIN) {
+            xc = (PX[ip1] - PX[i]) - h2 * (2.0 * MX[i] + MX[ip1]) * (1.0 / 6.0);
+            yc = (PY[ip1] - PY[i]) - h2 * (2.0 * MY[i] + MY[ip1]) * (1.0 / 6.0);
+        }
+        const double xpt = xc + (NX[ip1] * al[ip1] - NX[i] * al[i]) - h2 * (2.0 * zx + ZX[ip1]) * (1.0 / 6.0);
+        const double ypt = yc + (NY[ip1] * al[ip1] - NY[i] * al[i]) - h2 * (2.0 * zy + ZY[ip1]) * (1.0 / 6.0);
         const double q0 = xp * xp + yp * yp, q1 = xpt * xpt + ypt * ypt;
         const double c0 = (xp * ddy - yp * ddx) / (q0 * sqrt(q0));
         const double c1 = (xpt * ddy - ypt * ddx) / (q1 * sqrt(q1));
@@ -143,19 +152,26 @@ mincurv_prox_kernel(int n_max, const int32_t *__restrict__ n_pts, double *__rest
     for (int i = threadIdx.x; i < n; i += blockDim.x) F[i] = mu * q[i] - (HX[i] + mu * x[i]);
 }
 
+int mincurv_finalize(int B, int n_max, const int32_t *n_pts, const double *alpha, double kappa_bound, double *curv_error_max,
+                     double *kappa_lin_max, int32_t *status, bool lin, void *workspace, size_t workspace_bytes, void *stream) {
+    if (!alpha || !curv_error_max || !status) return bad("mc_mincurv_finalize_batch: NULL argument");
+    int rc = mincurv_args("mc_mincurv_finalize_batch", B, n_max, workspace, workspace_bytes);
+    if (rc) return rc;
+    auto kernel = lin ? mincurv_finalize_kernel<true> : mincurv_finalize_kernel<false>;
+    kernel<<<B, 256, 0, (cudaStream_t)stream>>>(n_max, n_pts, (double *)workspace, make_layout(n_max), alpha, kappa_bound,
+                                                curv_error_max, kappa_lin_max, status);
+    return check_cuda("mincurv_finalize_kernel");
+}
+
 }  // namespace mc
 
 extern "C" {
 
 int mc_mincurv_finalize_batch(int B, int n_max, const int32_t *n_pts, const double *alpha, double kappa_bound,
-                              double *curv_error_max, double *kappa_lin_max, int32_t *status, void *workspace,
+                              double *curv_error_max, double *kappa_lin_max, int32_t *status, int linearised, void *workspace,
                               size_t workspace_bytes, void *stream) {
-    if (!alpha || !curv_error_max || !status) return bad("mc_mincurv_finalize_batch: NULL argument");
-    int rc = mc::mincurv_args("mc_mincurv_finalize_batch", B, n_max, workspace, workspace_bytes);
-    if (rc) return rc;
-    mc::mincurv_finalize_kernel<<<B, 256, 0, (cudaStream_t)stream>>>(n_max, n_pts, (double *)workspace, mc::make_layout(n_max),
-                                                                     alpha, kappa_bound, curv_error_max, kappa_lin_max, status);
-    return check_cuda("mincurv_finalize_kernel");
+    return mc::mincurv_finalize(B, n_max, n_pts, alpha, kappa_bound, curv_error_max, kappa_lin_max, status, linearised != 0,
+                                workspace, workspace_bytes, stream);
 }
 
 int mc_mincurv_solve_batch(int B, int n_max, const int32_t *n_pts, const double *reftrack, const double *normvec,
@@ -163,21 +179,22 @@ int mc_mincurv_solve_batch(int B, int n_max, const int32_t *n_pts, const double 
                            double *curv_error_max, double *kappa_lin_max, int32_t *status, int32_t *iters,
                            void *workspace, size_t workspace_bytes, void *stream) {
     return mc_mincurv_solve_batch_ex(B, n_max, n_pts, reftrack, normvec, h, kappa_bound, w_veh, w_veh_batch, MC_F_SCALE_DEFAULT,
-                                     alpha, curv_error_max, kappa_lin_max, status, iters, 0.0, nullptr, nullptr, workspace,
-                                     workspace_bytes, stream);
+                                     alpha, curv_error_max, kappa_lin_max, status, iters, 0.0, nullptr, nullptr, nullptr,
+                                     workspace, workspace_bytes, stream);
 }
 
 // the projection QP: setup -> prox -> pdip -> finalize -> kappa (with prox_mu) -> finalize
 static int mincurv_prox_solve(int B, int n_max, const int32_t *n_pts, const double *reftrack, const double *normvec,
                               const double *h, double kappa_bound, double w_veh, const double *w_veh_batch, double f_scale,
                               double *alpha, double *curv_error_max, double *kappa_lin_max, int32_t *status, int32_t *iters,
-                              double prox_mu, const double *prox_x, const double *prox_q, void *workspace,
-                              size_t workspace_bytes, void *stream) {
+                              double prox_mu, const double *prox_x, const double *prox_q, const double *lin_alpha,
+                              void *workspace, size_t workspace_bytes, void *stream) {
     if (!reftrack || !normvec || !h || !alpha || !curv_error_max || !status || !prox_q)
         return bad("mc_mincurv_solve_batch_ex: NULL argument");
     if (!(prox_mu > 0.0) || !(prox_mu < INFINITY)) return bad("mc_mincurv_solve_batch_ex: prox_mu must be finite and positive");
-    int rc = mc_mincurv_setup_batch_shared(B, n_max, n_pts, reftrack, normvec, h, w_veh, w_veh_batch, f_scale, nullptr, status,
-                                           workspace, workspace_bytes, stream);
+    const bool lin = lin_alpha != nullptr;
+    int rc = mc::mincurv_setup(B, n_max, n_pts, reftrack, normvec, h, w_veh, w_veh_batch, f_scale, nullptr, lin_alpha, status,
+                               workspace, workspace_bytes, stream);
     if (rc) return rc;
     mc::mincurv_prox_kernel<<<B, 256, 0, (cudaStream_t)stream>>>(n_max, n_pts, (double *)workspace, mc::make_layout(n_max),
                                                                  prox_mu, prox_x, prox_q, status);
@@ -185,26 +202,13 @@ static int mincurv_prox_solve(int B, int n_max, const int32_t *n_pts, const doub
     if (rc) return rc;
     rc = mc_mincurv_pdip_batch(B, n_max, n_pts, alpha, status, iters, workspace, workspace_bytes, stream);
     if (rc) return rc;
-    rc = mc_mincurv_finalize_batch(B, n_max, n_pts, alpha, kappa_bound, curv_error_max, kappa_lin_max, status, workspace,
-                                   workspace_bytes, stream);
+    rc = mc::mincurv_finalize(B, n_max, n_pts, alpha, kappa_bound, curv_error_max, kappa_lin_max, status, lin, workspace,
+                              workspace_bytes, stream);
     if (rc) return rc;
     rc = mc::mincurv_kappa_phase(B, n_max, n_pts, kappa_bound, prox_mu, alpha, status, iters, workspace, workspace_bytes, stream);
     if (rc) return rc;
-    return mc_mincurv_finalize_batch(B, n_max, n_pts, alpha, kappa_bound, curv_error_max, kappa_lin_max, status, workspace,
-                                     workspace_bytes, stream);
-}
-
-int mc_mincurv_solve_batch_ex(int B, int n_max, const int32_t *n_pts, const double *reftrack, const double *normvec,
-                              const double *h, double kappa_bound, double w_veh, const double *w_veh_batch, double f_scale,
-                              double *alpha, double *curv_error_max, double *kappa_lin_max, int32_t *status, int32_t *iters,
-                              double prox_mu, const double *prox_x, const double *prox_q, void *workspace,
-                              size_t workspace_bytes, void *stream) {
-    if (prox_x)
-        return mincurv_prox_solve(B, n_max, n_pts, reftrack, normvec, h, kappa_bound, w_veh, w_veh_batch, f_scale, alpha,
-                                  curv_error_max, kappa_lin_max, status, iters, prox_mu, prox_x, prox_q, workspace,
-                                  workspace_bytes, stream);
-    return mc_mincurv_solve_batch_shared(B, n_max, n_pts, reftrack, normvec, h, kappa_bound, w_veh, w_veh_batch, f_scale, nullptr,
-                                         alpha, curv_error_max, kappa_lin_max, status, iters, workspace, workspace_bytes, stream);
+    return mc::mincurv_finalize(B, n_max, n_pts, alpha, kappa_bound, curv_error_max, kappa_lin_max, status, lin, workspace,
+                                workspace_bytes, stream);
 }
 
 // setup -> pdip -> finalize -> (export of the sensitivity data) -> kappa -> finalize -> (export of the curvature-row phase's
@@ -213,17 +217,18 @@ int mc_mincurv_solve_batch_ex(int B, int n_max, const int32_t *n_pts, const doub
 static int mincurv_solve(int B, int n_max, const int32_t *n_pts, const double *reftrack, const double *normvec, const double *h,
                          double kappa_bound, double w_veh, const double *w_veh_batch, double f_scale, const int32_t *centre_id,
                          double *alpha, double *curv_error_max, double *kappa_lin_max, int32_t *status, int32_t *iters,
-                         double *sens, int32_t *grad_status, double *sens_rows, int32_t *n_rows, void *workspace,
-                         size_t workspace_bytes, void *stream) {
+                         double *sens, int32_t *grad_status, double *sens_rows, int32_t *n_rows, const double *lin_alpha,
+                         void *workspace, size_t workspace_bytes, void *stream) {
     if (!reftrack || !normvec || !h || !alpha || !curv_error_max || !status)
         return bad("mc_mincurv_solve_batch: NULL argument");
-    int rc = mc_mincurv_setup_batch_shared(B, n_max, n_pts, reftrack, normvec, h, w_veh, w_veh_batch, f_scale, centre_id, status,
-                                           workspace, workspace_bytes, stream);
+    const bool lin = lin_alpha != nullptr;
+    int rc = mc::mincurv_setup(B, n_max, n_pts, reftrack, normvec, h, w_veh, w_veh_batch, f_scale, centre_id, lin_alpha, status,
+                               workspace, workspace_bytes, stream);
     if (rc) return rc;
     rc = mc_mincurv_pdip_batch(B, n_max, n_pts, alpha, status, iters, workspace, workspace_bytes, stream);
     if (rc) return rc;
-    rc = mc_mincurv_finalize_batch(B, n_max, n_pts, alpha, kappa_bound, curv_error_max, kappa_lin_max, status, workspace,
-                                   workspace_bytes, stream);
+    rc = mc::mincurv_finalize(B, n_max, n_pts, alpha, kappa_bound, curv_error_max, kappa_lin_max, status, lin, workspace,
+                              workspace_bytes, stream);
     if (rc) return rc;
     if (sens) {
         // the box phase's final iterate, before the curvature-row phase takes over the status-4 slabs
@@ -235,12 +240,26 @@ static int mincurv_solve(int B, int n_max, const int32_t *n_pts, const double *r
     // instances whose box-only optimum violates the curvature rows (status 4) are re-solved with the rows
     rc = mc_mincurv_kappa_batch(B, n_max, n_pts, kappa_bound, alpha, status, iters, workspace, workspace_bytes, stream);
     if (rc) return rc;
-    rc = mc_mincurv_finalize_batch(B, n_max, n_pts, alpha, kappa_bound, curv_error_max, kappa_lin_max, status, workspace,
-                                   workspace_bytes, stream);
+    rc = mc::mincurv_finalize(B, n_max, n_pts, alpha, kappa_bound, curv_error_max, kappa_lin_max, status, lin, workspace,
+                              workspace_bytes, stream);
     if (rc || !sens_rows) return rc;
     mc::mincurv_sens_rows_export_kernel<<<B, 256, 0, (cudaStream_t)stream>>>(n_max, n_pts, (double *)workspace, mc::make_layout(n_max),
                                                                              status, sens, sens_rows, n_rows, grad_status);
     return check_cuda("mincurv_sens_rows_export_kernel");
+}
+
+int mc_mincurv_solve_batch_ex(int B, int n_max, const int32_t *n_pts, const double *reftrack, const double *normvec,
+                              const double *h, double kappa_bound, double w_veh, const double *w_veh_batch, double f_scale,
+                              double *alpha, double *curv_error_max, double *kappa_lin_max, int32_t *status, int32_t *iters,
+                              double prox_mu, const double *prox_x, const double *prox_q, const double *lin_alpha,
+                              void *workspace, size_t workspace_bytes, void *stream) {
+    if (prox_x)
+        return mincurv_prox_solve(B, n_max, n_pts, reftrack, normvec, h, kappa_bound, w_veh, w_veh_batch, f_scale, alpha,
+                                  curv_error_max, kappa_lin_max, status, iters, prox_mu, prox_x, prox_q, lin_alpha, workspace,
+                                  workspace_bytes, stream);
+    return mincurv_solve(B, n_max, n_pts, reftrack, normvec, h, kappa_bound, w_veh, w_veh_batch, f_scale, nullptr, alpha,
+                         curv_error_max, kappa_lin_max, status, iters, nullptr, nullptr, nullptr, nullptr, lin_alpha, workspace,
+                         workspace_bytes, stream);
 }
 
 int mc_mincurv_solve_batch_shared(int B, int n_max, const int32_t *n_pts, const double *reftrack, const double *normvec,
@@ -248,7 +267,7 @@ int mc_mincurv_solve_batch_shared(int B, int n_max, const int32_t *n_pts, const 
                                   const int32_t *centre_id, double *alpha, double *curv_error_max, double *kappa_lin_max,
                                   int32_t *status, int32_t *iters, void *workspace, size_t workspace_bytes, void *stream) {
     return mincurv_solve(B, n_max, n_pts, reftrack, normvec, h, kappa_bound, w_veh, w_veh_batch, f_scale, centre_id, alpha,
-                         curv_error_max, kappa_lin_max, status, iters, nullptr, nullptr, nullptr, nullptr, workspace,
+                         curv_error_max, kappa_lin_max, status, iters, nullptr, nullptr, nullptr, nullptr, nullptr, workspace,
                          workspace_bytes, stream);
 }
 
@@ -260,7 +279,7 @@ int mc_mincurv_solve_batch_sens(int B, int n_max, const int32_t *n_pts, const do
     if (!sens || !grad_status) return bad("mc_mincurv_solve_batch_sens: NULL argument");
     if (!sens_rows != !n_rows) return bad("mc_mincurv_solve_batch_sens: sens_rows and n_rows go together");
     return mincurv_solve(B, n_max, n_pts, reftrack, normvec, h, kappa_bound, w_veh, w_veh_batch, f_scale, centre_id, alpha,
-                         curv_error_max, kappa_lin_max, status, iters, sens, grad_status, sens_rows, n_rows, workspace,
+                         curv_error_max, kappa_lin_max, status, iters, sens, grad_status, sens_rows, n_rows, nullptr, workspace,
                          workspace_bytes, stream);
 }
 

@@ -1950,15 +1950,16 @@ int mc_mincurv_adjoint_batch(int B, int n_max, const int32_t *n_pts, const doubl
                              const double *h, double w_veh, const double *w_veh_batch, double f_scale, const int32_t *centre_id,
                              const double *sens, int32_t *grad_status, const double *grad_alpha, double *grad_w_right,
                              double *grad_w_left, double *grad_w_veh, const double *sens_rows, const int32_t *n_rows,
-                             double *schur, int n_rows_cap, void *workspace, size_t workspace_bytes, void *stream) {
+                             double *schur, int n_rows_cap, const double *lin_alpha, void *workspace,
+                             size_t workspace_bytes, void *stream) {
     if (!sens || !grad_status || !grad_alpha || !grad_w_right || !grad_w_left || !grad_w_veh)
         return bad("mc_mincurv_adjoint_batch: NULL argument");
     if (sens_rows && (!n_rows || !schur)) return bad("mc_mincurv_adjoint_batch: sens_rows needs n_rows and schur");
     if (sens_rows && n_rows_cap < 0) return bad("mc_mincurv_adjoint_batch: n_rows_cap < 0");
     // the band of H and the bounds are rebuilt in the slabs; the assembly's status words (the forward pass's, recorded in
     // grad_status) go to grad_w_right, which the adjoint kernel overwrites
-    int rc = mc_mincurv_setup_batch_shared(B, n_max, n_pts, reftrack, normvec, h, w_veh, w_veh_batch, f_scale, centre_id,
-                                           reinterpret_cast<int32_t *>(grad_w_right), workspace, workspace_bytes, stream);
+    int rc = mc::mincurv_setup(B, n_max, n_pts, reftrack, normvec, h, w_veh, w_veh_batch, f_scale, centre_id, lin_alpha,
+                               reinterpret_cast<int32_t *>(grad_w_right), workspace, workspace_bytes, stream);
     if (rc) return rc;
     if (sens_rows) {
         // pass 0: the instances without row weights (reading their owner's band); pass 1: the curvature-row instances

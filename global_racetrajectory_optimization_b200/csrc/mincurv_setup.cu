@@ -17,16 +17,23 @@
 //   Mid_t(c, c'+1) = rho+_{c'+1} (Mid_t(c, c') + w_t[c'] Ti[c'][c] Ti[c'][c'])
 // (exact sums over all m -- no truncation of E -- verified against the explicit E^T E in tools/).
 // One CTA per QP instance; O(N) vectors and the B / H bands live in the instance's HBM slab.
+//
+// LIN: linearised about the line P + a n (a = lin_alpha) instead of the centre line P.  The first derivatives x', y'
+// (and with them S_x, S_y) are those of the spline through Ps = P + a n, from its moments Ms; k_ref = S_y m_y - S_x m_x
+// keeps the centre line's moments, since alpha still enters through E.  Then k_ref + E a is the knot curvature of the
+// spline through Ps, and H, f and the curvature rows follow from S_x, S_y, k_ref as about the centre line.
 #include "capi.cuh"
 #include "mincurv_ops.cuh"
 
 namespace mc {
 
+template <bool LIN>
 __global__ void __launch_bounds__(256)
 mincurv_setup_kernel(int n_max, const int32_t *__restrict__ n_pts,
                      const double *__restrict__ reftrack, const double *__restrict__ normvec,
                      const double *__restrict__ hin, double w_veh, const double *__restrict__ w_veh_batch, double f_scale,
-                     const int32_t *__restrict__ centre_id, double *__restrict__ ws, Layout L, int32_t *__restrict__ status) {
+                     const int32_t *__restrict__ centre_id, double *__restrict__ ws, Layout L, int32_t *__restrict__ status,
+                     const double *__restrict__ lin_alpha) {
     const int b = blockIdx.x;
     const int n = n_pts ? n_pts[b] : n_max;
     double *slab = ws + (size_t)b * L.stride;
@@ -99,12 +106,33 @@ mincurv_setup_kernel(int n_max, const int32_t *__restrict__ n_pts,
     __syncthreads();
     // ---- P4: moments of the reference line ----
     tri_solve2(LFW, INVD, H, T0, T1, T2, T3, MX, MY, n);
+    // LIN: moments Ms of the shifted points Ps = P + a n, in T4 / T5 (free until the E^T solve below)
+    const double *la = LIN ? lin_alpha + (size_t)b * n_max : nullptr;
+    if (LIN) {
+        for (int i = threadIdx.x; i < n; i += blockDim.x) {
+            const int im1 = (i == 0) ? n - 1 : i - 1;
+            const int ip1 = (i + 1 == n) ? 0 : i + 1;
+            const double hi = H[i], him = H[im1];
+            const double x = PX[i] + la[i] * NX[i], xm = PX[im1] + la[im1] * NX[im1], xp = PX[ip1] + la[ip1] * NX[ip1];
+            const double y = PY[i] + la[i] * NY[i], ym = PY[im1] + la[im1] * NY[im1], yp = PY[ip1] + la[ip1] * NY[ip1];
+            T0[i] = 6.0 * ((xp - x) / hi - (x - xm) / him);
+            T1[i] = 6.0 * ((yp - y) / hi - (y - ym) / him);
+        }
+        __syncthreads();
+        tri_solve2(LFW, INVD, H, T0, T1, T2, T3, T4, T5, n);
+    }
     // ---- P5: linearisation point; right-hand sides of f = F_SCALE E^T k_ref ----
     for (int i = threadIdx.x; i < n; i += blockDim.x) {
         const int ip1 = (i + 1 == n) ? 0 : i + 1;
         const double hi = H[i], h2 = hi * hi;
-        const double xp = (PX[ip1] - PX[i]) - h2 * (2.0 * MX[i] + MX[ip1]) * (1.0 / 6.0);
-        const double yp = (PY[ip1] - PY[i]) - h2 * (2.0 * MY[i] + MY[ip1]) * (1.0 / 6.0);
+        double xp, yp;
+        if constexpr (LIN) {                    // first derivatives of the spline through Ps (moments in T4 / T5)
+            xp = ((PX[ip1] + la[ip1] * NX[ip1]) - (PX[i] + la[i] * NX[i])) - h2 * (2.0 * T4[i] + T4[ip1]) * (1.0 / 6.0);
+            yp = ((PY[ip1] + la[ip1] * NY[ip1]) - (PY[i] + la[i] * NY[i])) - h2 * (2.0 * T5[i] + T5[ip1]) * (1.0 / 6.0);
+        } else {
+            xp = (PX[ip1] - PX[i]) - h2 * (2.0 * MX[i] + MX[ip1]) * (1.0 / 6.0);
+            yp = (PY[ip1] - PY[i]) - h2 * (2.0 * MY[i] + MY[ip1]) * (1.0 / 6.0);
+        }
         const double q = xp * xp + yp * yp;
         const double c = 1.0 / (q * sqrt(q));
         const double sy = c * xp * h2, sx = c * yp * h2;
@@ -160,6 +188,31 @@ mincurv_share_kernel(int B, int n_max, const int32_t *__restrict__ n_pts, const 
     if (threadIdx.x == 0) *band_owner(dst, L) = o;
 }
 
+int mincurv_setup(int B, int n_max, const int32_t *n_pts, const double *reftrack, const double *normvec, const double *h,
+                  double w_veh, const double *w_veh_batch, double f_scale, const int32_t *centre_id, const double *lin_alpha,
+                  int32_t *status, void *workspace, size_t workspace_bytes, void *stream) {
+    if (!reftrack || !normvec || !h || !status) return bad("mc_mincurv_setup_batch: NULL argument");
+    if (!(f_scale > 0.0)) return bad("mc_mincurv_setup_batch: f_scale must be positive");
+    int rc = mincurv_args("mc_mincurv_setup_batch", B, n_max, workspace, workspace_bytes);
+    if (rc) return rc;
+    const Layout L = make_layout(n_max);
+    double *ws = (double *)workspace;
+    cudaStream_t s = (cudaStream_t)stream;
+    constexpr int smem = hband_win_doubles(256) * (int)sizeof(double);      // 49 KB: above the static limit
+    // (per launch: the attribute is per device and a process may drive several)
+    if (lin_alpha) {
+        cudaFuncSetAttribute(mincurv_setup_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+        mincurv_setup_kernel<true><<<B, 256, smem, s>>>(n_max, n_pts, reftrack, normvec, h, w_veh, w_veh_batch, f_scale,
+                                                         centre_id, ws, L, status, lin_alpha);
+    } else {
+        cudaFuncSetAttribute(mincurv_setup_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+        mincurv_setup_kernel<false><<<B, 256, smem, s>>>(n_max, n_pts, reftrack, normvec, h, w_veh, w_veh_batch, f_scale,
+                                                          centre_id, ws, L, status, nullptr);
+    }
+    if (centre_id) mincurv_share_kernel<<<B, 256, 0, s>>>(B, n_max, n_pts, centre_id, ws, L, status);
+    return check_cuda("mincurv_setup_kernel");
+}
+
 }  // namespace mc
 
 extern "C" {
@@ -173,34 +226,22 @@ int mc_mincurv_setup_batch_shared(int B, int n_max, const int32_t *n_pts, const 
                                   const double *h, double w_veh, const double *w_veh_batch, double f_scale,
                                   const int32_t *centre_id, int32_t *status, void *workspace, size_t workspace_bytes,
                                   void *stream) {
-    if (!reftrack || !normvec || !h || !status) return bad("mc_mincurv_setup_batch: NULL argument");
-    if (!(f_scale > 0.0)) return bad("mc_mincurv_setup_batch: f_scale must be positive");
-    int rc = mc::mincurv_args("mc_mincurv_setup_batch", B, n_max, workspace, workspace_bytes);
-    if (rc) return rc;
-    const mc::Layout L = mc::make_layout(n_max);
-    double *ws = (double *)workspace;
-    cudaStream_t s = (cudaStream_t)stream;
-    constexpr int smem = mc::hband_win_doubles(256) * (int)sizeof(double);      // 49 KB: above the static limit
-    // (per launch: the attribute is per device and a process may drive several)
-    cudaFuncSetAttribute(mc::mincurv_setup_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-    mc::mincurv_setup_kernel<<<B, 256, smem, s>>>(n_max, n_pts, reftrack, normvec, h, w_veh, w_veh_batch, f_scale, centre_id,
-                                                  ws, L, status);
-    if (centre_id) mc::mincurv_share_kernel<<<B, 256, 0, s>>>(B, n_max, n_pts, centre_id, ws, L, status);
-    return check_cuda("mincurv_setup_kernel");
+    return mc::mincurv_setup(B, n_max, n_pts, reftrack, normvec, h, w_veh, w_veh_batch, f_scale, centre_id, nullptr, status,
+                             workspace, workspace_bytes, stream);
 }
 
 int mc_mincurv_setup_batch_ex(int B, int n_max, const int32_t *n_pts, const double *reftrack, const double *normvec,
                               const double *h, double w_veh, const double *w_veh_batch, double f_scale, int32_t *status,
-                              void *workspace, size_t workspace_bytes, void *stream) {
-    return mc_mincurv_setup_batch_shared(B, n_max, n_pts, reftrack, normvec, h, w_veh, w_veh_batch, f_scale, nullptr, status,
-                                         workspace, workspace_bytes, stream);
+                              const double *lin_alpha, void *workspace, size_t workspace_bytes, void *stream) {
+    return mc::mincurv_setup(B, n_max, n_pts, reftrack, normvec, h, w_veh, w_veh_batch, f_scale, nullptr, lin_alpha, status,
+                             workspace, workspace_bytes, stream);
 }
 
 int mc_mincurv_setup_batch(int B, int n_max, const int32_t *n_pts, const double *reftrack, const double *normvec,
                            const double *h, double w_veh, const double *w_veh_batch, int32_t *status, void *workspace,
                            size_t workspace_bytes, void *stream) {
     return mc_mincurv_setup_batch_ex(B, n_max, n_pts, reftrack, normvec, h, w_veh, w_veh_batch, MC_F_SCALE_DEFAULT, status,
-                                     workspace, workspace_bytes, stream);
+                                     nullptr, workspace, workspace_bytes, stream);
 }
 
 }  // extern "C"

@@ -77,6 +77,17 @@ __attribute__((visibility("hidden")))
 int mincurv_kappa_phase(int B, int n_max, const int32_t *n_pts, double kappa_bound, double prox_mu, double *alpha,
                         int32_t *status, int32_t *iters, void *workspace, size_t workspace_bytes, void *stream);
 
+// the assembly (mincurv_setup.cu) with shared centre lines (centre_id) and a linearisation point (lin_alpha [B][n_max]),
+// either NULL; and the finalize stage (mincurv_finalize.cu) of a workspace assembled about a linearisation point (lin)
+// or about the centre line.  Not exported.
+__attribute__((visibility("hidden")))
+int mincurv_setup(int B, int n_max, const int32_t *n_pts, const double *reftrack, const double *normvec, const double *h,
+                  double w_veh, const double *w_veh_batch, double f_scale, const int32_t *centre_id, const double *lin_alpha,
+                  int32_t *status, void *workspace, size_t workspace_bytes, void *stream);
+__attribute__((visibility("hidden")))
+int mincurv_finalize(int B, int n_max, const int32_t *n_pts, const double *alpha, double kappa_bound, double *curv_error_max,
+                     double *kappa_lin_max, int32_t *status, bool lin, void *workspace, size_t workspace_bytes, void *stream);
+
 __device__ __forceinline__ double *vec(double *slab, const Layout &L, int v) { return slab + (size_t)v * L.np; }
 
 // index of the instance whose slab holds this instance's band of H: its own, or with shared centre lines the owner's

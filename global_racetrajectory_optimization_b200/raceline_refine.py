@@ -46,6 +46,8 @@ STATUS_TEXT = {CONVERGED: "converged", ITER_CAP: "iteration cap reached", LINE_S
                NO_GRADIENT: "no usable gradient", EMPTY_BOX: "empty box (track narrower than w_veh)",
                NO_PROJECTION: "projection onto the curvature-limited set failed", INACTIVE: "inactive slot"}
 
+CURV_ERROR_ALLOWED = 0.01     # [1/m] refine_raceline_batch(relinearise=...): the reference's iqp_curverror_allowed
+
 # defaults of the method (Birgin, Martinez and Raydan 2000 use M = 10 and gamma = 1e-4 as well)
 MAX_ITERS = 100        # accepted steps per track
 PG_TOL = 1e-6          # on ||P(x - g) - x||_inf, x in m and g in s/m
@@ -387,9 +389,10 @@ class CurvatureMetric:
     through centre_id, so it costs a factorisation and no assembly).  Tracks outside the mask, and those with fewer than
     N_MIN points, are not launched (n_pts 0, grad_status -1: not ok); with n_max < N_MIN nothing is.  h, the chunk size
     and the chunk-local centre ids are computed once here, so a call does not synchronise the stream.  timer(name) as
-    LapTime's ('metric')."""
+    LapTime's ('metric').  lin_alpha [B, n_max] (None: the centre line): H is that of the QP linearised about the line
+    reftrack + lin_alpha * normvec (DESIGN.md section 3.2)."""
 
-    def __init__(self, reftrack, normvec, n_pts, length: float):
+    def __init__(self, reftrack, normvec, n_pts, length: float, lin_alpha: Optional[torch.Tensor] = None):
         B, n_max, _ = reftrack.shape
         dev = reftrack.device
         self.mu = float(length) ** -4
@@ -406,6 +409,7 @@ class CurvatureMetric:
         two = lambda t: t.repeat_interleave(2, dim=0).contiguous()      # noqa: E731
         self.reftrack = two(torch.cat((reftrack[:, :, :2], torch.ones_like(reftrack[:, :, 2:])), dim=2))
         self.normvec, self.h = two(normvec), two(h)
+        self.lin = None if lin_alpha is None else two(lin_alpha.to(torch.float64))
         chunk = _b._chunk(2 * B, _lib.load().mc_mincurv_workspace_bytes(1, n_max), dev)
         self.chunk = max(2, chunk - chunk % 2)                           # (a track's two rows share a launch)
         r = torch.arange(2 * B, dtype=torch.int32, device=dev)
@@ -432,7 +436,8 @@ class CurvatureMetric:
                 e = min(2 * B, s + self.chunk)
                 _b._mincurv_launch("mc_mincurv_adjoint_batch", e - s, n_pts[s:e], self.reftrack[s:e], self.normvec[s:e],
                                    self.h[s:e], None, 0.0, None, _b.F_SCALE, self.centre_id[s:e], sens[s:e], gs[s:e],
-                                   rhs[s:e], out[s:e], gwl[s:e], gwv[s:e], None, None, None, 0)
+                                   rhs[s:e], out[s:e], gwl[s:e], gwv[s:e], None, None, None, 0,
+                                   None if self.lin is None else self.lin[s:e])
             out, gs = out.reshape(B, 2, n_max), gs.reshape(B, 2)
             u, w = out[:, 0], (out[:, 1] if y is not None else None)
             ok = go & (gs[:, 0] == 0) & torch.isfinite(u).all(dim=1)
@@ -453,9 +458,12 @@ class CurvatureProjection:
     bind, the curvature-row phase).  ok: the QP's status is 0 and y is finite.  Tracks outside the mask get n_pts 0, those
     with fewer than N_MIN points are never launched (not ok); with n_max < N_MIN nothing is.  h and the chunk size are
     computed once here, so a call does not synchronise the stream.  kappa_lin(x, mask) -> kappa_lin_max [B], the QP's
-    max |k_ref + E x| at x (assembly and the finalize stage).  timer(name) as LapTime's ('projection')."""
+    max |k_ref + E x| at x (assembly and the finalize stage); evaluate(x, mask) -> (kappa_lin_max, curv_error_max) [B].
+    timer(name) as LapTime's ('projection').  lin_alpha [B, n_max] (None: the centre line): P and H are those of the QP
+    linearised about the line reftrack + lin_alpha * normvec (DESIGN.md section 3.2)."""
 
-    def __init__(self, reftrack, normvec, n_pts, w_veh, kappa_bound: float, length: float):
+    def __init__(self, reftrack, normvec, n_pts, w_veh, kappa_bound: float, length: float,
+                 lin_alpha: Optional[torch.Tensor] = None):
         B, n_max, _ = reftrack.shape
         dev = reftrack.device
         self.mu, self.kb = float(length) ** -4, float(kappa_bound)
@@ -464,6 +472,7 @@ class CurvatureProjection:
         self.w_scalar, self.w_batch = _b._wveh(w_veh, B, dev)
         self.timer = lambda name: contextlib.nullcontext()
         self.chunk = None
+        self.lin = None if lin_alpha is None else lin_alpha.to(torch.float64).contiguous()
         if n_max < _b.N_MIN:
             return
         self.reftrack, self.normvec = reftrack.contiguous(), normvec.contiguous()
@@ -485,15 +494,18 @@ class CurvatureProjection:
             _b._launch_chunks("mc_mincurv_solve_batch_ex", B, self.chunk, self._ws(), n_max,
                               *map(_b._rows, (self._n(mask), self.reftrack, self.normvec, self.h)), self.kb, self.w_scalar,
                               _b._rows(self.w_batch), _b.F_SCALE, *map(_b._rows, out.values()), self.mu,
-                              _b._rows(x.contiguous()), _b._rows(q.contiguous()))
+                              _b._rows(x.contiguous()), _b._rows(q.contiguous()), _b._rows(self.lin))
             ok = mask & self.launchable & (out["status"] == 0) & torch.isfinite(out["alpha"]).all(dim=1)
             return out["alpha"], ok
 
     def kappa_lin(self, x, mask):
+        return self.evaluate(x, mask)[0]
+
+    def evaluate(self, x, mask):
         B, n_max = x.shape
         kmax = torch.full((B,), math.nan, dtype=torch.float64, device=x.device)
         if self.chunk is None:
-            return kmax
+            return kmax, kmax.clone()
         out = _b._mincurv_results(B, n_max, x.device)
         n = self._n(mask)
         ws = self._ws()
@@ -502,10 +514,11 @@ class CurvatureProjection:
             e = min(B, s + self.chunk)
             _b._call("mc_mincurv_setup_batch_ex", e - s, n_max, n[s:e], self.reftrack[s:e], self.normvec[s:e], self.h[s:e],
                      self.w_scalar, None if self.w_batch is None else self.w_batch[s:e], _b.F_SCALE, out["status"][s:e],
-                     ws=ws)
+                     None if self.lin is None else self.lin[s:e], ws=ws)
             _b._call("mc_mincurv_finalize_batch", e - s, n_max, n[s:e], x[s:e], self.kb, out["curv_error_max"][s:e],
-                     out["kappa_lin_max"][s:e], out["status"][s:e], ws=ws)
-        return torch.where(mask & self.launchable & (out["status"] != 1) & (out["status"] >= 0), out["kappa_lin_max"], kmax)
+                     out["kappa_lin_max"][s:e], out["status"][s:e], int(self.lin is not None), ws=ws)
+        ok = mask & self.launchable & (out["status"] != 1) & (out["status"] >= 0)
+        return torch.where(ok, out["kappa_lin_max"], kmax), torch.where(ok, out["curv_error_max"], kmax)
 
 
 def refine_raceline_batch(reftrack: torch.Tensor, normvec: torch.Tensor, alpha0: torch.Tensor,
@@ -515,7 +528,8 @@ def refine_raceline_batch(reftrack: torch.Tensor, normvec: torch.Tensor, alpha0:
                           pg_tol: float = PG_TOL, memory: int = MEMORY, gamma: float = GAMMA, lam_min: float = LAM_MIN,
                           lam_max: float = LAM_MAX, max_halvings: int = MAX_HALVINGS,
                           callback: Optional[Callable] = None, objective: Optional[LapTime] = None,
-                          metric_length: Optional[float] = None, kappa_bound: Optional[float] = None) -> dict:
+                          metric_length: Optional[float] = None, kappa_bound: Optional[float] = None,
+                          relinearise: int = 0, curv_error_allowed: float = CURV_ERROR_ALLOWED) -> dict:
     """Lowers the quasi-steady-state lap time of every track's raceline by moving alpha inside opt_min_curv's box.
 
     reftrack [B, n_max, 4], normvec [B, n_max, 2] and alpha0 [B, n_max] (normally the opt_min_curv_batch result) as for
@@ -545,7 +559,22 @@ def refine_raceline_batch(reftrack: torch.Tensor, normvec: torch.Tensor, alpha0:
     points) alpha0 is returned with NaN lap times.  The result also holds kappa_lin_max [B] (the QP's max |k_ref + E alpha|
     at the result), kappa_max [B] (the raceline's max |kappa| from create_raceline_batch at the result; the rows are a
     linearisation, so it may exceed kb by about curv_error_max) and projection_failures [B] int32; kappa_lin_max and
-    kappa_max are NaN where alpha0 is returned."""
+    kappa_max are NaN where alpha0 is returned, and curv_error_max [B] (the QP's linearisation error at the result).
+
+    relinearise: r >= 0 outer rounds after the first (kappa_bound required), as the reference's iterative QP does on a
+    fixed grid.  Round 0 is the run above, about the centre line.  Round k >= 1 starts from the previous round's result
+    x_k, builds the projection and the metric about the line reftrack + x_k * normvec (DESIGN.md section 3.2), projects
+    x_k onto that set and runs spg() for up to max_iters iterations.  A track leaves after a round whose result has
+    curv_error_max (against that round's linearisation) <= curv_error_allowed, or after round relinearise; a track whose
+    round-start projection fails keeps the previous round's result with status NO_PROJECTION.  The result then also holds
+    rounds [B] int32 (the last round whose result is returned); iters, evals and projection_failures add up over the
+    rounds, laptime_start is that of round 0, and status, pg_norm, kappa_lin_max and curv_error_max are the last round's."""
+    if int(relinearise) != relinearise or relinearise < 0:
+        raise ValueError("refine_raceline_batch: relinearise must be an integer >= 0")
+    if relinearise and kappa_bound is None:
+        raise ValueError("refine_raceline_batch: relinearise needs kappa_bound (it re-linearises the curvature rows)")
+    if not (math.isfinite(float(curv_error_allowed)) and float(curv_error_allowed) >= 0.0):
+        raise ValueError("refine_raceline_batch: curv_error_allowed must be a finite curvature >= 0 [1/m]")
     if metric_length is not None and not (math.isfinite(float(metric_length)) and float(metric_length) > 0.0):
         raise ValueError("refine_raceline_batch: metric_length must be None or a finite length > 0 [m]")
     if kappa_bound is not None:
@@ -599,13 +628,48 @@ def refine_raceline_batch(reftrack: torch.Tensor, normvec: torch.Tensor, alpha0:
                pg_norm=res["pg_norm"])
     if project is not None:
         nan_b = torch.full_like(res["f"], math.nan)
-        out["kappa_lin_max"] = torch.where(kept, nan_b, project.kappa_lin(res["x"], ~kept))
+        kl, ce = project.evaluate(res["x"], ~kept)
+        out["kappa_lin_max"], out["curv_error_max"] = torch.where(kept, nan_b, kl), torch.where(kept, nan_b, ce)
+        out["projection_failures"] = res["projection_failures"]
+        if relinearise:
+            _rounds(out, fun, reftrack, normvec, n_pts, w_veh, lb, ub, kept, int(relinearise), float(curv_error_allowed),
+                    float(kappa_bound), float(metric_length), dict(max_iters=max_iters, pg_tol=pg_tol, memory=memory,
+                    gamma=gamma, lam_min=lam_min, lam_max=lam_max, max_halvings=max_halvings, callback=callback))
+        else:
+            out["rounds"] = torch.zeros_like(out["iters"])
         rl = _b.create_raceline_batch(reftrack, normvec, out["alpha"], stepsize_interp,
                                       n_pts=torch.where(kept, torch.zeros_like(project.n_pts), project.n_pts))
         k = rl["kappa"].abs()
         k = torch.where(torch.arange(k.shape[1], device=dev)[None, :] < rl["n_out"][:, None], k, torch.zeros_like(k))
         out["kappa_max"] = torch.where(kept | (rl["n_out"] <= 0), nan_b, k.amax(dim=1))
-        out["projection_failures"] = res["projection_failures"]
     elif metric is not None:
         out["metric_fallbacks"] = res["metric_fallbacks"]
     return out
+
+
+def _rounds(out, fun, reftrack, normvec, n_pts, w_veh, lb, ub, kept, relinearise, allowed, kb, length, spg_opts):
+    """The outer rounds of refine_raceline_batch(relinearise=...), updating out (round 0's result) in place."""
+    B = kept.shape[0]
+    rounds = torch.zeros((B,), dtype=torch.int32, device=kept.device)
+    done = kept | (out["curv_error_max"] <= allowed)
+    for r in range(1, relinearise + 1):
+        go = ~done
+        if not bool(go.any()):                                              # the round's one read
+            break
+        x0 = out["alpha"].clone()
+        project = CurvatureProjection(reftrack, normvec, n_pts, w_veh, kb, length, lin_alpha=x0)
+        metric = CurvatureMetric(reftrack, normvec, n_pts, length, lin_alpha=x0)
+        project.timer = metric.timer = fun.timer
+        res = spg(fun, x0, lb, ub, go, metric=metric, project=project, **spg_opts)
+        failed = go & (res["status"] == NO_PROJECTION) & (res["evals"] == 0)
+        ok = go & ~failed
+        kl, ce = project.evaluate(res["x"], ok)
+        out["alpha"] = torch.where(ok[:, None], res["x"], out["alpha"])
+        for k, v in (("laptime", res["f"]), ("pg_norm", res["pg_norm"]), ("kappa_lin_max", kl), ("curv_error_max", ce)):
+            out[k] = torch.where(ok, v, out[k])
+        out["status"] = torch.where(ok, res["status"], torch.where(failed, NO_PROJECTION, out["status"])).to(torch.int32)
+        for k in ("iters", "evals", "projection_failures"):
+            out[k] = (out[k] + torch.where(go, res[k], torch.zeros_like(res[k]))).to(torch.int32)
+        rounds = torch.where(ok, r, rounds).to(torch.int32)
+        done |= failed | (ok & (ce <= allowed))
+    out["rounds"] = rounds

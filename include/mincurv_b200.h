@@ -40,6 +40,9 @@ extern "C" {
  * may be 0), and NULL gives the entry's earlier behaviour exactly.  The package's ctypes binding lets a call leave them
  * out altogether, so code written for the earlier signature keeps working; C callers pass NULL / 0. */
 #define MC_OPTIONAL
+/* MC_OPTIONAL2 marks parameters added after the MC_OPTIONAL ones, alike NULL-able.  The binding lets a call leave out
+ * the MC_OPTIONAL2 parameters alone (the signature before they were added), or them and the MC_OPTIONAL ones. */
+#define MC_OPTIONAL2
 
 #define MC_STATUS_OK 0
 #define MC_STATUS_TOO_NARROW 1
@@ -111,13 +114,21 @@ int mc_mincurv_solve_batch(int B, int n_max, const int32_t *n_pts,
  *                    + q^T (alpha - x);  prox_mu > 0 and finite, prox_q required.  f_scale is checked but does not enter
  *                    the objective; the stages are those of mc_mincurv_solve_batch (assembly, box phase, finalize,
  *                    curvature-row phase, finalize) on H + prox_mu I, without shared centre lines.  kappa_lin_max and
- *                    curv_error_max are those of the result; status as above (4: the rows are still violated). */
+ *                    curv_error_max are those of the result; status as above (4: the rows are still violated).
+ *   lin_alpha [B][n_max] or NULL : the linearisation point a (DESIGN.md section 3.2), with or without prox_x.  NULL: the
+ *                    QP as tph builds it, its curvature rows linearised about the centre line P.  Otherwise about the line
+ *                    P + a n on the same grid (the step of tph's iterative QP, without re-sampling): the first
+ *                    derivatives x', y' in S_x, S_y are those of the spline through P + a n, k_ref = S_y m_y - S_x m_x
+ *                    keeps the centre line's moments, so that k_ref + E a is the knot curvature of the spline through
+ *                    P + a n.  H, f and the rows follow from these; the variable is still alpha about P.  curv_error_max
+ *                    and kappa_lin_max refer to this linearisation. */
 int mc_mincurv_solve_batch_ex(int B, int n_max, const int32_t *n_pts,
                               const double *reftrack, const double *normvec, const double *h,
                               double kappa_bound, double w_veh, const double *w_veh_batch, double f_scale,
                               double *alpha, double *curv_error_max, double *kappa_lin_max,
                               int32_t *status, int32_t *iters,
                               double prox_mu, const double *prox_x, const double *prox_q,
+                              MC_OPTIONAL2 const double *lin_alpha,
                               void *workspace, size_t workspace_bytes, void *stream);
 
 /* the same for batches in which several instances share a centreline (x, y, normal vectors, h and n_pts identical, only
@@ -143,17 +154,21 @@ int mc_mincurv_setup_batch_shared(int B, int n_max, const int32_t *n_pts, const 
 /* The three stages of mc_mincurv_solve_batch as separate stream-ordered calls on the same workspace
  * (assembly of the banded QP, interior-point solve, post-solve curvature check / linearisation error);
  * mc_mincurv_solve_batch is exactly setup -> pdip -> finalize.  Exposed so that a caller can time or
- * overlap the stages; arguments as above. */
+ * overlap the stages; arguments as above.  The finalize stage of a workspace assembled about a linearisation point
+ * (lin_alpha of mc_mincurv_setup_batch_ex) needs linearised = 1: the line P + alpha n takes the centre line's first
+ * derivatives, the linearised curvature those of the linearisation point. */
 int mc_mincurv_setup_batch(int B, int n_max, const int32_t *n_pts, const double *reftrack, const double *normvec,
                            const double *h, double w_veh, const double *w_veh_batch, int32_t *status,
                            void *workspace, size_t workspace_bytes, void *stream);
 int mc_mincurv_setup_batch_ex(int B, int n_max, const int32_t *n_pts, const double *reftrack, const double *normvec,
                               const double *h, double w_veh, const double *w_veh_batch, double f_scale, int32_t *status,
+                              MC_OPTIONAL2 const double *lin_alpha,
                               void *workspace, size_t workspace_bytes, void *stream);
 int mc_mincurv_pdip_batch(int B, int n_max, const int32_t *n_pts, double *alpha, int32_t *status, int32_t *iters,
                           void *workspace, size_t workspace_bytes, void *stream);
 int mc_mincurv_finalize_batch(int B, int n_max, const int32_t *n_pts, const double *alpha, double kappa_bound,
                               double *curv_error_max, double *kappa_lin_max, int32_t *status,
+                              MC_OPTIONAL2 int linearised,
                               void *workspace, size_t workspace_bytes, void *stream);
 
 /* Width sensitivities of this QP: alpha differentiated with respect to w_tr_right, w_tr_left and w_veh by one more
@@ -194,7 +209,10 @@ int mc_mincurv_finalize_batch(int B, int n_max, const int32_t *n_pts, const doub
  * is differentiated at the curvature-row phase's iterate: one factorisation of H + diag(sens[0] + sens[1]) + E^T W E
  * with the weak rows (W <= 1) in the band, and the n_rows[b] strong rows through their Schur complement, a dense
  * n_rows[b]^2 matrix kept in schur [B][n_rows_cap][n_rows_cap] (required with sens_rows); an instance with
- * n_rows[b] > n_rows_cap gets grad_status 3. */
+ * n_rows[b] > n_rows_cap gets grad_status 3.
+ * lin_alpha (NULL: the centre line): the linearisation point of H, as for mc_mincurv_solve_batch_ex; with centre_id a
+ * follower is linearised about its owner's row (the assembly is shared); alpha is not
+ * differentiated with respect to it. */
 int mc_mincurv_solve_batch_sens(int B, int n_max, const int32_t *n_pts,
                                 const double *reftrack, const double *normvec, const double *h,
                                 double kappa_bound, double w_veh, const double *w_veh_batch, double f_scale,
@@ -210,6 +228,7 @@ int mc_mincurv_adjoint_batch(int B, int n_max, const int32_t *n_pts,
                              double *grad_w_right, double *grad_w_left, double *grad_w_veh,
                              MC_OPTIONAL const double *sens_rows, MC_OPTIONAL const int32_t *n_rows,
                              MC_OPTIONAL double *schur, MC_OPTIONAL int n_rows_cap,
+                             MC_OPTIONAL2 const double *lin_alpha,
                              void *workspace, size_t workspace_bytes, void *stream);
 
 /* Fourth stage, run by mc_mincurv_solve_batch between two finalize passes: re-solves every instance flagged

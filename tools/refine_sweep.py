@@ -36,6 +36,7 @@ def main():
     ap.add_argument("--lengths", type=float, nargs="+", default=[5.0, 10.0, 20.0, 40.0, 80.0])
     ap.add_argument("--kappa-bounds", type=float, nargs="*", default=[CURVLIM])
     ap.add_argument("--max-iters", type=int, default=R.MAX_ITERS)
+    ap.add_argument("--relinearise", type=int, default=0, help="outer rounds that re-linearise the curvature rows")
     ap.add_argument("--out", default=None)
     args = ap.parse_args()
     if not torch.cuda.is_available():
@@ -57,7 +58,8 @@ def main():
     runs = []
     for ell, kb in [(None, None)] + [(ell, kb) for ell in args.lengths for kb in [None] + list(args.kappa_bounds)]:
         res = R.refine_raceline_batch(rt, nv, al, wv, n_pts=npts, stepsize_interp=STEP, max_iters=args.max_iters,
-                                      metric_length=ell, kappa_bound=kb, **veh)
+                                      metric_length=ell, kappa_bound=kb,
+                                      relinearise=args.relinearise if kb is not None else 0, **veh)
         rl = B_.create_raceline_batch(rt, nv, res["alpha"], STEP, n_pts=npts)
         tracks = {}
         for b, nm in enumerate(NAMES):

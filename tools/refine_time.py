@@ -78,6 +78,7 @@ def main():
     ap.add_argument("--max-iters", type=int, default=R.MAX_ITERS)
     ap.add_argument("--metric-length", type=float, default=None)
     ap.add_argument("--kappa-bound", type=float, default=None)
+    ap.add_argument("--relinearise", type=int, default=0, help="outer rounds that re-linearise the curvature rows")
     ap.add_argument("--out", default=None)
     args = ap.parse_args()
     if not torch.cuda.is_available():
@@ -94,7 +95,8 @@ def main():
             obj.timer = rec
         return R.refine_raceline_batch(rt, nv, alpha, 2.0, GGV, MACH, stepsize_interp=STEP, max_iters=max_iters,
                                        objective=obj, callback=None if rec is None else rec.callback,
-                                       metric_length=args.metric_length, kappa_bound=args.kappa_bound, **VEH)
+                                       metric_length=args.metric_length, kappa_bound=args.kappa_bound,
+                                       relinearise=args.relinearise, **VEH)
 
     run(2)                                                    # warm-up: every launch and allocation size once
     torch.cuda.synchronize()
