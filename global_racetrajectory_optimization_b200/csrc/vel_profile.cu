@@ -50,7 +50,10 @@ __global__ void __launch_bounds__(128, 5) vel_profile_kernel(const VpArgs a) {
     if (p >= P) return;
     const int b = (int)(p / a.V), v = (int)(p - (size_t)b * a.V);
     const int n = a.n_pts ? a.n_pts[b] : a.n_max;
-    if (n < 2 || n > a.n_max) {          // inactive / invalid track: no profile
+    // inactive / invalid track: no profile.  A track shorter than the half-width of the moving-average window is refused
+    // too: tph's cyclic conv_filt returns a profile of the wrong length there (the kernel would average over more than one
+    // lap).
+    if (n < 2 || n > a.n_max || (a.pr.filt_window > 1 && (a.pr.filt_window - 1) / 2 > n)) {
         a.laptime[p] = 0.0;
         // n == 0: an inactive slot (ok); n < 0: the producer reported an overflow (create_raceline's -needed) -- never a lap time
         if (a.status) a.status[p] = (n == 0) ? vp::VP_STATUS_OK : MC_STATUS_BREAKDOWN;
@@ -118,7 +121,7 @@ __global__ void __launch_bounds__(128) vel_profile_adjoint_kernel(const VpAdjArg
     const int b = (int)(p / a.V), v = (int)(p - (size_t)b * a.V);
     const int n = a.n_pts ? a.n_pts[b] : a.n_max;
     const size_t row = (size_t)b * a.n_max;
-    const bool active = n >= 2 && n <= a.n_max;
+    const bool active = n >= 2 && n <= a.n_max && !(a.pr.filt_window > 1 && (a.pr.filt_window - 1) / 2 > n);   // as K5
     double *g_kappa = (a.V == 1 && a.g_kappa) ? a.g_kappa + row : nullptr;
     double *g_el = (a.V == 1 && a.g_el) ? a.g_el + row : nullptr;
     int st = (n == 0) ? vp::VP_STATUS_OK : MC_STATUS_BREAKDOWN;          // an inactive slot: K5's status, zeros

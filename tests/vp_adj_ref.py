@@ -53,6 +53,19 @@ class Harness:
                                                    _p(vx), _p(ax), _p(t), _p(lap))
         return st, vx, float(lap[0])
 
+    def profile(self, kappa, el, ggv, mach, v_max, scale=1.0, exp=1.0, filt=0, mu=None, upper=1, drag_coeff=0.75,
+                m_veh=1200.0, stride=1):
+        """dict(status, vx [n], ax [n], t [n + 1], laptime) of profile_thread, with a ggv scale and per-point mu."""
+        n = kappa.size
+        kappa, el = np.ascontiguousarray(kappa, dtype=float), np.ascontiguousarray(el, dtype=float)
+        ggv, mach = np.ascontiguousarray(ggv, dtype=float), np.ascontiguousarray(mach, dtype=float)
+        mu = None if mu is None else np.ascontiguousarray(mu, dtype=float)
+        vx, ax, t, lap = np.zeros(n), np.zeros(n), np.zeros(n + 1), np.zeros(1)
+        st = self.libs[int(upper)].vp_host_profile(n, _p(kappa), _p(el), _p(mu), float(scale), float(v_max), ggv.shape[0],
+                                                   _p(ggv), mach.shape[0], _p(mach), float(exp), drag_coeff, m_veh, int(filt),
+                                                   int(stride), _p(vx), _p(ax), _p(t), _p(lap))
+        return dict(status=st, vx=vx, ax=ax, t=t, laptime=float(lap[0]))
+
     def adjoint(self, kappa, el, ggv, mach, v_max, g_lap, g_vx=None, exp=1.0, filt=0, upper=1, drag_coeff=0.75,
                 m_veh=1200.0, stride=1):
         """dict(status, g_kappa, g_el, laptime, codes [4n] (forward pass, then backward pass), iters) of
