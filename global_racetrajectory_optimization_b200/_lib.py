@@ -61,6 +61,35 @@ def optional_parameters(path: str, marker: str = "MC_OPTIONAL") -> dict:
     return out
 
 
+def header_struct(path: str, name: str):
+    """A ctypes.Structure with the fields of `typedef struct { ... } name;` in the C header at path (the scalar and
+    pointer types of header_signatures)."""
+    m = re.search(rf"typedef\s+struct\s*\{{([^}}]*)\}}\s*{name}\s*;", _c_source(path))
+    if m is None:
+        raise MinCurvLibError(f"{path}: no typedef struct {name}")
+    fields = []
+    for decl in filter(str.strip, m.group(1).split(";")):
+        base, *rest = decl.split(",")
+        first = re.match(r"\s*(.*?)([\s*]+)(\w+)\s*$", base)
+        if first is None:
+            raise MinCurvLibError(f"{name}: cannot read the field declaration '{decl.strip()}'")
+        typ = first.group(1).strip()
+        for stars, field in [(first.group(2), first.group(3))] + [re.match(r"\s*([\s*]*)(\w+)\s*$", r).groups()
+                                                                  for r in rest]:
+            stars = stars.strip()        # (a const scalar is passed as the scalar)
+            fields.append((field, _ctype(typ + " " + stars if stars else re.sub(r"\bconst\b", "", typ), name)))
+    return type(name, (ctypes.Structure,), {"_fields_": fields})
+
+
+def header_define(path: str, name: str) -> int:
+    """The integer value of `#define name value` (or `(value)`) in the C header at path."""
+    with open(path) as f:
+        m = re.search(rf"^[ \t]*#[ \t]*define[ \t]+{name}[ \t]+\(?(-?\d+)\)?", f.read(), flags=re.M)
+    if m is None:
+        raise MinCurvLibError(f"{path}: no #define {name}")
+    return int(m.group(1))
+
+
 _SIGS = header_signatures(_build.HEADER)
 _OPTIONAL = optional_parameters(_build.HEADER)
 _OPTIONAL2 = optional_parameters(_build.HEADER, "MC_OPTIONAL2")

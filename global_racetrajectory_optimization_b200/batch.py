@@ -771,13 +771,139 @@ def _to_device(t: torch.Tensor, dev) -> torch.Tensor:
     return t.to(dev).contiguous()
 
 
+class Vehicles:
+    """K vehicles for the vehicles= argument of the velocity-profile entry points (vel_profile_batch, vel_profile_diff,
+    lap_time_matrix_batch, lap_time_matrix_diff, raceline_refine.refine_raceline_batch), each with its own tables and
+    scalars; veh_id [B] then picks the vehicle of each track.
+
+    ggv, ax_max_machines: sequences of K tables ([rows, 3] and [rows, 2], 1 to 256 rows each; e.g. the pairs
+    import_veh_dyn_info returns); v_max, drag_coeff, m_veh: K-sequences (a number stands for all K).  The checks of tph
+    run here, once, per vehicle (each table must cover that vehicle's v_max; a call with per-variant top speeds checks
+    those against every vehicle's tables on the host).  The tables are packed back to back and copied to device once,
+    through pinned memory: a reused object costs no copy and no stream synchronisation per call.  device: where the
+    tracks will be (default: the current CUDA device)."""
+
+    def __init__(self, ggv, ax_max_machines, v_max, drag_coeff, m_veh, device=None):
+        if isinstance(ggv, torch.Tensor) or isinstance(ax_max_machines, torch.Tensor):
+            raise TypeError("Vehicles: ggv and ax_max_machines are sequences of one table per vehicle")
+        ggv, mach = list(ggv), list(ax_max_machines)
+        K = len(ggv)
+        if K < 1 or len(mach) != K:
+            raise ValueError("Vehicles: ggv and ax_max_machines need one table per vehicle (at least one vehicle)")
+        vm, drag, mass = (self._per_vehicle(x, K, name) for x, name in ((v_max, "v_max"), (drag_coeff, "drag_coeff"),
+                                                                         (m_veh, "m_veh")))
+        ggv = [_table(g, 3, f"ggv[{k}]") for k, g in enumerate(ggv)]
+        mach = [_table(m, 2, f"ax_max_machines[{k}]") for k, m in enumerate(mach)]
+        for k in range(K):
+            if ggv[k].shape[0] < 1 or mach[k].shape[0] < 1:
+                raise ValueError(f"Vehicles: vehicle {k} has an empty table")
+            if not (math.isfinite(vm[k]) and vm[k] > 0.0):
+                raise ValueError(f"Vehicles: v_max[{k}] must be a finite speed > 0")
+            if not (math.isfinite(mass[k]) and mass[k] > 0.0):
+                raise ValueError(f"Vehicles: m_veh[{k}] must be > 0")
+        self.n_veh = K
+        self.v_max, self.drag_coeff, self.m_veh = vm, drag, mass
+        self._ggv_top = [float(g[-1, 0]) for g in ggv]
+        self._mach_top = [float(m[-1, 0]) for m in mach]
+        for k in range(K):
+            self.check_covers(vm[k], k)
+        rows = torch.zeros((K + 1, 2), dtype=torch.int32)
+        rows[1:, 0] = torch.cumsum(torch.tensor([g.shape[0] for g in ggv]), 0)
+        rows[1:, 1] = torch.cumsum(torch.tensor([m.shape[0] for m in mach]), 0)
+        par = torch.tensor([vm, drag, mass], dtype=torch.float64).T.contiguous()
+        dev = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
+        self.ggv, self.ax_max_machines = _to_device(torch.cat(ggv), dev), _to_device(torch.cat(mach), dev)
+        self.rows, self.par = _to_device(rows, dev), _to_device(par, dev)
+        self.device = self.ggv.device
+
+    @staticmethod
+    def _per_vehicle(x, K, name):
+        if isinstance(x, torch.Tensor):
+            x = x.detach().cpu().reshape(-1).tolist()
+        elif not hasattr(x, "__len__"):
+            x = [x] * K
+        x = [float(v) for v in x]
+        if len(x) != K:
+            raise ValueError(f"Vehicles: {name} needs one value per vehicle ({K})")
+        return x
+
+    def check_covers(self, v_top: float, k: Optional[int] = None) -> None:
+        """tph's range checks: the tables of vehicle k (None: of every vehicle) cover the speed v_top."""
+        for j in range(self.n_veh) if k is None else (k,):
+            if self._mach_top[j] < v_top:
+                raise RuntimeError("ax_max_machines has to cover the entire velocity range of the car (i.e. >= v_max)!")
+            if self._ggv_top[j] < v_top:
+                raise RuntimeError("ggv has to cover the entire velocity range of the car (i.e. >= v_max)!")
+
+    def veh_id(self, veh_id, B: int, dev) -> torch.Tensor:
+        """veh_id as the [B] int32 device tensor the C-ABI takes.  None: one vehicle per track (K == B).  A host veh_id
+        is range-checked here and copied through pinned memory; a device veh_id is not read (the kernels refuse a track
+        whose id is out of range)."""
+        if veh_id is None:
+            if self.n_veh != B:
+                raise ValueError(f"veh_id is required unless there is one vehicle per track ({self.n_veh} vehicles, "
+                                 f"{B} tracks)")
+            veh_id = torch.arange(B, dtype=torch.int32)
+        if isinstance(veh_id, torch.Tensor) and veh_id.device.type != "cpu":
+            if veh_id.numel() != B or veh_id.dtype.is_floating_point or veh_id.dtype == torch.bool:
+                raise ValueError("veh_id must hold one integer per track")
+            return veh_id.to(device=dev, dtype=torch.int32).reshape(B).contiguous()
+        ids = torch.as_tensor(veh_id).reshape(-1)
+        if ids.numel() != B or ids.dtype.is_floating_point or ids.dtype == torch.bool:
+            raise ValueError("veh_id must hold one integer per track")
+        if bool(((ids < 0) | (ids >= self.n_veh)).any()):
+            raise ValueError(f"veh_id must be in 0 .. {self.n_veh - 1}")
+        return _to_device(ids.to(torch.int32), dev)
+
+
+# vehicle mode of the velocity-profile entries: n_ggv = MC_VP_VEHICLES, ggv = the address of an mc_vp_vehicles
+VP_VEHICLES = _lib.header_define(_lib._build.HEADER, "MC_VP_VEHICLES")
+_VpVehiclesDesc = _lib.header_struct(_lib._build.HEADER, "mc_vp_vehicles")
+
+
+def _vp_vehicles(vehicles: Vehicles, veh_id, ggv, ax_max_machines, v_max, ggv_scales, drag_coeff, m_veh, B, dev):
+    """The vehicle-mode part of _vp_inputs: (V, vmax_t, scale_t, the table arguments of the C-ABI (n_ggv, ggv, n_mach,
+    ax_max_machines)).  ggv is a callable of the chunk (s, e) as _launch_chunks takes it: a reference to the
+    mc_vp_vehicles of tracks s:e (held by the reference until the call has read it)."""
+    if not isinstance(vehicles, Vehicles):
+        raise TypeError("vehicles must be a batch.Vehicles")
+    if (any(x is not None for x in (ggv, ax_max_machines, drag_coeff, m_veh))
+            or (v_max is not None and ggv_scales is None)):
+        raise ValueError("with vehicles= the ggv, ax_max_machines, v_max, drag_coeff and m_veh arguments must be None "
+                         "(each vehicle has its own; v_max may give per-variant top speeds with ggv_scales)")
+    if vehicles.device != torch.device(dev):
+        raise ValueError(f"vehicles are on {vehicles.device}, the tracks on {dev}")
+    ids = vehicles.veh_id(veh_id, B, dev)
+    V, vmax_t, scale_t = 1, None, None
+    if ggv_scales is not None:
+        sc = torch.as_tensor(ggv_scales, dtype=torch.float64).reshape(-1)
+        V, scale_t = int(sc.numel()), sc.to(dev).contiguous()
+        if v_max is not None:
+            vm = torch.as_tensor(v_max, dtype=torch.float64).reshape(-1)
+            if vm.numel() == 1 and V > 1:
+                vm = vm.expand(V).clone()
+            if vm.numel() != V:
+                raise ValueError("v_max and ggv_scales must have one entry per variant")
+            vehicles.check_covers(float(vm.max().item()))
+            vmax_t = vm.to(dev).contiguous()
+    def desc(s, e):
+        d = _VpVehiclesDesc(n_veh=vehicles.n_veh, n_ggv=int(vehicles.ggv.shape[0]),
+                            n_mach=int(vehicles.ax_max_machines.shape[0]), ggv=vehicles.ggv.data_ptr(),
+                            ax_max_machines=vehicles.ax_max_machines.data_ptr(), veh_rows=vehicles.rows.data_ptr(),
+                            veh_par=vehicles.par.data_ptr(), veh_id=ids[s:e].data_ptr())
+        d.tensors = (vehicles, ids)                       # (the buffers outlive the descriptor)
+        return ctypes.byref(d)
+    return V, vmax_t, scale_t, (VP_VEHICLES, desc, 0, None)
+
+
 def _vp_inputs(kappa, el_lengths, ggv, ax_max_machines, v_max, ggv_scales, drag_coeff, m_veh, dyn_model_exp, filt_window,
-               n_pts, decel_slice_upper, mu=None, max_chunk=None):
+               n_pts, decel_slice_upper, mu=None, max_chunk=None, vehicles=None, veh_id=None):
     """The checked and normalised inputs of vel_profile_batch, vel_profile_diff and lap_time_matrix_diff: kappa and
     el_lengths as contiguous float64 CUDA tensors [B, n_max], and a namespace of the rest as the C-ABI takes it: B, n_max,
     dev, mu, n_pts, V variants per track with their top speeds vmax_t and ggv scales scale_t ([V] on the device; both None
     for one profile per track at top speed v_scalar), common: the arguments from n_ggv to decel_slice_upper, which
-    mc_vel_profile_batch_ex and mc_vel_profile_adjoint_batch take alike, and max_chunk (see _vp_chunk)."""
+    mc_vel_profile_batch_ex and mc_vel_profile_adjoint_batch take alike (with vehicles: n_ggv = MC_VP_VEHICLES and the
+    chunk's mc_vp_vehicles in place of ggv), and max_chunk (see _vp_chunk)."""
     kappa = _f64(kappa, "kappa")
     el_lengths = _f64(el_lengths, "el_lengths")
     B, n_max = kappa.shape
@@ -789,10 +915,22 @@ def _vp_inputs(kappa, el_lengths, ggv, ax_max_machines, v_max, ggv_scales, drag_
         if mu.shape != (B, n_max):
             raise RuntimeError("kappa and mu must have the same length!")
     n_pts = _npts(n_pts, B, dev)
-    ggv_h = _table(ggv, 3, "ggv")
-    mach_h = _table(ax_max_machines, 2, "ax_max_machines")
     if filt_window is not None and int(filt_window) % 2 != 1:
         raise RuntimeError("Window width of moving average filter must be odd!")
+    upper = int(VP_DECEL_SLICE_UPPER if decel_slice_upper is None else decel_slice_upper)
+    filt = 0 if filt_window is None else int(filt_window)
+    if vehicles is not None or veh_id is not None:
+        if vehicles is None:
+            raise ValueError("veh_id needs vehicles=")
+        V, vmax_t, scale_t, tables = _vp_vehicles(vehicles, veh_id, ggv, ax_max_machines, v_max, ggv_scales, drag_coeff,
+                                                  m_veh, B, dev)
+        return kappa, el_lengths, SimpleNamespace(B=B, n_max=n_max, dev=dev, mu=mu, n_pts=n_pts, V=V, vmax_t=vmax_t,
+                                                  scale_t=scale_t, v_scalar=0.0, max_chunk=max_chunk,
+                                                  common=(*tables, float(dyn_model_exp), 0.0, 0.0, filt, upper))
+    if any(x is None for x in (ggv, ax_max_machines, v_max, drag_coeff, m_veh)):
+        raise TypeError("the velocity profile needs ggv, ax_max_machines, v_max, drag_coeff and m_veh (or vehicles=)")
+    ggv_h = _table(ggv, 3, "ggv")
+    mach_h = _table(ax_max_machines, 2, "ax_max_machines")
     vmax_t = scale_t = None
     if ggv_scales is not None or isinstance(v_max, torch.Tensor) or hasattr(v_max, "__len__"):
         vm = torch.as_tensor(v_max, dtype=torch.float64).reshape(-1)
@@ -813,8 +951,7 @@ def _vp_inputs(kappa, el_lengths, ggv, ax_max_machines, v_max, ggv_scales, drag_
         raise RuntimeError("ggv has to cover the entire velocity range of the car (i.e. >= v_max)!")
     ggv_t, mach_t = _to_device(ggv_h, dev), _to_device(mach_h, dev)
     common = (int(ggv_t.shape[0]), ggv_t, int(mach_t.shape[0]), mach_t, float(dyn_model_exp), float(drag_coeff), float(m_veh),
-              0 if filt_window is None else int(filt_window),
-              int(VP_DECEL_SLICE_UPPER if decel_slice_upper is None else decel_slice_upper))
+              filt, upper)
     return kappa, el_lengths, SimpleNamespace(B=B, n_max=n_max, dev=dev, mu=mu, n_pts=n_pts, V=V, vmax_t=vmax_t,
                                               scale_t=scale_t, v_scalar=v_scalar, common=common, max_chunk=max_chunk)
 
@@ -850,11 +987,12 @@ def _vel_profile_launch(kappa: torch.Tensor, el_lengths: torch.Tensor, p: Simple
 
 
 @_device_guard
-def vel_profile_batch(kappa: torch.Tensor, el_lengths: torch.Tensor, ggv, ax_max_machines, v_max,
-                      drag_coeff: float, m_veh: float, dyn_model_exp: float = 1.0, filt_window: Optional[int] = None,
-                      mu: Optional[torch.Tensor] = None, n_pts: Optional[torch.Tensor] = None,
-                      ggv_scales=None, want_profiles: bool = True, max_chunk: Optional[int] = None,
-                      decel_slice_upper: Optional[int] = None) -> dict:
+def vel_profile_batch(kappa: torch.Tensor, el_lengths: torch.Tensor, ggv=None, ax_max_machines=None, v_max=None,
+                      drag_coeff: Optional[float] = None, m_veh: Optional[float] = None, dyn_model_exp: float = 1.0,
+                      filt_window: Optional[int] = None, mu: Optional[torch.Tensor] = None,
+                      n_pts: Optional[torch.Tensor] = None, ggv_scales=None, want_profiles: bool = True,
+                      max_chunk: Optional[int] = None, decel_slice_upper: Optional[int] = None,
+                      vehicles: Optional[Vehicles] = None, veh_id=None) -> dict:
     """Batched tph.calc_vel_profile (closed, ggv branch) + calc_ax_profile + calc_t_profile.
 
     kappa, el_lengths: [B, n_max] device tensors (n_pts[b] valid entries), e.g. the ``kappa`` /
@@ -862,10 +1000,17 @@ def vel_profile_batch(kappa: torch.Tensor, el_lengths: torch.Tensor, ggv, ax_max
     ``ggv_scales`` -- a sequence of V per-variant values: variant v of every track runs with
     ggv[:, 1:] * ggv_scales[v] and top speed v_max[v] (one cell of the reference's lap-time matrix,
     main_globaltraj.py:442-496).  Returns dict(laptime [B, V], status [B, V] and, if want_profiles,
-    vx [B, V, n_max], ax [B, V, n_max], t [B, V, n_max + 1])."""
+    vx [B, V, n_max], ax [B, V, n_max], t [B, V, n_max + 1]).
+
+    vehicles: a Vehicles of K vehicles, one per track picked by veh_id [B] (host or device integers; None: K == B, track
+    b drives vehicle b).  ggv, ax_max_machines, drag_coeff and m_veh are then None, and so is v_max unless ggv_scales is
+    given (v_max then gives per-variant top speeds; None: each track's variants run at its vehicle's v_max).  A track's
+    results are bit for bit those of a call with its vehicle alone.  A track whose device veh_id is out of range gets
+    lap time 0 and status 5 (VP_STATUS_BAD_VEHICLE), its neighbours are untouched."""
     _require_cuda()
     kappa, el_lengths, p = _vp_inputs(kappa, el_lengths, ggv, ax_max_machines, v_max, ggv_scales, drag_coeff, m_veh,
-                                      dyn_model_exp, filt_window, n_pts, decel_slice_upper, mu=mu, max_chunk=max_chunk)
+                                      dyn_model_exp, filt_window, n_pts, decel_slice_upper, mu=mu, max_chunk=max_chunk,
+                                      vehicles=vehicles, veh_id=veh_id)
     return _vel_profile_launch(kappa, el_lengths, p, want_profiles)
 
 
@@ -911,10 +1056,12 @@ class _VelProfileDiff(torch.autograd.Function):
 
 
 @_device_guard
-def vel_profile_diff(kappa: torch.Tensor, el_lengths: torch.Tensor, ggv, ax_max_machines, v_max: float, drag_coeff: float,
-                     m_veh: float, dyn_model_exp: float = 1.0, filt_window: Optional[int] = None,
+def vel_profile_diff(kappa: torch.Tensor, el_lengths: torch.Tensor, ggv=None, ax_max_machines=None,
+                     v_max: Optional[float] = None, drag_coeff: Optional[float] = None, m_veh: Optional[float] = None,
+                     dyn_model_exp: float = 1.0, filt_window: Optional[int] = None,
                      n_pts: Optional[torch.Tensor] = None, decel_slice_upper: Optional[int] = None,
-                     strict: bool = True) -> dict:
+                     strict: bool = True, vehicles: Optional[Vehicles] = None, veh_id=None,
+                     max_chunk: Optional[int] = None) -> dict:
     """vel_profile_batch for one profile per track (no ggv scales, one top speed, no mu) with the lap time and the speed
     profile differentiable with respect to kappa and el_lengths (autograd).
 
@@ -926,36 +1073,49 @@ def vel_profile_diff(kappa: torch.Tensor, el_lengths: torch.Tensor, ggv, ax_max_
     frozen.  Chain it to create_raceline_batch's kappa / el_lengths_interp with n_pts=rl["n_out"].
     grad_status: 0 = the gradient is computed; 3 = a non-finite lap time or gradient; for an inactive slot (n_pts < 2)
     the forward's status.  strict=True: backward raises if an instance with a nonzero upstream gradient has
-    grad_status != 0; strict=False: such instances get zero gradients."""
+    grad_status != 0; strict=False: such instances get zero gradients.  vehicles, veh_id: a vehicle per track, as for
+    vel_profile_batch (each track at its vehicle's v_max; grad_status 5 for a refused veh_id).  max_chunk: at most that
+    many tracks per launch (the results do not depend on it)."""
     _require_cuda()
     if isinstance(v_max, torch.Tensor) or hasattr(v_max, "__len__"):
         raise ValueError("vel_profile_diff: v_max must be one number (no per-variant top speeds)")
     kappa, el_lengths, p = _vp_inputs(kappa, el_lengths, ggv, ax_max_machines, v_max, None, drag_coeff, m_veh, dyn_model_exp,
-                                      filt_window, n_pts, decel_slice_upper)
+                                      filt_window, n_pts, decel_slice_upper, max_chunk=max_chunk, vehicles=vehicles,
+                                      veh_id=veh_id)
     p.strict = bool(strict)
     laptime, vx, ax, t, status, grad_status = _VelProfileDiff.apply(kappa, el_lengths, p)
     return dict(laptime=laptime, vx=vx, ax=ax, t=t, status=status, grad_status=grad_status)
 
 
-def _lap_time_variants(ggv_scales, top_speeds):
+def _lap_time_variants(ggv_scales, top_speeds, vehicles=None):
     """(top speed [V], ggv scale [V], T, S): the V = T * S variants of the lap-time matrix in its order, variant
-    v = (top-speed index) * S + (scale index)."""
-    ts = torch.as_tensor(top_speeds, dtype=torch.float64).reshape(-1)
+    v = (top-speed index) * S + (scale index).  With vehicles, top_speeds None stands for each vehicle's v_max (T = 1,
+    top speed None)."""
+    if ggv_scales is None or (top_speeds is None and vehicles is None):
+        raise TypeError("the lap-time matrix needs ggv_scales and top_speeds (top_speeds may be None with vehicles=)")
     gs = torch.as_tensor(ggv_scales, dtype=torch.float64).reshape(-1)
+    if top_speeds is None:
+        return None, gs, 1, gs.numel()
+    ts = torch.as_tensor(top_speeds, dtype=torch.float64).reshape(-1)
     return ts.repeat_interleave(gs.numel()), gs.repeat(ts.numel()), ts.numel(), gs.numel()
 
 
-def lap_time_matrix_batch(kappa: torch.Tensor, el_lengths: torch.Tensor, ggv, ax_max_machines, ggv_scales, top_speeds,
-                          drag_coeff: float, m_veh: float, dyn_model_exp: float = 1.0,
-                          filt_window: Optional[int] = None, n_pts: Optional[torch.Tensor] = None) -> torch.Tensor:
+def lap_time_matrix_batch(kappa: torch.Tensor, el_lengths: torch.Tensor, ggv=None, ax_max_machines=None,
+                          ggv_scales=None, top_speeds=None, drag_coeff: Optional[float] = None, m_veh: Optional[float] = None,
+                          dyn_model_exp: float = 1.0, filt_window: Optional[int] = None,
+                          n_pts: Optional[torch.Tensor] = None, vehicles: Optional[Vehicles] = None,
+                          veh_id=None) -> torch.Tensor:
     """The lap-time matrix of main_globaltraj.py:442-496 for every track of the batch in one launch:
-    returns [B, len(top_speeds), len(ggv_scales)] lap times (top speeds in m/s)."""
-    vm, sc, T, S = _lap_time_variants(ggv_scales, top_speeds)
+    returns [B, len(top_speeds), len(ggv_scales)] lap times (top speeds in m/s).  vehicles, veh_id: a vehicle per track
+    as for vel_profile_batch; cell v then scales the ggv of the track's vehicle, and top_speeds None runs every cell at
+    the vehicle's v_max ([B, 1, len(ggv_scales)])."""
+    vm, sc, T, S = _lap_time_variants(ggv_scales, top_speeds, vehicles)
     res = vel_profile_batch(kappa, el_lengths, ggv, ax_max_machines, vm, drag_coeff, m_veh, dyn_model_exp, filt_window,
-                            n_pts=n_pts, ggv_scales=sc, want_profiles=False)
+                            n_pts=n_pts, ggv_scales=sc, want_profiles=False, vehicles=vehicles, veh_id=veh_id)
     bad_ = res["status"] != 0
     if bool(bad_.any().item()):
-        raise RuntimeError("lap_time_matrix_batch: non-finite lap time for %i profile(s)" % int(bad_.sum().item()))
+        raise RuntimeError("lap_time_matrix_batch: non-finite lap time or refused vehicle for %i profile(s)"
+                           % int(bad_.sum().item()))
     return res["laptime"].reshape(kappa.shape[0], T, S)
 
 
@@ -1002,10 +1162,12 @@ class _LapTimeMatrixDiff(torch.autograd.Function):
 
 
 @_device_guard
-def lap_time_matrix_diff(kappa: torch.Tensor, el_lengths: torch.Tensor, ggv, ax_max_machines, ggv_scales, top_speeds,
-                         drag_coeff: float, m_veh: float, dyn_model_exp: float = 1.0, filt_window: Optional[int] = None,
+def lap_time_matrix_diff(kappa: torch.Tensor, el_lengths: torch.Tensor, ggv=None, ax_max_machines=None,
+                         ggv_scales=None, top_speeds=None, drag_coeff: Optional[float] = None,
+                         m_veh: Optional[float] = None, dyn_model_exp: float = 1.0, filt_window: Optional[int] = None,
                          n_pts: Optional[torch.Tensor] = None, decel_slice_upper: Optional[int] = None,
-                         strict: bool = True) -> dict:
+                         strict: bool = True, vehicles: Optional[Vehicles] = None, veh_id=None,
+                         max_chunk: Optional[int] = None) -> dict:
     """lap_time_matrix_batch with the lap-time matrix differentiable with respect to kappa and el_lengths (autograd).
 
     Returns dict(laptime, status, grad_status), each [B, len(top_speeds), len(ggv_scales)]: laptime holds the values of
@@ -1016,11 +1178,14 @@ def lap_time_matrix_diff(kappa: torch.Tensor, el_lengths: torch.Tensor, ggv, ax_
     tape (17 n_max + 1 doubles per profile; tracks are chunked by free device memory).
     grad_status per cell: 0 = the gradient is computed; 3 = a non-finite lap time or gradient; for an inactive slot
     (n_pts < 2) the forward's status.  strict=True: backward raises if a cell with a nonzero upstream gradient has
-    grad_status != 0; strict=False: such cells add nothing to their track's gradient."""
+    grad_status != 0; strict=False: such cells add nothing to their track's gradient.  vehicles, veh_id: a vehicle per
+    track, as for lap_time_matrix_batch.  max_chunk: at most that many tracks per launch (the results do not depend on
+    it)."""
     _require_cuda()
-    vm, sc, T, S = _lap_time_variants(ggv_scales, top_speeds)
+    vm, sc, T, S = _lap_time_variants(ggv_scales, top_speeds, vehicles)
     kappa, el_lengths, p = _vp_inputs(kappa, el_lengths, ggv, ax_max_machines, vm, sc, drag_coeff, m_veh, dyn_model_exp,
-                                      filt_window, n_pts, decel_slice_upper)
+                                      filt_window, n_pts, decel_slice_upper, max_chunk=max_chunk, vehicles=vehicles,
+                                      veh_id=veh_id)
     p.strict = bool(strict)
     laptime, status, grad_status = _LapTimeMatrixDiff.apply(kappa, el_lengths, p)
     B = p.B

@@ -37,6 +37,7 @@ namespace vp {
 constexpr int VP_UNROLL = 4;             // elements per block of the streaming loops (loads first, then arithmetic)
 constexpr int VP_STATUS_OK = 0;
 constexpr int VP_STATUS_NONFINITE = 3;   // NaN/inf lap time (tph would raise a math domain error or return NaN)
+constexpr int VP_STATUS_BAD_VEHICLE = 5; // vehicle mode: the track's veh_id or its vehicle's rows / mass are invalid
 
 VP_HD double mul(double a, double b) {
 #if defined(__CUDA_ARCH__)
@@ -60,12 +61,38 @@ VP_HD double sub(double a, double b) {
 #endif
 }
 
-struct Tables {
-    const double *gv, *gax, *gay;   // ggv diagram columns v, ax_max, ay_max (n_ggv rows)
+// The ggv and machine tables as the arithmetic reads them: columns C3 of the ggv diagram and C2 of ax_max_machines,
+// each indexed by row.  Tables: contiguous columns (the shared-memory copy of vel_profile_kernel).  VehTables: the
+// columns read in place from the C-ABI's row layout (stride 3 / 2) through the read-only path, one vehicle's rows per
+// thread (the vehicle kernels).  The arithmetic is the same for both: only the loads differ.
+template <class C3, class C2>
+struct TablesT {
+    C3 gv, gax, gay;                // ggv diagram columns v, ax_max, ay_max (n_ggv rows)
     int n_ggv;
-    const double *mv, *ma;          // ax_max_machines columns v, ax_max_machines (n_mach rows)
+    C2 mv, ma;                      // ax_max_machines columns v, ax_max_machines (n_mach rows)
     int n_mach;
 };
+using Tables = TablesT<const double *, const double *>;
+
+// Column of a row-major table of S doubles per row: element k at p[S k].
+template <int S>
+struct RowCol {
+    const double *p;
+    VP_HD double operator[](int k) const {
+#if defined(__CUDA_ARCH__)
+        return __ldg(p + S * k);
+#else
+        return p[S * k];
+#endif
+    }
+};
+using VehTables = TablesT<RowCol<3>, RowCol<2>>;
+
+// The tables of rows [g0, g0 + n_ggv) of ggv [.][3] and [m0, m0 + n_mach) of mach [.][2], read in place.
+VP_HD VehTables row_tables(const double *ggv, int g0, int n_ggv, const double *mach, int m0, int n_mach) {
+    const double *g = ggv + 3 * (size_t)g0, *m = mach + 2 * (size_t)m0;
+    return VehTables{{g}, {g + 1}, {g + 2}, n_ggv, {m}, {m + 1}, n_mach};
+}
 
 struct Params {
     double dyn_model_exp, drag_coeff, m_veh;
@@ -82,7 +109,8 @@ struct Strided {
 // numpy.interp(x, xp, fp * s) for a scalar x (xp increasing): clamped outside the table, exact at the knots.
 // `hint`: segment found by the previous call of the same caller (speeds change slowly along a lap, so the search is
 // skipped almost always); any value in [0, n - 2] is valid, the result does not depend on it.
-VP_HD int find_segment(double x, const double *xp, int n, int &hint) {     // requires xp[0] <= x < xp[n - 1]
+template <class X>
+VP_HD int find_segment(double x, X xp, int n, int &hint) {     // requires xp[0] <= x < xp[n - 1]
     int lo = hint;
     if (xp[lo] <= x && x < xp[lo + 1]) return lo;
     lo = 0;
@@ -95,7 +123,8 @@ VP_HD int find_segment(double x, const double *xp, int n, int &hint) {     // re
     return lo;
 }
 
-VP_HD double interp(double x, const double *xp, const double *fp, int n, double s, int &hint) {
+template <class X, class F>
+VP_HD double interp(double x, X xp, F fp, int n, double s, int &hint) {
     if (x != x) return x;
     if (x >= xp[n - 1]) return mul(fp[n - 1], s);
     if (x < xp[0]) return mul(fp[0], s);
@@ -109,8 +138,8 @@ VP_HD double interp(double x, const double *xp, const double *fp, int n, double 
 
 // Both columns of the ggv diagram at one speed: numpy.interp(x, xp, fa * s), numpy.interp(x, xp, fb * s) with one
 // search of xp (the two interpolations of calc_ax_poss share their abscissa).
-VP_HD void interp2(double x, const double *xp, const double *fa, const double *fb, int n, double s, double &oa,
-                   double &ob, int &hint) {
+template <class X, class F>
+VP_HD void interp2(double x, X xp, F fa, F fb, int n, double s, double &oa, double &ob, int &hint) {
     if (x != x) { oa = x; ob = x; return; }
     if (x >= xp[n - 1]) { oa = mul(fa[n - 1], s); ob = mul(fb[n - 1], s); return; }
     if (x < xp[0]) { oa = mul(fa[0], s); ob = mul(fb[0], s); return; }
@@ -127,7 +156,8 @@ VP_HD void interp2(double x, const double *xp, const double *fa, const double *f
 // accel_forw == true: forward acceleration (machine limit applies, drag opposes);
 // false: "decel_backw", the deceleration pass walked backwards (drag helps).
 struct Hints { int g, m; };   // last segments of the ggv / machine tables
-VP_HD double ax_poss(double vx, double radius, double mu, bool has_mu, bool accel_forw, const Tables &tb, double s,
+template <class Tab>
+VP_HD double ax_poss(double vx, double radius, double mu, bool has_mu, bool accel_forw, const Tab &tb, double s,
                      const Params &pr, Hints &h) {
     double ax_max_tires, ay_max_tires;
     interp2(vx, tb.gv, tb.gax, tb.gay, tb.n_ggv, s, ax_max_tires, ay_max_tires, h.g);
@@ -159,7 +189,8 @@ VP_HD double v_next(double v, double a, double el) { return sqrt(add(mul(v, v), 
 // Tape policy of profile_thread that records nothing (the forward kernel); TapeRecorder below records what the adjoint
 // needs.  The hooks see the values of the forward statements and never change them.
 struct NoTape {
-    VP_HD void initial(int, int, double, double, double, double, const Tables &, double) const {}
+    template <class Tab>
+    VP_HD void initial(int, int, double, double, double, double, const Tab &, double) const {}
     VP_HD void fwd(int, double, int) const {}
     VP_HD void bwd(int, double, int) const {}
 };
@@ -176,10 +207,10 @@ constexpr int VP_BR_CLAMP2 = 64;    // set by the adjoint: the radicand of the c
 // One closed-track profile.  kappa/el/mu: this profile's track rows (contiguous, n entries; mu may be null).
 // R, EL, MU, V, W: scratch vectors of n entries each (MU unused without mu, W unused without filter).
 // vx_out/ax_out [n], t_out [n + 1] may each be null; *laptime always written.  Returns the status code.
-// tp: the tape policy (NoTape: the forward alone).
-template <class Tape = NoTape>
+// tp: the tape policy (NoTape: the forward alone).  tb: Tables or VehTables.
+template <class Tape = NoTape, class Tab = Tables>
 VP_HD int profile_thread(int n, const double *kappa, const double *el, const double *mu, double scale, double v_max,
-                         const Tables &tb, const Params &pr, Strided R, Strided EL, Strided MU, Strided V, Strided W,
+                         const Tab &tb, const Params &pr, Strided R, Strided EL, Strided MU, Strided V, Strided W,
                          double *vx_out, double *ax_out, double *t_out, double *laptime, const Tape &tp = Tape()) {
     const bool has_mu = (mu != nullptr);
     // radii = |1 / kappa| (inf where kappa == 0); private coalesced copies of the track rows.
@@ -386,7 +417,8 @@ VP_HD int profile_thread(int n, const double *kappa, const double *el, const dou
 
 // d/dx of numpy.interp(x, xp, fp * s) on the segment interp takes (the right-hand one at a knot), 0 where interp clamps.
 // *seg: that segment, -1 where clamped.
-VP_HD double interp_slope(double x, const double *xp, const double *fp, int n, double s, int *seg) {
+template <class X, class F>
+VP_HD double interp_slope(double x, X xp, F fp, int n, double s, int *seg) {
     if (!(x >= xp[0]) || x >= xp[n - 1]) {
         *seg = -1;
         return 0.0;
@@ -408,7 +440,8 @@ VP_HD double interp_slope(double x, const double *xp, const double *fp, int n, d
 struct TapeRecorder {
     Strided V0, D, CF, CB, KF, KB, iters;
     bool keep_codes;
-    VP_HD void initial(int it, int i, double r, double vp, double ay, double vn, const Tables &tb, double scale) const {
+    template <class Tab>
+    VP_HD void initial(int it, int i, double r, double vp, double ay, double vn, const Tab &tb, double scale) const {
         V0[i] = vn;
         if (i == 0) iters[0] = it;
         if (!(r < (double)INFINITY)) {           // kappa == 0: V0 = inf is clipped, nothing flows back
@@ -427,7 +460,8 @@ struct TapeRecorder {
 // Partial derivatives of ax_poss (no mu) at (vx, radius): da/dvx, da/dradius.  Returns the frozen decisions of the call
 // as a code: VP_BR_CLAMP, VP_BR_MACH, the ggv segment + 1 in bits 8..15 and (accel_forw) the machine segment + 1 in
 // bits 16..23.
-VP_HD int ax_poss_lin(double vx, double radius, bool accel_forw, const Tables &tb, double s, const Params &pr,
+template <class Tab>
+VP_HD int ax_poss_lin(double vx, double radius, bool accel_forw, const Tab &tb, double s, const Params &pr,
                       double &da_dv, double &da_dr) {
     int hint = 0, seg_g, seg_m = -1;
     double ax_t, ay_t;
@@ -478,7 +512,8 @@ VP_HD int ax_poss_lin(double vx, double radius, bool accel_forw, const Tables &t
 // Upstream: g_lap (d L / d laptime) and g_vx [n] (d L / d vx, may be null).  Writes g_kappa [n] and g_el [n] (either may
 // be null).  GV, GR, GE: scratch vectors of n entries (adjoints of the speeds, the radii and the lengths).
 // Returns the forward's status, or VP_STATUS_NONFINITE for a non-finite gradient; the gradients are zero unless it is 0.
-VP_HD int profile_adjoint_thread(int n, const double *kappa, const double *el, double scale, double v_max, const Tables &tb,
+template <class Tab>
+VP_HD int profile_adjoint_thread(int n, const double *kappa, const double *el, double scale, double v_max, const Tab &tb,
                                  const Params &pr, Strided R, Strided EL, Strided V, Strided W, const TapeRecorder &tp,
                                  Strided GV, Strided GR, Strided GE, double g_lap, const double *g_vx, double *g_kappa,
                                  double *g_el, double *laptime) {

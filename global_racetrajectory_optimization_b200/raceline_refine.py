@@ -322,15 +322,21 @@ class LapTime:
     n_out_max is derived as create_raceline_batch derives it, from the start point (unless it was set before); a trial
     that overflows it is reported in redo and grow() enlarges it to what the kernel asked for.  The ggv and machine
     tables are kept on the host (pinned), so that the checks of vel_profile_batch read no device memory and their copy
-    does not synchronise the stream.  timer(name), a context manager, brackets the launches of each part ('trial',
+    does not synchronise the stream; with a vehicle per track (vp_args holds vehicles= and veh_id=) the batch.Vehicles
+    object, whose tables are on the device already, is passed through, with veh_id checked and put on the device once
+    here.  timer(name), a context manager, brackets the launches of each part ('trial',
     'forward', 'backward'); tools/refine_time.py times them."""
 
     def __init__(self, reftrack, normvec, n_pts, stepsize_interp, vp_args: dict):
         self.reftrack, self.normvec, self.step = reftrack, normvec, float(stepsize_interp)
-        host = lambda t: torch.as_tensor(t, dtype=torch.float64).cpu().contiguous()     # noqa: E731
-        pin = (lambda t: t.pin_memory()) if reftrack.is_cuda else (lambda t: t)          # noqa: E731
-        self.vp = dict(vp_args, ggv=pin(host(vp_args["ggv"])), ax_max_machines=pin(host(vp_args["ax_max_machines"])))
         B, n_max, _ = reftrack.shape
+        if vp_args.get("vehicles") is not None:
+            veh = vp_args["vehicles"]
+            self.vp = dict(vp_args, veh_id=veh.veh_id(vp_args.get("veh_id"), B, reftrack.device))
+        else:
+            host = lambda t: torch.as_tensor(t, dtype=torch.float64).cpu().contiguous()     # noqa: E731
+            pin = (lambda t: t.pin_memory()) if reftrack.is_cuda else (lambda t: t)          # noqa: E731
+            self.vp = dict(vp_args, ggv=pin(host(vp_args["ggv"])), ax_max_machines=pin(host(vp_args["ax_max_machines"])))
         self.n_pts = n_pts if n_pts is not None else torch.full((B,), n_max, dtype=torch.int32, device=reftrack.device)
         self.n_out_max = None
         self._need = None
@@ -522,14 +528,15 @@ class CurvatureProjection:
 
 
 def refine_raceline_batch(reftrack: torch.Tensor, normvec: torch.Tensor, alpha0: torch.Tensor,
-                          w_veh: Union[float, torch.Tensor], ggv, ax_max_machines, v_max: float, drag_coeff: float,
-                          m_veh: float, stepsize_interp: float = 2.0, n_pts: Optional[torch.Tensor] = None,
+                          w_veh: Union[float, torch.Tensor], ggv=None, ax_max_machines=None, v_max: Optional[float] = None,
+                          drag_coeff: Optional[float] = None, m_veh: Optional[float] = None, stepsize_interp: float = 2.0, n_pts: Optional[torch.Tensor] = None,
                           dyn_model_exp: float = 1.0, filt_window: Optional[int] = None, max_iters: int = MAX_ITERS,
                           pg_tol: float = PG_TOL, memory: int = MEMORY, gamma: float = GAMMA, lam_min: float = LAM_MIN,
                           lam_max: float = LAM_MAX, max_halvings: int = MAX_HALVINGS,
                           callback: Optional[Callable] = None, objective: Optional[LapTime] = None,
                           metric_length: Optional[float] = None, kappa_bound: Optional[float] = None,
-                          relinearise: int = 0, curv_error_allowed: float = CURV_ERROR_ALLOWED) -> dict:
+                          relinearise: int = 0, curv_error_allowed: float = CURV_ERROR_ALLOWED,
+                          vehicles: Optional[_b.Vehicles] = None, veh_id=None) -> dict:
     """Lowers the quasi-steady-state lap time of every track's raceline by moving alpha inside opt_min_curv's box.
 
     reftrack [B, n_max, 4], normvec [B, n_max, 2] and alpha0 [B, n_max] (normally the opt_min_curv_batch result) as for
@@ -568,7 +575,12 @@ def refine_raceline_batch(reftrack: torch.Tensor, normvec: torch.Tensor, alpha0:
     curv_error_max (against that round's linearisation) <= curv_error_allowed, or after round relinearise; a track whose
     round-start projection fails keeps the previous round's result with status NO_PROJECTION.  The result then also holds
     rounds [B] int32 (the last round whose result is returned); iters, evals and projection_failures add up over the
-    rounds, laptime_start is that of round 0, and status, pg_norm, kappa_lin_max and curv_error_max are the last round's."""
+    rounds, laptime_start is that of round 0, and status, pg_norm, kappa_lin_max and curv_error_max are the last round's.
+
+    vehicles, veh_id: a vehicle per track (batch.Vehicles; veh_id [B], None for one vehicle per track), each track
+    driven at its vehicle's v_max; ggv, ax_max_machines, v_max, drag_coeff and m_veh are then None.  Tracks are refined
+    independently, so a track's result is that of the track refined alone with its vehicle.  A track whose vehicle the
+    kernels refuse gets no gradient (NO_GRADIENT)."""
     if int(relinearise) != relinearise or relinearise < 0:
         raise ValueError("refine_raceline_batch: relinearise must be an integer >= 0")
     if relinearise and kappa_bound is None:
@@ -588,7 +600,7 @@ def refine_raceline_batch(reftrack: torch.Tensor, normvec: torch.Tensor, alpha0:
     B, n_max, four = reftrack.shape
     if four != 4 or normvec.shape != (B, n_max, 2) or alpha0.shape != (B, n_max):
         raise RuntimeError("refine_raceline_batch: reftrack must be [B, n_max, 4], normvec [B, n_max, 2], alpha0 [B, n_max]")
-    if isinstance(v_max, torch.Tensor) or hasattr(v_max, "__len__"):
+    if vehicles is None and (isinstance(v_max, torch.Tensor) or hasattr(v_max, "__len__")):
         raise ValueError("refine_raceline_batch: v_max must be one number")
     if not float(stepsize_interp) > 0.0:
         raise ValueError("refine_raceline_batch: stepsize_interp must be positive")
@@ -602,8 +614,16 @@ def refine_raceline_batch(reftrack: torch.Tensor, normvec: torch.Tensor, alpha0:
     finite = torch.isfinite(reftrack).all(dim=2) & torch.isfinite(normvec).all(dim=2) & torch.isfinite(alpha0)
     broken = (~finite & valid).any(dim=1)
     active = (n_pts > 0 if n_pts is not None else torch.ones((B,), dtype=torch.bool, device=dev)) & ~empty & ~broken
-    vp = dict(ggv=ggv, ax_max_machines=ax_max_machines, v_max=float(v_max), drag_coeff=float(drag_coeff),
-              m_veh=float(m_veh), dyn_model_exp=float(dyn_model_exp), filt_window=filt_window)
+    if vehicles is not None:
+        if any(x is not None for x in (ggv, ax_max_machines, v_max, drag_coeff, m_veh)):
+            raise ValueError("refine_raceline_batch: with vehicles= the ggv, ax_max_machines, v_max, drag_coeff and m_veh "
+                             "arguments must be None (each vehicle has its own)")
+        vp = dict(vehicles=vehicles, veh_id=veh_id, dyn_model_exp=float(dyn_model_exp), filt_window=filt_window)
+    else:
+        if any(x is None for x in (ggv, ax_max_machines, v_max, drag_coeff, m_veh)):
+            raise TypeError("refine_raceline_batch needs ggv, ax_max_machines, v_max, drag_coeff and m_veh (or vehicles=)")
+        vp = dict(ggv=ggv, ax_max_machines=ax_max_machines, v_max=float(v_max), drag_coeff=float(drag_coeff),
+                  m_veh=float(m_veh), dyn_model_exp=float(dyn_model_exp), filt_window=filt_window)
     fun = objective if objective is not None else LapTime(reftrack, normvec, n_pts, stepsize_interp, vp)
     x0 = torch.minimum(torch.maximum(alpha0, lb), ub)
     if kappa_bound is None:

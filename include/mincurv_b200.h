@@ -369,6 +369,19 @@ int mc_scale_alpha_batch(int B, int n_max, double *alpha, const double *scale_ba
  *   laptime [B*V] (= t[n_pts]), status [B*V] (0 ok, 3 non-finite result) or NULL
  * workspace: mc_vel_profile_workspace_bytes(B, V, n_max)
  */
+#define MC_VP_VEHICLES (-1)
+/* The vehicles of a call with n_ggv = MC_VP_VEHICLES (in host memory; every pointer in it is a device array):
+ * K = n_veh >= 1 vehicles, their tables back to back in ggv [n_ggv][3] (v, ax_max, ay_max) and ax_max_machines
+ * [n_mach][2] (v, ax); veh_rows [K + 1][2] the prefix row offsets (vehicle k has ggv rows veh_rows[k][0] ..
+ * veh_rows[k + 1][0] - 1 and machine rows veh_rows[k][1] .. veh_rows[k + 1][1] - 1, 1 to 256 of each); veh_par [K][3]
+ * its v_max, drag_coeff, m_veh; veh_id [B] the vehicle of each track of the call. */
+typedef struct {
+    int n_veh, n_ggv, n_mach;
+    const double *ggv, *ax_max_machines;
+    const int32_t *veh_rows;
+    const double *veh_par;
+    const int32_t *veh_id;
+} mc_vp_vehicles;
 size_t mc_vel_profile_workspace_bytes(int B, int V, int n_max);
 int mc_vel_profile_batch(int B, int n_max, const int32_t *n_pts, const double *kappa, const double *el_lengths,
                          const double *mu, int V, const double *ggv_scale, const double *v_max_batch, double v_max,
@@ -389,7 +402,17 @@ int mc_vel_profile_batch(int B, int n_max, const int32_t *n_pts, const double *k
  *   mu), and the forward is run again inside: the other arguments are those of the forward call.
  * workspace: mc_vel_profile_workspace_bytes(B, V, n_max) for the forward,
  *            mc_vel_profile_adjoint_workspace_bytes(B * V, n_max) with grad_laptime (the tape of every profile; the
- *            sum over the variants reads it and needs nothing more) */
+ *            sum over the variants reads it and needs nothing more)
+ *
+ * A vehicle per track (here, in mc_vel_profile_batch, which forwards to this entry, and in
+ * mc_vel_profile_adjoint_batch): n_ggv = MC_VP_VEHICLES and ggv = (const double *) a HOST pointer to an mc_vp_vehicles
+ * below, which the entry reads before it returns; n_mach and ax_max_machines are then not read, nor are the scalar
+ * v_max, drag_coeff and m_veh.  A variant's top speed is v_max_batch[v] if given, else its vehicle's v_max;
+ * ggv_scale[v] scales its vehicle's ggv.  A track's results are bit for bit those of a call with its vehicle's tables
+ * and scalars alone.  A track whose veh_id is outside 0 .. n_veh - 1, or whose vehicle has rows outside the tables or
+ * outside 1 .. 256, m_veh <= 0 or (without v_max_batch) v_max <= 0, is refused alone: lap time 0, zero gradients and
+ * status / grad_status 5 (an inactive slot, n_pts 0, stays status 0).  The workspace sizes are those above (the
+ * kernels read the tables in place). */
 int mc_vel_profile_batch_ex(int B, int n_max, const int32_t *n_pts, const double *kappa, const double *el_lengths,
                             const double *mu, int V, const double *ggv_scale, const double *v_max_batch, double v_max,
                             int n_ggv, const double *ggv, int n_mach, const double *ax_max_machines,
@@ -415,7 +438,7 @@ int mc_vel_profile_batch_ex(int B, int n_max, const int32_t *n_pts, const double
  *   grad_kappa      [B][n_max] or NULL = dL / dkappa
  *   grad_el_lengths [B][n_max] or NULL = dL / del_lengths
  * both zero beyond n_pts[b].  The other arguments are those of the forward call; the forward is run again inside (its
- * outputs are not inputs here). */
+ * outputs are not inputs here).  n_ggv = MC_VP_VEHICLES: a vehicle per track, as for mc_vel_profile_batch_ex. */
 size_t mc_vel_profile_adjoint_workspace_bytes(int B, int n_max);
 int mc_vel_profile_adjoint_batch(int B, int n_max, const int32_t *n_pts, const double *kappa, const double *el_lengths,
                                  double v_max, int n_ggv, const double *ggv, int n_mach, const double *ax_max_machines,
