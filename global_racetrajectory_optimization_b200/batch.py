@@ -152,6 +152,22 @@ def _wveh(w_veh, B, dev):
     return float(w_veh), None
 
 
+def _kappa_bound(kappa_bound, B, dev):
+    """(scalar, None) for a number, (0.0, [B] float64 tensor on dev) for a tensor: the kappa_bound / kappa_bound_batch
+    pair of the C-ABI.  A host tensor is checked here; a device tensor is not read (the kernels give an instance whose
+    limit is not finite or not > 0 status -1, its neighbours untouched)."""
+    if not isinstance(kappa_bound, torch.Tensor):
+        return float(kappa_bound), None
+    if kappa_bound.numel() != B:
+        raise ValueError("kappa_bound tensor must have one entry per track")
+    kb = kappa_bound.detach().to(dtype=torch.float64).reshape(B)
+    if kb.device.type == "cpu":
+        if not bool((torch.isfinite(kb) & (kb > 0.0)).all()):
+            raise ValueError("kappa_bound must be a finite curvature > 0 [1/m] for every track")
+        return 0.0, _to_device(kb, dev)
+    return 0.0, kb.to(dev).contiguous()
+
+
 def _chunk(B: int, per_item_bytes: int, device) -> int:
     free, _ = torch.cuda.mem_get_info(device)
     budget = max(int(free * 0.6), per_item_bytes)
@@ -216,8 +232,8 @@ def _mincurv_results(B: int, n_max: int, dev) -> dict:
 
 
 @_device_guard
-def opt_min_curv_batch(reftrack: torch.Tensor, normvec: torch.Tensor, h: torch.Tensor, kappa_bound: float,
-                       w_veh: Union[float, torch.Tensor], n_pts: Optional[torch.Tensor] = None,
+def opt_min_curv_batch(reftrack: torch.Tensor, normvec: torch.Tensor, h: torch.Tensor,
+                       kappa_bound: Union[float, torch.Tensor], w_veh: Union[float, torch.Tensor], n_pts: Optional[torch.Tensor] = None,
                        max_chunk: Optional[int] = None, f_scale: Optional[float] = None,
                        centre_id: Optional[torch.Tensor] = None, lin_alpha: Optional[torch.Tensor] = None) -> dict:
     """Batched tph.opt_min_curv (closed tracks).  Returns a dict of device tensors:
@@ -230,13 +246,19 @@ def opt_min_curv_batch(reftrack: torch.Tensor, normvec: torch.Tensor, h: torch.T
     lin_alpha [B, n_max] (optional): the QP linearised about the line reftrack + lin_alpha * normvec on the same grid
     instead of the centre line (the step of tph's iterative QP without re-sampling; DESIGN.md section 3.2): the curvature
     rows, H and f use that line's first derivatives, and curv_error_max and kappa_lin_max refer to that linearisation.
-    alpha is still the shift from the centre line.  With centre_id a follower is linearised about its owner's row."""
+    alpha is still the shift from the centre line.  With centre_id a follower is linearised about its owner's row.
+    kappa_bound: a float, or a [B] tensor of one curvature limit per instance (e.g. a car per track).  Each instance's
+    results are then bit for bit those of the call with its own limit as the float, with the same chunking; status 4 and
+    the curvature-row phase follow each instance's limit.  A host tensor must hold finite limits > 0; in a device tensor
+    (not read on the host) an instance whose limit is not finite or not > 0 gets status -1 and the others are untouched.
+    With a tensor the solve goes through mc_mincurv_solve_batch_ex, which runs the same stages with kappa_bound_batch."""
     _require_cuda()
     if lin_alpha is not None and (lin_alpha.shape != h.shape):
         raise ValueError(f"opt_min_curv_batch: lin_alpha must be [B, n_max] like h, got {tuple(lin_alpha.shape)}")
     a = _mincurv_inputs(dict(reftrack=(reftrack, 4), normvec=(normvec, 2), h=(h, None)),
                         "Array size of reftrack should be the same as normvectors!", n_pts, w_veh, centre_id, max_chunk, f_scale)
     out = _mincurv_results(a.B, a.n_max, a.dev)
+    kb, kbb = _kappa_bound(kappa_bound, a.B, a.dev)
     if lin_alpha is not None:
         lin = _f64(lin_alpha, "lin_alpha")
         invalid = None
@@ -251,14 +273,31 @@ def opt_min_curv_batch(reftrack: torch.Tensor, normvec: torch.Tensor, h: torch.T
             lin = lin[oc].contiguous()
         ws = _workspace("mincurv", _lib.load().mc_mincurv_workspace_bytes(a.chunk, a.n_max), a.dev)
         _launch_chunks("mc_mincurv_solve_batch_ex", a.B, a.chunk, ws, a.n_max, *map(_rows, (a.n_pts, a.reftrack, a.normvec,
-                       a.h)), float(kappa_bound), a.w_scalar, _rows(a.w_batch), a.f_scale, *map(_rows, out.values()), 0.0,
-                       None, None, _rows(lin))
+                       a.h)), kb, a.w_scalar, _rows(a.w_batch), a.f_scale, *map(_rows, out.values()), 0.0, None, None,
+                       _rows(lin), _rows(kbb), *(None,) * 5)
         if invalid is not None:
             out["status"] = torch.where(invalid, -1, out["status"]).to(torch.int32)
         return out
-    _mincurv_launch("mc_mincurv_solve_batch_shared", a.chunk, a.n_pts, a.reftrack, a.normvec, a.h, float(kappa_bound),
+    if kbb is not None:
+        _mincurv_per_instance(a.chunk, a.n_pts, a.reftrack, a.normvec, a.h, kbb, a.w_scalar, a.w_batch, a.f_scale,
+                              a.centre_id, out.values())
+        return out
+    _mincurv_launch("mc_mincurv_solve_batch_shared", a.chunk, a.n_pts, a.reftrack, a.normvec, a.h, kb,
                     a.w_scalar, a.w_batch, a.f_scale, a.centre_id, *out.values())
     return out
+
+
+def _mincurv_per_instance(chunk: int, n_pts, reftrack, normvec, h, kbb, w_scalar, w_batch, f_scale, centre_id, outputs,
+                          export=(None,) * 4) -> None:
+    """mc_mincurv_solve_batch_shared, or with export (sens, grad_status, sens_rows, n_rows) mc_mincurv_solve_batch_sens,
+    with a curvature limit per instance (kbb [B]), which those entries do not take: mc_mincurv_solve_batch_ex runs the
+    same solve with kappa_bound_batch, centre ids and the export, on chunks of at most chunk instances (centre ids
+    re-indexed inside each chunk).  outputs: alpha, curv_error_max, kappa_lin_max, status, iters."""
+    B, n_max = h.shape
+    ws = _workspace("mincurv", _lib.load().mc_mincurv_workspace_bytes(chunk, n_max), h.device)
+    _launch_chunks("mc_mincurv_solve_batch_ex", B, chunk, ws, n_max, *map(_rows, (n_pts, reftrack, normvec, h)), 0.0,
+                   w_scalar, _rows(w_batch), f_scale, *map(_rows, outputs), 0.0, None, None, None, _rows(kbb),
+                   _chunk_centre_ids(centre_id, B), *map(_rows, export))
 
 
 def shared_centre_ids(group: torch.Tensor) -> torch.Tensor:
@@ -315,7 +354,7 @@ class _MinCurvDiff(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, widths, w_veh_t, centre, normvec, h, kappa_bound, w_scalar, n_pts, centre_id, chunk, f_scale, strict,
-                curvature_rows):
+                curvature_rows, kappa_bound_t):
         B, n_max, _ = centre.shape
         dev = centre.device
         reftrack = torch.cat((centre, widths), dim=2).contiguous()
@@ -324,8 +363,13 @@ class _MinCurvDiff(torch.autograd.Function):
         grad_status = torch.empty((B,), dtype=torch.int32, device=dev)
         sens_rows = torch.empty((B, n_max), dtype=torch.float64, device=dev) if curvature_rows else None
         n_rows = torch.empty((B,), dtype=torch.int32, device=dev) if curvature_rows else None
-        _mincurv_launch("mc_mincurv_solve_batch_sens", chunk, n_pts, reftrack, normvec, h, kappa_bound, w_scalar, w_veh_t,
-                        f_scale, centre_id, alpha, cerr, kmax, status, iters, sens, grad_status, sens_rows, n_rows)
+        if kappa_bound_t is None:
+            _mincurv_launch("mc_mincurv_solve_batch_sens", chunk, n_pts, reftrack, normvec, h, kappa_bound, w_scalar,
+                            w_veh_t, f_scale, centre_id, alpha, cerr, kmax, status, iters, sens, grad_status, sens_rows,
+                            n_rows)
+        else:
+            _mincurv_per_instance(chunk, n_pts, reftrack, normvec, h, kappa_bound_t, w_scalar, w_veh_t, f_scale, centre_id,
+                                  (alpha, cerr, kmax, status, iters), (sens, grad_status, sens_rows, n_rows))
         ctx.save_for_backward(widths, centre, normvec, h, w_veh_t, n_pts, centre_id, sens, grad_status, sens_rows, n_rows)
         ctx.w_scalar, ctx.chunk, ctx.f_scale, ctx.strict = w_scalar, chunk, f_scale, strict
         ctx.mark_non_differentiable(cerr, kmax, status, iters, grad_status)
@@ -357,12 +401,12 @@ class _MinCurvDiff(torch.autograd.Function):
         _mincurv_launch("mc_mincurv_adjoint_batch", chunk, n_pts, reftrack, normvec, h, None, ctx.w_scalar, w_veh_t,
                         ctx.f_scale, centre_id, sens, gs, grad_alpha, gwr, gwl, gwv, *rows, None)
         _refuse(ctx.strict, wanted, gs, who, "whose adjoint factorisation broke down")
-        return (torch.stack((gwr, gwl), dim=2), gwv if w_veh_t is not None else None) + (None,) * 11
+        return (torch.stack((gwr, gwl), dim=2), gwv if w_veh_t is not None else None) + (None,) * 12
 
 
 @_device_guard
-def opt_min_curv_diff(centre: torch.Tensor, widths: torch.Tensor, normvec: torch.Tensor, h: torch.Tensor, kappa_bound: float,
-                      w_veh: Union[float, torch.Tensor], n_pts: Optional[torch.Tensor] = None,
+def opt_min_curv_diff(centre: torch.Tensor, widths: torch.Tensor, normvec: torch.Tensor, h: torch.Tensor,
+                      kappa_bound: Union[float, torch.Tensor], w_veh: Union[float, torch.Tensor], n_pts: Optional[torch.Tensor] = None,
                       centre_id: Optional[torch.Tensor] = None, max_chunk: Optional[int] = None,
                       f_scale: Optional[float] = None, strict: bool = True, curvature_rows: bool = False) -> dict:
     """opt_min_curv_batch with alpha differentiable with respect to the track widths and the vehicle width (autograd).
@@ -381,7 +425,8 @@ def opt_min_curv_diff(centre: torch.Tensor, widths: torch.Tensor, normvec: torch
     iterate (DESIGN.md section 3.10, curvature rows): the forward exports 8 more bytes per point, grad_status is the final
     solve status (4 only where the rows stay violated), and the backward reads the largest count of strongly active rows
     once from the device to size their Schur complements.  The forward's values are those of curvature_rows=False bit
-    for bit, and so are the gradients of the instances the box phase solved."""
+    for bit, and so are the gradients of the instances the box phase solved.
+    kappa_bound: a float or a [B] tensor, as for opt_min_curv_batch (a constant: not differentiated)."""
     _require_cuda()
     for t, name in ((centre, "centre"), (normvec, "normvec"), (h, "h")):
         if isinstance(t, torch.Tensor) and t.requires_grad:
@@ -389,9 +434,10 @@ def opt_min_curv_diff(centre: torch.Tensor, widths: torch.Tensor, normvec: torch
     a = _mincurv_inputs(dict(centre=(centre, 2), widths=(widths, 2), normvec=(normvec, 2), h=(h, None)),
                         "opt_min_curv_diff: centre and widths must be [B, n_max, 2], normvec [B, n_max, 2], h [B, n_max]",
                         n_pts, w_veh, centre_id, max_chunk, f_scale)
+    kb, kbb = _kappa_bound(kappa_bound, a.B, a.dev)
     alpha, cerr, kmax, status, iters, grad_status = _MinCurvDiff.apply(
-        a.widths, a.w_batch, a.centre, a.normvec, a.h, float(kappa_bound), a.w_scalar, a.n_pts, a.centre_id, a.chunk,
-        a.f_scale, bool(strict), bool(curvature_rows))
+        a.widths, a.w_batch, a.centre, a.normvec, a.h, kb, a.w_scalar, a.n_pts, a.centre_id, a.chunk,
+        a.f_scale, bool(strict), bool(curvature_rows), kbb)
     return dict(alpha=alpha, curv_error_max=cerr, kappa_lin_max=kmax, status=status, iters=iters, grad_status=grad_status)
 
 
@@ -652,7 +698,7 @@ def scale_alpha_batch(alpha: torch.Tensor, scale: Union[float, torch.Tensor]) ->
 
 
 @_device_guard
-def iqp_batch(reftrack: torch.Tensor, normvec: torch.Tensor, h: torch.Tensor, kappa_bound: float,
+def iqp_batch(reftrack: torch.Tensor, normvec: torch.Tensor, h: torch.Tensor, kappa_bound: Union[float, torch.Tensor],
               w_veh: Union[float, torch.Tensor], stepsize_interp: float, iters_min: int = 3,
               curv_error_allowed: float = 0.01, n_pts: Optional[torch.Tensor] = None, max_iters: int = 50,
               fixed_iters: Optional[int] = None, _n_cap_min: int = 0) -> dict:
@@ -666,7 +712,10 @@ def iqp_batch(reftrack: torch.Tensor, normvec: torch.Tensor, h: torch.Tensor, ka
     fixed_iters: run exactly that many outer iterations for every instance (bench config C3).  Nothing has to be decided
     on the host between the iterations then, so they are queued back to back and the one thing the host would have
     looked at -- a re-sampled track that does not fit the capacity -- is checked once at the end (and the call repeated
-    with the larger capacity, which the 5 % + 50 m of slack makes a rare event)."""
+    with the larger capacity, which the 5 % + 50 m of slack makes a rare event).
+
+    kappa_bound: a float or a [B] tensor of one limit per instance, as for opt_min_curv_batch (every QP of an instance
+    takes its own limit)."""
     _require_cuda()
     reftrack0, normvec0, h0 = reftrack, normvec, h           # (the caller's arrays: never written)
     reftrack = _f64(reftrack, "reftrack").clone()
@@ -674,6 +723,8 @@ def iqp_batch(reftrack: torch.Tensor, normvec: torch.Tensor, h: torch.Tensor, ka
     h = _f64(h, "h").clone()
     B, n_max, _ = reftrack.shape
     dev = reftrack.device
+    if isinstance(kappa_bound, torch.Tensor):           # (checked and put on the device once, not per outer iteration)
+        kappa_bound = _kappa_bound(kappa_bound, B, dev)[1]
     cur_n = (n_pts.to(device=dev, dtype=torch.int32).clone() if n_pts is not None
              else torch.full((B,), n_max, dtype=torch.int32, device=dev))
     # capacity of the re-sampled tracks: the raceline is re-sampled every stepsize_interp metres, so its point count
@@ -781,9 +832,18 @@ class Vehicles:
     run here, once, per vehicle (each table must cover that vehicle's v_max; a call with per-variant top speeds checks
     those against every vehicle's tables on the host).  The tables are packed back to back and copied to device once,
     through pinned memory: a reused object costs no copy and no stream synchronisation per call.  device: where the
-    tracks will be (default: the current CUDA device)."""
+    tracks will be (default: the current CUDA device).
 
-    def __init__(self, ggv, ax_max_machines, v_max, drag_coeff, m_veh, device=None):
+    curvlim, width_opt, length, width (optional, keyword): the rest of racecar.ini's veh_params / optim_opts per vehicle,
+    K-sequences as above, for globaltraj.globaltraj_batch(vehicles=) and check_traj_flags(vehicles=): the curvature
+    limit of the minimum-curvature QPs [1/m], the vehicle width the QPs plan with [m], and the vehicle size check_traj
+    tests [m].  None (the default) leaves a field unset; the attribute is then None.  per_track() gathers a field by
+    veh_id on the device; the table maxima check_traj compares with are kept on the host at construction."""
+
+    FIELDS = ("curvlim", "width_opt", "length", "width")
+
+    def __init__(self, ggv, ax_max_machines, v_max, drag_coeff, m_veh, device=None, *, curvlim=None, width_opt=None,
+                 length=None, width=None):
         if isinstance(ggv, torch.Tensor) or isinstance(ax_max_machines, torch.Tensor):
             raise TypeError("Vehicles: ggv and ax_max_machines are sequences of one table per vehicle")
         ggv, mach = list(ggv), list(ax_max_machines)
@@ -801,10 +861,22 @@ class Vehicles:
                 raise ValueError(f"Vehicles: v_max[{k}] must be a finite speed > 0")
             if not (math.isfinite(mass[k]) and mass[k] > 0.0):
                 raise ValueError(f"Vehicles: m_veh[{k}] must be > 0")
+        extra = {}
+        for name, x in zip(self.FIELDS, (curvlim, width_opt, length, width)):
+            if x is not None:
+                extra[name] = self._per_vehicle(x, K, name)
+                if not all(math.isfinite(v) and v > 0.0 for v in extra[name]):
+                    raise ValueError(f"Vehicles: every {name} must be finite and > 0")
         self.n_veh = K
         self.v_max, self.drag_coeff, self.m_veh = vm, drag, mass
+        self.curvlim, self.width_opt, self.length, self.width = (extra.get(name) for name in self.FIELDS)
         self._ggv_top = [float(g[-1, 0]) for g in ggv]
         self._mach_top = [float(m[-1, 0]) for m in mach]
+        # the maxima check_traj compares with (check_traj.py:74-139), per vehicle, on the host
+        self._limits = {"v_max": vm,
+                        "ay": [float(g[:, 2].max()) for g in ggv], "ax_pos": [float(g[:, 1].max()) for g in ggv],
+                        "ax_neg": [float((-g[:, 1]).min()) for g in ggv], "a_tot": [float(g[:, 1:].max()) for g in ggv],
+                        "ax_machines": [float(m[:, 1].max()) for m in mach]}
         for k in range(K):
             self.check_covers(vm[k], k)
         rows = torch.zeros((K + 1, 2), dtype=torch.int32)
@@ -815,6 +887,14 @@ class Vehicles:
         self.ggv, self.ax_max_machines = _to_device(torch.cat(ggv), dev), _to_device(torch.cat(mach), dev)
         self.rows, self.par = _to_device(rows, dev), _to_device(par, dev)
         self.device = self.ggv.device
+        # the per-vehicle numbers per_track() gathers, one column each, and a row of NaN for an id out of range
+        self._cols = {"v_max": 0, "drag_coeff": 1, "m_veh": 2}
+        cols = [vm, drag, mass]
+        for name, vals in list(extra.items()) + list(self._limits.items())[1:]:
+            self._cols[name] = len(cols)
+            cols.append(vals)
+        table = torch.tensor(cols, dtype=torch.float64).T
+        self._table = _to_device(torch.cat((table, torch.full((1, len(cols)), math.nan, dtype=torch.float64))), dev)
 
     @staticmethod
     def _per_vehicle(x, K, name):
@@ -834,6 +914,20 @@ class Vehicles:
                 raise RuntimeError("ax_max_machines has to cover the entire velocity range of the car (i.e. >= v_max)!")
             if self._ggv_top[j] < v_top:
                 raise RuntimeError("ggv has to cover the entire velocity range of the car (i.e. >= v_max)!")
+
+    def per_track(self, name: str, veh_id: torch.Tensor) -> torch.Tensor:
+        """[B] float64 device tensor of the field name ('v_max', 'drag_coeff', 'm_veh', a set one of FIELDS, or a table
+        maximum of check_traj_flags) for each track's vehicle; veh_id: the [B] device tensor veh_id() returns.  Gathered
+        on the device without a read.  A track whose id is out of range gets NaN.  What that does depends on the field:
+        a NaN curvlim or width_opt refuses the track's minimum-curvature QP (status -1), a NaN width_opt ends its
+        shortest-path QP with status 3, a NaN mass refuses its check_traj extrema (NaN row), and the velocity profile
+        refuses the id itself (status 5); a NaN length or width gives that track NaN distances.  The other tracks are
+        untouched."""
+        if name not in self._cols:
+            raise ValueError(f"Vehicles: {name} is not set" if name in self.FIELDS else f"Vehicles: no field {name}")
+        ids = veh_id.long()
+        ids = torch.where((ids >= 0) & (ids < self.n_veh), ids, self.n_veh)
+        return self._table[ids, self._cols[name]].contiguous()
 
     def veh_id(self, veh_id, B: int, dev) -> torch.Tensor:
         """veh_id as the [B] int32 device tensor the C-ABI takes.  None: one vehicle per track (K == B).  A host veh_id
@@ -1251,12 +1345,24 @@ def interp_track_batch(pts: torch.Tensor, stepsize_approx: float = 1.0, n_pts: O
         n_out_max = need + 8
 
 
+def _per_track(x, B: int, dev, name: str):
+    """(scalar, None) for a number, (0.0, [B] float64 tensor on dev) for a tensor: a scalar / per-track array pair of
+    the C-ABI (a host tensor goes through pinned memory)."""
+    if not isinstance(x, torch.Tensor):
+        return float(x), None
+    if x.numel() != B:
+        raise ValueError(f"{name} tensor must have one entry per track")
+    return 0.0, _to_device(x.detach().to(dtype=torch.float64).reshape(B), dev)
+
+
 @_device_guard
 def min_bound_dists_batch(xy: torch.Tensor, psi: torch.Tensor, bound1: torch.Tensor, bound2: torch.Tensor,
-                          length_veh: float, width_veh: float, n_traj: Optional[torch.Tensor] = None,
-                          nb1: Optional[torch.Tensor] = None, nb2: Optional[torch.Tensor] = None) -> torch.Tensor:
+                          length_veh: Union[float, torch.Tensor], width_veh: Union[float, torch.Tensor],
+                          n_traj: Optional[torch.Tensor] = None, nb1: Optional[torch.Tensor] = None,
+                          nb2: Optional[torch.Tensor] = None) -> torch.Tensor:
     """Batched helper_funcs_glob.src.calc_min_bound_dists.calc_min_bound_dists: [B, n_traj_max] minimum distances of
-    the vehicle corners to the boundary points (bound1/bound2: [B, nb_max, >= 2], x and y first)."""
+    the vehicle corners to the boundary points (bound1/bound2: [B, nb_max, >= 2], x and y first).  length_veh and
+    width_veh: floats or [B] tensors (a vehicle size per trajectory)."""
     _require_cuda()
     xy, psi, bound1, bound2 = _f64(xy, "xy"), _f64(psi, "psi"), _f64(bound1, "bound1"), _f64(bound2, "bound2")
     B, n_traj_max, _ = xy.shape
@@ -1265,8 +1371,9 @@ def min_bound_dists_batch(xy: torch.Tensor, psi: torch.Tensor, bound1: torch.Ten
     dev = xy.device
     out = torch.zeros((B, n_traj_max), dtype=torch.float64, device=dev)
     n_traj, nb1, nb2 = _npts(n_traj, B, dev), _npts(nb1, B, dev), _npts(nb2, B, dev)
+    (length, length_t), (width, width_t) = _per_track(length_veh, B, dev, "length_veh"), _per_track(width_veh, B, dev, "width_veh")
     _call("mc_min_bound_dists_batch", B, n_traj_max, n_traj, xy, psi, int(bound1.shape[1]), nb1, bound1, int(bound2.shape[1]),
-          nb2, bound2, int(bound1.shape[2]), float(length_veh), float(width_veh), out)
+          nb2, bound2, int(bound1.shape[2]), length, width, out, length_t, width_t)
     return out
 
 
@@ -1274,9 +1381,12 @@ EXTREMA = ("min_dist", "kappa_abs_max", "ay_max", "ax_wo_drag_max", "ax_wo_drag_
 
 
 @_device_guard
-def traj_extrema_batch(kappa: torch.Tensor, vx: torch.Tensor, ax: torch.Tensor, dragcoeff: float, mass_veh: float,
-                       min_dists: Optional[torch.Tensor] = None, n_traj: Optional[torch.Tensor] = None) -> torch.Tensor:
-    """[B, 8] extrema per trajectory, columns as in EXTREMA (min_dist = inf without min_dists)."""
+def traj_extrema_batch(kappa: torch.Tensor, vx: torch.Tensor, ax: torch.Tensor, dragcoeff: Union[float, torch.Tensor],
+                       mass_veh: Union[float, torch.Tensor], min_dists: Optional[torch.Tensor] = None,
+                       n_traj: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """[B, 8] extrema per trajectory, columns as in EXTREMA (min_dist = inf without min_dists).  dragcoeff and mass_veh:
+    floats or [B] tensors (per trajectory).  A host mass tensor must be > 0; a trajectory whose mass in a device tensor
+    is not > 0 gets a row of NaN but for n_points."""
     _require_cuda()
     kappa, vx, ax = _f64(kappa, "kappa"), _f64(vx, "vx"), _f64(ax, "ax")
     B, n_max = kappa.shape
@@ -1284,22 +1394,26 @@ def traj_extrema_batch(kappa: torch.Tensor, vx: torch.Tensor, ax: torch.Tensor, 
     if min_dists is not None:
         min_dists = _f64(min_dists, "min_dists")
     ext = torch.zeros((B, 8), dtype=torch.float64, device=dev)
-    _call("mc_traj_extrema_batch", B, n_max, _npts(n_traj, B, dev), kappa, vx, ax, min_dists, float(dragcoeff), float(mass_veh),
-          ext)
+    if isinstance(mass_veh, torch.Tensor) and mass_veh.device.type == "cpu" and not bool((mass_veh > 0.0).all()):
+        raise ValueError("mass_veh must be > 0 for every trajectory")
+    (drag, drag_t), (mass, mass_t) = _per_track(dragcoeff, B, dev, "dragcoeff"), _per_track(mass_veh, B, dev, "mass_veh")
+    _call("mc_traj_extrema_batch", B, n_max, _npts(n_traj, B, dev), kappa, vx, ax, min_dists, drag, mass, ext, drag_t, mass_t)
     return ext
 
 
 @_device_guard
 def check_traj_batch(reftrack: torch.Tensor, normvec: torch.Tensor, xy: torch.Tensor, psi: torch.Tensor,
-                     kappa: torch.Tensor, vx: torch.Tensor, ax: torch.Tensor, length_veh: float, width_veh: float,
-                     dragcoeff: float, mass_veh: float, n_pts: Optional[torch.Tensor] = None,
+                     kappa: torch.Tensor, vx: torch.Tensor, ax: torch.Tensor, length_veh: Union[float, torch.Tensor],
+                     width_veh: Union[float, torch.Tensor], dragcoeff: Union[float, torch.Tensor],
+                     mass_veh: Union[float, torch.Tensor], n_pts: Optional[torch.Tensor] = None,
                      n_traj: Optional[torch.Tensor] = None, bound_stepsize: float = 1.0) -> dict:
     """The quantities helper_funcs_glob.src.check_traj.check_traj tests, for a batch of trajectories: boundaries
     re-sampled every ``bound_stepsize`` metres, minimum distance of the vehicle corners to them for every trajectory
     point (against ALL boundary points -- the reference passes only the first point of each boundary, check_traj.py:58-61,
     which the single-track mirror reproduces), and the extrema of curvature, accelerations and speed.
     Returns dict(min_dists [B, n_traj_max], bound_r/bound_l [B, nb, 4] with nb_r/nb_l [B], and one [B] tensor per name
-    in EXTREMA)."""
+    in EXTREMA).  length_veh, width_veh, dragcoeff and mass_veh: floats or [B] tensors (a vehicle per trajectory), as for
+    min_bound_dists_batch and traj_extrema_batch."""
     _require_cuda()
     kappa = _f64(kappa, "kappa")
     B = kappa.shape[0]
@@ -1313,8 +1427,28 @@ def check_traj_batch(reftrack: torch.Tensor, normvec: torch.Tensor, xy: torch.Te
     return out
 
 
-def check_traj_flags(chk: dict, ggv, ax_max_machines, v_max: float, curvlim: float, min_dist_warn: float = 1.0) -> dict:
-    """The comparisons of check_traj.py:74-139 as boolean [B] tensors (True = the reference would print the warning)."""
+def check_traj_flags(chk: dict, ggv=None, ax_max_machines=None, v_max=None, curvlim=None, min_dist_warn: float = 1.0,
+                     vehicles: Optional[Vehicles] = None, veh_id=None) -> dict:
+    """The comparisons of check_traj.py:74-139 as boolean [B] tensors (True = the reference would print the warning).
+
+    vehicles, veh_id: each track against its own vehicle (batch.Vehicles; veh_id as for vel_profile_batch): its v_max, its
+    curvlim (if the object sets one; else the curvlim argument, a float or [B] tensor) and the maxima of its tables, which
+    Vehicles keeps from construction, so no device memory is read.  ggv, ax_max_machines and v_max are then None.  A
+    track whose device veh_id is out of range gets NaN limits (no flag)."""
+    if vehicles is not None:
+        if any(x is not None for x in (ggv, ax_max_machines, v_max)):
+            raise ValueError("check_traj_flags: with vehicles= the ggv, ax_max_machines and v_max arguments must be None")
+        kappa = chk["kappa_abs_max"]
+        ids = vehicles.veh_id(veh_id, kappa.shape[0], kappa.device)
+        lim = lambda name: vehicles.per_track(name, ids)            # noqa: E731
+        if vehicles.curvlim is not None:
+            curvlim = lim("curvlim")
+        elif curvlim is None:
+            raise TypeError("check_traj_flags needs curvlim (the vehicles set none)")
+        return dict(min_dist=chk["min_dist"] < min_dist_warn, curvature=kappa > curvlim, v_max=chk["vx_max"] > lim("v_max") + 0.1,
+                    ay=chk["ay_max"] > lim("ay") + 0.1, ax_pos=chk["ax_wo_drag_max"] > lim("ax_pos") + 0.1,
+                    ax_neg=chk["ax_wo_drag_min"] < lim("ax_neg") - 0.1, a_tot=chk["a_tot_max"] > lim("a_tot") + 0.1,
+                    ax_machines=chk["ax_wo_drag_max"] > lim("ax_machines") + 0.1)
     import numpy as _np
     f = dict(min_dist=chk["min_dist"] < min_dist_warn, curvature=chk["kappa_abs_max"] > curvlim,
              v_max=chk["vx_max"] > v_max + 0.1)

@@ -5,21 +5,31 @@
 // LIN: the workspace was assembled about a linearisation point (mincurv_setup.cu): V_XP / V_YP hold its first
 // derivatives, which the linearised curvature uses, while the line P + alpha n takes those of the centre line, recomputed
 // here from its points and moments.
+// KBB: the curvature limit of each instance is kappa_bound_batch[b] (the scalar kappa_bound is not read).  An instance whose
+// limit is not finite or not > 0 is refused with status -1 (in the first pass: afterwards its status is negative).  The
+// array is the last parameter, so that the scalar instantiations keep their parameter offsets.
 #include "capi.cuh"
 #include "mincurv_ops.cuh"
 
 namespace mc {
 
-template <bool LIN>
+template <bool LIN, bool KBB>
 __global__ void __launch_bounds__(256)
 mincurv_finalize_kernel(int n_max, const int32_t *__restrict__ n_pts, double *__restrict__ ws, Layout L,
                         const double *__restrict__ alpha, double kappa_bound,
                         double *__restrict__ curv_error_max, double *__restrict__ kappa_lin_max,
-                        int32_t *__restrict__ status) {
+                        int32_t *__restrict__ status, const double *__restrict__ kappa_bound_batch) {
     const int b = blockIdx.x;
     const int n = n_pts ? n_pts[b] : n_max;
     __shared__ double red[32];
-    const int st = status[b];
+    int st = status[b];
+    if constexpr (KBB) {
+        kappa_bound = kappa_bound_batch[b];
+        if (st >= 0 && !(kappa_bound > 0.0 && kappa_bound < INFINITY)) {
+            if (threadIdx.x == 0) status[b] = -1;
+            st = -1;
+        }
+    }
     if (st == 1 || st < 0) {
         if (threadIdx.x == 0) {
             curv_error_max[b] = 0.0;
@@ -153,13 +163,15 @@ mincurv_prox_kernel(int n_max, const int32_t *__restrict__ n_pts, double *__rest
 }
 
 int mincurv_finalize(int B, int n_max, const int32_t *n_pts, const double *alpha, double kappa_bound, double *curv_error_max,
-                     double *kappa_lin_max, int32_t *status, bool lin, void *workspace, size_t workspace_bytes, void *stream) {
+                     double *kappa_lin_max, int32_t *status, bool lin, const double *kappa_bound_batch, void *workspace,
+                     size_t workspace_bytes, void *stream) {
     if (!alpha || !curv_error_max || !status) return bad("mc_mincurv_finalize_batch: NULL argument");
     int rc = mincurv_args("mc_mincurv_finalize_batch", B, n_max, workspace, workspace_bytes);
     if (rc) return rc;
-    auto kernel = lin ? mincurv_finalize_kernel<true> : mincurv_finalize_kernel<false>;
+    auto kernel = kappa_bound_batch ? (lin ? mincurv_finalize_kernel<true, true> : mincurv_finalize_kernel<false, true>)
+                                    : (lin ? mincurv_finalize_kernel<true, false> : mincurv_finalize_kernel<false, false>);
     kernel<<<B, 256, 0, (cudaStream_t)stream>>>(n_max, n_pts, (double *)workspace, make_layout(n_max), alpha, kappa_bound,
-                                                curv_error_max, kappa_lin_max, status);
+                                                curv_error_max, kappa_lin_max, status, kappa_bound_batch);
     return check_cuda("mincurv_finalize_kernel");
 }
 
@@ -168,10 +180,10 @@ int mincurv_finalize(int B, int n_max, const int32_t *n_pts, const double *alpha
 extern "C" {
 
 int mc_mincurv_finalize_batch(int B, int n_max, const int32_t *n_pts, const double *alpha, double kappa_bound,
-                              double *curv_error_max, double *kappa_lin_max, int32_t *status, int linearised, void *workspace,
-                              size_t workspace_bytes, void *stream) {
+                              double *curv_error_max, double *kappa_lin_max, int32_t *status, int linearised,
+                              const double *kappa_bound_batch, void *workspace, size_t workspace_bytes, void *stream) {
     return mc::mincurv_finalize(B, n_max, n_pts, alpha, kappa_bound, curv_error_max, kappa_lin_max, status, linearised != 0,
-                                workspace, workspace_bytes, stream);
+                                kappa_bound_batch, workspace, workspace_bytes, stream);
 }
 
 int mc_mincurv_solve_batch(int B, int n_max, const int32_t *n_pts, const double *reftrack, const double *normvec,
@@ -180,7 +192,7 @@ int mc_mincurv_solve_batch(int B, int n_max, const int32_t *n_pts, const double 
                            void *workspace, size_t workspace_bytes, void *stream) {
     return mc_mincurv_solve_batch_ex(B, n_max, n_pts, reftrack, normvec, h, kappa_bound, w_veh, w_veh_batch, MC_F_SCALE_DEFAULT,
                                      alpha, curv_error_max, kappa_lin_max, status, iters, 0.0, nullptr, nullptr, nullptr,
-                                     workspace, workspace_bytes, stream);
+                                     nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, workspace, workspace_bytes, stream);
 }
 
 // the projection QP: setup -> prox -> pdip -> finalize -> kappa (with prox_mu) -> finalize
@@ -188,7 +200,7 @@ static int mincurv_prox_solve(int B, int n_max, const int32_t *n_pts, const doub
                               const double *h, double kappa_bound, double w_veh, const double *w_veh_batch, double f_scale,
                               double *alpha, double *curv_error_max, double *kappa_lin_max, int32_t *status, int32_t *iters,
                               double prox_mu, const double *prox_x, const double *prox_q, const double *lin_alpha,
-                              void *workspace, size_t workspace_bytes, void *stream) {
+                              const double *kbb, void *workspace, size_t workspace_bytes, void *stream) {
     if (!reftrack || !normvec || !h || !alpha || !curv_error_max || !status || !prox_q)
         return bad("mc_mincurv_solve_batch_ex: NULL argument");
     if (!(prox_mu > 0.0) || !(prox_mu < INFINITY)) return bad("mc_mincurv_solve_batch_ex: prox_mu must be finite and positive");
@@ -202,13 +214,14 @@ static int mincurv_prox_solve(int B, int n_max, const int32_t *n_pts, const doub
     if (rc) return rc;
     rc = mc_mincurv_pdip_batch(B, n_max, n_pts, alpha, status, iters, workspace, workspace_bytes, stream);
     if (rc) return rc;
-    rc = mc::mincurv_finalize(B, n_max, n_pts, alpha, kappa_bound, curv_error_max, kappa_lin_max, status, lin, workspace,
-                              workspace_bytes, stream);
+    rc = mc::mincurv_finalize(B, n_max, n_pts, alpha, kappa_bound, curv_error_max, kappa_lin_max, status, lin, kbb,
+                              workspace, workspace_bytes, stream);
     if (rc) return rc;
-    rc = mc::mincurv_kappa_phase(B, n_max, n_pts, kappa_bound, prox_mu, alpha, status, iters, workspace, workspace_bytes, stream);
+    rc = mc::mincurv_kappa_phase(B, n_max, n_pts, kappa_bound, kbb, prox_mu, alpha, status, iters, workspace, workspace_bytes,
+                                 stream);
     if (rc) return rc;
-    return mc::mincurv_finalize(B, n_max, n_pts, alpha, kappa_bound, curv_error_max, kappa_lin_max, status, lin, workspace,
-                                workspace_bytes, stream);
+    return mc::mincurv_finalize(B, n_max, n_pts, alpha, kappa_bound, curv_error_max, kappa_lin_max, status, lin, kbb,
+                                workspace, workspace_bytes, stream);
 }
 
 // setup -> pdip -> finalize -> (export of the sensitivity data) -> kappa -> finalize -> (export of the curvature-row phase's
@@ -218,7 +231,7 @@ static int mincurv_solve(int B, int n_max, const int32_t *n_pts, const double *r
                          double kappa_bound, double w_veh, const double *w_veh_batch, double f_scale, const int32_t *centre_id,
                          double *alpha, double *curv_error_max, double *kappa_lin_max, int32_t *status, int32_t *iters,
                          double *sens, int32_t *grad_status, double *sens_rows, int32_t *n_rows, const double *lin_alpha,
-                         void *workspace, size_t workspace_bytes, void *stream) {
+                         const double *kbb, void *workspace, size_t workspace_bytes, void *stream) {
     if (!reftrack || !normvec || !h || !alpha || !curv_error_max || !status)
         return bad("mc_mincurv_solve_batch: NULL argument");
     const bool lin = lin_alpha != nullptr;
@@ -227,8 +240,8 @@ static int mincurv_solve(int B, int n_max, const int32_t *n_pts, const double *r
     if (rc) return rc;
     rc = mc_mincurv_pdip_batch(B, n_max, n_pts, alpha, status, iters, workspace, workspace_bytes, stream);
     if (rc) return rc;
-    rc = mc::mincurv_finalize(B, n_max, n_pts, alpha, kappa_bound, curv_error_max, kappa_lin_max, status, lin, workspace,
-                              workspace_bytes, stream);
+    rc = mc::mincurv_finalize(B, n_max, n_pts, alpha, kappa_bound, curv_error_max, kappa_lin_max, status, lin, kbb,
+                              workspace, workspace_bytes, stream);
     if (rc) return rc;
     if (sens) {
         // the box phase's final iterate, before the curvature-row phase takes over the status-4 slabs
@@ -238,10 +251,10 @@ static int mincurv_solve(int B, int n_max, const int32_t *n_pts, const double *r
         if (rc) return rc;
     }
     // instances whose box-only optimum violates the curvature rows (status 4) are re-solved with the rows
-    rc = mc_mincurv_kappa_batch(B, n_max, n_pts, kappa_bound, alpha, status, iters, workspace, workspace_bytes, stream);
+    rc = mc_mincurv_kappa_batch(B, n_max, n_pts, kappa_bound, alpha, status, iters, kbb, workspace, workspace_bytes, stream);
     if (rc) return rc;
-    rc = mc::mincurv_finalize(B, n_max, n_pts, alpha, kappa_bound, curv_error_max, kappa_lin_max, status, lin, workspace,
-                              workspace_bytes, stream);
+    rc = mc::mincurv_finalize(B, n_max, n_pts, alpha, kappa_bound, curv_error_max, kappa_lin_max, status, lin, kbb,
+                              workspace, workspace_bytes, stream);
     if (rc || !sens_rows) return rc;
     mc::mincurv_sens_rows_export_kernel<<<B, 256, 0, (cudaStream_t)stream>>>(n_max, n_pts, (double *)workspace, mc::make_layout(n_max),
                                                                              status, sens, sens_rows, n_rows, grad_status);
@@ -252,14 +265,19 @@ int mc_mincurv_solve_batch_ex(int B, int n_max, const int32_t *n_pts, const doub
                               const double *h, double kappa_bound, double w_veh, const double *w_veh_batch, double f_scale,
                               double *alpha, double *curv_error_max, double *kappa_lin_max, int32_t *status, int32_t *iters,
                               double prox_mu, const double *prox_x, const double *prox_q, const double *lin_alpha,
-                              void *workspace, size_t workspace_bytes, void *stream) {
+                              const double *kappa_bound_batch, const int32_t *centre_id, double *sens, int32_t *grad_status,
+                              double *sens_rows, int32_t *n_rows, void *workspace, size_t workspace_bytes, void *stream) {
+    if (!sens != !grad_status) return bad("mc_mincurv_solve_batch_ex: sens and grad_status go together");
+    if (!sens_rows != !n_rows || (sens_rows && !sens))
+        return bad("mc_mincurv_solve_batch_ex: sens_rows and n_rows go together, and with sens");
+    if (prox_x && (centre_id || sens)) return bad("mc_mincurv_solve_batch_ex: prox_x takes neither centre_id nor sens");
     if (prox_x)
         return mincurv_prox_solve(B, n_max, n_pts, reftrack, normvec, h, kappa_bound, w_veh, w_veh_batch, f_scale, alpha,
-                                  curv_error_max, kappa_lin_max, status, iters, prox_mu, prox_x, prox_q, lin_alpha, workspace,
-                                  workspace_bytes, stream);
-    return mincurv_solve(B, n_max, n_pts, reftrack, normvec, h, kappa_bound, w_veh, w_veh_batch, f_scale, nullptr, alpha,
-                         curv_error_max, kappa_lin_max, status, iters, nullptr, nullptr, nullptr, nullptr, lin_alpha, workspace,
-                         workspace_bytes, stream);
+                                  curv_error_max, kappa_lin_max, status, iters, prox_mu, prox_x, prox_q, lin_alpha,
+                                  kappa_bound_batch, workspace, workspace_bytes, stream);
+    return mincurv_solve(B, n_max, n_pts, reftrack, normvec, h, kappa_bound, w_veh, w_veh_batch, f_scale, centre_id, alpha,
+                         curv_error_max, kappa_lin_max, status, iters, sens, grad_status, sens_rows, n_rows, lin_alpha,
+                         kappa_bound_batch, workspace, workspace_bytes, stream);
 }
 
 int mc_mincurv_solve_batch_shared(int B, int n_max, const int32_t *n_pts, const double *reftrack, const double *normvec,
@@ -267,8 +285,8 @@ int mc_mincurv_solve_batch_shared(int B, int n_max, const int32_t *n_pts, const 
                                   const int32_t *centre_id, double *alpha, double *curv_error_max, double *kappa_lin_max,
                                   int32_t *status, int32_t *iters, void *workspace, size_t workspace_bytes, void *stream) {
     return mincurv_solve(B, n_max, n_pts, reftrack, normvec, h, kappa_bound, w_veh, w_veh_batch, f_scale, centre_id, alpha,
-                         curv_error_max, kappa_lin_max, status, iters, nullptr, nullptr, nullptr, nullptr, nullptr, workspace,
-                         workspace_bytes, stream);
+                         curv_error_max, kappa_lin_max, status, iters, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr,
+                         workspace, workspace_bytes, stream);
 }
 
 int mc_mincurv_solve_batch_sens(int B, int n_max, const int32_t *n_pts, const double *reftrack, const double *normvec,
@@ -279,8 +297,8 @@ int mc_mincurv_solve_batch_sens(int B, int n_max, const int32_t *n_pts, const do
     if (!sens || !grad_status) return bad("mc_mincurv_solve_batch_sens: NULL argument");
     if (!sens_rows != !n_rows) return bad("mc_mincurv_solve_batch_sens: sens_rows and n_rows go together");
     return mincurv_solve(B, n_max, n_pts, reftrack, normvec, h, kappa_bound, w_veh, w_veh_batch, f_scale, centre_id, alpha,
-                         curv_error_max, kappa_lin_max, status, iters, sens, grad_status, sens_rows, n_rows, nullptr, workspace,
-                         workspace_bytes, stream);
+                         curv_error_max, kappa_lin_max, status, iters, sens, grad_status, sens_rows, n_rows, nullptr,
+                         nullptr, workspace, workspace_bytes, stream);
 }
 
 }  // extern "C"

@@ -1429,16 +1429,24 @@ static int launch_solver(void (*kernel)(P...), int grid, int *work_counter, cuda
 // PROX: the Hessian is H + prox_mu I (the projection QP of mc_mincurv_solve_batch_ex, whose prox stage put prox_mu on the
 // band's diagonal and its linear term in V_F for the box phase): + prox_mu a in the gradient and the residuals, + prox_mu
 // on the factored diagonal.  Without PROX prox_mu is not read.
+// kb_batch [B] or NULL: the bound of each instance's rows (NULL: kb for all).  A flagged instance whose bound is not finite
+// or not > 0 is refused with status -1 (the finalize stage refuses it before it could be flagged).
 // ================================================================================================
 template <bool PROX>
 __global__ void __launch_bounds__(IP_THREADS, 8)
 mincurv_pdip_kappa_kernel(int B, int n_max, const int32_t *__restrict__ n_pts, double *__restrict__ ws, Layout L,
-                          PdipParams prm, double kb, double *__restrict__ alpha_out, int32_t *__restrict__ status,
-                          int32_t *__restrict__ iters_out, int *__restrict__ work_counter, double prox_mu) {
+                          PdipParams prm, double kb_scalar, double *__restrict__ alpha_out, int32_t *__restrict__ status,
+                          int32_t *__restrict__ iters_out, int *__restrict__ work_counter, double prox_mu,
+                          const double *__restrict__ kb_batch) {
     IpShared &sh = ip_init_shared();
     unsigned tick = 0;
     for (int b; (b = next_instance(sh, work_counter)) < B;) {
         if (status[b] != 4) continue;
+        const double kb = kb_batch ? kb_batch[b] : kb_scalar;
+        if (!(kb > 0.0 && kb < INFINITY)) {     // (a thread that reads the -1 already leaves above: both go on to the
+            if (threadIdx.x == 0) status[b] = -1;   //  next instance's barrier)
+            continue;
+        }
         const int n = n_pts ? n_pts[b] : n_max;
         double *aout = alpha_out + (size_t)b * n_max;
         double *slab = ws + (size_t)b * L.stride;
@@ -1869,8 +1877,9 @@ mincurv_adjoint_rows_kernel(int B, int n_max, const int32_t *__restrict__ n_pts,
 
 // the curvature-row phase of mc_mincurv_kappa_batch (prox_mu 0) or of the projection QP of mc_mincurv_solve_batch_ex
 // (Hessian H + prox_mu I, prox_mu > 0)
-int mincurv_kappa_phase(int B, int n_max, const int32_t *n_pts, double kappa_bound, double prox_mu, double *alpha,
-                        int32_t *status, int32_t *iters, void *workspace, size_t workspace_bytes, void *stream) {
+int mincurv_kappa_phase(int B, int n_max, const int32_t *n_pts, double kappa_bound, const double *kappa_bound_batch,
+                        double prox_mu, double *alpha, int32_t *status, int32_t *iters, void *workspace,
+                        size_t workspace_bytes, void *stream) {
     if (!alpha || !status) return bad("mc_mincurv_kappa_batch: NULL argument");
     int rc = mincurv_args("mc_mincurv_kappa_batch", B, n_max, workspace, workspace_bytes);
     if (rc) return rc;
@@ -1884,7 +1893,8 @@ int mincurv_kappa_phase(int B, int n_max, const int32_t *n_pts, double kappa_bou
     auto kernel = prox_mu > 0.0 ? mincurv_pdip_kappa_kernel<true> : mincurv_pdip_kappa_kernel<false>;
     const SolverGrid g = solver_grid(B, n_max, workspace, ctas_per_sm(kernel));
     if (launch_solver(kernel, g.grid, g.counter, (cudaStream_t)stream, B, n_max, n_pts, (double *)workspace,
-                      make_layout(n_max), prm, kappa_bound, alpha, status, iters, g.counter, prox_mu) != 0) {
+                      make_layout(n_max), prm, kappa_bound, alpha, status, iters, g.counter, prox_mu,
+                      kappa_bound_batch) != 0) {
         snprintf(g_err, sizeof(g_err), "mincurv_pdip_kappa_kernel: cudaFuncSetAttribute failed");
         return MC_ECUDA;
     }
@@ -1942,8 +1952,10 @@ int mc_mincurv_pdip_batch(int B, int n_max, const int32_t *n_pts, double *alpha,
 }
 
 int mc_mincurv_kappa_batch(int B, int n_max, const int32_t *n_pts, double kappa_bound, double *alpha, int32_t *status,
-                           int32_t *iters, void *workspace, size_t workspace_bytes, void *stream) {
-    return mc::mincurv_kappa_phase(B, n_max, n_pts, kappa_bound, 0.0, alpha, status, iters, workspace, workspace_bytes, stream);
+                           int32_t *iters, const double *kappa_bound_batch, void *workspace, size_t workspace_bytes,
+                           void *stream) {
+    return mc::mincurv_kappa_phase(B, n_max, n_pts, kappa_bound, kappa_bound_batch, 0.0, alpha, status, iters, workspace,
+                                   workspace_bytes, stream);
 }
 
 int mc_mincurv_adjoint_batch(int B, int n_max, const int32_t *n_pts, const double *reftrack, const double *normvec,

@@ -47,6 +47,7 @@ mincurv_setup_kernel(int n_max, const int32_t *__restrict__ n_pts,
     }
     if (threadIdx.x == 0) *band_owner(slab, L) = b;       // (a follower's is set by mincurv_share_kernel)
     const double wv = w_veh_batch ? w_veh_batch[b] : w_veh;
+    const bool bad_wv = !(fabs(wv) < INFINITY);           // refused with status -1 (an owner still assembles)
     const double *rt = reftrack + (size_t)b * n_max * 4;
     const double *nv = normvec + (size_t)b * n_max * 2;
     const double *hb = hin + (size_t)b * n_max;
@@ -84,8 +85,8 @@ mincurv_setup_kernel(int n_max, const int32_t *__restrict__ n_pts,
     // mincurv_share_kernel copies its O(N) vectors into the followers' slabs; the band of H stays in the owner's slab.  An
     // owner finishes the assembly even when its own bounds are infeasible (its followers need it).
     const bool follower = centre_id && centre_id[b] != b;
-    if (s_flag || follower) {
-        if (threadIdx.x == 0) status[b] = s_flag ? 1 : 0;
+    if (s_flag || bad_wv || follower) {
+        if (threadIdx.x == 0) status[b] = bad_wv ? -1 : s_flag ? 1 : 0;
         if (follower || !centre_id) return;
     }
     // ---- P2/P3: periodic LDL^T of the spline system, decay ratios of its inverse ----
@@ -155,7 +156,7 @@ mincurv_setup_kernel(int n_max, const int32_t *__restrict__ n_pts,
     assemble_hband(slab, L, n, nullptr, s_win);
     double *HB = slab + L.o_hb;
     for (int i = threadIdx.x; i < n; i += blockDim.x) HB[(size_t)i * HB_PITCH + HBW + 1] = 0.0;
-    if (threadIdx.x == 0 && !s_flag) status[b] = 0;
+    if (threadIdx.x == 0 && !s_flag && !bad_wv) status[b] = 0;
 }
 
 // followers of a shared centreline: copy the vectors the owner assembled (V_H .. V_KREF, V_F, V_IH) and point the

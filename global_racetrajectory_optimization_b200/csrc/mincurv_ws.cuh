@@ -74,8 +74,9 @@ struct PdipParams {
 // the curvature-row phase (mincurv_ipm.cu): mc_mincurv_kappa_batch with prox_mu = 0, the projection QP of
 // mc_mincurv_solve_batch_ex (Hessian H + prox_mu I) with prox_mu > 0.  Not exported.
 __attribute__((visibility("hidden")))
-int mincurv_kappa_phase(int B, int n_max, const int32_t *n_pts, double kappa_bound, double prox_mu, double *alpha,
-                        int32_t *status, int32_t *iters, void *workspace, size_t workspace_bytes, void *stream);
+int mincurv_kappa_phase(int B, int n_max, const int32_t *n_pts, double kappa_bound, const double *kappa_bound_batch,
+                        double prox_mu, double *alpha, int32_t *status, int32_t *iters, void *workspace,
+                        size_t workspace_bytes, void *stream);
 
 // the assembly (mincurv_setup.cu) with shared centre lines (centre_id) and a linearisation point (lin_alpha [B][n_max]),
 // either NULL; and the finalize stage (mincurv_finalize.cu) of a workspace assembled about a linearisation point (lin)
@@ -86,7 +87,8 @@ int mincurv_setup(int B, int n_max, const int32_t *n_pts, const double *reftrack
                   int32_t *status, void *workspace, size_t workspace_bytes, void *stream);
 __attribute__((visibility("hidden")))
 int mincurv_finalize(int B, int n_max, const int32_t *n_pts, const double *alpha, double kappa_bound, double *curv_error_max,
-                     double *kappa_lin_max, int32_t *status, bool lin, void *workspace, size_t workspace_bytes, void *stream);
+                     double *kappa_lin_max, int32_t *status, bool lin, const double *kappa_bound_batch, void *workspace,
+                     size_t workspace_bytes, void *stream);
 
 __device__ __forceinline__ double *vec(double *slab, const Layout &L, int v) { return slab + (size_t)v * L.np; }
 

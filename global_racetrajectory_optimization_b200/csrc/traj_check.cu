@@ -68,13 +68,21 @@ __global__ void __launch_bounds__(IT_THREADS) interp_track_kernel(int B, int n_m
 }
 
 // ---- calc_min_bound_dists -----------------------------------------------------------------------------------------
+// PER_TRACK: the vehicle length of trajectory b is length_b[b], its width width_b[b] (either array may be NULL: the scalar).
+// The arrays are the last parameters, so that the scalar instantiation keeps its parameter offsets.
+template <bool PER_TRACK>
 __global__ void __launch_bounds__(MB_THREADS) min_bound_dists_kernel(int n_traj_max, const int32_t *n_traj, const double *xy,
                                                                      const double *psi, int nb_max1, const int32_t *nb1,
                                                                      const double *bound1, int nb_max2, const int32_t *nb2,
                                                                      const double *bound2, int bstride, double length_veh,
-                                                                     double width_veh, double *min_dists) {
+                                                                     double width_veh, double *min_dists,
+                                                                     const double *length_b, const double *width_b) {
     __shared__ double sbx[MB_TILE], sby[MB_TILE];
     const int b = blockIdx.y;
+    if constexpr (PER_TRACK) {
+        if (length_b) length_veh = length_b[b];
+        if (width_b) width_veh = width_b[b];
+    }
     const int nt = n_traj ? n_traj[b] : n_traj_max;
     if ((int)(blockIdx.x * blockDim.x) >= nt) return;              // whole CTA beyond this track's trajectory
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -117,13 +125,25 @@ __global__ void __launch_bounds__(MB_THREADS) min_bound_dists_kernel(int n_traj_
 
 // ---- extrema tested by check_traj ---------------------------------------------------------------------------------
 // extrema[b][0..7] = min(min_dists), max |kappa|, max ay, max ax_wo_drag, min ax_wo_drag, max a_tot, max vx, n points
+// PER_TRACK: drag and mass of trajectory b are drag_b[b], mass_b[b] (either may be NULL: the scalar); a mass that is not > 0
+// gives a row of NaN but for the number of points.  The arrays are the last parameters, as for min_bound_dists_kernel.
+template <bool PER_TRACK>
 __global__ void __launch_bounds__(256) traj_extrema_kernel(int n_max, const int32_t *n_traj, const double *kappa,
                                                            const double *vx, const double *ax, const double *min_dists,
-                                                           double dragcoeff, double mass_veh, double *extrema) {
+                                                           double dragcoeff, double mass_veh, double *extrema,
+                                                           const double *drag_b, const double *mass_b) {
     __shared__ double red[32];
     const int b = blockIdx.x;
     const int n = n_traj ? n_traj[b] : n_max;
     const size_t o = (size_t)b * n_max;
+    if constexpr (PER_TRACK) {
+        if (drag_b) dragcoeff = drag_b[b];
+        if (mass_b) mass_veh = mass_b[b];
+        if (!(mass_veh > 0.0)) {
+            if (threadIdx.x < 8) extrema[(size_t)b * 8 + threadIdx.x] = threadIdx.x == 7 ? (double)n : NAN;
+            return;
+        }
+    }
     double mn_d = INFINITY, mx_k = -INFINITY, mx_ay = -INFINITY, mx_ax = -INFINITY, mn_ax = INFINITY, mx_at = -INFINITY,
            mx_v = -INFINITY;
     for (int i = threadIdx.x; i < n && i < n_max; i += blockDim.x) {
@@ -213,27 +233,33 @@ int mc_interp_track_batch(int B, int n_max, const int32_t *n_pts, const double *
 
 int mc_min_bound_dists_batch(int B, int n_traj_max, const int32_t *n_traj, const double *xy, const double *psi, int nb1_max,
                              const int32_t *nb1, const double *bound1, int nb2_max, const int32_t *nb2, const double *bound2,
-                             int bound_stride, double length_veh, double width_veh, double *min_dists, void *stream) {
+                             int bound_stride, double length_veh, double width_veh, double *min_dists,
+                             const double *length_veh_batch, const double *width_veh_batch, void *stream) {
     if (B <= 0 || n_traj_max <= 0 || !xy || !psi || !bound1 || !bound2 || nb1_max <= 0 || nb2_max <= 0 ||
         bound_stride < 2 || !min_dists)
         return bad("mc_min_bound_dists_batch: bad argument");
+    const bool per_track = length_veh_batch || width_veh_batch;
     mc::for_grid_y_chunks(B, [&](int b0, int nb) {
         const size_t ot = (size_t)b0 * n_traj_max;
         dim3 grid((n_traj_max + mc::MB_THREADS - 1) / mc::MB_THREADS, nb);
-        mc::min_bound_dists_kernel<<<grid, mc::MB_THREADS, 0, (cudaStream_t)stream>>>(
+        auto kernel = per_track ? mc::min_bound_dists_kernel<true> : mc::min_bound_dists_kernel<false>;
+        kernel<<<grid, mc::MB_THREADS, 0, (cudaStream_t)stream>>>(
             n_traj_max, n_traj ? n_traj + b0 : nullptr, xy + 2 * ot, psi + ot, nb1_max, nb1 ? nb1 + b0 : nullptr,
             bound1 + (size_t)b0 * nb1_max * bound_stride, nb2_max, nb2 ? nb2 + b0 : nullptr,
-            bound2 + (size_t)b0 * nb2_max * bound_stride, bound_stride, length_veh, width_veh, min_dists + ot);
+            bound2 + (size_t)b0 * nb2_max * bound_stride, bound_stride, length_veh, width_veh, min_dists + ot,
+            length_veh_batch ? length_veh_batch + b0 : nullptr, width_veh_batch ? width_veh_batch + b0 : nullptr);
     });
     return check_cuda("min_bound_dists_kernel");
 }
 
 int mc_traj_extrema_batch(int B, int n_max, const int32_t *n_traj, const double *kappa, const double *vx, const double *ax,
-                          const double *min_dists, double dragcoeff, double mass_veh, double *extrema, void *stream) {
-    if (B <= 0 || n_max <= 0 || !kappa || !vx || !ax || !extrema || !(mass_veh > 0.0))
+                          const double *min_dists, double dragcoeff, double mass_veh, double *extrema,
+                          const double *dragcoeff_batch, const double *mass_veh_batch, void *stream) {
+    if (B <= 0 || n_max <= 0 || !kappa || !vx || !ax || !extrema || !(mass_veh_batch || mass_veh > 0.0))
         return bad("mc_traj_extrema_batch: bad argument");
-    mc::traj_extrema_kernel<<<B, 256, 0, (cudaStream_t)stream>>>(n_max, n_traj, kappa, vx, ax, min_dists, dragcoeff, mass_veh,
-                                                                 extrema);
+    auto kernel = (dragcoeff_batch || mass_veh_batch) ? mc::traj_extrema_kernel<true> : mc::traj_extrema_kernel<false>;
+    kernel<<<B, 256, 0, (cudaStream_t)stream>>>(n_max, n_traj, kappa, vx, ax, min_dists, dragcoeff, mass_veh, extrema,
+                                                dragcoeff_batch, mass_veh_batch);
     return check_cuda("traj_extrema_kernel");
 }
 

@@ -9,6 +9,7 @@ The parameter names are those of params/racecar.ini (``pars["veh_params"]``, ``p
 ``pars["stepsize_opts"]``, ``pars["vel_calc_opts"]``); ``default_pars()`` returns the stock values."""
 from __future__ import annotations
 
+from types import SimpleNamespace
 from typing import Optional
 
 import torch
@@ -25,8 +26,9 @@ def default_pars() -> dict:
             "optim_opts": {"width_opt": 3.4, "iqp_iters_min": 3, "iqp_curverror_allowed": 0.01}}
 
 
-def globaltraj_batch(reftrack: torch.Tensor, opt_type: str, pars: dict, ggv, ax_max_machines,
-                     n_pts: Optional[torch.Tensor] = None, check: bool = True, refine: Optional[dict] = None) -> dict:
+def globaltraj_batch(reftrack: torch.Tensor, opt_type: str, pars: dict, ggv=None, ax_max_machines=None,
+                     n_pts: Optional[torch.Tensor] = None, check: bool = True, refine: Optional[dict] = None,
+                     vehicles: Optional[_b.Vehicles] = None, veh_id=None) -> dict:
     """Runs the flow for every track of ``reftrack`` [B, n_max, 4] (prepared tracks: what prep_track returns).
 
     Returns a dict of device tensors: alpha, reftrack / normvec / n_pts (of the last QP: they change for 'mincurv_iqp'),
@@ -39,7 +41,20 @@ def globaltraj_batch(reftrack: torch.Tensor, opt_type: str, pars: dict, ggv, ax_
     and every later stage uses the refined alpha; ``qp_alpha``, ``laptime_start`` (the lap time at the QP's alpha),
     ``refine_status``, ``refine_iters`` and ``refine_evals`` are added.  A track whose QP failed (status != 0) is not
     refined: it keeps the QP's alpha and gets refine_status -1.  Not for 'mincurv_iqp', whose reftrack changes per
-    iteration."""
+    iteration.
+
+    ``vehicles``, ``veh_id``: a car per track (batch.Vehicles; veh_id [B] host or device integers, None for one vehicle
+    per track), so that one call sweeps cars.  Every stage runs with each track's car: the QPs with its curvlim and
+    width_opt, the velocity profile (and the refinement's lap time) with its tables, v_max, dragcoeff and mass, and the
+    check_traj quantities with its length, width, dragcoeff and mass.  A field the Vehicles object leaves unset
+    (curvlim, width_opt, length, width) is taken from ``pars`` for every track.  ggv and ax_max_machines are then None.
+    The refinement plans with each track's width_opt and drives each track's car.  Its curvature limit is, as with
+    ``pars``, refine's own ``kappa_bound`` and not curvlim: with ``pars`` the refinement enforces no limit unless refine
+    asks for one, and the vehicles path keeps that meaning, so that a track's outputs stay those of the call with its
+    car's scalar ``pars`` and tables alone.  For each car's limit pass it per track, e.g.
+    ``refine={"metric_length": 10.0, "kappa_bound": vehicles.per_track("curvlim", vehicles.veh_id(veh_id, B, dev))}``.
+    Still one per call: dyn_model_exp, the filter window, the step sizes and the iterative
+    QP's options."""
     if opt_type not in ("mincurv", "mincurv_iqp", "shortest_path"):
         raise IOError("Unknown optimization type!" if opt_type != "mintime" else
                       "opt_type 'mintime' (CasADi/IPOPT NLP) is outside the CUDA path")
@@ -48,35 +63,34 @@ def globaltraj_batch(reftrack: torch.Tensor, opt_type: str, pars: dict, ggv, ax_
     if refine is not None and opt_type == "mincurv_iqp":
         raise NotImplementedError("refine: not for 'mincurv_iqp' (its reftrack changes per iteration)")
     veh, opt, steps, vel = pars["veh_params"], pars["optim_opts"], pars["stepsize_opts"], pars["vel_calc_opts"]
+    car = _car(reftrack, veh, opt, ggv, ax_max_machines, vehicles, veh_id)
     cx, cy, nv, h = _b.calc_splines_batch(reftrack, n_pts=n_pts, want_coeffs=False)
     rt_used, nv_used, n_used = reftrack, nv, n_pts
     if opt_type == "mincurv":
-        qp = _b.opt_min_curv_batch(reftrack, nv, h, veh["curvlim"], opt["width_opt"], n_pts=n_pts)
+        qp = _b.opt_min_curv_batch(reftrack, nv, h, car.curvlim, car.width_opt, n_pts=n_pts)
         alpha, status = qp["alpha"], qp["status"]
     elif opt_type == "mincurv_iqp":
-        qp = _b.iqp_batch(reftrack, nv, h, veh["curvlim"], opt["width_opt"], steps["stepsize_reg"],
+        qp = _b.iqp_batch(reftrack, nv, h, car.curvlim, car.width_opt, steps["stepsize_reg"],
                           iters_min=opt["iqp_iters_min"], curv_error_allowed=opt["iqp_curverror_allowed"], n_pts=n_pts)
         alpha, status = qp["alpha"], qp["status"]
         rt_used, nv_used, n_used = qp["reftrack"], qp["normvec"], qp["n_pts"]
     else:
-        qp = _b.opt_shortest_path_batch(reftrack, nv, opt["width_opt"], n_pts=n_pts)
+        qp = _b.opt_shortest_path_batch(reftrack, nv, car.width_opt, n_pts=n_pts)
         alpha, status = qp["alpha"], qp["status"]
     refined = {}
     if refine is not None:
         n_all = n_pts if n_pts is not None else torch.full_like(status, reftrack.shape[1])
-        ref = _refine.refine_raceline_batch(reftrack, nv, alpha, opt["width_opt"], ggv, ax_max_machines, float(veh["v_max"]),
-                                            veh["dragcoeff"], veh["mass"], stepsize_interp=steps["stepsize_interp_after_opt"],
+        ref = _refine.refine_raceline_batch(reftrack, nv, alpha, car.width_opt, stepsize_interp=steps["stepsize_interp_after_opt"],
                                             n_pts=torch.where(status == 0, n_all.to(status), torch.zeros_like(status)),
                                             dyn_model_exp=vel["dyn_model_exp"],
-                                            filt_window=vel["vel_profile_conv_filt_window"], **refine)
+                                            filt_window=vel["vel_profile_conv_filt_window"], **car.vp, **refine)
         refined = dict(qp_alpha=alpha, laptime_start=ref["laptime_start"], refine_status=ref["status"],
                        refine_iters=ref["iters"], refine_evals=ref["evals"])
         alpha = ref["alpha"]
     rl = _b.create_raceline_batch(rt_used, nv_used, alpha, steps["stepsize_interp_after_opt"], n_pts=n_used)
     n_out = rl["n_out"]
-    vp = _b.vel_profile_batch(rl["kappa"], rl["el_lengths_interp"], ggv, ax_max_machines, float(veh["v_max"]),
-                              veh["dragcoeff"], veh["mass"], dyn_model_exp=vel["dyn_model_exp"],
-                              filt_window=vel["vel_profile_conv_filt_window"], n_pts=n_out)
+    vp = _b.vel_profile_batch(rl["kappa"], rl["el_lengths_interp"], dyn_model_exp=vel["dyn_model_exp"],
+                              filt_window=vel["vel_profile_conv_filt_window"], n_pts=n_out, **car.vp)
     vx, ax, t = vp["vx"][:, 0].contiguous(), vp["ax"][:, 0].contiguous(), vp["t"][:, 0].contiguous()
     traj = _b.assemble_trajectory_batch(rl["s_interp"], rl["raceline_interp"], rl["psi"], rl["kappa"], vx, ax,
                                         rl["spline_lengths"], n_traj=n_out, n_spl=n_used)
@@ -86,6 +100,30 @@ def globaltraj_batch(reftrack: torch.Tensor, opt_type: str, pars: dict, ggv, ax_
     out.update(refined)
     if check:
         out.update(_b.check_traj_batch(rt_used, nv_used, rl["raceline_interp"], rl["psi"], rl["kappa"], vx, ax,
-                                       veh["length"], veh["width"], veh["dragcoeff"], veh["mass"], n_pts=n_used,
-                                       n_traj=n_out))
+                                       car.length, car.width, car.dragcoeff, car.mass, n_pts=n_used, n_traj=n_out))
     return out
+
+
+def _car(reftrack, veh: dict, opt: dict, ggv, ax_max_machines, vehicles, veh_id) -> SimpleNamespace:
+    """The vehicle parameters of globaltraj_batch's stages: curvlim, width_opt, length, width, dragcoeff, mass (a number
+    from pars, or with vehicles a [B] device tensor gathered by veh_id, pars where the Vehicles leave a field unset) and
+    vp, the vehicle arguments of the velocity profile and the refinement."""
+    if vehicles is None:
+        if veh_id is not None:
+            raise ValueError("veh_id needs vehicles=")
+        if ggv is None or ax_max_machines is None:
+            raise TypeError("globaltraj_batch needs ggv and ax_max_machines (or vehicles=)")
+        return SimpleNamespace(curvlim=veh["curvlim"], width_opt=opt["width_opt"], length=veh["length"], width=veh["width"],
+                               dragcoeff=veh["dragcoeff"], mass=veh["mass"],
+                               vp=dict(ggv=ggv, ax_max_machines=ax_max_machines, v_max=float(veh["v_max"]),
+                                       drag_coeff=veh["dragcoeff"], m_veh=veh["mass"]))
+    if ggv is not None or ax_max_machines is not None:
+        raise ValueError("globaltraj_batch: with vehicles= ggv and ax_max_machines must be None (each vehicle has its own)")
+    if not isinstance(vehicles, _b.Vehicles):
+        raise TypeError("vehicles must be a batch.Vehicles")
+    ids = vehicles.veh_id(veh_id, reftrack.shape[0], reftrack.device)
+    field = lambda name, default: default if getattr(vehicles, name) is None else vehicles.per_track(name, ids)  # noqa: E731
+    return SimpleNamespace(curvlim=field("curvlim", veh["curvlim"]), width_opt=field("width_opt", opt["width_opt"]),
+                           length=field("length", veh["length"]), width=field("width", veh["width"]),
+                           dragcoeff=vehicles.per_track("drag_coeff", ids), mass=vehicles.per_track("m_veh", ids),
+                           vp=dict(vehicles=vehicles, veh_id=ids))

@@ -466,13 +466,15 @@ class CurvatureProjection:
     computed once here, so a call does not synchronise the stream.  kappa_lin(x, mask) -> kappa_lin_max [B], the QP's
     max |k_ref + E x| at x (assembly and the finalize stage); evaluate(x, mask) -> (kappa_lin_max, curv_error_max) [B].
     timer(name) as LapTime's ('projection').  lin_alpha [B, n_max] (None: the centre line): P and H are those of the QP
-    linearised about the line reftrack + lin_alpha * normvec (DESIGN.md section 3.2)."""
+    linearised about the line reftrack + lin_alpha * normvec (DESIGN.md section 3.2).  kappa_bound: a float or a [B]
+    tensor (a limit per track, as for batch.opt_min_curv_batch)."""
 
-    def __init__(self, reftrack, normvec, n_pts, w_veh, kappa_bound: float, length: float,
+    def __init__(self, reftrack, normvec, n_pts, w_veh, kappa_bound: Union[float, torch.Tensor], length: float,
                  lin_alpha: Optional[torch.Tensor] = None):
         B, n_max, _ = reftrack.shape
         dev = reftrack.device
-        self.mu, self.kb = float(length) ** -4, float(kappa_bound)
+        self.mu = float(length) ** -4
+        self.kb, self.kb_batch = _b._kappa_bound(kappa_bound, B, dev)
         self.n_pts = n_pts if n_pts is not None else torch.full((B,), n_max, dtype=torch.int32, device=dev)
         self.launchable = self.n_pts >= _b.N_MIN
         self.w_scalar, self.w_batch = _b._wveh(w_veh, B, dev)
@@ -500,7 +502,8 @@ class CurvatureProjection:
             _b._launch_chunks("mc_mincurv_solve_batch_ex", B, self.chunk, self._ws(), n_max,
                               *map(_b._rows, (self._n(mask), self.reftrack, self.normvec, self.h)), self.kb, self.w_scalar,
                               _b._rows(self.w_batch), _b.F_SCALE, *map(_b._rows, out.values()), self.mu,
-                              _b._rows(x.contiguous()), _b._rows(q.contiguous()), _b._rows(self.lin))
+                              _b._rows(x.contiguous()), _b._rows(q.contiguous()), _b._rows(self.lin),
+                              _b._rows(self.kb_batch), *(None,) * 5)
             ok = mask & self.launchable & (out["status"] == 0) & torch.isfinite(out["alpha"]).all(dim=1)
             return out["alpha"], ok
 
@@ -522,7 +525,8 @@ class CurvatureProjection:
                      self.w_scalar, None if self.w_batch is None else self.w_batch[s:e], _b.F_SCALE, out["status"][s:e],
                      None if self.lin is None else self.lin[s:e], ws=ws)
             _b._call("mc_mincurv_finalize_batch", e - s, n_max, n[s:e], x[s:e], self.kb, out["curv_error_max"][s:e],
-                     out["kappa_lin_max"][s:e], out["status"][s:e], int(self.lin is not None), ws=ws)
+                     out["kappa_lin_max"][s:e], out["status"][s:e], int(self.lin is not None),
+                     None if self.kb_batch is None else self.kb_batch[s:e], ws=ws)
         ok = mask & self.launchable & (out["status"] != 1) & (out["status"] >= 0)
         return torch.where(ok, out["kappa_lin_max"], kmax), torch.where(ok, out["curv_error_max"], kmax)
 
@@ -534,7 +538,7 @@ def refine_raceline_batch(reftrack: torch.Tensor, normvec: torch.Tensor, alpha0:
                           pg_tol: float = PG_TOL, memory: int = MEMORY, gamma: float = GAMMA, lam_min: float = LAM_MIN,
                           lam_max: float = LAM_MAX, max_halvings: int = MAX_HALVINGS,
                           callback: Optional[Callable] = None, objective: Optional[LapTime] = None,
-                          metric_length: Optional[float] = None, kappa_bound: Optional[float] = None,
+                          metric_length: Optional[float] = None, kappa_bound: Union[None, float, torch.Tensor] = None,
                           relinearise: int = 0, curv_error_allowed: float = CURV_ERROR_ALLOWED,
                           vehicles: Optional[_b.Vehicles] = None, veh_id=None) -> dict:
     """Lowers the quasi-steady-state lap time of every track's raceline by moving alpha inside opt_min_curv's box.
@@ -559,7 +563,9 @@ def refine_raceline_batch(reftrack: torch.Tensor, normvec: torch.Tensor, alpha0:
 
     kappa_bound: None (alpha stays in the box only), or kb > 0 [1/m] (metric_length required): alpha stays in opt_min_curv's
     feasible set for this kappa_bound, the box and the linearised curvature rows |k_ref + E alpha| <= kb about the centre
-    line.  alpha0 is projected onto it in the metric (replacing the clamp to the box), and every step is the projected
+    line (a [B] tensor: a limit per track, e.g. each car's curvlim; a host tensor must hold finite limits > 0, a track
+    whose entry in a device tensor is not finite or not > 0 has no projection (status NO_PROJECTION, alpha0 returned)).
+    alpha0 is projected onto it in the metric (replacing the clamp to the box), and every step is the projected
     gradient step in the metric (CurvatureProjection, spg's project: one QP per iteration; no pins, no metric_fallbacks).
     pg_norm is then ||d||_inf / lam of that step.  A track whose projection fails, or gives no descent direction, stops
     with status NO_PROJECTION (5) at its last accepted point; where alpha0's projection fails (e.g. fewer than N_MIN
@@ -590,7 +596,10 @@ def refine_raceline_batch(reftrack: torch.Tensor, normvec: torch.Tensor, alpha0:
     if metric_length is not None and not (math.isfinite(float(metric_length)) and float(metric_length) > 0.0):
         raise ValueError("refine_raceline_batch: metric_length must be None or a finite length > 0 [m]")
     if kappa_bound is not None:
-        if not (math.isfinite(float(kappa_bound)) and float(kappa_bound) > 0.0):
+        if isinstance(kappa_bound, torch.Tensor):
+            if kappa_bound.device.type == "cpu" and not bool((torch.isfinite(kappa_bound) & (kappa_bound > 0.0)).all()):
+                raise ValueError("refine_raceline_batch: kappa_bound must be None or finite curvatures > 0 [1/m]")
+        elif not (math.isfinite(float(kappa_bound)) and float(kappa_bound) > 0.0):
             raise ValueError("refine_raceline_batch: kappa_bound must be None or a finite curvature > 0 [1/m]")
         if metric_length is None:
             raise ValueError("refine_raceline_batch: kappa_bound needs metric_length (the projection runs in the "
@@ -633,7 +642,13 @@ def refine_raceline_batch(reftrack: torch.Tensor, normvec: torch.Tensor, alpha0:
         metric = CurvatureMetric(reftrack, normvec, n_pts, float(metric_length))
         metric.timer = fun.timer
     if kappa_bound is not None:
-        project = CurvatureProjection(reftrack, normvec, n_pts, w_veh, float(kappa_bound), float(metric_length))
+        if isinstance(kappa_bound, torch.Tensor):            # (checked and on the device once, for every round)
+            if kappa_bound.numel() != B:
+                raise ValueError("refine_raceline_batch: kappa_bound tensor must have one entry per track")
+            kappa_bound = _b._kappa_bound(kappa_bound, B, dev)[1]
+        else:
+            kappa_bound = float(kappa_bound)
+        project = CurvatureProjection(reftrack, normvec, n_pts, w_veh, kappa_bound, float(metric_length))
         project.timer = fun.timer
     res = spg(fun, x0, lb, ub, active, max_iters=max_iters, pg_tol=pg_tol, memory=memory, gamma=gamma,
               lam_min=lam_min, lam_max=lam_max, max_halvings=max_halvings, callback=callback, metric=metric,
@@ -653,7 +668,7 @@ def refine_raceline_batch(reftrack: torch.Tensor, normvec: torch.Tensor, alpha0:
         out["projection_failures"] = res["projection_failures"]
         if relinearise:
             _rounds(out, fun, reftrack, normvec, n_pts, w_veh, lb, ub, kept, int(relinearise), float(curv_error_allowed),
-                    float(kappa_bound), float(metric_length), dict(max_iters=max_iters, pg_tol=pg_tol, memory=memory,
+                    kappa_bound, float(metric_length), dict(max_iters=max_iters, pg_tol=pg_tol, memory=memory,
                     gamma=gamma, lam_min=lam_min, lam_max=lam_max, max_halvings=max_halvings, callback=callback))
         else:
             out["rounds"] = torch.zeros_like(out["iters"])

@@ -43,6 +43,12 @@ extern "C" {
 /* MC_OPTIONAL2 marks parameters added after the MC_OPTIONAL ones, alike NULL-able.  The binding lets a call leave out
  * the MC_OPTIONAL2 parameters alone (the signature before they were added), or them and the MC_OPTIONAL ones. */
 #define MC_OPTIONAL2
+/* MC_OPTIONAL3 marks parameters added after the MC_OPTIONAL2 ones, alike NULL-able: those of a vehicle per track (a
+ * curvature limit, a vehicle size, drag and mass per track) and, on mc_mincurv_solve_batch_ex only, the shared centre
+ * lines and the sensitivity export, so that a limit per instance reaches the solves of mc_mincurv_solve_batch_shared
+ * and mc_mincurv_solve_batch_sens, whose signatures keep the scalar limit.  The binding lets a call leave out the
+ * MC_OPTIONAL3 parameters alone, or them and each earlier group in turn. */
+#define MC_OPTIONAL3
 
 #define MC_STATUS_OK 0
 #define MC_STATUS_TOO_NARROW 1
@@ -91,7 +97,8 @@ int mc_calc_splines_batch(int B, int n_max, const int32_t *n_pts,
  *   normvec   [B][n_max][2]
  *   h         [B][n_max]     : parameter scales of the spline system (h_out of mc_calc_splines_batch;
  *                              what the reference passes as the dense matrix `A`)
- *   w_veh_batch [B] or NULL  : per-instance vehicle width; NULL => the scalar w_veh for all
+ *   w_veh_batch [B] or NULL  : per-instance vehicle width; NULL => the scalar w_veh for all (an instance whose width is
+ *                              not finite gets status -1 from the assembly: here and in every minimum-curvature entry)
  *   alpha     [B][n_max]     : lateral shift of every point along its normal [m]
  *   curv_error_max [B]       : tph's linearisation error (second tuple element of opt_min_curv)
  *   kappa_lin_max  [B] or NULL : max |k_ref + E alpha| of the linearised curvature at the solution
@@ -121,7 +128,18 @@ int mc_mincurv_solve_batch(int B, int n_max, const int32_t *n_pts,
  *                    derivatives x', y' in S_x, S_y are those of the spline through P + a n, k_ref = S_y m_y - S_x m_x
  *                    keeps the centre line's moments, so that k_ref + E a is the knot curvature of the spline through
  *                    P + a n.  H, f and the rows follow from these; the variable is still alpha about P.  curv_error_max
- *                    and kappa_lin_max refer to this linearisation. */
+ *                    and kappa_lin_max refer to this linearisation.
+ *   kappa_bound_batch [B] or NULL : a curvature limit per instance (NULL: the scalar kappa_bound for all; with the array
+ *                    the scalar is not read).  Also taken by mc_mincurv_finalize_batch and mc_mincurv_kappa_batch.  An
+ *                    instance whose limit is not finite or not > 0 gets status -1 in the first finalize pass (the
+ *                    curvature-row phase never takes it up); the other instances are those of a call with their own
+ *                    limit as the scalar, bit for bit.
+ *   centre_id, sens, grad_status, sens_rows, n_rows (all NULL: none of this): without prox_x, the shared centre lines of
+ *                    mc_mincurv_solve_batch_shared and the export of mc_mincurv_solve_batch_sens (sens and grad_status
+ *                    together, sens_rows and n_rows together and only with them), as documented there.  This entry is
+ *                    the one way to those two solves with kappa_bound_batch: their own signatures keep the scalar limit
+ *                    (a parameter before their workspace would change what existing callers' argument lists bind to).
+ *                    Not with prox_x. */
 int mc_mincurv_solve_batch_ex(int B, int n_max, const int32_t *n_pts,
                               const double *reftrack, const double *normvec, const double *h,
                               double kappa_bound, double w_veh, const double *w_veh_batch, double f_scale,
@@ -129,6 +147,9 @@ int mc_mincurv_solve_batch_ex(int B, int n_max, const int32_t *n_pts,
                               int32_t *status, int32_t *iters,
                               double prox_mu, const double *prox_x, const double *prox_q,
                               MC_OPTIONAL2 const double *lin_alpha,
+                              MC_OPTIONAL3 const double *kappa_bound_batch, MC_OPTIONAL3 const int32_t *centre_id,
+                              MC_OPTIONAL3 double *sens, MC_OPTIONAL3 int32_t *grad_status, MC_OPTIONAL3 double *sens_rows,
+                              MC_OPTIONAL3 int32_t *n_rows,
                               void *workspace, size_t workspace_bytes, void *stream);
 
 /* the same for batches in which several instances share a centreline (x, y, normal vectors, h and n_pts identical, only
@@ -138,7 +159,10 @@ int mc_mincurv_solve_batch_ex(int B, int n_max, const int32_t *n_pts,
  *   centre_id [B] or NULL : centre_id[b] = index (in this batch) of the instance that owns b's centreline; owners have
  *                           centre_id[b] == b.  NULL: every instance is assembled on its own.  A follower whose owner is
  *                           not an owner itself, is out of range or has another n_pts gets status -1.
- * The results are identical to the unshared call (the shared quantities are bitwise the same). */
+ * The results are identical to the unshared call (the shared quantities are bitwise the same).
+ * This entry takes the scalar kappa_bound only; shared centre lines with a limit per instance are the stages
+ * mc_mincurv_setup_batch_shared -> mc_mincurv_pdip_batch -> mc_mincurv_finalize_batch -> mc_mincurv_kappa_batch ->
+ * mc_mincurv_finalize_batch on one workspace with kappa_bound_batch, the sequence this entry runs. */
 int mc_mincurv_solve_batch_shared(int B, int n_max, const int32_t *n_pts,
                                   const double *reftrack, const double *normvec, const double *h,
                                   double kappa_bound, double w_veh, const double *w_veh_batch, double f_scale,
@@ -169,6 +193,7 @@ int mc_mincurv_pdip_batch(int B, int n_max, const int32_t *n_pts, double *alpha,
 int mc_mincurv_finalize_batch(int B, int n_max, const int32_t *n_pts, const double *alpha, double kappa_bound,
                               double *curv_error_max, double *kappa_lin_max, int32_t *status,
                               MC_OPTIONAL2 int linearised,
+                              MC_OPTIONAL3 const double *kappa_bound_batch,
                               void *workspace, size_t workspace_bytes, void *stream);
 
 /* Width sensitivities of this QP: alpha differentiated with respect to w_tr_right, w_tr_left and w_veh by one more
@@ -233,9 +258,12 @@ int mc_mincurv_adjoint_batch(int B, int n_max, const int32_t *n_pts,
 
 /* Fourth stage, run by mc_mincurv_solve_batch between two finalize passes: re-solves every instance flagged
  * status 4 (curvature rows violated by the box-only optimum) as the full QP tph hands to quadprog, rows
- * |k_ref + E alpha| <= kappa_bound included; leaves all other instances untouched. */
+ * |k_ref + E alpha| <= kappa_bound included; leaves all other instances untouched.  kappa_bound_batch [B] or NULL: the
+ * limit of each instance's rows, as for mc_mincurv_solve_batch_ex (a flagged instance whose limit is not finite or not
+ * > 0 gets status -1). */
 int mc_mincurv_kappa_batch(int B, int n_max, const int32_t *n_pts, double kappa_bound, double *alpha, int32_t *status,
-                           int32_t *iters, void *workspace, size_t workspace_bytes, void *stream);
+                           int32_t *iters, MC_OPTIONAL3 const double *kappa_bound_batch,
+                           void *workspace, size_t workspace_bytes, void *stream);
 
 /* -------------------------------------------------------------------------------------------------
  * tph.opt_shortest_path.opt_shortest_path(reftrack, normvectors, w_veh, print_debug)
@@ -482,20 +510,30 @@ int mc_interp_track_batch(int B, int n_max, const int32_t *n_pts, const double *
  *   xy [B][n_traj_max][2], psi [B][n_traj_max], n_traj [B] or NULL
  *   bound1/bound2 [B][nb*_max][bound_stride] (x at +0, y at +1), nb1/nb2 [B] or NULL
  *   min_dists [B][n_traj_max]
+ *   length_veh_batch, width_veh_batch [B] or NULL : the vehicle size per trajectory (NULL: the scalars for all; each
+ *                    array replaces its scalar alone)
  */
 int mc_min_bound_dists_batch(int B, int n_traj_max, const int32_t *n_traj, const double *xy, const double *psi,
                              int nb1_max, const int32_t *nb1, const double *bound1, int nb2_max, const int32_t *nb2,
                              const double *bound2, int bound_stride, double length_veh, double width_veh,
-                             double *min_dists, void *stream);
+                             double *min_dists,
+                             MC_OPTIONAL3 const double *length_veh_batch, MC_OPTIONAL3 const double *width_veh_batch,
+                             void *stream);
 
 /* The quantities helper_funcs_glob.src.check_traj.check_traj compares with its limits
  * (helper_funcs_glob/src/check_traj.py:74-139; call site main_globaltraj.py:520-532), per trajectory:
  *   extrema [B][8] = min(min_dists) (inf if min_dists is NULL), max |kappa|, max ay = vx^2 / radius,
  *                    max and min of ax_wo_drag = ax + vx^2 dragcoeff / mass_veh, max sqrt(ax_wo_drag^2 + ay^2), max vx,
  *                    number of points
+ *   dragcoeff_batch, mass_veh_batch [B] or NULL : drag and mass per trajectory (NULL: the scalars for all; each array
+ *                    replaces its scalar alone).  The scalar mass_veh must be > 0 unless mass_veh_batch is given; a
+ *                    trajectory whose mass_veh_batch entry is not > 0 is refused alone: its row is NaN but for the
+ *                    number of points.
  */
 int mc_traj_extrema_batch(int B, int n_max, const int32_t *n_traj, const double *kappa, const double *vx, const double *ax,
-                          const double *min_dists, double dragcoeff, double mass_veh, double *extrema, void *stream);
+                          const double *min_dists, double dragcoeff, double mass_veh, double *extrema,
+                          MC_OPTIONAL3 const double *dragcoeff_batch, MC_OPTIONAL3 const double *mass_veh_batch,
+                          void *stream);
 
 /* trajectory_opt / traj_race_cl of main_globaltraj.py:501-512: rows [s, x, y, psi, kappa, vx, ax];
  * row n_traj[b] closes the lap (copy of row 0 with s = sum(spline_lengths)).  traj [B][n_max + 1][7].
