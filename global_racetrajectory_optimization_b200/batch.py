@@ -109,9 +109,13 @@ def _f64(t: torch.Tensor, name: str) -> torch.Tensor:
     return t.contiguous()
 
 
-def _npts(n_pts, B, device):
+def _npts(n_pts, B, device, cap: Optional[int] = None, name: str = "n_pts"):
+    """The per-track counts as an int32 tensor on device.  With cap, counts in a host tensor must be <= cap (the row
+    holds cap entries); counts in a device tensor are not read here, and the kernels refuse a track whose count is larger."""
     if n_pts is None:
         return None
+    if cap is not None and n_pts.device.type == "cpu" and n_pts.numel() and int(n_pts.max()) > cap:
+        raise ValueError(f"{name}: a count is larger than its row ({int(n_pts.max())} > {cap})")
     n_pts = n_pts.to(device=device, dtype=torch.int32).contiguous()
     if n_pts.numel() != B:
         raise ValueError("n_pts must have one entry per track")
@@ -1332,6 +1336,8 @@ def interp_track_batch(pts: torch.Tensor, stepsize_approx: float = 1.0, n_pts: O
         else:       # the boundary polyline p + sign * w n: the width column of the track is the per-point shift (stride 4)
             poly = _closed_polygon_length(pts, n_pts, normvec=normvec, shift=pts.reshape(-1)[int(width_col):].view(-1),
                                           shift_stride=4, sign=float(normal_sign))
+        # (a NaN or infinite lap, which the kernel refuses, does not size the buffer)
+        poly = torch.nan_to_num(poly, nan=0.0, posinf=0.0)
         n_out_max = int(math.ceil(float(poly.max().item()) / float(stepsize_approx))) + 8
     ws = _workspace("interp_track", _lib.load().mc_interp_track_workspace_bytes(B, n_max), dev)
     while True:
@@ -1362,7 +1368,9 @@ def min_bound_dists_batch(xy: torch.Tensor, psi: torch.Tensor, bound1: torch.Ten
                           nb2: Optional[torch.Tensor] = None) -> torch.Tensor:
     """Batched helper_funcs_glob.src.calc_min_bound_dists.calc_min_bound_dists: [B, n_traj_max] minimum distances of
     the vehicle corners to the boundary points (bound1/bound2: [B, nb_max, >= 2], x and y first).  length_veh and
-    width_veh: floats or [B] tensors (a vehicle size per trajectory)."""
+    width_veh: floats or [B] tensors (a vehicle size per trajectory).  A NaN coordinate propagates like np.amin: a NaN
+    boundary point makes the track's row NaN, a NaN trajectory point its entry.  Host counts beyond their rows raise
+    ValueError; a track whose device count is beyond its row gets a row of NaN."""
     _require_cuda()
     xy, psi, bound1, bound2 = _f64(xy, "xy"), _f64(psi, "psi"), _f64(bound1, "bound1"), _f64(bound2, "bound2")
     B, n_traj_max, _ = xy.shape
@@ -1370,7 +1378,8 @@ def min_bound_dists_batch(xy: torch.Tensor, psi: torch.Tensor, bound1: torch.Ten
         raise ValueError("bound1 and bound2 must have the same row layout")
     dev = xy.device
     out = torch.zeros((B, n_traj_max), dtype=torch.float64, device=dev)
-    n_traj, nb1, nb2 = _npts(n_traj, B, dev), _npts(nb1, B, dev), _npts(nb2, B, dev)
+    n_traj = _npts(n_traj, B, dev, n_traj_max, "n_traj")
+    nb1, nb2 = _npts(nb1, B, dev, int(bound1.shape[1]), "nb1"), _npts(nb2, B, dev, int(bound2.shape[1]), "nb2")
     (length, length_t), (width, width_t) = _per_track(length_veh, B, dev, "length_veh"), _per_track(width_veh, B, dev, "width_veh")
     _call("mc_min_bound_dists_batch", B, n_traj_max, n_traj, xy, psi, int(bound1.shape[1]), nb1, bound1, int(bound2.shape[1]),
           nb2, bound2, int(bound1.shape[2]), length, width, out, length_t, width_t)
@@ -1386,7 +1395,9 @@ def traj_extrema_batch(kappa: torch.Tensor, vx: torch.Tensor, ax: torch.Tensor, 
                        n_traj: Optional[torch.Tensor] = None) -> torch.Tensor:
     """[B, 8] extrema per trajectory, columns as in EXTREMA (min_dist = inf without min_dists).  dragcoeff and mass_veh:
     floats or [B] tensors (per trajectory).  A host mass tensor must be > 0; a trajectory whose mass in a device tensor
-    is not > 0 gets a row of NaN but for n_points."""
+    is not > 0, or whose device n_traj is larger than n_max, gets a row of NaN but for n_points.  min_dist and
+    kappa_abs_max are NaN if a point's is (np.amin / np.amax, as the reference tests them); the other maxima skip NaN
+    points (the reference tests those with np.any(x > limit))."""
     _require_cuda()
     kappa, vx, ax = _f64(kappa, "kappa"), _f64(vx, "vx"), _f64(ax, "ax")
     B, n_max = kappa.shape
@@ -1397,7 +1408,7 @@ def traj_extrema_batch(kappa: torch.Tensor, vx: torch.Tensor, ax: torch.Tensor, 
     if isinstance(mass_veh, torch.Tensor) and mass_veh.device.type == "cpu" and not bool((mass_veh > 0.0).all()):
         raise ValueError("mass_veh must be > 0 for every trajectory")
     (drag, drag_t), (mass, mass_t) = _per_track(dragcoeff, B, dev, "dragcoeff"), _per_track(mass_veh, B, dev, "mass_veh")
-    _call("mc_traj_extrema_batch", B, n_max, _npts(n_traj, B, dev), kappa, vx, ax, min_dists, drag, mass, ext, drag_t, mass_t)
+    _call("mc_traj_extrema_batch", B, n_max, _npts(n_traj, B, dev, n_max, "n_traj"), kappa, vx, ax, min_dists, drag, mass, ext, drag_t, mass_t)
     return ext
 
 
@@ -1467,7 +1478,8 @@ def assemble_trajectory_batch(s: torch.Tensor, xy: torch.Tensor, psi: torch.Tens
                               ax: torch.Tensor, spline_lengths: torch.Tensor, n_traj: Optional[torch.Tensor] = None,
                               n_spl: Optional[torch.Tensor] = None) -> torch.Tensor:
     """trajectory_opt / traj_race_cl of main_globaltraj.py:501-512 for a batch: [B, n_max + 1, 7] rows
-    [s, x, y, psi, kappa, vx, ax]; row n_traj[b] closes the lap with s = sum(spline_lengths[b])."""
+    [s, x, y, psi, kappa, vx, ax]; row n_traj[b] closes the lap with s = sum(spline_lengths[b]), summed left to right.
+    Host counts beyond their rows raise ValueError; a track whose device n_traj or n_spl is beyond its row is left zero."""
     _require_cuda()
     s, xy, psi, kappa, vx, ax = (_f64(t, nm) for t, nm in ((s, "s"), (xy, "xy"), (psi, "psi"), (kappa, "kappa"), (vx, "vx"),
                                                           (ax, "ax")))
@@ -1475,8 +1487,8 @@ def assemble_trajectory_batch(s: torch.Tensor, xy: torch.Tensor, psi: torch.Tens
     B, n_max = s.shape
     dev = s.device
     traj = torch.zeros((B, n_max + 1, 7), dtype=torch.float64, device=dev)
-    _call("mc_assemble_trajectory_batch", B, n_max, _npts(n_traj, B, dev), s, xy, psi, kappa, vx, ax, int(spline_lengths.shape[1]),
-          _npts(n_spl, B, dev), spline_lengths, traj)
+    _call("mc_assemble_trajectory_batch", B, n_max, _npts(n_traj, B, dev, n_max, "n_traj"), s, xy, psi, kappa, vx, ax,
+          int(spline_lengths.shape[1]), _npts(n_spl, B, dev, int(spline_lengths.shape[1]), "n_spl"), spline_lengths, traj)
     return traj
 
 

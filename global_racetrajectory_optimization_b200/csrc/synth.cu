@@ -72,6 +72,10 @@ polygon_length_kernel(int n_max, const int32_t *__restrict__ n_pts, const double
                       double *__restrict__ length) {
     const int b = blockIdx.x;
     const int n = n_pts ? n_pts[b] : n_max;
+    if (n > n_max) {                   // a count beyond the row: length 0 (the re-sampling kernels refuse the track)
+        if (threadIdx.x == 0) length[b] = 0.0;
+        return;
+    }
     __shared__ double red[32];
     double acc = 0.0;
     const double *P = pts + (size_t)b * n_max * stride;

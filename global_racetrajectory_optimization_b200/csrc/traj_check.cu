@@ -49,8 +49,9 @@ __global__ void __launch_bounds__(IT_THREADS) interp_track_kernel(int B, int n_m
     const double total = dc[n];
     const int num = tc::resample_count(total, stepsize);     // includes the closing point, which is dropped
     const int m = num - 1;
-    if (!(total > 0.0) || m > n_out_max) {
-        if (threadIdx.x == 0) n_out[b] = (total > 0.0) ? -m : 0;
+    const bool usable = total > 0.0 && total < (double)INFINITY;      // a NaN or infinite lap is refused: n_out 0
+    if (!usable || m > n_out_max) {
+        if (threadIdx.x == 0) n_out[b] = usable ? -m : 0;
         return;
     }
     if (threadIdx.x == 0) n_out[b] = m;
@@ -69,7 +70,8 @@ __global__ void __launch_bounds__(IT_THREADS) interp_track_kernel(int B, int n_m
 
 // ---- calc_min_bound_dists -----------------------------------------------------------------------------------------
 // PER_TRACK: the vehicle length of trajectory b is length_b[b], its width width_b[b] (either array may be NULL: the scalar).
-// The arrays are the last parameters, so that the scalar instantiation keeps its parameter offsets.
+// The arrays are the last parameters, so that the scalar instantiation keeps its parameter offsets.  A track with
+// n_traj[b] > n_traj_max, nb1[b] > nb_max1 or nb2[b] > nb_max2 is refused: its whole row is NaN.
 template <bool PER_TRACK>
 __global__ void __launch_bounds__(MB_THREADS) min_bound_dists_kernel(int n_traj_max, const int32_t *n_traj, const double *xy,
                                                                      const double *psi, int nb_max1, const int32_t *nb1,
@@ -84,37 +86,55 @@ __global__ void __launch_bounds__(MB_THREADS) min_bound_dists_kernel(int n_traj_
         if (width_b) width_veh = width_b[b];
     }
     const int nt = n_traj ? n_traj[b] : n_traj_max;
-    if ((int)(blockIdx.x * blockDim.x) >= nt) return;              // whole CTA beyond this track's trajectory
+    const int nbs[2] = {nb1 ? nb1[b] : nb_max1, nb2 ? nb2[b] : nb_max2};
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (nt > n_traj_max || nbs[0] > nb_max1 || nbs[1] > nb_max2) {     // counts beyond the row: the track is refused
+        if (i < n_traj_max) min_dists[(size_t)b * n_traj_max + i] = NAN;
+        return;
+    }
+    if ((int)(blockIdx.x * blockDim.x) >= nt) return;              // whole CTA beyond this track's trajectory
     const bool live = i < nt;
     double c[8];
+    bool corners_finite = true;
     if (live) {
         const size_t o = (size_t)b * n_traj_max + i;
         tc::vehicle_corners(xy[2 * o], xy[2 * o + 1], psi[o], length_veh, width_veh, c);
+#pragma unroll
+        for (int k = 0; k < 8; ++k) corners_finite = corners_finite && isfinite(c[k]);
     } else {
 #pragma unroll
         for (int k = 0; k < 8; ++k) c[k] = 0.0;
     }
+    // Finite corners and boundary points give no NaN distance, and there fmin is np.amin.  Otherwise (a NaN, or inf - inf)
+    // the tile takes nan_min, so that a NaN propagates as through np.amin.
     double best = INFINITY;
     for (int side = 0; side < 2; ++side) {
         const double *bd = side == 0 ? bound1 + (size_t)b * nb_max1 * bstride : bound2 + (size_t)b * nb_max2 * bstride;
-        int nb = side == 0 ? (nb1 ? nb1[b] : nb_max1) : (nb2 ? nb2[b] : nb_max2);
-        if (nb < 0) nb = 0;
+        const int nb = max(nbs[side], 0);
         for (int t0 = 0; t0 < nb; t0 += MB_TILE) {
             const int cnt = min(MB_TILE, nb - t0);
             __syncthreads();
+            bool staged_finite = true;
             for (int k = threadIdx.x; k < cnt; k += blockDim.x) {
                 sbx[k] = bd[(size_t)(t0 + k) * bstride];
                 sby[k] = bd[(size_t)(t0 + k) * bstride + 1];
+                staged_finite = staged_finite && isfinite(sbx[k]) && isfinite(sby[k]);
             }
-            __syncthreads();
-            if (live) {
+            const bool tile_finite = !__syncthreads_or(!staged_finite);
+            if (live && tile_finite && corners_finite && best == best) {     // (fmin would drop an earlier tile's NaN)
 #pragma unroll 4
                 for (int k = 0; k < cnt; ++k) {
                     const double bx = sbx[k], by = sby[k];
                     const double d0 = tc::dist2(bx, by, c[0], c[1]), d1 = tc::dist2(bx, by, c[2], c[3]);
                     const double d2 = tc::dist2(bx, by, c[4], c[5]), d3 = tc::dist2(bx, by, c[6], c[7]);
                     best = fmin(best, fmin(fmin(d0, d1), fmin(d2, d3)));
+                }
+            } else if (live) {
+                for (int k = 0; k < cnt; ++k) {
+                    const double bx = sbx[k], by = sby[k];
+                    const double d0 = tc::dist2(bx, by, c[0], c[1]), d1 = tc::dist2(bx, by, c[2], c[3]);
+                    const double d2 = tc::dist2(bx, by, c[4], c[5]), d3 = tc::dist2(bx, by, c[6], c[7]);
+                    best = tc::nan_min(best, tc::nan_min(tc::nan_min(d0, d1), tc::nan_min(d2, d3)));
                 }
             }
         }
@@ -125,8 +145,9 @@ __global__ void __launch_bounds__(MB_THREADS) min_bound_dists_kernel(int n_traj_
 
 // ---- extrema tested by check_traj ---------------------------------------------------------------------------------
 // extrema[b][0..7] = min(min_dists), max |kappa|, max ay, max ax_wo_drag, min ax_wo_drag, max a_tot, max vx, n points
-// PER_TRACK: drag and mass of trajectory b are drag_b[b], mass_b[b] (either may be NULL: the scalar); a mass that is not > 0
-// gives a row of NaN but for the number of points.  The arrays are the last parameters, as for min_bound_dists_kernel.
+// PER_TRACK: drag and mass of trajectory b are drag_b[b], mass_b[b] (either may be NULL: the scalar).  A mass that is not
+// > 0, or n_traj[b] > n_max, gives a row of NaN but for the number of points.  The arrays are the last parameters, as for
+// min_bound_dists_kernel.
 template <bool PER_TRACK>
 __global__ void __launch_bounds__(256) traj_extrema_kernel(int n_max, const int32_t *n_traj, const double *kappa,
                                                            const double *vx, const double *ax, const double *min_dists,
@@ -139,16 +160,23 @@ __global__ void __launch_bounds__(256) traj_extrema_kernel(int n_max, const int3
     if constexpr (PER_TRACK) {
         if (drag_b) dragcoeff = drag_b[b];
         if (mass_b) mass_veh = mass_b[b];
-        if (!(mass_veh > 0.0)) {
-            if (threadIdx.x < 8) extrema[(size_t)b * 8 + threadIdx.x] = threadIdx.x == 7 ? (double)n : NAN;
-            return;
-        }
     }
+    if (n > n_max || (PER_TRACK && !(mass_veh > 0.0))) {
+        if (threadIdx.x < 8) extrema[(size_t)b * 8 + threadIdx.x] = threadIdx.x == 7 ? (double)n : NAN;
+        return;
+    }
+    // min_dist and max |kappa| propagate a NaN (the reference tests them with np.amin / np.amax); the other maxima drop
+    // it (the reference tests them with np.any(x > limit))
     double mn_d = INFINITY, mx_k = -INFINITY, mx_ay = -INFINITY, mx_ax = -INFINITY, mn_ax = INFINITY, mx_at = -INFINITY,
            mx_v = -INFINITY;
-    for (int i = threadIdx.x; i < n && i < n_max; i += blockDim.x) {
+    bool nan_d = false, nan_k = false;
+    for (int i = threadIdx.x; i < n; i += blockDim.x) {
         const tc::PointChecks q = tc::point_checks(kappa[o + i], vx[o + i], ax[o + i], dragcoeff, mass_veh);
-        if (min_dists) mn_d = fmin(mn_d, min_dists[o + i]);
+        if (min_dists) {
+            mn_d = fmin(mn_d, min_dists[o + i]);
+            nan_d = nan_d || min_dists[o + i] != min_dists[o + i];
+        }
+        nan_k = nan_k || q.kappa_abs != q.kappa_abs;
         mx_k = fmax(mx_k, q.kappa_abs);
         mx_ay = fmax(mx_ay, q.ay);
         mx_ax = fmax(mx_ax, q.ax_wo_drag);
@@ -163,6 +191,8 @@ __global__ void __launch_bounds__(256) traj_extrema_kernel(int n_max, const int3
     mn_ax = block_reduce<2>(mn_ax, red);
     mx_at = block_reduce<1>(mx_at, red);
     mx_v = block_reduce<1>(mx_v, red);
+    if (__syncthreads_or(nan_d)) mn_d = NAN;
+    if (__syncthreads_or(nan_k)) mx_k = NAN;
     if (threadIdx.x == 0) {
         double *e = extrema + (size_t)b * 8;
         e[0] = mn_d; e[1] = mx_k; e[2] = mx_ay; e[3] = mx_ax; e[4] = mn_ax; e[5] = mx_at; e[6] = mx_v; e[7] = (double)n;
@@ -171,7 +201,8 @@ __global__ void __launch_bounds__(256) traj_extrema_kernel(int n_max, const int3
 
 // ---- trajectory_opt / traj_race_cl --------------------------------------------------------------------------------
 // traj[b][j][0..6] = s, x, y, psi, kappa, vx, ax for j < n; row n = row 0 with s = sum(spline_lengths) (closed race
-// trajectory); rows beyond stay untouched.
+// trajectory, summed left to right); rows beyond stay untouched.  A track with n <= 0, n > n_max or n_spl > n_spl_max is
+// refused: its rows stay untouched.
 __global__ void __launch_bounds__(256) assemble_trajectory_kernel(int n_max, const int32_t *n_traj, const double *s,
                                                                   const double *xy, const double *psi, const double *kappa,
                                                                   const double *vx, const double *ax, int n_spl_max,
@@ -179,7 +210,8 @@ __global__ void __launch_bounds__(256) assemble_trajectory_kernel(int n_max, con
                                                                   double *traj) {
     const int b = blockIdx.x;
     const int n = n_traj ? n_traj[b] : n_max;
-    if (n <= 0 || n > n_max) return;
+    const int ns = n_spl ? n_spl[b] : n_spl_max;
+    if (n <= 0 || n > n_max || ns > n_spl_max) return;
     const size_t o = (size_t)b * n_max;
     double *t = traj + (size_t)b * ((size_t)n_max + 1) * 7;
     for (int j = threadIdx.x; j < n; j += blockDim.x) {
@@ -188,7 +220,6 @@ __global__ void __launch_bounds__(256) assemble_trajectory_kernel(int n_max, con
         r[5] = vx[o + j]; r[6] = ax[o + j];
     }
     if (threadIdx.x == 0) {
-        const int ns = n_spl ? n_spl[b] : n_spl_max;
         double total = 0.0;
         for (int i = 0; i < ns; ++i) total += spline_lengths[(size_t)b * n_spl_max + i];
         double *r = t + (size_t)n * 7;

@@ -35,23 +35,36 @@ def check_traj(reftrack: np.ndarray, reftrack_normvec_normalized: np.ndarray, tr
     ext = _b.traj_extrema_batch(up(traj[:, 4]), up(traj[:, 5]), up(traj[:, 6]), dragcoeff, mass_veh)[0].cpu().numpy()
     kappa_max, ay_max, ax_max, ax_min, a_tot_max, vx_max = ext[1:7]
 
+    # The device maxima of ay, ax, a_tot and vx skip NaN points, as the reference's np.any(x > limit) tests do.  Its
+    # messages print np.amax / np.amin, which is nan if a point is, so a printed value is NaN where the trajectory's
+    # quantity has a NaN point.
+    def shown(x, q):
+        return np.nan if np.isnan(q).any() else x
+
+    k, v, a = traj[:, 4], traj[:, 5], traj[:, 6]
+    with np.errstate(divide="ignore", invalid="ignore"):
+        ay = np.power(v, 2) / np.abs(np.divide(1.0, k, out=np.full(k.shape[0], np.inf), where=k != 0))
+        ax_wo = a - (-np.power(v, 2) * dragcoeff / mass_veh)
+        a_tot = np.sqrt(np.power(ax_wo, 2) + np.power(ay, 2))
+
     if kappa_max > curvlim:
         print("WARNING: Curvature limit is exceeded: %.3frad/m" % kappa_max)
     if ggv is not None:
         ggv = np.asarray(ggv, dtype=np.float64)
         if ay_max > np.amax(ggv[:, 2]) + 0.1:
-            print("WARNING: Lateral ggv acceleration limit is exceeded: %.2fm/s2" % ay_max)
+            print("WARNING: Lateral ggv acceleration limit is exceeded: %.2fm/s2" % shown(ay_max, ay))
         if ax_max > np.amax(ggv[:, 1]) + 0.1:
-            print("WARNING: Longitudinal ggv acceleration limit (positive) is exceeded: %.2fm/s2" % ax_max)
+            print("WARNING: Longitudinal ggv acceleration limit (positive) is exceeded: %.2fm/s2" % shown(ax_max, ax_wo))
         if ax_min < np.amin(-ggv[:, 1]) - 0.1:
-            print("WARNING: Longitudinal ggv acceleration limit (negative) is exceeded: %.2fm/s2" % ax_min)
+            print("WARNING: Longitudinal ggv acceleration limit (negative) is exceeded: %.2fm/s2" % shown(ax_min, ax_wo))
         if a_tot_max > np.amax(ggv[:, 1:]) + 0.1:
-            print("WARNING: Total ggv acceleration limit is exceeded: %.2fm/s2" % a_tot_max)
+            print("WARNING: Total ggv acceleration limit is exceeded: %.2fm/s2" % shown(a_tot_max, a_tot))
     else:
         print("WARNING: Since ggv-diagram was not given the according checks cannot be performed!")
     if ax_max_machines is not None:
         if ax_max > np.amax(np.asarray(ax_max_machines, dtype=np.float64)[:, 1]) + 0.1:
-            print("WARNING: Longitudinal acceleration machine limits are exceeded: %.2fm/s2" % ax_max)
+            print("WARNING: Longitudinal acceleration machine limits are exceeded: %.2fm/s2" % shown(ax_max, ax_wo))
     if vx_max > v_max + 0.1:
-        print("WARNING: Maximum velocity of final trajectory exceeds the maximal velocity of the vehicle: %.2fm/s!" % vx_max)
+        print("WARNING: Maximum velocity of final trajectory exceeds the maximal velocity of the vehicle: %.2fm/s!"
+              % shown(vx_max, v))
     return bound_r, bound_l

@@ -512,6 +512,9 @@ int mc_interp_track_batch(int B, int n_max, const int32_t *n_pts, const double *
  *   min_dists [B][n_traj_max]
  *   length_veh_batch, width_veh_batch [B] or NULL : the vehicle size per trajectory (NULL: the scalars for all; each
  *                    array replaces its scalar alone)
+ * A NaN propagates as through np.amin: a NaN boundary point makes every min_dists entry of its trajectory NaN, a NaN
+ * trajectory point its own entry.  A trajectory with n_traj[b] > n_traj_max, nb1[b] > nb1_max or nb2[b] > nb2_max is
+ * refused alone: its whole min_dists row is NaN, and nothing outside its rows is read.
  */
 int mc_min_bound_dists_batch(int B, int n_traj_max, const int32_t *n_traj, const double *xy, const double *psi,
                              int nb1_max, const int32_t *nb1, const double *bound1, int nb2_max, const int32_t *nb2,
@@ -529,6 +532,9 @@ int mc_min_bound_dists_batch(int B, int n_traj_max, const int32_t *n_traj, const
  *                    replaces its scalar alone).  The scalar mass_veh must be > 0 unless mass_veh_batch is given; a
  *                    trajectory whose mass_veh_batch entry is not > 0 is refused alone: its row is NaN but for the
  *                    number of points.
+ * A trajectory with n_traj[b] > n_max is refused the same way.  min(min_dists) and max |kappa| are NaN if a point's is
+ * (the reference tests them with np.amin / np.amax); the other maxima and the minimum skip NaN points (the reference
+ * tests those with np.any(x > limit)).
  */
 int mc_traj_extrema_batch(int B, int n_max, const int32_t *n_traj, const double *kappa, const double *vx, const double *ax,
                           const double *min_dists, double dragcoeff, double mass_veh, double *extrema,
@@ -536,7 +542,8 @@ int mc_traj_extrema_batch(int B, int n_max, const int32_t *n_traj, const double 
                           void *stream);
 
 /* trajectory_opt / traj_race_cl of main_globaltraj.py:501-512: rows [s, x, y, psi, kappa, vx, ax];
- * row n_traj[b] closes the lap (copy of row 0 with s = sum(spline_lengths)).  traj [B][n_max + 1][7].
+ * row n_traj[b] closes the lap (copy of row 0 with s = sum(spline_lengths), summed left to right).  traj [B][n_max + 1][7].
+ * A track with n_traj[b] <= 0, n_traj[b] > n_max or n_spl[b] > n_spl_max is refused alone: its rows stay untouched.
  */
 int mc_assemble_trajectory_batch(int B, int n_max, const int32_t *n_traj, const double *s, const double *xy,
                                  const double *psi, const double *kappa, const double *vx, const double *ax,

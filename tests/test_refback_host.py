@@ -8,15 +8,12 @@ unmodified): this row is parity-PINNED.
 import contextlib
 import ctypes
 import io
-import os
-import shutil
-import subprocess
 
 import numpy as np
 import pytest
 
-from conftest import ROOT
 from global_racetrajectory_optimization_b200 import helper_funcs_glob as hf
+from refback_edge_cases import load_tc_host
 
 DP = ctypes.POINTER(ctypes.c_double)
 NAMES = ["berlin", "handling", "synth333"]
@@ -28,23 +25,9 @@ def _p(a):
 
 @pytest.fixture(scope="module")
 def tc(tmp_path_factory):
-    cxx = shutil.which("g++")
-    if cxx is None:
+    lib = load_tc_host(tmp_path_factory.mktemp("tc_host"))
+    if lib is None:
         pytest.skip("g++ not available")
-    so = str(tmp_path_factory.mktemp("tc_host") / "libtc_host.so")
-    subprocess.check_call([cxx, "-O2", "-ffp-contract=off", "-fPIC", "-shared", "-x", "c++", "-std=c++17", "-o", so,
-                           os.path.join(ROOT, "tests", "host_harness", "tc_host.cpp")])
-    lib = ctypes.CDLL(so)
-    lib.tc_host_interp_track.restype = ctypes.c_int
-    lib.tc_host_interp_track.argtypes = [ctypes.c_int, DP, ctypes.c_int, DP, ctypes.c_double, ctypes.c_int, ctypes.c_double,
-                                         ctypes.c_int, DP]
-    lib.tc_host_min_bound_dists.restype = None
-    lib.tc_host_min_bound_dists.argtypes = [ctypes.c_int, DP, DP, ctypes.c_int, DP, ctypes.c_int, DP, ctypes.c_int,
-                                            ctypes.c_double, ctypes.c_double, DP]
-    lib.tc_host_normals_crossing.restype = ctypes.c_int
-    lib.tc_host_normals_crossing.argtypes = [ctypes.c_int, DP, DP, ctypes.c_int]
-    lib.tc_host_extrema.restype = None
-    lib.tc_host_extrema.argtypes = [ctypes.c_int, DP, DP, DP, DP, ctypes.c_double, ctypes.c_double, DP]
     return lib
 
 
@@ -73,11 +56,11 @@ def test_min_bound_dists_and_extrema_statements_reproduce_the_reference(golden, 
     br, bl = np.ascontiguousarray(r["bound_r_interp"]), np.ascontiguousarray(r["bound_l_interp"])
     md = np.zeros(tr.shape[0])
     tc.tc_host_min_bound_dists(tr.shape[0], _p(xy), _p(psi), br.shape[0], _p(br), bl.shape[0], _p(bl), 4,
-                               float(r["length_veh"]), float(r["width_veh"]), _p(md))
+                               float(r["length_veh"]), float(r["width_veh"]), _p(md), None)
     assert np.abs(md - r["min_dists_full"]).max() <= 1e-12
     b1, b2 = np.ascontiguousarray(br[:1]), np.ascontiguousarray(bl[:1])                     # what check_traj.py:58-68 passes
     tc.tc_host_min_bound_dists(tr.shape[0], _p(xy), _p(psi), 1, _p(b1), 1, _p(b2), 4, float(r["length_veh"]),
-                               float(r["width_veh"]), _p(md))
+                               float(r["width_veh"]), _p(md), None)
     assert np.abs(md - r["min_dists_as_called"]).max() <= 1e-12
     # the quantities of check_traj.py:93-131, formed exactly like the reference forms them
     k, v, a = (np.ascontiguousarray(tr[:, c]) for c in (4, 5, 6))

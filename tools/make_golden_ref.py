@@ -16,7 +16,10 @@ Inputs: the raceline of the committed fixtures (tests/golden/<name>.npz, made by
 profile of oracle/tph_velprofile.py, assembled into the trajectory array exactly like
 the reference's main_globaltraj.py:501-512.
 
-    MC_REFERENCE_DIR=<reference checkout> python tools/make_golden_ref.py
+    MC_REFERENCE_DIR=<reference checkout> python tools/make_golden_ref.py [edges]
+
+With ``edges`` only tests/golden/refback_edges.npz is written: constructed cases where the K6 kernels change code path
+(see edges() below), each run through the same unmodified helpers.
 """
 from __future__ import annotations
 
@@ -136,5 +139,185 @@ def main():
     np.savez_compressed(os.path.join(GOLD, "refback_import_track.npz"), **imp)
 
 
+def _normals(xy):
+    """Unit normals (tangent of the neighbours turned right) of a closed polyline; any unit vectors would do."""
+    t = np.roll(xy, -1, axis=0) - np.roll(xy, 1, axis=0)
+    for alt in (np.roll(xy, -1, axis=0) - xy, xy - np.roll(xy, 1, axis=0)):     # 2 points, repeated points
+        t = np.where(np.all(t == 0.0, axis=1)[:, None], alt, t)
+    n = np.column_stack((t[:, 1], -t[:, 0]))
+    return n / np.sqrt(np.sum(n * n, axis=1))[:, None]
+
+
+def _ring(rng, n, r, jitter, smooth=False):
+    """n points around a circle of radius r (radius jittered by a factor up to 1 +- jitter), random widths 1 .. 3 m (with
+    smooth, the same at every point, so that the boundaries stay as short as the ring)"""
+    ang = 2.0 * np.pi * np.arange(n) / n
+    rad = r * (1.0 + jitter * rng.uniform(-1.0, 1.0, n))
+    xy = np.round(np.column_stack((rad * np.cos(ang), rad * np.sin(ang))) * 4096.0) / 4096.0    # (a smaller fixture)
+    w = np.round(rng.uniform(1.0, 3.0, (1 if smooth else n, 2)) * 64.0) / 64.0
+    return np.column_stack((xy, np.broadcast_to(w, (n, 2))))
+
+
+IT_STEPS = (1.0, 2.5, 0.1 / 3)
+
+
+def edge_interp_tracks(rng):
+    """name -> (track [n, 4], its steps: IT_STEPS, and a step longer than the lap for some)"""
+    sq = np.array([[0.0, 0.0, 1.0, 2.0], [10.0, 0.0, 1.5, 1.0], [10.0, 10.0, 2.0, 1.5], [0.0, 10.0, 1.0, 1.0]])
+    return {
+        "n2": (np.array([[0.0, 0.0, 1.0, 2.0], [3.0, 4.0, 1.5, 2.5]]), IT_STEPS + (1000.0,)),          # lap 10 m: multiples of 1, 2.5
+        "n3": (np.array([[0.0, 0.0, 1.0, 1.0], [4.0, 0.0, 1.2, 0.8], [0.0, 3.0, 0.9, 1.1]]), IT_STEPS),  # lap 12 m
+        "ring127": (_ring(rng, 127, 3.0, 0.1), IT_STEPS + (1000.0,)),
+        "ring128": (_ring(rng, 128, 3.0, 0.1), IT_STEPS),
+        "ring129": (_ring(rng, 129, 3.0, 0.1), IT_STEPS),
+        "ring3000": (_ring(rng, 3000, 20.0, 0.0, smooth=True) , (1.0, 2.5, 0.7)),        # lap ~126 m
+        "square10": (sq, IT_STEPS),                                                               # lap 40 m
+        "repeat": (np.array([[0.0, 0.0, 1.0, 1.0], [4.0, 0.0, 1.0, 1.0], [4.0, 0.0, 2.0, 3.0], [4.0, 3.0, 1.5, 1.0],
+                             [0.0, 3.0, 1.0, 2.0]]), IT_STEPS),                             # zero-length element
+        "offset": (sq + np.array([1e5, 1e5, 0.0, 0.0]), IT_STEPS),
+        "ring_offset": (_ring(rng, 16, 3.0, 0.1) + np.array([1e5, -1e5, 0.0, 0.0]), IT_STEPS),
+    }
+
+
+MB_SIZES = (1, 511, 512, 513, 1024, 1025, 1537)
+MB_NTRAJ = (1, 127, 128, 129, 257)
+MB_PSI = {"p_half_pi": np.pi / 2, "m_half_pi": -np.pi / 2, "p_pi": np.pi, "m_pi": -np.pi, "three": 3.0}
+
+
+def edge_min_bound_dists_cases(rng):
+    """list of dicts: xy [n, 2], psi [n], bounds [nb, 2] (split into bound1 = bounds[:s], bound2 = bounds[s:] for every s
+    in splits), length, width, near (index of the planted nearest boundary point, -1 for none)."""
+    ang = 2.0 * np.pi * np.arange(1537) / 1537
+    base = np.round(np.column_stack((60.0 * np.cos(ang), 60.0 * np.sin(ang))) * 64.0) / 64.0     # far from the car
+    near = np.array([0.15625, 0.3125])                                  # closer to every corner than any base point
+    cases, c = [], 0
+    for nb in MB_SIZES:
+        for k in sorted({0, 511, 512, 513, nb - 1} & set(range(nb))):
+            n = MB_NTRAJ[c % len(MB_NTRAJ)]
+            c += 1
+            b = base[:nb].copy()
+            b[k] = near
+            cases.append(dict(tag=f"nb{nb}_k{k}", xy=np.round(rng.uniform(-0.5, 0.5, (n, 2)) * 256.0) / 256.0,
+                              psi=np.zeros(n), bounds=b, length=4.7, width=2.0, near=k,
+                              splits=sorted({nb, nb // 2, 1, min(512, nb), 0} & set(range(nb + 1)))))
+    b = base[:1025].copy()
+    b[700] = near
+    for tag, psi in MB_PSI.items():
+        cases.append(dict(tag="psi_" + tag, xy=rng.uniform(-0.5, 0.5, (257, 2)), psi=np.full(257, psi), bounds=b,
+                          length=4.7, width=2.0, near=700, splits=[600]))
+    cases.append(dict(tag="psi_mixed", xy=rng.uniform(-40.0, 40.0, (257, 2)), psi=rng.uniform(-np.pi, np.pi, 257),
+                      bounds=base, length=4.7, width=2.0, near=-1, splits=[768]))
+    cases.append(dict(tag="spread", xy=np.round(rng.uniform(-50.0, 50.0, (257, 2)) * 256.0) / 256.0, psi=np.zeros(257),
+                      bounds=base, length=4.7, width=2.0, near=-1, splits=[0, 511, 1025, 1537]))
+    b = base[:513].copy()
+    b[512] = near
+    cases.append(dict(tag="zero_vehicle", xy=np.round(rng.uniform(-0.5, 0.5, (129, 2)) * 256.0) / 256.0, psi=np.zeros(129),
+                      bounds=b, length=0.0, width=0.0, near=512, splits=[513, 200]))
+    b = base[:513].copy()
+    b[300, 0] = np.nan
+    cases.append(dict(tag="nan_bound", xy=rng.uniform(-0.5, 0.5, (129, 2)), psi=np.zeros(129), bounds=b, length=4.7,
+                      width=2.0, near=-1, splits=[513, 300, 301]))
+    xy = rng.uniform(-0.5, 0.5, (128, 2))
+    xy[5, 1] = np.nan
+    cases.append(dict(tag="nan_traj", xy=xy, psi=np.zeros(128), bounds=base[:1024], length=4.7, width=2.0, near=-1,
+                      splits=[1024, 512]))
+    return cases
+
+
+def edge_check_traj_cases(rng):
+    """(reftrack, normvec, name -> trajectory [n, 7]): trajectories along a 30 m circle inside the reftrack's corridor."""
+    rt = _ring(rng, 40, 30.0, 0.0)
+    rt[:, 2:] = rng.uniform(3.0, 4.0, (40, 2))
+    nv = _normals(rt[:, :2])
+
+    def lap(n, v_lo=20.0, v_hi=40.0):
+        a = 2.0 * np.pi * np.arange(n) / max(n, 1)
+        s = 30.0 * a
+        return np.column_stack((s, 30.0 * np.cos(a), 30.0 * np.sin(a), a + np.pi / 2, np.full(n, 1.0 / 30.0),
+                                rng.uniform(v_lo, v_hi, n), rng.uniform(-8.0, 6.0, n)))
+
+    tr = {}
+    t = lap(100)
+    t[::7, 4] = 0.0                                                     # kappa exactly 0: radius inf, ay 0
+    tr["kappa_zero"] = t
+    t = lap(100)
+    t[:, 6] = rng.uniform(-12.0, -2.0, 100)                             # ax_wo_drag < 0 everywhere
+    tr["ax_negative"] = t
+    t = lap(100)
+    t[:, 5] = 0.0
+    t[::3, 4] = 0.0                                                     # v = 0 (and 0 / inf)
+    tr["v_zero"] = t
+    for n in (1, 255, 256, 257):
+        tr[f"n{n}"] = lap(n)
+    t = lap(100)
+    t[10, 4] = np.nan
+    tr["nan_kappa"] = t
+    t = lap(100, 20.0, 80.0)
+    t[20, 5] = np.nan
+    tr["nan_vx"] = t
+    return rt, nv, tr
+
+
+def edges():
+    """tests/golden/refback_edges.npz: the reference's interp_track, calc_min_bound_dists and check_traj on constructed
+    cases (tile edges, block-reduction sizes, exact-multiple laps, zero-length elements, NaN)."""
+    hf = load_reference_helpers()
+    from oracle import tph_velprofile as VP
+    rng = np.random.default_rng(20261018)
+    out = dict(numpy_version=np.array(np.__version__))
+    names = []
+    for name, (rt, steps) in edge_interp_tracks(rng).items():
+        names.append(name)
+        nv = _normals(rt[:, :2])
+        out[f"it_{name}_track"], out[f"it_{name}_normvec"] = rt, nv
+        out[f"it_{name}_steps"] = np.array(steps)
+        for i, step in enumerate(steps):
+            out[f"it_{name}_{i}"] = hf.src.interp_track.interp_track(reftrack=rt, stepsize_approx=step)
+        for side, bound in (("r", rt[:, :2] + nv * np.expand_dims(rt[:, 2], 1)),          # check_traj.py:50-55
+                            ("l", rt[:, :2] - nv * np.expand_dims(rt[:, 3], 1))):
+            out[f"it_{name}_bound_{side}"] = hf.src.interp_track.interp_track(
+                reftrack=np.column_stack((bound, np.zeros((bound.shape[0], 2)))), stepsize_approx=1.0)
+    out["it_names"] = np.array(names)
+    cases = edge_min_bound_dists_cases(rng)
+    for i, c in enumerate(cases):
+        traj = np.column_stack((np.zeros(c["xy"].shape[0]), c["xy"], c["psi"]))
+        res = [hf.src.calc_min_bound_dists.calc_min_bound_dists(trajectory=traj, bound1=c["bounds"][:s],
+                                                                bound2=c["bounds"][s:], length_veh=c["length"],
+                                                                width_veh=c["width"]) for s in c["splits"]]
+        out.update({f"mb_{i}_xy": c["xy"], f"mb_{i}_psi": c["psi"], f"mb_{i}_bounds": c["bounds"],
+                    f"mb_{i}_splits": np.array(c["splits"], dtype=np.int64), f"mb_{i}_out": np.array(res),
+                    f"mb_{i}_veh": np.array([c["length"], c["width"]]), f"mb_{i}_near": np.array(c["near"]),
+                    f"mb_{i}_tag": np.array(c["tag"])})
+    out["mb_count"] = np.array(len(cases))
+    ggv_file = os.path.join(REF, "inputs", "veh_dyn_info", "ggv.csv")
+    ggv, axm = VP.import_veh_dyn_info(ggv_file, os.path.join(REF, "inputs", "veh_dyn_info", "ax_max_machines.csv"))
+    veh = dict(v_max=70.0, length=4.7, width=2.0, mass=1200.0, dragcoeff=0.75, curvlim=0.12)   # params/racecar.ini:44-50
+    tight = dict(v_max=30.0, curvlim=0.02, ggv=ggv * np.array([1.0, 0.5, 0.5]), ax_max_machines=axm * np.array([1.0, 0.5]))
+    rt, nv, trs = edge_check_traj_cases(rng)
+    out.update(ct_reftrack=rt, ct_normvec=nv, ct_names=np.array(list(trs)), ct_ggv=ggv, ct_ax_max_machines=axm,
+               ct_veh=np.array([veh[k] for k in ("v_max", "length", "width", "mass", "dragcoeff", "curvlim")]),
+               ct_tight_ggv=tight["ggv"], ct_tight_ax_max_machines=tight["ax_max_machines"],
+               ct_tight_v_max=np.array(tight["v_max"]), ct_tight_curvlim=np.array(tight["curvlim"]))
+    for name, tr in trs.items():
+        out[f"ct_{name}"] = tr
+        for tag, kw in (("stock", {}), ("tight", tight)):
+            args = dict(reftrack=rt, reftrack_normvec_normalized=nv, length_veh=veh["length"], width_veh=veh["width"],
+                        debug=True, trajectory=tr, ggv=ggv, ax_max_machines=axm, v_max=veh["v_max"],
+                        curvlim=veh["curvlim"], mass_veh=veh["mass"], dragcoeff=veh["dragcoeff"])
+            args.update(kw)
+            buf = io.StringIO()
+            with contextlib.redirect_stdout(buf), np.errstate(all="ignore"):
+                hf.src.check_traj.check_traj(**args)
+            out[f"ct_{name}_{tag}_stdout"] = np.array(buf.getvalue())
+    path = os.path.join(GOLD, "refback_edges.npz")
+    np.savez_compressed(path, **out)
+    print(f"  refback_edges: {len(names)} interp_track tracks, {len(cases)} calc_min_bound_dists cases, {len(trs)} "
+          f"check_traj trajectories, {os.path.getsize(path)} bytes (numpy {np.__version__})")
+
+
 if __name__ == "__main__":
-    main()
+    if sys.argv[1:] == ["edges"]:
+        edges()
+    else:
+        main()
+        edges()
