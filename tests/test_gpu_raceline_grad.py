@@ -14,7 +14,7 @@ from global_racetrajectory_optimization_b200 import _lib, batch as B_, synth
 pytestmark = pytest.mark.gpu
 DEV = "cuda"
 VEH = dict(drag_coeff=0.75, m_veh=1200.0)
-REF_TOL = 1e-8          # |device - reference| / max |reference| per gradient; measured on the H100: see DESIGN.md 3.12
+REF_TOL = 1e-10         # |device - reference| / max |reference| per gradient; measured 7.1e-12 (n = 4000) on an H100 80GB HBM3
 STEP = 2.0
 # |central difference - chain gradient| / |chain gradient| per track.  The difference runs through the QP solvers, whose
 # active sets are not held (the raceline's station segments and the profile's decisions are): measured on the H100,
@@ -75,6 +75,7 @@ def _reference_errors(golden, big):
 
 def test_adjoint_matches_the_torch_reference_in_every_regime_of_the_moment_solve(golden):
     for n, e in _reference_errors(golden, (2500, 4000)):
+        print(f"  n={n}: measured {max(e):.3e}, bound {REF_TOL:.0e}")
         assert max(e) <= REF_TOL, (n, e)
 
 
