@@ -25,6 +25,7 @@ from . import _lib
 SLAB_VECTORS, _CONSTS = _lib.slab_mirror()
 HB_PITCH, ZB_PITCH = _CONSTS["HB_PITCH"], _CONSTS["ZB_PITCH"]
 N_MIN = _CONSTS["N_MIN"]     # smallest closed track the banded solver supports
+N_DENSE_MAX = _lib.header_define(_lib._build.HEADER, "MC_DENSE_N_MAX")    # largest the dense small-track solver takes
 STATUS_TEXT = {
     0: "ok",
     1: "Problem not solvable, track might be too small to run with current safety distance!",
@@ -203,17 +204,19 @@ def _launch_chunks(entry: str, B: int, chunk: int, ws: torch.Tensor, *args) -> N
         _call(entry, e - s, *(a(s, e) if callable(a) else a for a in args), ws=ws)
 
 
-def _mincurv_inputs(tracks: dict, shape_error: str, n_pts, w_veh, centre_id, max_chunk, f_scale) -> SimpleNamespace:
+def _mincurv_inputs(tracks: dict, shape_error: str, n_pts, w_veh, centre_id, max_chunk, f_scale,
+                    small: bool = False) -> SimpleNamespace:
     """The checked and normalised inputs of opt_min_curv_batch and opt_min_curv_diff.  tracks: name -> (tensor, cols), every
     tensor [B, n_max, cols] ([B, n_max] for cols None; the first fixes B and n_max).  Returns a namespace of the tracks as
     contiguous float64 CUDA tensors, B, n_max, dev, n_pts, w_scalar and w_batch (see _wveh), centre_id (int32 or None),
-    f_scale (None: F_SCALE) and chunk, the instances per launch."""
+    f_scale (None: F_SCALE) and chunk, the instances per launch.  small: the dense solver takes the tracks below N_MIN,
+    so n_max < N_MIN is accepted (its workspace is then 0 bytes per instance)."""
     t = {name: _f64(x, name) for name, (x, _) in tracks.items()}
     first = next(iter(t.values()))
     B, n_max = first.shape[:2]
     if any(t[name].shape != (B, n_max) + ((cols,) if cols else ()) for name, (_, cols) in tracks.items()):
         raise RuntimeError(shape_error)
-    if n_max < N_MIN:
+    if n_max < N_MIN and not small:
         raise NotImplementedError(f"closed tracks with fewer than {N_MIN} points are not supported by the banded solver")
     dev = first.device
     n_pts = _npts(n_pts, B, dev)
@@ -239,7 +242,8 @@ def _mincurv_results(B: int, n_max: int, dev) -> dict:
 def opt_min_curv_batch(reftrack: torch.Tensor, normvec: torch.Tensor, h: torch.Tensor,
                        kappa_bound: Union[float, torch.Tensor], w_veh: Union[float, torch.Tensor], n_pts: Optional[torch.Tensor] = None,
                        max_chunk: Optional[int] = None, f_scale: Optional[float] = None,
-                       centre_id: Optional[torch.Tensor] = None, lin_alpha: Optional[torch.Tensor] = None) -> dict:
+                       centre_id: Optional[torch.Tensor] = None, lin_alpha: Optional[torch.Tensor] = None,
+                       small_tracks: bool = False, _dense_below: int = 0) -> dict:
     """Batched tph.opt_min_curv (closed tracks).  Returns a dict of device tensors:
     alpha [B, n_max], curv_error_max [B], kappa_lin_max [B], status [B] (int32), iters [B] (int32).
     f_scale: None = the module default F_SCALE (see there).
@@ -255,12 +259,20 @@ def opt_min_curv_batch(reftrack: torch.Tensor, normvec: torch.Tensor, h: torch.T
     results are then bit for bit those of the call with its own limit as the float, with the same chunking; status 4 and
     the curvature-row phase follow each instance's limit.  A host tensor must hold finite limits > 0; in a device tensor
     (not read on the host) an instance whose limit is not finite or not > 0 gets status -1 and the others are untouched.
-    With a tensor the solve goes through mc_mincurv_solve_batch_ex, which runs the same stages with kappa_bound_batch."""
+    With a tensor the solve goes through mc_mincurv_solve_batch_ex, which runs the same stages with kappa_bound_batch.
+    small_tracks: also solve the closed tracks with 3 <= n < N_MIN points, which the banded solver refuses (status -1), by
+    the dense small-track kernel (DESIGN.md section 3.14): the same QP, statuses and outputs; n_max < N_MIN is then
+    accepted.  Every launch goes through mc_mincurv_solve_batch_ex; tracks of N_MIN points or more get what they get
+    without the flag, bit for bit.  A follower of centre_id is checked as on the banded path and assembles its own QP.
+    _dense_below (tests only): the dense kernel takes the tracks below this count instead (N_MIN .. N_DENSE_MAX + 1), so
+    that the two solvers can be compared on the same track."""
     _require_cuda()
+    dense_below = int(_dense_below) if _dense_below else (N_MIN if small_tracks else 0)
     if lin_alpha is not None and (lin_alpha.shape != h.shape):
         raise ValueError(f"opt_min_curv_batch: lin_alpha must be [B, n_max] like h, got {tuple(lin_alpha.shape)}")
     a = _mincurv_inputs(dict(reftrack=(reftrack, 4), normvec=(normvec, 2), h=(h, None)),
-                        "Array size of reftrack should be the same as normvectors!", n_pts, w_veh, centre_id, max_chunk, f_scale)
+                        "Array size of reftrack should be the same as normvectors!", n_pts, w_veh, centre_id, max_chunk, f_scale,
+                        small=dense_below != 0)
     out = _mincurv_results(a.B, a.n_max, a.dev)
     kb, kbb = _kappa_bound(kappa_bound, a.B, a.dev)
     if lin_alpha is not None:
@@ -278,13 +290,13 @@ def opt_min_curv_batch(reftrack: torch.Tensor, normvec: torch.Tensor, h: torch.T
         ws = _workspace("mincurv", _lib.load().mc_mincurv_workspace_bytes(a.chunk, a.n_max), a.dev)
         _launch_chunks("mc_mincurv_solve_batch_ex", a.B, a.chunk, ws, a.n_max, *map(_rows, (a.n_pts, a.reftrack, a.normvec,
                        a.h)), kb, a.w_scalar, _rows(a.w_batch), a.f_scale, *map(_rows, out.values()), 0.0, None, None,
-                       _rows(lin), _rows(kbb), *(None,) * 5)
+                       _rows(lin), _rows(kbb), *(None,) * 5, dense_below)
         if invalid is not None:
             out["status"] = torch.where(invalid, -1, out["status"]).to(torch.int32)
         return out
-    if kbb is not None:
+    if kbb is not None or dense_below:
         _mincurv_per_instance(a.chunk, a.n_pts, a.reftrack, a.normvec, a.h, kbb, a.w_scalar, a.w_batch, a.f_scale,
-                              a.centre_id, out.values())
+                              a.centre_id, out.values(), kb=kb, dense_below=dense_below)
         return out
     _mincurv_launch("mc_mincurv_solve_batch_shared", a.chunk, a.n_pts, a.reftrack, a.normvec, a.h, kb,
                     a.w_scalar, a.w_batch, a.f_scale, a.centre_id, *out.values())
@@ -292,16 +304,17 @@ def opt_min_curv_batch(reftrack: torch.Tensor, normvec: torch.Tensor, h: torch.T
 
 
 def _mincurv_per_instance(chunk: int, n_pts, reftrack, normvec, h, kbb, w_scalar, w_batch, f_scale, centre_id, outputs,
-                          export=(None,) * 4) -> None:
+                          export=(None,) * 4, kb: float = 0.0, dense_below: int = 0) -> None:
     """mc_mincurv_solve_batch_shared, or with export (sens, grad_status, sens_rows, n_rows) mc_mincurv_solve_batch_sens,
     with a curvature limit per instance (kbb [B]), which those entries do not take: mc_mincurv_solve_batch_ex runs the
     same solve with kappa_bound_batch, centre ids and the export, on chunks of at most chunk instances (centre ids
-    re-indexed inside each chunk).  outputs: alpha, curv_error_max, kappa_lin_max, status, iters."""
+    re-indexed inside each chunk).  outputs: alpha, curv_error_max, kappa_lin_max, status, iters.  With dense_below (and
+    kbb None: the scalar limit kb) the same solve with the dense small-track kernel below that count."""
     B, n_max = h.shape
     ws = _workspace("mincurv", _lib.load().mc_mincurv_workspace_bytes(chunk, n_max), h.device)
-    _launch_chunks("mc_mincurv_solve_batch_ex", B, chunk, ws, n_max, *map(_rows, (n_pts, reftrack, normvec, h)), 0.0,
+    _launch_chunks("mc_mincurv_solve_batch_ex", B, chunk, ws, n_max, *map(_rows, (n_pts, reftrack, normvec, h)), kb,
                    w_scalar, _rows(w_batch), f_scale, *map(_rows, outputs), 0.0, None, None, None, _rows(kbb),
-                   _chunk_centre_ids(centre_id, B), *map(_rows, export))
+                   _chunk_centre_ids(centre_id, B), *map(_rows, export), dense_below)
 
 
 def shared_centre_ids(group: torch.Tensor) -> torch.Tensor:
@@ -705,7 +718,7 @@ def scale_alpha_batch(alpha: torch.Tensor, scale: Union[float, torch.Tensor]) ->
 def iqp_batch(reftrack: torch.Tensor, normvec: torch.Tensor, h: torch.Tensor, kappa_bound: Union[float, torch.Tensor],
               w_veh: Union[float, torch.Tensor], stepsize_interp: float, iters_min: int = 3,
               curv_error_allowed: float = 0.01, n_pts: Optional[torch.Tensor] = None, max_iters: int = 50,
-              fixed_iters: Optional[int] = None, _n_cap_min: int = 0) -> dict:
+              fixed_iters: Optional[int] = None, _n_cap_min: int = 0, small_tracks: bool = False) -> dict:
     """Batched tph.iqp_handler (SURVEY.md A.5): per-instance outer iterations with damping and
     re-linearisation; an instance leaves the loop once iter >= iters_min and its curv_error_max <=
     curv_error_allowed.  Returns dict(alpha [B, n_cap], reftrack [B, n_cap, 4], normvec [B, n_cap, 2],
@@ -719,7 +732,10 @@ def iqp_batch(reftrack: torch.Tensor, normvec: torch.Tensor, h: torch.Tensor, ka
     with the larger capacity, which the 5 % + 50 m of slack makes a rare event).
 
     kappa_bound: a float or a [B] tensor of one limit per instance, as for opt_min_curv_batch (every QP of an instance
-    takes its own limit)."""
+    takes its own limit).
+
+    small_tracks: every QP also solves the tracks below N_MIN points (opt_min_curv_batch(small_tracks=True)), including
+    those whose re-sampled raceline drops below N_MIN part-way."""
     _require_cuda()
     reftrack0, normvec0, h0 = reftrack, normvec, h           # (the caller's arrays: never written)
     reftrack = _f64(reftrack, "reftrack").clone()
@@ -757,7 +773,8 @@ def iqp_batch(reftrack: torch.Tensor, normvec: torch.Tensor, h: torch.Tensor, ka
     while True:
         it += 1
         n_cur_max = reftrack.shape[1]
-        res = opt_min_curv_batch(reftrack, normvec, h, kappa_bound, w_veh, n_pts=cur_n)     # (finished tracks: n_pts = 0, skipped)
+        res = opt_min_curv_batch(reftrack, normvec, h, kappa_bound, w_veh, n_pts=cur_n,      # (finished tracks: n_pts = 0,
+                                 small_tracks=small_tracks)                                 #  skipped)
         qp_solves += n_active
         alpha = res["alpha"]
         if it < iters_min:
@@ -798,7 +815,7 @@ def iqp_batch(reftrack: torch.Tensor, normvec: torch.Tensor, h: torch.Tensor, ka
         if n_min < 0:         # a re-sampled track did not fit: its later iterations ran on nothing -- repeat with room for it
             return iqp_batch(reftrack0, normvec0, h0, kappa_bound, w_veh, stepsize_interp, iters_min=iters_min,
                              curv_error_allowed=curv_error_allowed, n_pts=n_pts, max_iters=max_iters,
-                             fixed_iters=fixed_iters, _n_cap_min=-n_min + 64)
+                             fixed_iters=fixed_iters, _n_cap_min=-n_min + 64, small_tracks=small_tracks)
     fin["qp_solves"] = qp_solves
     return fin
 

@@ -192,7 +192,7 @@ int mc_mincurv_solve_batch(int B, int n_max, const int32_t *n_pts, const double 
                            void *workspace, size_t workspace_bytes, void *stream) {
     return mc_mincurv_solve_batch_ex(B, n_max, n_pts, reftrack, normvec, h, kappa_bound, w_veh, w_veh_batch, MC_F_SCALE_DEFAULT,
                                      alpha, curv_error_max, kappa_lin_max, status, iters, 0.0, nullptr, nullptr, nullptr,
-                                     nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, workspace, workspace_bytes, stream);
+                                     nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, 0, workspace, workspace_bytes, stream);
 }
 
 // the projection QP: setup -> prox -> pdip -> finalize -> kappa (with prox_mu) -> finalize
@@ -266,18 +266,36 @@ int mc_mincurv_solve_batch_ex(int B, int n_max, const int32_t *n_pts, const doub
                               double *alpha, double *curv_error_max, double *kappa_lin_max, int32_t *status, int32_t *iters,
                               double prox_mu, const double *prox_x, const double *prox_q, const double *lin_alpha,
                               const double *kappa_bound_batch, const int32_t *centre_id, double *sens, int32_t *grad_status,
-                              double *sens_rows, int32_t *n_rows, void *workspace, size_t workspace_bytes, void *stream) {
+                              double *sens_rows, int32_t *n_rows, int dense_below, void *workspace, size_t workspace_bytes,
+                              void *stream) {
     if (!sens != !grad_status) return bad("mc_mincurv_solve_batch_ex: sens and grad_status go together");
     if (!sens_rows != !n_rows || (sens_rows && !sens))
         return bad("mc_mincurv_solve_batch_ex: sens_rows and n_rows go together, and with sens");
     if (prox_x && (centre_id || sens)) return bad("mc_mincurv_solve_batch_ex: prox_x takes neither centre_id nor sens");
+    if (dense_below != 0) {
+        if (dense_below < mc::N_MIN || dense_below > MC_DENSE_N_MAX + 1)
+            return bad("mc_mincurv_solve_batch_ex: dense_below must be 0 or in [%d, %d]", mc::N_MIN, MC_DENSE_N_MAX + 1);
+        if (prox_x || sens) return bad("mc_mincurv_solve_batch_ex: dense_below takes neither prox_x nor sens");
+        if (B <= 0 || n_max <= 0) return bad("mc_mincurv_solve_batch_ex: B <= 0 or n_max <= 0");
+        if (!reftrack || !normvec || !h || !alpha || !curv_error_max || !status)
+            return bad("mc_mincurv_solve_batch_ex: NULL argument");
+        if (!(f_scale > 0.0)) return bad("mc_mincurv_solve_batch_ex: f_scale must be positive");
+    }
     if (prox_x)
         return mincurv_prox_solve(B, n_max, n_pts, reftrack, normvec, h, kappa_bound, w_veh, w_veh_batch, f_scale, alpha,
                                   curv_error_max, kappa_lin_max, status, iters, prox_mu, prox_x, prox_q, lin_alpha,
                                   kappa_bound_batch, workspace, workspace_bytes, stream);
-    return mincurv_solve(B, n_max, n_pts, reftrack, normvec, h, kappa_bound, w_veh, w_veh_batch, f_scale, centre_id, alpha,
-                         curv_error_max, kappa_lin_max, status, iters, sens, grad_status, sens_rows, n_rows, lin_alpha,
-                         kappa_bound_batch, workspace, workspace_bytes, stream);
+    const bool banded = dense_below == 0 || n_max >= mc::N_MIN;
+    if (banded) {
+        const int rc = mincurv_solve(B, n_max, n_pts, reftrack, normvec, h, kappa_bound, w_veh, w_veh_batch, f_scale, centre_id,
+                                     alpha, curv_error_max, kappa_lin_max, status, iters, sens, grad_status, sens_rows, n_rows,
+                                     lin_alpha, kappa_bound_batch, workspace, workspace_bytes, stream);
+        if (rc || dense_below == 0) return rc;
+    }
+    // the small tracks: the dense kernel, last on the stream
+    return mc::mincurv_dense(B, n_max, dense_below, banded, n_pts, reftrack, normvec, h, kappa_bound, kappa_bound_batch, w_veh,
+                             w_veh_batch, f_scale, centre_id, lin_alpha, alpha, curv_error_max, kappa_lin_max, status, iters,
+                             stream);
 }
 
 int mc_mincurv_solve_batch_shared(int B, int n_max, const int32_t *n_pts, const double *reftrack, const double *normvec,

@@ -90,6 +90,14 @@ int mincurv_finalize(int B, int n_max, const int32_t *n_pts, const double *alpha
                      double *kappa_lin_max, int32_t *status, bool lin, const double *kappa_bound_batch, void *workspace,
                      size_t workspace_bytes, void *stream);
 
+// the dense small-track kernel (mincurv_dense.cu) of mc_mincurv_solve_batch_ex on the instances with
+// 3 <= n_pts[b] < dense_below; banded: the banded stages ran before it on this batch.  Not exported.
+__attribute__((visibility("hidden")))
+int mincurv_dense(int B, int n_max, int dense_below, bool banded, const int32_t *n_pts, const double *reftrack,
+                  const double *normvec, const double *h, double kappa_bound, const double *kappa_bound_batch, double w_veh,
+                  const double *w_veh_batch, double f_scale, const int32_t *centre_id, const double *lin_alpha, double *alpha,
+                  double *curv_error_max, double *kappa_lin_max, int32_t *status, int32_t *iters, void *stream);
+
 __device__ __forceinline__ double *vec(double *slab, const Layout &L, int v) { return slab + (size_t)v * L.np; }
 
 // index of the instance whose slab holds this instance's band of H: its own, or with shared centre lines the owner's

@@ -28,7 +28,7 @@ def default_pars() -> dict:
 
 def globaltraj_batch(reftrack: torch.Tensor, opt_type: str, pars: dict, ggv=None, ax_max_machines=None,
                      n_pts: Optional[torch.Tensor] = None, check: bool = True, refine: Optional[dict] = None,
-                     vehicles: Optional[_b.Vehicles] = None, veh_id=None) -> dict:
+                     vehicles: Optional[_b.Vehicles] = None, veh_id=None, small_tracks: bool = False) -> dict:
     """Runs the flow for every track of ``reftrack`` [B, n_max, 4] (prepared tracks: what prep_track returns).
 
     Returns a dict of device tensors: alpha, reftrack / normvec / n_pts (of the last QP: they change for 'mincurv_iqp'),
@@ -54,7 +54,11 @@ def globaltraj_batch(reftrack: torch.Tensor, opt_type: str, pars: dict, ggv=None
     car's scalar ``pars`` and tables alone.  For each car's limit pass it per track, e.g.
     ``refine={"metric_length": 10.0, "kappa_bound": vehicles.per_track("curvlim", vehicles.veh_id(veh_id, B, dev))}``.
     Still one per call: dyn_model_exp, the filter window, the step sizes and the iterative
-    QP's options."""
+    QP's options.
+
+    ``small_tracks``: the 'mincurv' and 'mincurv_iqp' QPs also solve the tracks below batch.N_MIN points (the dense
+    small-track solver, batch.opt_min_curv_batch); without it those get status -1.  'shortest_path' takes every size
+    anyway.  With ``refine`` a solved short track is refined as the refinement documents for tracks below N_MIN."""
     if opt_type not in ("mincurv", "mincurv_iqp", "shortest_path"):
         raise IOError("Unknown optimization type!" if opt_type != "mintime" else
                       "opt_type 'mintime' (CasADi/IPOPT NLP) is outside the CUDA path")
@@ -67,11 +71,12 @@ def globaltraj_batch(reftrack: torch.Tensor, opt_type: str, pars: dict, ggv=None
     cx, cy, nv, h = _b.calc_splines_batch(reftrack, n_pts=n_pts, want_coeffs=False)
     rt_used, nv_used, n_used = reftrack, nv, n_pts
     if opt_type == "mincurv":
-        qp = _b.opt_min_curv_batch(reftrack, nv, h, car.curvlim, car.width_opt, n_pts=n_pts)
+        qp = _b.opt_min_curv_batch(reftrack, nv, h, car.curvlim, car.width_opt, n_pts=n_pts, small_tracks=small_tracks)
         alpha, status = qp["alpha"], qp["status"]
     elif opt_type == "mincurv_iqp":
         qp = _b.iqp_batch(reftrack, nv, h, car.curvlim, car.width_opt, steps["stepsize_reg"],
-                          iters_min=opt["iqp_iters_min"], curv_error_allowed=opt["iqp_curverror_allowed"], n_pts=n_pts)
+                          iters_min=opt["iqp_iters_min"], curv_error_allowed=opt["iqp_curverror_allowed"], n_pts=n_pts,
+                          small_tracks=small_tracks)
         alpha, status = qp["alpha"], qp["status"]
         rt_used, nv_used, n_used = qp["reftrack"], qp["normvec"], qp["n_pts"]
     else:

@@ -503,7 +503,7 @@ class CurvatureProjection:
                               *map(_b._rows, (self._n(mask), self.reftrack, self.normvec, self.h)), self.kb, self.w_scalar,
                               _b._rows(self.w_batch), _b.F_SCALE, *map(_b._rows, out.values()), self.mu,
                               _b._rows(x.contiguous()), _b._rows(q.contiguous()), _b._rows(self.lin),
-                              _b._rows(self.kb_batch), *(None,) * 5)
+                              _b._rows(self.kb_batch), *(None,) * 5, 0)
             ok = mask & self.launchable & (out["status"] == 0) & torch.isfinite(out["alpha"]).all(dim=1)
             return out["alpha"], ok
 

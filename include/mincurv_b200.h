@@ -49,6 +49,10 @@ extern "C" {
  * and mc_mincurv_solve_batch_sens, whose signatures keep the scalar limit.  The binding lets a call leave out the
  * MC_OPTIONAL3 parameters alone, or them and each earlier group in turn. */
 #define MC_OPTIONAL3
+/* MC_OPTIONAL4 marks parameters added after the MC_OPTIONAL3 ones, alike 0 / NULL-able: on mc_mincurv_solve_batch_ex, the
+ * dense solver of small closed tracks (dense_below).  The binding lets a call leave out the MC_OPTIONAL4 parameters alone,
+ * or them and each earlier group in turn. */
+#define MC_OPTIONAL4
 
 #define MC_STATUS_OK 0
 #define MC_STATUS_TOO_NARROW 1
@@ -63,6 +67,9 @@ extern "C" {
  *                      quadratic term does not; 1.0 would be the consistent Gauss-Newton scaling)
  *   decel_slice_upper  tph.calc_vel_profile (closed): which half of the doubled lap is kept after the backward pass */
 #define MC_F_SCALE_DEFAULT 2.0
+/* largest closed track the dense small-track solver of mc_mincurv_solve_batch_ex takes (dense_below <= MC_DENSE_N_MAX + 1):
+ * its E and normal matrix, MC_DENSE_N_MAX^2 doubles each, and its vectors fill one CTA's 227 KB of shared memory */
+#define MC_DENSE_N_MAX 108
 #define MC_VP_DECEL_SLICE_UPPER_DEFAULT 1
 
 /* library version (major*10000 + minor*100 + patch) and last CUDA error text of this thread */
@@ -139,7 +146,16 @@ int mc_mincurv_solve_batch(int B, int n_max, const int32_t *n_pts,
  *                    together, sens_rows and n_rows together and only with them), as documented there.  This entry is
  *                    the one way to those two solves with kappa_bound_batch: their own signatures keep the scalar limit
  *                    (a parameter before their workspace would change what existing callers' argument lists bind to).
- *                    Not with prox_x. */
+ *                    Not with prox_x.
+ *   dense_below (0: none of this): the closed tracks with 3 <= n_pts[b] < dense_below are solved by the dense small-track
+ *                    kernel (DESIGN.md section 3.14), N_MIN (80) <= dense_below <= MC_DENSE_N_MAX + 1.  It runs last on the
+ *                    stream and owns every output of those instances; the banded stages (which give the ones below N_MIN
+ *                    status -1) are launched only if n_max >= N_MIN, so that n_max < N_MIN is accepted, with any workspace
+ *                    (NULL and 0 bytes included).  The dense kernel solves the full QP of tph.opt_min_curv without band
+ *                    truncation: the bounds, the statuses -1 and 1, kappa_bound_batch, w_veh_batch and lin_alpha as above;
+ *                    a follower of centre_id is checked as above and then assembled on its own.  Status 2 and 3 as for
+ *                    the banded solve; status 4 when the rows are still violated at the end (whatever ended it).  dense_below > N_MIN lets the two
+ *                    solvers be compared on the same instance.  Not with prox_x or the sensitivity export. */
 int mc_mincurv_solve_batch_ex(int B, int n_max, const int32_t *n_pts,
                               const double *reftrack, const double *normvec, const double *h,
                               double kappa_bound, double w_veh, const double *w_veh_batch, double f_scale,
@@ -150,6 +166,7 @@ int mc_mincurv_solve_batch_ex(int B, int n_max, const int32_t *n_pts,
                               MC_OPTIONAL3 const double *kappa_bound_batch, MC_OPTIONAL3 const int32_t *centre_id,
                               MC_OPTIONAL3 double *sens, MC_OPTIONAL3 int32_t *grad_status, MC_OPTIONAL3 double *sens_rows,
                               MC_OPTIONAL3 int32_t *n_rows,
+                              MC_OPTIONAL4 int dense_below,
                               void *workspace, size_t workspace_bytes, void *stream);
 
 /* the same for batches in which several instances share a centreline (x, y, normal vectors, h and n_pts identical, only
