@@ -397,12 +397,14 @@ mincurv_dense_kernel(int n_max, int m, int dense_below, int banded, const int32_
     __syncthreads();
     tri_solve2(LFW, INVD, H, U0, U1, W0, W1, ZX, ZY, n);
     double kmax = 0.0, emax = 0.0, viol = 0.0;
+    bool nan_k = false, nan_e = false;           // (both maxima propagate a NaN, as in mincurv_finalize_kernel)
     for (int i = threadIdx.x; i < n; i += DENSE_THREADS) {
         const int ip1 = (i + 1 == n) ? 0 : i + 1;
         const double hi = H[i], h2 = hi * hi;
         const double zx = ZX[i], zy = ZY[i];
         const double kl = fabs(KR[i] + SY[i] * zy - SX[i] * zx);
         kmax = fmax(kmax, kl);
+        nan_k = nan_k || kl != kl;
         if (!(kl <= kb * (1.0 + 1e-7))) viol = 1.0;         // (a NaN iterate counts as a violation)
         const double ddx = h2 * (MX[i] + zx), ddy = h2 * (MY[i] + zy);
         const double xp = XP[i], yp = YP[i];
@@ -417,10 +419,13 @@ mincurv_dense_kernel(int n_max, int m, int dense_below, int banded, const int32_
         const double c0 = (xp * ddy - yp * ddx) / (q0 * sqrt(q0));
         const double c1 = (xpt * ddy - ypt * ddx) / (q1 * sqrt(q1));
         emax = fmax(emax, fabs(c1 - c0));
+        nan_e = nan_e || c1 - c0 != c1 - c0;
     }
     kmax = block_reduce<1>(kmax, red);
     emax = block_reduce<1>(emax, red);
     viol = block_reduce<1>(viol, red);
+    if (__syncthreads_or(nan_k)) kmax = NAN;
+    if (__syncthreads_or(nan_e)) emax = NAN;
     if (threadIdx.x == 0) {
         curv_error_max[b] = emax;
         if (kappa_lin_max) kappa_lin_max[b] = kmax;

@@ -56,13 +56,17 @@ mincurv_finalize_kernel(int n_max, const int32_t *__restrict__ n_pts, double *__
     }
     __syncthreads();
     tri_solve2(LFW, INVD, H, T0, T1, T2, T3, ZX, ZY, n);
+    // both maxima propagate a NaN as tph's np.amax does (fmax drops it, and the chunked solve confines a NaN of alpha to
+    // about 64 points around it, so the maximum over the others would be finite)
     double kmax = 0.0, emax = 0.0;
+    bool nan_k = false, nan_e = false;
     for (int i = threadIdx.x; i < n; i += blockDim.x) {
         const int ip1 = (i + 1 == n) ? 0 : i + 1;
         const double hi = H[i], h2 = hi * hi;
         const double zx = ZX[i], zy = ZY[i];
         const double klin = KREF[i] + SY[i] * zy - SX[i] * zx;
         kmax = fmax(kmax, fabs(klin));
+        nan_k = nan_k || klin != klin;
         const double ddx = h2 * (MX[i] + zx), ddy = h2 * (MY[i] + zy);
         const double xp = XP[i], yp = YP[i];
         double xc = xp, yc = yp;                // first derivatives of the centre line
@@ -76,9 +80,12 @@ mincurv_finalize_kernel(int n_max, const int32_t *__restrict__ n_pts, double *__
         const double c0 = (xp * ddy - yp * ddx) / (q0 * sqrt(q0));
         const double c1 = (xpt * ddy - ypt * ddx) / (q1 * sqrt(q1));
         emax = fmax(emax, fabs(c1 - c0));
+        nan_e = nan_e || c1 - c0 != c1 - c0;
     }
     kmax = block_reduce<1>(kmax, red);
     emax = block_reduce<1>(emax, red);
+    if (__syncthreads_or(nan_k)) kmax = NAN;
+    if (__syncthreads_or(nan_e)) emax = NAN;
     if (threadIdx.x == 0) {
         curv_error_max[b] = emax;
         if (kappa_lin_max) kappa_lin_max[b] = kmax;

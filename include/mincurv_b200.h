@@ -197,7 +197,12 @@ int mc_mincurv_setup_batch_shared(int B, int n_max, const int32_t *n_pts, const 
  * mc_mincurv_solve_batch is exactly setup -> pdip -> finalize.  Exposed so that a caller can time or
  * overlap the stages; arguments as above.  The finalize stage of a workspace assembled about a linearisation point
  * (lin_alpha of mc_mincurv_setup_batch_ex) needs linearised = 1: the line P + alpha n takes the centre line's first
- * derivatives, the linearised curvature those of the linearisation point. */
+ * derivatives, the linearised curvature those of the linearisation point.
+ * mc_mincurv_finalize_batch, per instance: status 1 or negative gives kappa_lin_max = curv_error_max = 0 and leaves the
+ * status (with kappa_bound_batch a limit that is not finite or not > 0 first turns a status >= 0 into -1); otherwise
+ * kappa_lin_max = max |k_ref + E alpha| and curv_error_max = max |kappa_sol_lin - kappa_orig_lin| over the n points, each
+ * NaN if any of its terms is NaN (as tph's np.amax; a NaN or infinite alpha makes both NaN), and status 0 becomes 4
+ * iff kappa_lin_max > kappa_bound * (1 + 1e-7) in float64 (a NaN maximum leaves 0); statuses 2, 3 and 4 are kept. */
 int mc_mincurv_setup_batch(int B, int n_max, const int32_t *n_pts, const double *reftrack, const double *normvec,
                            const double *h, double w_veh, const double *w_veh_batch, int32_t *status,
                            void *workspace, size_t workspace_bytes, void *stream);
