@@ -371,7 +371,7 @@ class _MinCurvDiff(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, widths, w_veh_t, centre, normvec, h, kappa_bound, w_scalar, n_pts, centre_id, chunk, f_scale, strict,
-                curvature_rows, kappa_bound_t):
+                curvature_rows, kappa_bound_t, dense_below):
         B, n_max, _ = centre.shape
         dev = centre.device
         reftrack = torch.cat((centre, widths), dim=2).contiguous()
@@ -380,15 +380,16 @@ class _MinCurvDiff(torch.autograd.Function):
         grad_status = torch.empty((B,), dtype=torch.int32, device=dev)
         sens_rows = torch.empty((B, n_max), dtype=torch.float64, device=dev) if curvature_rows else None
         n_rows = torch.empty((B,), dtype=torch.int32, device=dev) if curvature_rows else None
-        if kappa_bound_t is None:
+        if kappa_bound_t is None and not dense_below:
             _mincurv_launch("mc_mincurv_solve_batch_sens", chunk, n_pts, reftrack, normvec, h, kappa_bound, w_scalar,
                             w_veh_t, f_scale, centre_id, alpha, cerr, kmax, status, iters, sens, grad_status, sens_rows,
                             n_rows)
         else:
             _mincurv_per_instance(chunk, n_pts, reftrack, normvec, h, kappa_bound_t, w_scalar, w_veh_t, f_scale, centre_id,
-                                  (alpha, cerr, kmax, status, iters), (sens, grad_status, sens_rows, n_rows))
+                                  (alpha, cerr, kmax, status, iters), (sens, grad_status, sens_rows, n_rows), kb=kappa_bound,
+                                  dense_below=dense_below)
         ctx.save_for_backward(widths, centre, normvec, h, w_veh_t, n_pts, centre_id, sens, grad_status, sens_rows, n_rows)
-        ctx.w_scalar, ctx.chunk, ctx.f_scale, ctx.strict = w_scalar, chunk, f_scale, strict
+        ctx.w_scalar, ctx.chunk, ctx.f_scale, ctx.strict, ctx.dense_below = w_scalar, chunk, f_scale, strict, dense_below
         ctx.mark_non_differentiable(cerr, kmax, status, iters, grad_status)
         return alpha, cerr, kmax, status, iters, grad_status
 
@@ -416,16 +417,17 @@ class _MinCurvDiff(torch.autograd.Function):
             schur = torch.empty((chunk, max(cap * cap, 1)), dtype=torch.float64, device=dev)
             rows = (sens_rows, n_rows, lambda s, e: schur, cap)
         _mincurv_launch("mc_mincurv_adjoint_batch", chunk, n_pts, reftrack, normvec, h, None, ctx.w_scalar, w_veh_t,
-                        ctx.f_scale, centre_id, sens, gs, grad_alpha, gwr, gwl, gwv, *rows, None)
+                        ctx.f_scale, centre_id, sens, gs, grad_alpha, gwr, gwl, gwv, *rows, None, ctx.dense_below)
         _refuse(ctx.strict, wanted, gs, who, "whose adjoint factorisation broke down")
-        return (torch.stack((gwr, gwl), dim=2), gwv if w_veh_t is not None else None) + (None,) * 12
+        return (torch.stack((gwr, gwl), dim=2), gwv if w_veh_t is not None else None) + (None,) * 13
 
 
 @_device_guard
 def opt_min_curv_diff(centre: torch.Tensor, widths: torch.Tensor, normvec: torch.Tensor, h: torch.Tensor,
                       kappa_bound: Union[float, torch.Tensor], w_veh: Union[float, torch.Tensor], n_pts: Optional[torch.Tensor] = None,
                       centre_id: Optional[torch.Tensor] = None, max_chunk: Optional[int] = None,
-                      f_scale: Optional[float] = None, strict: bool = True, curvature_rows: bool = False) -> dict:
+                      f_scale: Optional[float] = None, strict: bool = True, curvature_rows: bool = False,
+                      small_tracks: bool = False, _dense_below: int = 0) -> dict:
     """opt_min_curv_batch with alpha differentiable with respect to the track widths and the vehicle width (autograd).
 
     centre [B, n_max, 2] (x, y) and widths [B, n_max, 2] (w_tr_right, w_tr_left) make up the reftrack of
@@ -443,18 +445,27 @@ def opt_min_curv_diff(centre: torch.Tensor, widths: torch.Tensor, normvec: torch
     solve status (4 only where the rows stay violated), and the backward reads the largest count of strongly active rows
     once from the device to size their Schur complements.  The forward's values are those of curvature_rows=False bit
     for bit, and so are the gradients of the instances the box phase solved.
-    kappa_bound: a float or a [B] tensor, as for opt_min_curv_batch (a constant: not differentiated)."""
+    kappa_bound: a float or a [B] tensor, as for opt_min_curv_batch (a constant: not differentiated).
+    small_tracks=True (with curvature_rows=True): the closed tracks with 3 <= n < N_MIN points are solved by the dense
+    small-track kernel, as by opt_min_curv_batch(small_tracks=True) (the same values bit for bit), and differentiated at
+    its final iterate by a dense adjoint (DESIGN.md section 3.14); n_max < N_MIN is then accepted.  The dense iterate
+    always carries the curvature rows, so it is only differentiable with them.  Tracks of N_MIN points or more get what
+    they get without the flag.  _dense_below (tests only): as for opt_min_curv_batch."""
     _require_cuda()
+    dense_below = int(_dense_below) if _dense_below else (N_MIN if small_tracks else 0)
+    if dense_below and not curvature_rows:
+        raise ValueError("opt_min_curv_diff: small_tracks needs curvature_rows=True (the dense small-track solver's "
+                         "iterate is differentiated with its curvature rows)")
     for t, name in ((centre, "centre"), (normvec, "normvec"), (h, "h")):
         if isinstance(t, torch.Tensor) and t.requires_grad:
             raise ValueError(f"opt_min_curv_diff: {name} is a constant (no gradient with respect to it); detach it")
     a = _mincurv_inputs(dict(centre=(centre, 2), widths=(widths, 2), normvec=(normvec, 2), h=(h, None)),
                         "opt_min_curv_diff: centre and widths must be [B, n_max, 2], normvec [B, n_max, 2], h [B, n_max]",
-                        n_pts, w_veh, centre_id, max_chunk, f_scale)
+                        n_pts, w_veh, centre_id, max_chunk, f_scale, small=dense_below != 0)
     kb, kbb = _kappa_bound(kappa_bound, a.B, a.dev)
     alpha, cerr, kmax, status, iters, grad_status = _MinCurvDiff.apply(
         a.widths, a.w_batch, a.centre, a.normvec, a.h, kb, a.w_scalar, a.n_pts, a.centre_id, a.chunk,
-        a.f_scale, bool(strict), bool(curvature_rows), kbb)
+        a.f_scale, bool(strict), bool(curvature_rows), kbb, dense_below)
     return dict(alpha=alpha, curv_error_max=cerr, kappa_lin_max=kmax, status=status, iters=iters, grad_status=grad_status)
 
 

@@ -105,63 +105,19 @@ __device__ void dense_solve(const double *L, int m, int n, double *r, double *x)
 __device__ __forceinline__ double d_affine_step(double r) { return (r > 1.0) ? 1.0 / r : 1.0; }
 __device__ __forceinline__ double d_damped_step(double eta, double r) { return (eta < r) ? eta / r : 1.0; }
 
-// banded: the banded stages ran on this batch (they own the status of every instance outside [3, dense_below)); otherwise
-// this kernel writes the refusal (status -1) of instances with n < 3 or n > n_max too.
+// The QP of one instance in shared memory (mincurv_setup.cu P1-P5): bounds LB / UB, the spline quantities, E, k_ref and
+// f = f_scale E^T k_ref; false (every thread alike) when a box is empty (lb > ub: status 1).  LIN: about the line P + la n.
+// Called by every thread of the CTA; its scratch lives in the iterate vectors D_AL .. D_L4.
 template <bool LIN>
-__global__ void __launch_bounds__(DENSE_THREADS)
-mincurv_dense_kernel(int n_max, int m, int dense_below, int banded, const int32_t *__restrict__ n_pts,
-                     const double *__restrict__ reftrack, const double *__restrict__ normvec, const double *__restrict__ hin,
-                     double kappa_bound, const double *__restrict__ kappa_bound_batch, double w_veh,
-                     const double *__restrict__ w_veh_batch, double f_scale, const int32_t *__restrict__ centre_id,
-                     const double *__restrict__ lin_alpha, PdipParams prm, double *__restrict__ alpha,
-                     double *__restrict__ curv_error_max, double *__restrict__ kappa_lin_max, int32_t *__restrict__ status,
-                     int32_t *__restrict__ iters) {
-    const int b = blockIdx.x;
-    const int n = n_pts ? n_pts[b] : n_max;
-    __shared__ double red[32];
-    __shared__ int s_flag;
-    extern __shared__ __align__(16) double s_dense[];
-    double *aout = alpha + (size_t)b * n_max;
-    // the outputs of a refused instance: those of the banded path (alpha 0 over the whole row, no iterations)
-    auto refuse = [&](int st) {
-        for (int i = threadIdx.x; i < n_max; i += DENSE_THREADS) aout[i] = 0.0;
-        if (threadIdx.x == 0) {
-            status[b] = st;
-            curv_error_max[b] = 0.0;
-            if (kappa_lin_max) kappa_lin_max[b] = 0.0;
-            if (iters) iters[b] = 0;
-        }
-    };
-    const bool owned = n >= 3 && n < dense_below && n <= n_max;
-    if (!owned) {
-        if (!banded && (n < 3 || n > n_max)) refuse(-1);
-        return;
-    }
-    if (centre_id && centre_id[b] != b) {       // a follower: the banded path's validity rule; its QP is assembled here
-        const int o = centre_id[b];
-        if (o < 0 || o >= (int)gridDim.x || centre_id[o] != o || (n_pts ? n_pts[o] : n_max) != n) { refuse(-1); return; }
-    }
-    const double wv = w_veh_batch ? w_veh_batch[b] : w_veh;
-    const double kb = kappa_bound_batch ? kappa_bound_batch[b] : kappa_bound;
-    if (!(fabs(wv) < INFINITY) || !(kb > 0.0 && kb < INFINITY)) { refuse(-1); return; }
-
-    double *E = s_dense, *K = s_dense + (size_t)m * m;
+__device__ __forceinline__ bool dense_assemble(double *s_dense, int m, int n, const double *rt, const double *nv,
+                                               const double *hb, const double *la, double wv, double f_scale, int &s_flag) {
+    double *E = s_dense;
     auto dv = [&](int v) { return s_dense + 2 * (size_t)m * m + (size_t)v * m; };
     double *PX = dv(D_PX), *PY = dv(D_PY), *NX = dv(D_NX), *NY = dv(D_NY), *H = dv(D_H), *LFW = dv(D_LFW);
     double *INVD = dv(D_INVD), *MX = dv(D_MX), *MY = dv(D_MY), *XP = dv(D_XP), *YP = dv(D_YP), *SX = dv(D_SX);
     double *SY = dv(D_SY), *KR = dv(D_KR), *LB = dv(D_LB), *UB = dv(D_UB), *F = dv(D_F);
-    double *AL = dv(D_AL), *LU = dv(D_LU), *LL = dv(D_LL), *SU = dv(D_SU), *SL = dv(D_SL), *S3 = dv(D_S3);
-    double *S4 = dv(D_S4), *L3 = dv(D_L3), *L4 = dv(D_L4), *KL = dv(D_KL), *DX = dv(D_DX), *ED = dv(D_ED);
-    double *RHS = dv(D_RHS), *DD = dv(D_DD), *WK = dv(D_WK), *TU = dv(D_TU), *TL = dv(D_TL), *T3 = dv(D_T3);
-    double *T4 = dv(D_T4), *VV = dv(D_VV), *ETV = dv(D_ETV);
-    // assembly scratch (in the iterate vectors)
     double *DG = dv(D_AL), *DFW = dv(D_LU), *DBW = dv(D_LL), *T0 = dv(D_SU), *T1 = dv(D_SL), *Y0 = dv(D_S3);
     double *Y1 = dv(D_S4), *Z0 = dv(D_L3), *Z1 = dv(D_L4);
-
-    const double *rt = reftrack + (size_t)b * n_max * 4;
-    const double *nv = normvec + (size_t)b * n_max * 2;
-    const double *hb = hin + (size_t)b * n_max;
-    const double *la = LIN ? lin_alpha + (size_t)b * n_max : nullptr;
 
     // ---- bounds (mincurv_setup.cu P1) ----
     if (threadIdx.x == 0) s_flag = 0;
@@ -180,7 +136,7 @@ mincurv_dense_kernel(int n_max, int m, int dense_below, int banded, const int32_
         LB[i] = lb; UB[i] = ub;
     }
     __syncthreads();
-    if (s_flag) { refuse(1); return; }
+    if (s_flag) return false;
 
     // ---- spline quantities (mincurv_setup.cu P2-P5) ----
     tri_pivots(DG, H, DFW, DBW, n);
@@ -247,6 +203,81 @@ mincurv_dense_kernel(int n_max, int m, int dense_below, int banded, const int32_
     dense_Et(E, m, n, KR, F);
     for (int i = threadIdx.x; i < n; i += DENSE_THREADS) F[i] *= f_scale;
     __syncthreads();
+    return true;
+}
+
+// a follower of centre_id: the banded path's validity rule (its QP is assembled on its own all the same)
+__device__ __forceinline__ bool dense_follower_ok(const int32_t *centre_id, const int32_t *n_pts, int n_max, int b, int n) {
+    const int o = centre_id[b];
+    return !(o < 0 || o >= (int)gridDim.x || centre_id[o] != o || (n_pts ? n_pts[o] : n_max) != n);
+}
+
+// banded: the banded stages ran on this batch (they own the status of every instance outside [3, dense_below)); otherwise
+// this kernel writes the refusal (status -1) of instances with n < 3 or n > n_max too.
+// EXPORT: the row export of mincurv_sens_rows_export_kernel for the instances this kernel writes the status of: the final
+// iterate's sens[b] = (lu / su, ll / sl), sens_rows[b] = l3 / s3 + l4 / s4, n_rows[b] = #{weight > 1} and grad_status[b]
+// = status[b]; zeros beyond n and wherever the status is not 0.  It is written before the post-solve quantities, which
+// take the iterate vectors as scratch.
+template <bool LIN, bool EXPORT>
+__global__ void __launch_bounds__(DENSE_THREADS)
+mincurv_dense_kernel(int n_max, int m, int dense_below, int banded, const int32_t *__restrict__ n_pts,
+                     const double *__restrict__ reftrack, const double *__restrict__ normvec, const double *__restrict__ hin,
+                     double kappa_bound, const double *__restrict__ kappa_bound_batch, double w_veh,
+                     const double *__restrict__ w_veh_batch, double f_scale, const int32_t *__restrict__ centre_id,
+                     const double *__restrict__ lin_alpha, PdipParams prm, double *__restrict__ alpha,
+                     double *__restrict__ curv_error_max, double *__restrict__ kappa_lin_max, int32_t *__restrict__ status,
+                     int32_t *__restrict__ iters, double *__restrict__ sens, double *__restrict__ sens_rows,
+                     int32_t *__restrict__ n_rows, int32_t *__restrict__ grad_status) {
+    const int b = blockIdx.x;
+    const int n = n_pts ? n_pts[b] : n_max;
+    __shared__ double red[32];
+    __shared__ int s_flag;
+    extern __shared__ __align__(16) double s_dense[];
+    double *aout = alpha + (size_t)b * n_max;
+    double *du = EXPORT ? sens + (size_t)b * 2 * n_max : nullptr, *dl = du + n_max;
+    double *wr = EXPORT ? sens_rows + (size_t)b * n_max : nullptr;
+    auto export_zeros = [&]() {
+        for (int i = threadIdx.x; i < n_max; i += DENSE_THREADS) { du[i] = 0.0; dl[i] = 0.0; wr[i] = 0.0; }
+        if (threadIdx.x == 0) n_rows[b] = 0;
+    };
+    // the outputs of a refused instance: those of the banded path (alpha 0 over the whole row, no iterations)
+    auto refuse = [&](int st) {
+        for (int i = threadIdx.x; i < n_max; i += DENSE_THREADS) aout[i] = 0.0;
+        if constexpr (EXPORT) export_zeros();
+        if (threadIdx.x == 0) {
+            status[b] = st;
+            curv_error_max[b] = 0.0;
+            if (kappa_lin_max) kappa_lin_max[b] = 0.0;
+            if (iters) iters[b] = 0;
+            if constexpr (EXPORT) grad_status[b] = st;
+        }
+    };
+    const bool owned = n >= 3 && n < dense_below && n <= n_max;
+    if (!owned) {
+        if (!banded && (n < 3 || n > n_max)) refuse(-1);
+        return;
+    }
+    if (centre_id && centre_id[b] != b && !dense_follower_ok(centre_id, n_pts, n_max, b, n)) { refuse(-1); return; }
+    const double wv = w_veh_batch ? w_veh_batch[b] : w_veh;
+    const double kb = kappa_bound_batch ? kappa_bound_batch[b] : kappa_bound;
+    if (!(fabs(wv) < INFINITY) || !(kb > 0.0 && kb < INFINITY)) { refuse(-1); return; }
+
+    double *E = s_dense, *K = s_dense + (size_t)m * m;
+    auto dv = [&](int v) { return s_dense + 2 * (size_t)m * m + (size_t)v * m; };
+    double *PX = dv(D_PX), *PY = dv(D_PY), *NX = dv(D_NX), *NY = dv(D_NY), *H = dv(D_H), *LFW = dv(D_LFW);
+    double *INVD = dv(D_INVD), *MX = dv(D_MX), *MY = dv(D_MY), *XP = dv(D_XP), *YP = dv(D_YP), *SX = dv(D_SX);
+    double *SY = dv(D_SY), *KR = dv(D_KR), *LB = dv(D_LB), *UB = dv(D_UB), *F = dv(D_F);
+    double *AL = dv(D_AL), *LU = dv(D_LU), *LL = dv(D_LL), *SU = dv(D_SU), *SL = dv(D_SL), *S3 = dv(D_S3);
+    double *S4 = dv(D_S4), *L3 = dv(D_L3), *L4 = dv(D_L4), *KL = dv(D_KL), *DX = dv(D_DX), *ED = dv(D_ED);
+    double *RHS = dv(D_RHS), *DD = dv(D_DD), *WK = dv(D_WK), *TU = dv(D_TU), *TL = dv(D_TL), *T3 = dv(D_T3);
+    double *T4 = dv(D_T4), *VV = dv(D_VV), *ETV = dv(D_ETV);
+
+    const double *rt = reftrack + (size_t)b * n_max * 4;
+    const double *nv = normvec + (size_t)b * n_max * 2;
+    const double *hb = hin + (size_t)b * n_max;
+    const double *la = LIN ? lin_alpha + (size_t)b * n_max : nullptr;
+
+    if (!dense_assemble<LIN>(s_dense, m, n, rt, nv, hb, la, wv, f_scale, s_flag)) { refuse(1); return; }
 
     // ---- interior point on the box and the curvature rows (the iteration of mincurv_pdip_kappa_kernel) ----
     const double m4 = 4.0 * n;
@@ -382,6 +413,19 @@ mincurv_dense_kernel(int n_max, int m, int dense_below, int banded, const int32_
         if (mu <= 1e-2 * prm.mu_rel * mu0) { result = (rdmax <= 1e3 * rd_tol && rpmax <= 1e-6 * kb) ? 0 : 2; ++it; break; }
     }
     for (int i = threadIdx.x; i < n_max; i += DENSE_THREADS) aout[i] = (i < n) ? AL[i] : 0.0;
+    if constexpr (EXPORT) {         // (status 4 from the post-solve check zeroes it again below)
+        const int ne = (result == 0) ? n : 0;
+        double strong = 0.0;
+        for (int i = threadIdx.x; i < n_max; i += DENSE_THREADS) {
+            const double w = (i < ne) ? L3[i] / S3[i] + L4[i] / S4[i] : 0.0;
+            du[i] = (i < ne) ? LU[i] / SU[i] : 0.0;
+            dl[i] = (i < ne) ? LL[i] / SL[i] : 0.0;
+            wr[i] = w;
+            strong += (w > 1.0) ? 1.0 : 0.0;
+        }
+        strong = block_reduce<0>(strong, red);
+        if (threadIdx.x == 0) n_rows[b] = (int32_t)strong;
+    }
 
     // ---- post-solve quantities (mincurv_finalize_kernel) ----
     double *U0 = dv(D_LU), *U1 = dv(D_LL), *W0 = dv(D_SU), *W1 = dv(D_SL), *ZX = dv(D_S3), *ZY = dv(D_S4);
@@ -426,6 +470,10 @@ mincurv_dense_kernel(int n_max, int m, int dense_below, int banded, const int32_
     viol = block_reduce<1>(viol, red);
     if (__syncthreads_or(nan_k)) kmax = NAN;
     if (__syncthreads_or(nan_e)) emax = NAN;
+    if constexpr (EXPORT) {
+        if (result == 0 && viol > 0.0) export_zeros();
+        if (threadIdx.x == 0) grad_status[b] = (viol > 0.0) ? 4 : result;
+    }
     if (threadIdx.x == 0) {
         curv_error_max[b] = emax;
         if (kappa_lin_max) kappa_lin_max[b] = kmax;
@@ -434,11 +482,193 @@ mincurv_dense_kernel(int n_max, int m, int dense_below, int banded, const int32_
     }
 }
 
+// A = C C^T in place (lower triangle, row-major with leading dimension lda), every thread of the CTA; false on a
+// non-positive pivot
+__device__ bool dense_chol(double *A, int lda, int n) {
+    for (int j = 0; j < n; ++j) {
+        __syncthreads();
+        const double p = A[(size_t)j * lda + j];
+        if (!(p > 0.0)) return false;          // (every thread reads the same pivot: the exit is uniform)
+        const double c = sqrt(p), ic = 1.0 / c;
+        __syncthreads();
+        if (threadIdx.x == 0) A[(size_t)j * lda + j] = c;
+        for (int i = j + 1 + threadIdx.x; i < n; i += DENSE_THREADS) A[(size_t)i * lda + j] *= ic;
+        __syncthreads();
+        const int r = n - j - 1;
+        for (int idx = threadIdx.x; idx < r * r; idx += DENSE_THREADS) {
+            const int i = j + 1 + idx / r, k = j + 1 + idx % r;
+            if (k <= i) A[(size_t)i * lda + k] -= A[(size_t)i * lda + j] * A[(size_t)k * lda + j];
+        }
+    }
+    __syncthreads();
+    return true;
+}
+
+// ================================================================================================
+// K2e-d -- width sensitivities of the small tracks (DESIGN.md section 3.14): the derivative of K2d' (mincurv_ipm.cu) at the
+// dense kernel's final iterate, which is always a curvature-row iterate, without band truncation.  With D = d_u + d_l
+// (sens) and the row weights W (sens_rows) of the export:
+//   (E^T E + D + E^T W E) v = g,   dL/dub = d_u v,  dL/dlb = d_l v
+// split at W = 1 as K2d' does: K = E^T (I + W_weak) E + D by dense_factor, and the ms = n_rows[b] strong rows S
+// (ascending) by Woodbury, Sigma = W_S^-1 + E_S K^-1 E_S^T in `schur` (n_rows_cap^2 doubles per instance, column j from
+// one solve against row S_j of E), v = K^-1 g - K^-1 E_S^T Sigma^-1 E_S K^-1 g.  The split is needed without truncation
+// too: W reaches 1e12 and more, and the late-accept exit returns status 0 at an iterate whose full normal matrix did not
+// factor.  The bounds and E are re-assembled as the forward does; the gradients follow the collapsed-box rule of
+// mincurv_adjoint_kernel.  One CTA per instance; those with 3 <= n < dense_below, n <= n_max.  banded: the banded
+// adjoint ran before on this batch, with these instances held out (grad_status ^ DENSE_HOLD, restored here); otherwise
+// this kernel writes the zero gradients of the other instances too.  grad_status 3 (zero gradients): more strong rows
+// than n_rows_cap, or a non-positive pivot in K or in Sigma; any other grad_status != 0 is kept, with zero gradients.
+__global__ void __launch_bounds__(DENSE_THREADS)
+mincurv_dense_adjoint_kernel(int n_max, int m, int dense_below, int banded, const int32_t *__restrict__ n_pts,
+                             const double *__restrict__ reftrack, const double *__restrict__ normvec,
+                             const double *__restrict__ hin, double w_veh, const double *__restrict__ w_veh_batch,
+                             double f_scale, const int32_t *__restrict__ centre_id, const double *__restrict__ sens,
+                             const double *__restrict__ sens_rows, const int32_t *__restrict__ n_rows, double *schur,
+                             int n_rows_cap, const double *__restrict__ grad_alpha, int32_t *__restrict__ grad_status,
+                             double *__restrict__ grad_w_right, double *__restrict__ grad_w_left,
+                             double *__restrict__ grad_w_veh) {
+    const int b = blockIdx.x;
+    const int n = n_pts ? n_pts[b] : n_max;
+    __shared__ double red[32];
+    __shared__ int s_flag;
+    extern __shared__ __align__(16) double s_dense[];
+    double *gwr = grad_w_right + (size_t)b * n_max, *gwl = grad_w_left + (size_t)b * n_max;
+    const bool owned = n >= 3 && n < dense_below && n <= n_max;
+    if (!owned && banded) return;
+    int gs = owned ? grad_status[b] : -1;
+    if (banded) gs ^= DENSE_HOLD;
+    if (owned && centre_id && centre_id[b] != b && !dense_follower_ok(centre_id, n_pts, n_max, b, n)) gs = -1;
+    const int ms = owned ? n_rows[b] : 0;
+    bool ok = gs == 0 && ms <= n_rows_cap;
+    const double *rt = reftrack + (size_t)b * n_max * 4;
+    const double wv = w_veh_batch ? w_veh_batch[b] : w_veh;
+    if (ok) ok = dense_assemble<false>(s_dense, m, n, rt, normvec + (size_t)b * n_max * 2, hin + (size_t)b * n_max, nullptr,
+                                       wv, f_scale, s_flag);
+    if (ok) {
+        double *E = s_dense, *K = s_dense + (size_t)m * m;
+        auto dv = [&](int v) { return s_dense + 2 * (size_t)m * m + (size_t)v * m; };
+        double *DD = dv(D_DD), *WK = dv(D_WK), *X = dv(D_DX), *Y = dv(D_RHS), *U = dv(D_VV);
+        int *S = reinterpret_cast<int *>(dv(D_ETV));        // the strong rows, ascending
+        const double *DU = sens + (size_t)b * 2 * n_max, *DL = DU + n_max, *WR = sens_rows + (size_t)b * n_max;
+        const double *GA = grad_alpha + (size_t)b * n_max;
+        const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+        for (int i = threadIdx.x; i < n; i += DENSE_THREADS) {
+            DD[i] = DU[i] + DL[i];
+            WK[i] = (WR[i] <= 1.0) ? WR[i] : 0.0;
+            X[i] = GA[i];
+        }
+        if (warp == 0) {
+            int cnt = 0;
+            for (int base = 0; base < n; base += 32) {
+                const bool st = base + lane < n && WR[base + lane] > 1.0;
+                const unsigned bal = __ballot_sync(0xffffffffu, st);
+                if (st) S[cnt + __popc(bal & ((1u << lane) - 1u))] = base + lane;
+                cnt += __popc(bal);
+            }
+        }
+        __syncthreads();
+        ok = dense_factor(E, K, m, n, WK, DD);
+        if (ok) dense_solve(K, m, n, X, X);                // K^-1 g
+        if (ok && ms > 0) {
+            double *Sg = schur + (size_t)b * n_rows_cap * n_rows_cap;      // Sigma, row-major, lower triangle used
+            for (int j = 0; j < ms; ++j) {          // column j: E_S K^-1 E_{S_j}^T + e_j / W_{S_j}
+                for (int i = threadIdx.x; i < n; i += DENSE_THREADS) Y[i] = E[(size_t)S[j] * m + i];
+                __syncthreads();
+                dense_solve(K, m, n, Y, Y);
+                for (int k = j + warp; k < ms; k += DENSE_THREADS / 32) {
+                    double t = 0.0;
+                    for (int i = lane; i < n; i += 32) t += E[(size_t)S[k] * m + i] * Y[i];
+                    t = warp_sum(t);
+                    if (lane == 0) Sg[(size_t)k * n_rows_cap + j] = t + ((k == j) ? 1.0 / WR[S[j]] : 0.0);
+                }
+                __syncthreads();
+            }
+            for (int k = warp; k < ms; k += DENSE_THREADS / 32) {       // u = E_S K^-1 g
+                double t = 0.0;
+                for (int i = lane; i < n; i += 32) t += E[(size_t)S[k] * m + i] * X[i];
+                t = warp_sum(t);
+                if (lane == 0) U[k] = t;
+            }
+            ok = dense_chol(Sg, n_rows_cap, ms);
+            if (ok) {
+                dense_solve(Sg, n_rows_cap, ms, U, U);                 // z = Sigma^-1 u
+                for (int i = threadIdx.x; i < n; i += DENSE_THREADS) {  // v = K^-1 g - K^-1 E_S^T z
+                    double t = 0.0;
+                    for (int k = 0; k < ms; ++k) t += E[(size_t)S[k] * m + i] * U[k];
+                    Y[i] = t;
+                }
+                __syncthreads();
+                dense_solve(K, m, n, Y, Y);
+                for (int i = threadIdx.x; i < n; i += DENSE_THREADS) X[i] -= Y[i];
+                __syncthreads();
+            }
+        }
+        if (ok) {       // the widths (mincurv_setup.cu P1); a collapsed box follows its mid point
+            double gv = 0.0;
+            for (int i = threadIdx.x; i < n_max; i += DENSE_THREADS) {
+                double gr = 0.0, gl = 0.0;
+                if (i < n) {
+                    const double v = X[i], gu = DU[i] * v, glb = DL[i] * v;
+                    const double ub = rt[(size_t)i * 4 + 2] - 0.5 * wv, lb = -(rt[(size_t)i * 4 + 3] - 0.5 * wv);
+                    if (ub - lb < 2.0 * FIX_EPS) {
+                        gr = 0.5 * (gu + glb);
+                        gl = -gr;
+                    } else {
+                        gr = gu;
+                        gl = -glb;
+                        gv += 0.5 * (glb - gu);
+                    }
+                }
+                gwr[i] = gr;
+                gwl[i] = gl;
+            }
+            gv = block_reduce<0>(gv, red);
+            if (threadIdx.x == 0) grad_w_veh[b] = gv;
+        }
+    }
+    if (!ok) {
+        for (int i = threadIdx.x; i < n_max; i += DENSE_THREADS) { gwr[i] = 0.0; gwl[i] = 0.0; }
+        if (threadIdx.x == 0) grad_w_veh[b] = 0.0;
+    }
+    if (owned && threadIdx.x == 0) grad_status[b] = (gs == 0 && !ok) ? 3 : gs;
+}
+
+// held out of the banded adjoint kernels, which factor every instance with grad_status 0 (a track below N_MIN would wrap
+// their band onto itself): the instances the dense adjoint takes get grad_status ^ DENSE_HOLD, nonzero whatever it was
+__global__ void mincurv_dense_hold_kernel(int B, int n_max, int dense_below, const int32_t *__restrict__ n_pts,
+                                          int32_t *__restrict__ grad_status) {
+    const int b = blockIdx.x * blockDim.x + threadIdx.x;
+    if (b >= B) return;
+    const int n = n_pts ? n_pts[b] : n_max;
+    if (n >= 3 && n < dense_below && n <= n_max) grad_status[b] ^= DENSE_HOLD;
+}
+
+int mincurv_dense_hold(int B, int n_max, int dense_below, const int32_t *n_pts, int32_t *grad_status, void *stream) {
+    mincurv_dense_hold_kernel<<<(B + 255) / 256, 256, 0, (cudaStream_t)stream>>>(B, n_max, dense_below, n_pts, grad_status);
+    return check_cuda("mincurv_dense_hold_kernel");
+}
+
+int mincurv_dense_adjoint(int B, int n_max, int dense_below, bool banded, const int32_t *n_pts, const double *reftrack,
+                          const double *normvec, const double *h, double w_veh, const double *w_veh_batch, double f_scale,
+                          const int32_t *centre_id, const double *sens, int32_t *grad_status, const double *grad_alpha,
+                          double *grad_w_right, double *grad_w_left, double *grad_w_veh, const double *sens_rows,
+                          const int32_t *n_rows, double *schur, int n_rows_cap, void *stream) {
+    const int m = n_max < dense_below - 1 ? n_max : dense_below - 1;
+    const int smem = (int)dense_smem_bytes(m);
+    if (cudaFuncSetAttribute(mincurv_dense_adjoint_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) != cudaSuccess)
+        return check_cuda("mincurv_dense_adjoint_kernel: cudaFuncSetAttribute");
+    mincurv_dense_adjoint_kernel<<<B, DENSE_THREADS, smem, (cudaStream_t)stream>>>(
+        n_max, m, dense_below, banded ? 1 : 0, n_pts, reftrack, normvec, h, w_veh, w_veh_batch, f_scale, centre_id, sens,
+        sens_rows, n_rows, schur, n_rows_cap, grad_alpha, grad_status, grad_w_right, grad_w_left, grad_w_veh);
+    return check_cuda("mincurv_dense_adjoint_kernel");
+}
+
 // launched after the banded stages (banded != 0), or alone when n_max < N_MIN
 int mincurv_dense(int B, int n_max, int dense_below, bool banded, const int32_t *n_pts, const double *reftrack,
                   const double *normvec, const double *h, double kappa_bound, const double *kappa_bound_batch, double w_veh,
                   const double *w_veh_batch, double f_scale, const int32_t *centre_id, const double *lin_alpha, double *alpha,
-                  double *curv_error_max, double *kappa_lin_max, int32_t *status, int32_t *iters, void *stream) {
+                  double *curv_error_max, double *kappa_lin_max, int32_t *status, int32_t *iters, double *sens,
+                  int32_t *grad_status, double *sens_rows, int32_t *n_rows, void *stream) {
     PdipParams prm;                     // those of the curvature-row phase (mincurv_kappa_phase)
     prm.max_iter = 40;
     prm.mu_rel = 1e-11;
@@ -448,14 +678,15 @@ int mincurv_dense(int B, int n_max, int dense_below, bool banded, const int32_t 
     prm.lam0_rel = 1e-2;
     const int m = n_max < dense_below - 1 ? n_max : dense_below - 1;
     const int smem = (int)dense_smem_bytes(m);
-    auto kernel = lin_alpha ? mincurv_dense_kernel<true> : mincurv_dense_kernel<false>;
+    auto kernel = sens ? (lin_alpha ? mincurv_dense_kernel<true, true> : mincurv_dense_kernel<false, true>)
+                       : (lin_alpha ? mincurv_dense_kernel<true, false> : mincurv_dense_kernel<false, false>);
     // (per launch: the attribute is per device and a process may drive several)
     if (cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) != cudaSuccess)
         return check_cuda("mincurv_dense_kernel: cudaFuncSetAttribute");
     kernel<<<B, DENSE_THREADS, smem, (cudaStream_t)stream>>>(n_max, m, dense_below, banded ? 1 : 0, n_pts, reftrack, normvec,
                                                              h, kappa_bound, kappa_bound_batch, w_veh, w_veh_batch, f_scale,
                                                              centre_id, lin_alpha, prm, alpha, curv_error_max, kappa_lin_max,
-                                                             status, iters);
+                                                             status, iters, sens, sens_rows, n_rows, grad_status);
     return check_cuda("mincurv_dense_kernel");
 }
 

@@ -282,7 +282,9 @@ int mc_mincurv_solve_batch_ex(int B, int n_max, const int32_t *n_pts, const doub
     if (dense_below != 0) {
         if (dense_below < mc::N_MIN || dense_below > MC_DENSE_N_MAX + 1)
             return bad("mc_mincurv_solve_batch_ex: dense_below must be 0 or in [%d, %d]", mc::N_MIN, MC_DENSE_N_MAX + 1);
-        if (prox_x || sens) return bad("mc_mincurv_solve_batch_ex: dense_below takes neither prox_x nor sens");
+        if (prox_x) return bad("mc_mincurv_solve_batch_ex: dense_below does not take prox_x");
+        // (the dense iterate always carries the curvature rows: its export is the row export)
+        if (sens && !sens_rows) return bad("mc_mincurv_solve_batch_ex: dense_below takes sens only with sens_rows and n_rows");
         if (B <= 0 || n_max <= 0) return bad("mc_mincurv_solve_batch_ex: B <= 0 or n_max <= 0");
         if (!reftrack || !normvec || !h || !alpha || !curv_error_max || !status)
             return bad("mc_mincurv_solve_batch_ex: NULL argument");
@@ -299,10 +301,10 @@ int mc_mincurv_solve_batch_ex(int B, int n_max, const int32_t *n_pts, const doub
                                      lin_alpha, kappa_bound_batch, workspace, workspace_bytes, stream);
         if (rc || dense_below == 0) return rc;
     }
-    // the small tracks: the dense kernel, last on the stream
+    // the small tracks: the dense kernel, last on the stream (it overwrites the export of its instances)
     return mc::mincurv_dense(B, n_max, dense_below, banded, n_pts, reftrack, normvec, h, kappa_bound, kappa_bound_batch, w_veh,
                              w_veh_batch, f_scale, centre_id, lin_alpha, alpha, curv_error_max, kappa_lin_max, status, iters,
-                             stream);
+                             sens, grad_status, sens_rows, n_rows, stream);
 }
 
 int mc_mincurv_solve_batch_shared(int B, int n_max, const int32_t *n_pts, const double *reftrack, const double *normvec,

@@ -1903,6 +1903,42 @@ int mincurv_kappa_phase(int B, int n_max, const int32_t *n_pts, double kappa_bou
 
 }  // namespace mc
 
+// the banded adjoint of mc_mincurv_adjoint_batch (K2d, or K2d' with sens_rows) after its argument checks
+static int adjoint_banded(int B, int n_max, const int32_t *n_pts, const double *reftrack, const double *normvec,
+                          const double *h, double w_veh, const double *w_veh_batch, double f_scale, const int32_t *centre_id,
+                          const double *sens, int32_t *grad_status, const double *grad_alpha, double *grad_w_right,
+                          double *grad_w_left, double *grad_w_veh, const double *sens_rows, const int32_t *n_rows,
+                          double *schur, int n_rows_cap, const double *lin_alpha, void *workspace, size_t workspace_bytes,
+                          void *stream) {
+    // the band of H and the bounds are rebuilt in the slabs; the assembly's status words (the forward pass's, recorded in
+    // grad_status) go to grad_w_right, which the adjoint kernel overwrites
+    int rc = mc::mincurv_setup(B, n_max, n_pts, reftrack, normvec, h, w_veh, w_veh_batch, f_scale, centre_id, lin_alpha,
+                               reinterpret_cast<int32_t *>(grad_w_right), workspace, workspace_bytes, stream);
+    if (rc) return rc;
+    if (sens_rows) {
+        // pass 0: the instances without row weights (reading their owner's band); pass 1: the curvature-row instances
+        const mc::SolverGrid g = mc::solver_grid(B, n_max, workspace, mc::ctas_per_sm(mc::mincurv_adjoint_rows_kernel));
+        for (int pass = 0; pass < 2; ++pass) {
+            if (mc::launch_solver(mc::mincurv_adjoint_rows_kernel, g.grid, g.counter, (cudaStream_t)stream, B, n_max, n_pts,
+                                  reftrack, w_veh, w_veh_batch, (double *)workspace, mc::make_layout(n_max), sens, sens_rows,
+                                  n_rows, schur, n_rows_cap, pass, grad_alpha, grad_status, grad_w_right, grad_w_left,
+                                  grad_w_veh, g.counter) != 0) {
+                snprintf(mc::g_err, sizeof(mc::g_err), "mincurv_adjoint_rows_kernel: cudaFuncSetAttribute failed");
+                return MC_ECUDA;
+            }
+        }
+        return check_cuda("mincurv_adjoint_rows_kernel");
+    }
+    const mc::SolverGrid g = mc::solver_grid(B, n_max, workspace, mc::ctas_per_sm(mc::mincurv_adjoint_kernel));
+    if (mc::launch_solver(mc::mincurv_adjoint_kernel, g.grid, g.counter, (cudaStream_t)stream, B, n_max, n_pts, reftrack, w_veh,
+                          w_veh_batch, (double *)workspace, mc::make_layout(n_max), sens, grad_alpha, grad_status, grad_w_right,
+                          grad_w_left, grad_w_veh, g.counter) != 0) {
+        snprintf(mc::g_err, sizeof(mc::g_err), "mincurv_adjoint_kernel: cudaFuncSetAttribute failed");
+        return MC_ECUDA;
+    }
+    return check_cuda("mincurv_adjoint_kernel");
+}
+
 static constexpr int PDIP_SLICE_DEFAULT = 8;      // DESIGN.md section 3.3: the predictor of the remaining iterations is
                                                   // no better than chance after 4 iterations, within one iteration after 8
 
@@ -1962,39 +1998,37 @@ int mc_mincurv_adjoint_batch(int B, int n_max, const int32_t *n_pts, const doubl
                              const double *h, double w_veh, const double *w_veh_batch, double f_scale, const int32_t *centre_id,
                              const double *sens, int32_t *grad_status, const double *grad_alpha, double *grad_w_right,
                              double *grad_w_left, double *grad_w_veh, const double *sens_rows, const int32_t *n_rows,
-                             double *schur, int n_rows_cap, const double *lin_alpha, void *workspace,
+                             double *schur, int n_rows_cap, const double *lin_alpha, int dense_below, void *workspace,
                              size_t workspace_bytes, void *stream) {
     if (!sens || !grad_status || !grad_alpha || !grad_w_right || !grad_w_left || !grad_w_veh)
         return bad("mc_mincurv_adjoint_batch: NULL argument");
     if (sens_rows && (!n_rows || !schur)) return bad("mc_mincurv_adjoint_batch: sens_rows needs n_rows and schur");
     if (sens_rows && n_rows_cap < 0) return bad("mc_mincurv_adjoint_batch: n_rows_cap < 0");
-    // the band of H and the bounds are rebuilt in the slabs; the assembly's status words (the forward pass's, recorded in
-    // grad_status) go to grad_w_right, which the adjoint kernel overwrites
-    int rc = mc::mincurv_setup(B, n_max, n_pts, reftrack, normvec, h, w_veh, w_veh_batch, f_scale, centre_id, lin_alpha,
-                               reinterpret_cast<int32_t *>(grad_w_right), workspace, workspace_bytes, stream);
-    if (rc) return rc;
-    if (sens_rows) {
-        // pass 0: the instances without row weights (reading their owner's band); pass 1: the curvature-row instances
-        const mc::SolverGrid g = mc::solver_grid(B, n_max, workspace, mc::ctas_per_sm(mc::mincurv_adjoint_rows_kernel));
-        for (int pass = 0; pass < 2; ++pass) {
-            if (mc::launch_solver(mc::mincurv_adjoint_rows_kernel, g.grid, g.counter, (cudaStream_t)stream, B, n_max, n_pts,
-                                  reftrack, w_veh, w_veh_batch, (double *)workspace, mc::make_layout(n_max), sens, sens_rows,
-                                  n_rows, schur, n_rows_cap, pass, grad_alpha, grad_status, grad_w_right, grad_w_left,
-                                  grad_w_veh, g.counter) != 0) {
-                snprintf(mc::g_err, sizeof(mc::g_err), "mincurv_adjoint_rows_kernel: cudaFuncSetAttribute failed");
-                return MC_ECUDA;
-            }
+    if (dense_below != 0) {
+        if (dense_below < mc::N_MIN || dense_below > MC_DENSE_N_MAX + 1)
+            return bad("mc_mincurv_adjoint_batch: dense_below must be 0 or in [%d, %d]", mc::N_MIN, MC_DENSE_N_MAX + 1);
+        if (!sens_rows) return bad("mc_mincurv_adjoint_batch: dense_below needs sens_rows, n_rows and schur");
+        if (lin_alpha) return bad("mc_mincurv_adjoint_batch: dense_below does not take lin_alpha");
+        if (B <= 0 || n_max <= 0) return bad("mc_mincurv_adjoint_batch: B <= 0 or n_max <= 0");
+        if (!reftrack || !normvec || !h) return bad("mc_mincurv_adjoint_batch: NULL argument");
+    }
+    // dense_below: the banded kernels run (if n_max >= N_MIN) with the dense adjoint's instances held out, then the dense one
+    const bool banded = dense_below == 0 || n_max >= mc::N_MIN;
+    if (banded) {
+        int rc = 0;
+        if (dense_below) {      // (the banded stage's own checks first: nothing is launched before every check passed)
+            rc = mc::mincurv_args("mc_mincurv_adjoint_batch", B, n_max, workspace, workspace_bytes);
+            if (!rc) rc = mc::mincurv_dense_hold(B, n_max, dense_below, n_pts, grad_status, stream);
+            if (rc) return rc;
         }
-        return check_cuda("mincurv_adjoint_rows_kernel");
+        rc = adjoint_banded(B, n_max, n_pts, reftrack, normvec, h, w_veh, w_veh_batch, f_scale, centre_id, sens, grad_status,
+                            grad_alpha, grad_w_right, grad_w_left, grad_w_veh, sens_rows, n_rows, schur, n_rows_cap, lin_alpha,
+                            workspace, workspace_bytes, stream);
+        if (rc || dense_below == 0) return rc;
     }
-    const mc::SolverGrid g = mc::solver_grid(B, n_max, workspace, mc::ctas_per_sm(mc::mincurv_adjoint_kernel));
-    if (mc::launch_solver(mc::mincurv_adjoint_kernel, g.grid, g.counter, (cudaStream_t)stream, B, n_max, n_pts, reftrack, w_veh,
-                          w_veh_batch, (double *)workspace, mc::make_layout(n_max), sens, grad_alpha, grad_status, grad_w_right,
-                          grad_w_left, grad_w_veh, g.counter) != 0) {
-        snprintf(mc::g_err, sizeof(mc::g_err), "mincurv_adjoint_kernel: cudaFuncSetAttribute failed");
-        return MC_ECUDA;
-    }
-    return check_cuda("mincurv_adjoint_kernel");
+    return mc::mincurv_dense_adjoint(B, n_max, dense_below, banded, n_pts, reftrack, normvec, h, w_veh, w_veh_batch, f_scale,
+                                     centre_id, sens, grad_status, grad_alpha, grad_w_right, grad_w_left, grad_w_veh,
+                                     sens_rows, n_rows, schur, n_rows_cap, stream);
 }
 
 /* debug aid (tests/test_gpu_factor.py): one factorisation + the two kinds of solve of the interior-point kernel on slabs

@@ -91,12 +91,27 @@ int mincurv_finalize(int B, int n_max, const int32_t *n_pts, const double *alpha
                      size_t workspace_bytes, void *stream);
 
 // the dense small-track kernel (mincurv_dense.cu) of mc_mincurv_solve_batch_ex on the instances with
-// 3 <= n_pts[b] < dense_below; banded: the banded stages ran before it on this batch.  Not exported.
+// 3 <= n_pts[b] < dense_below; banded: the banded stages ran before it on this batch; sens (with grad_status, sens_rows
+// and n_rows) or NULL: the row export of its instances.  Not exported.
 __attribute__((visibility("hidden")))
 int mincurv_dense(int B, int n_max, int dense_below, bool banded, const int32_t *n_pts, const double *reftrack,
                   const double *normvec, const double *h, double kappa_bound, const double *kappa_bound_batch, double w_veh,
                   const double *w_veh_batch, double f_scale, const int32_t *centre_id, const double *lin_alpha, double *alpha,
-                  double *curv_error_max, double *kappa_lin_max, int32_t *status, int32_t *iters, void *stream);
+                  double *curv_error_max, double *kappa_lin_max, int32_t *status, int32_t *iters, double *sens,
+                  int32_t *grad_status, double *sens_rows, int32_t *n_rows, void *stream);
+
+// the dense adjoint (mincurv_dense.cu) of mc_mincurv_adjoint_batch on the same instances.  Before the banded adjoint runs
+// on the batch, mincurv_dense_hold marks them (grad_status ^ DENSE_HOLD) so that it leaves them alone; the dense adjoint
+// (banded = true) restores their grad_status.  Not exported.
+constexpr int32_t DENSE_HOLD = 0x40000000;
+__attribute__((visibility("hidden")))
+int mincurv_dense_hold(int B, int n_max, int dense_below, const int32_t *n_pts, int32_t *grad_status, void *stream);
+__attribute__((visibility("hidden")))
+int mincurv_dense_adjoint(int B, int n_max, int dense_below, bool banded, const int32_t *n_pts, const double *reftrack,
+                          const double *normvec, const double *h, double w_veh, const double *w_veh_batch, double f_scale,
+                          const int32_t *centre_id, const double *sens, int32_t *grad_status, const double *grad_alpha,
+                          double *grad_w_right, double *grad_w_left, double *grad_w_veh, const double *sens_rows,
+                          const int32_t *n_rows, double *schur, int n_rows_cap, void *stream);
 
 __device__ __forceinline__ double *vec(double *slab, const Layout &L, int v) { return slab + (size_t)v * L.np; }
 

@@ -443,7 +443,7 @@ class CurvatureMetric:
                 _b._mincurv_launch("mc_mincurv_adjoint_batch", e - s, n_pts[s:e], self.reftrack[s:e], self.normvec[s:e],
                                    self.h[s:e], None, 0.0, None, _b.F_SCALE, self.centre_id[s:e], sens[s:e], gs[s:e],
                                    rhs[s:e], out[s:e], gwl[s:e], gwv[s:e], None, None, None, 0,
-                                   None if self.lin is None else self.lin[s:e])
+                                   None if self.lin is None else self.lin[s:e], 0)
             out, gs = out.reshape(B, 2, n_max), gs.reshape(B, 2)
             u, w = out[:, 0], (out[:, 1] if y is not None else None)
             ok = go & (gs[:, 0] == 0) & torch.isfinite(u).all(dim=1)

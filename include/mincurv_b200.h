@@ -53,6 +53,10 @@ extern "C" {
  * dense solver of small closed tracks (dense_below).  The binding lets a call leave out the MC_OPTIONAL4 parameters alone,
  * or them and each earlier group in turn. */
 #define MC_OPTIONAL4
+/* MC_OPTIONAL5 marks parameters added after the MC_OPTIONAL4 ones, alike 0 / NULL-able: on mc_mincurv_adjoint_batch, the
+ * dense adjoint of small closed tracks (dense_below).  The binding lets a call leave out the MC_OPTIONAL5 parameters alone,
+ * or them and each earlier group in turn. */
+#define MC_OPTIONAL5
 
 #define MC_STATUS_OK 0
 #define MC_STATUS_TOO_NARROW 1
@@ -155,7 +159,12 @@ int mc_mincurv_solve_batch(int B, int n_max, const int32_t *n_pts,
  *                    truncation: the bounds, the statuses -1 and 1, kappa_bound_batch, w_veh_batch and lin_alpha as above;
  *                    a follower of centre_id is checked as above and then assembled on its own.  Status 2 and 3 as for
  *                    the banded solve; status 4 when the rows are still violated at the end (whatever ended it).  dense_below > N_MIN lets the two
- *                    solvers be compared on the same instance.  Not with prox_x or the sensitivity export. */
+ *                    solvers be compared on the same instance.  Not with prox_x.  With the sensitivity export only as
+ *                    the full row export (sens, grad_status, sens_rows and n_rows; sens and grad_status alone are
+ *                    refused): the dense iterate always carries the curvature rows.  The banded stages export as
+ *                    documented at mc_mincurv_solve_batch_sens, then the dense kernel overwrites the export of its
+ *                    instances with that of its final iterate (ratios, row weights, strong-row count, grad_status =
+ *                    status; zeros where the status is not 0), for mc_mincurv_adjoint_batch with the same dense_below. */
 int mc_mincurv_solve_batch_ex(int B, int n_max, const int32_t *n_pts,
                               const double *reftrack, const double *normvec, const double *h,
                               double kappa_bound, double w_veh, const double *w_veh_batch, double f_scale,
@@ -259,7 +268,13 @@ int mc_mincurv_finalize_batch(int B, int n_max, const int32_t *n_pts, const doub
  * n_rows[b] > n_rows_cap gets grad_status 3.
  * lin_alpha (NULL: the centre line): the linearisation point of H, as for mc_mincurv_solve_batch_ex; with centre_id a
  * follower is linearised about its owner's row (the assembly is shared); alpha is not
- * differentiated with respect to it. */
+ * differentiated with respect to it.
+ * dense_below (0: none of this): that of the mc_mincurv_solve_batch_ex call with the full row export that produced sens,
+ * grad_status, sens_rows and n_rows; N_MIN <= dense_below <= MC_DENSE_N_MAX + 1, with sens_rows, n_rows and schur, not
+ * with lin_alpha.  The instances with 3 <= n_pts[b] < dense_below are differentiated by the dense adjoint (DESIGN.md
+ * section 3.14) at the dense kernel's final iterate, the same derivative without band truncation, its strong rows
+ * through the same Schur complement in schur; the banded kernels, launched only if n_max >= N_MIN (so that n_max <
+ * N_MIN is accepted with any workspace), leave them alone.  grad_status as above. */
 int mc_mincurv_solve_batch_sens(int B, int n_max, const int32_t *n_pts,
                                 const double *reftrack, const double *normvec, const double *h,
                                 double kappa_bound, double w_veh, const double *w_veh_batch, double f_scale,
@@ -276,6 +291,7 @@ int mc_mincurv_adjoint_batch(int B, int n_max, const int32_t *n_pts,
                              MC_OPTIONAL const double *sens_rows, MC_OPTIONAL const int32_t *n_rows,
                              MC_OPTIONAL double *schur, MC_OPTIONAL int n_rows_cap,
                              MC_OPTIONAL2 const double *lin_alpha,
+                             MC_OPTIONAL5 int dense_below,
                              void *workspace, size_t workspace_bytes, void *stream);
 
 /* Fourth stage, run by mc_mincurv_solve_batch between two finalize passes: re-solves every instance flagged
