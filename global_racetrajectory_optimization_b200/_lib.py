@@ -44,13 +44,14 @@ def _declarations(path: str):
 
 def header_signatures(path: str) -> dict:
     """name -> (restype, argtypes) of every declaration `ret mc_name(type name, ...);` in the C header at path."""
-    return {name: (_ctype(ret, name, ret=True), [_ctype(re.sub(r"\bMC_OPTIONAL[2345]?\b", " ", p), name) for p in params])
+    return {name: (_ctype(ret, name, ret=True), [_ctype(re.sub(r"\bMC_OPTIONAL[2-6]?\b", " ", p), name) for p in params])
             for ret, name, params in _declarations(path)}
 
 
 def optional_parameters(path: str, marker: str = "MC_OPTIONAL") -> dict:
     """name -> (first, count) of the MC_OPTIONAL parameters (or those of another marker, such as MC_OPTIONAL2,
-    MC_OPTIONAL3, MC_OPTIONAL4 or MC_OPTIONAL5) of each declaration in the C header at path that has them (one run of consecutive parameters)."""
+    MC_OPTIONAL3, MC_OPTIONAL4, MC_OPTIONAL5 or MC_OPTIONAL6) of each declaration in the C header at path that has them
+    (one run of consecutive parameters)."""
     out = {}
     for _, name, params in _declarations(path):
         k = [i for i, p in enumerate(params) if re.search(rf"\b{marker}\b", p)]
@@ -96,18 +97,20 @@ _OPTIONAL2 = optional_parameters(_build.HEADER, "MC_OPTIONAL2")
 _OPTIONAL3 = optional_parameters(_build.HEADER, "MC_OPTIONAL3")
 _OPTIONAL4 = optional_parameters(_build.HEADER, "MC_OPTIONAL4")
 _OPTIONAL5 = optional_parameters(_build.HEADER, "MC_OPTIONAL5")
+_OPTIONAL6 = optional_parameters(_build.HEADER, "MC_OPTIONAL6")
 EXPORTED_SYMBOLS = tuple(_SIGS)
 
 
 def _with_optional(fn, *groups):
     """fn, which may also be called without its parameters [first, first + count) of the last of groups ((first, count)
-    each, in release order), or without those of the last two, and so on: they are then NULL (0 for an int), as the
-    header documents for the MC_OPTIONAL .. MC_OPTIONAL5 parameters, so that a call written for the entry
-    before they were added still binds its arguments to the right parameters."""
+    each, in release order), or without those of the last two, and so on: they are then NULL (0 for an int or a
+    double), as the header documents for the MC_OPTIONAL .. MC_OPTIONAL6 parameters, so that a call written for the
+    entry before they were added still binds its arguments to the right parameters."""
     forms = {}
     left_out = []
     for first, count in sorted(groups, reverse=True):       # (the later groups come after the earlier ones)
-        left_out.append((first, tuple(0 if t is ctypes.c_int else None for t in fn.argtypes[first:first + count])))
+        left_out.append((first, tuple(0 if t is ctypes.c_int else 0.0 if t is ctypes.c_double else None
+                                      for t in fn.argtypes[first:first + count])))
         forms[len(fn.argtypes) - sum(len(f) for _, f in left_out)] = list(reversed(left_out))
 
     def call(*args):
@@ -154,7 +157,8 @@ def load(build_if_missing: bool = True):
         fn = getattr(lib, name)
         fn.restype = res
         fn.argtypes = args
-        groups = [g[name] for g in (_OPTIONAL, _OPTIONAL2, _OPTIONAL3, _OPTIONAL4, _OPTIONAL5) if name in g]
+        groups = [g[name] for g in (_OPTIONAL, _OPTIONAL2, _OPTIONAL3, _OPTIONAL4, _OPTIONAL5, _OPTIONAL6)
+                  if name in g]
         if groups:
             setattr(lib, name, _with_optional(fn, *groups))
     _LIB = lib

@@ -290,7 +290,7 @@ def opt_min_curv_batch(reftrack: torch.Tensor, normvec: torch.Tensor, h: torch.T
         ws = _workspace("mincurv", _lib.load().mc_mincurv_workspace_bytes(a.chunk, a.n_max), a.dev)
         _launch_chunks("mc_mincurv_solve_batch_ex", a.B, a.chunk, ws, a.n_max, *map(_rows, (a.n_pts, a.reftrack, a.normvec,
                        a.h)), kb, a.w_scalar, _rows(a.w_batch), a.f_scale, *map(_rows, out.values()), 0.0, None, None,
-                       _rows(lin), _rows(kbb), *(None,) * 5, dense_below)
+                       _rows(lin), _rows(kbb), *(None,) * 5, dense_below, 0)
         if invalid is not None:
             out["status"] = torch.where(invalid, -1, out["status"]).to(torch.int32)
         return out
@@ -314,7 +314,7 @@ def _mincurv_per_instance(chunk: int, n_pts, reftrack, normvec, h, kbb, w_scalar
     ws = _workspace("mincurv", _lib.load().mc_mincurv_workspace_bytes(chunk, n_max), h.device)
     _launch_chunks("mc_mincurv_solve_batch_ex", B, chunk, ws, n_max, *map(_rows, (n_pts, reftrack, normvec, h)), kb,
                    w_scalar, _rows(w_batch), f_scale, *map(_rows, outputs), 0.0, None, None, None, _rows(kbb),
-                   _chunk_centre_ids(centre_id, B), *map(_rows, export), dense_below)
+                   _chunk_centre_ids(centre_id, B), *map(_rows, export), dense_below, 0)
 
 
 def shared_centre_ids(group: torch.Tensor) -> torch.Tensor:

@@ -14,6 +14,9 @@
 // as violating them), however the iteration ended: rows that cannot be met drive their weights l / s up until the
 // iteration cap or a non-positive pivot stops it.
 // No global workspace: shared memory holds E and K (m x m each, m = min(n_max, dense_below - 1)) and DV vectors of m.
+// The same kernel with PROX solves the lap-time refinement's projection QP (mc_mincurv_solve_batch_ex with prox_x and
+// prox_dense_below), and mincurv_dense_eval_kernel its post-solve evaluation (mc_mincurv_finalize_batch with
+// dense_below), both on the tracks below dense_below; the refinement's metric is the dense adjoint below.
 #include "capi.cuh"
 #include "mincurv_ws.cuh"
 
@@ -206,6 +209,61 @@ __device__ __forceinline__ bool dense_assemble(double *s_dense, int m, int n, co
     return true;
 }
 
+// The post-solve quantities of mincurv_finalize_kernel at alpha = D_AL, for the QP dense_assemble<LIN> left in s_dense:
+// kmax = max |k_ref + E alpha| and emax = curv_error_max (each NaN if any of its terms is, as there), and viol = 1 where
+// some point has |k_ref + E alpha| > kb (1 + 1e-7) or a NaN there, else 0.  The iterate vectors D_LU .. D_S4 are scratch.
+// Called by every thread of the CTA; the forward kernel and mincurv_dense_eval_kernel share it.
+template <bool LIN>
+__device__ __forceinline__ void dense_post_solve(double *s_dense, int m, int n, double kb, double *red, double &kmax,
+                                                 double &emax, double &viol) {
+    auto dv = [&](int v) { return s_dense + 2 * (size_t)m * m + (size_t)v * m; };
+    const double *PX = dv(D_PX), *PY = dv(D_PY), *NX = dv(D_NX), *NY = dv(D_NY), *H = dv(D_H), *LFW = dv(D_LFW);
+    const double *INVD = dv(D_INVD), *MX = dv(D_MX), *MY = dv(D_MY), *XP = dv(D_XP), *YP = dv(D_YP), *SX = dv(D_SX);
+    const double *SY = dv(D_SY), *KR = dv(D_KR), *AL = dv(D_AL);
+    double *U0 = dv(D_LU), *U1 = dv(D_LL), *W0 = dv(D_SU), *W1 = dv(D_SL), *ZX = dv(D_S3), *ZY = dv(D_S4);
+    __syncthreads();
+    for (int i = threadIdx.x; i < n; i += DENSE_THREADS) {
+        const int im1 = (i == 0) ? n - 1 : i - 1, ip1 = (i + 1 == n) ? 0 : i + 1;
+        const double hi = H[i], him = H[im1];
+        const double vx = NX[i] * AL[i], vxm = NX[im1] * AL[im1], vxp = NX[ip1] * AL[ip1];
+        const double vy = NY[i] * AL[i], vym = NY[im1] * AL[im1], vyp = NY[ip1] * AL[ip1];
+        U0[i] = 6.0 * ((vxp - vx) / hi - (vx - vxm) / him);
+        U1[i] = 6.0 * ((vyp - vy) / hi - (vy - vym) / him);
+    }
+    __syncthreads();
+    tri_solve2(LFW, INVD, H, U0, U1, W0, W1, ZX, ZY, n);
+    kmax = 0.0; emax = 0.0; viol = 0.0;
+    bool nan_k = false, nan_e = false;           // (both maxima propagate a NaN, as in mincurv_finalize_kernel)
+    for (int i = threadIdx.x; i < n; i += DENSE_THREADS) {
+        const int ip1 = (i + 1 == n) ? 0 : i + 1;
+        const double hi = H[i], h2 = hi * hi;
+        const double zx = ZX[i], zy = ZY[i];
+        const double kl = fabs(KR[i] + SY[i] * zy - SX[i] * zx);
+        kmax = fmax(kmax, kl);
+        nan_k = nan_k || kl != kl;
+        if (!(kl <= kb * (1.0 + 1e-7))) viol = 1.0;         // (a NaN iterate counts as a violation)
+        const double ddx = h2 * (MX[i] + zx), ddy = h2 * (MY[i] + zy);
+        const double xp = XP[i], yp = YP[i];
+        double xc = xp, yc = yp;                // first derivatives of the centre line
+        if (LIN) {
+            xc = (PX[ip1] - PX[i]) - h2 * (2.0 * MX[i] + MX[ip1]) * (1.0 / 6.0);
+            yc = (PY[ip1] - PY[i]) - h2 * (2.0 * MY[i] + MY[ip1]) * (1.0 / 6.0);
+        }
+        const double xpt = xc + (NX[ip1] * AL[ip1] - NX[i] * AL[i]) - h2 * (2.0 * zx + ZX[ip1]) * (1.0 / 6.0);
+        const double ypt = yc + (NY[ip1] * AL[ip1] - NY[i] * AL[i]) - h2 * (2.0 * zy + ZY[ip1]) * (1.0 / 6.0);
+        const double q0 = xp * xp + yp * yp, q1 = xpt * xpt + ypt * ypt;
+        const double c0 = (xp * ddy - yp * ddx) / (q0 * sqrt(q0));
+        const double c1 = (xpt * ddy - ypt * ddx) / (q1 * sqrt(q1));
+        emax = fmax(emax, fabs(c1 - c0));
+        nan_e = nan_e || c1 - c0 != c1 - c0;
+    }
+    kmax = block_reduce<1>(kmax, red);
+    emax = block_reduce<1>(emax, red);
+    viol = block_reduce<1>(viol, red);
+    if (__syncthreads_or(nan_k)) kmax = NAN;
+    if (__syncthreads_or(nan_e)) emax = NAN;
+}
+
 // a follower of centre_id: the banded path's validity rule (its QP is assembled on its own all the same)
 __device__ __forceinline__ bool dense_follower_ok(const int32_t *centre_id, const int32_t *n_pts, int n_max, int b, int n) {
     const int o = centre_id[b];
@@ -218,7 +276,11 @@ __device__ __forceinline__ bool dense_follower_ok(const int32_t *centre_id, cons
 // iterate's sens[b] = (lu / su, ll / sl), sens_rows[b] = l3 / s3 + l4 / s4, n_rows[b] = #{weight > 1} and grad_status[b]
 // = status[b]; zeros beyond n and wherever the status is not 0.  It is written before the post-solve quantities, which
 // take the iterate vectors as scratch.
-template <bool LIN, bool EXPORT>
+// PROX: the projection QP of mc_mincurv_solve_batch_ex(prox_x, prox_dense_below), Hessian E^T E + prox_mu I and linear term
+// c = prox_mu q - (E^T E + prox_mu I) x (x = prox_x[b], q = prox_q[b]; f_scale does not enter): c replaces f, and prox_mu
+// goes on the diagonal of K and, as + prox_mu a, into the gradient, the right-hand sides and the dual residual, as in
+// mincurv_pdip_kappa_kernel<true>.  Not with EXPORT.  Without PROX prox_mu, prox_x and prox_q are not read.
+template <bool LIN, bool EXPORT, bool PROX>
 __global__ void __launch_bounds__(DENSE_THREADS)
 mincurv_dense_kernel(int n_max, int m, int dense_below, int banded, const int32_t *__restrict__ n_pts,
                      const double *__restrict__ reftrack, const double *__restrict__ normvec, const double *__restrict__ hin,
@@ -227,7 +289,9 @@ mincurv_dense_kernel(int n_max, int m, int dense_below, int banded, const int32_
                      const double *__restrict__ lin_alpha, PdipParams prm, double *__restrict__ alpha,
                      double *__restrict__ curv_error_max, double *__restrict__ kappa_lin_max, int32_t *__restrict__ status,
                      int32_t *__restrict__ iters, double *__restrict__ sens, double *__restrict__ sens_rows,
-                     int32_t *__restrict__ n_rows, int32_t *__restrict__ grad_status) {
+                     int32_t *__restrict__ n_rows, int32_t *__restrict__ grad_status, double prox_mu,
+                     const double *__restrict__ prox_x, const double *__restrict__ prox_q) {
+    static_assert(!(PROX && EXPORT), "the projection QP has no sensitivity export");
     const int b = blockIdx.x;
     const int n = n_pts ? n_pts[b] : n_max;
     __shared__ double red[32];
@@ -278,6 +342,16 @@ mincurv_dense_kernel(int n_max, int m, int dense_below, int banded, const int32_
     const double *la = LIN ? lin_alpha + (size_t)b * n_max : nullptr;
 
     if (!dense_assemble<LIN>(s_dense, m, n, rt, nv, hb, la, wv, f_scale, s_flag)) { refuse(1); return; }
+    const double pmu = PROX ? prox_mu : 0.0;        // (+ pmu a below: only in the PROX instantiations)
+    if constexpr (PROX) {       // c = mu q - (H + mu I) x in F (mincurv_prox_kernel); AL, ED and ETV as scratch
+        const double *px = prox_x + (size_t)b * n_max, *pq = prox_q + (size_t)b * n_max;
+        for (int i = threadIdx.x; i < n; i += DENSE_THREADS) AL[i] = px[i];
+        __syncthreads();
+        dense_E(E, m, n, AL, ED);
+        dense_Et(E, m, n, ED, ETV);
+        for (int i = threadIdx.x; i < n; i += DENSE_THREADS) F[i] = pmu * pq[i] - (ETV[i] + pmu * AL[i]);
+        __syncthreads();
+    }
 
     // ---- interior point on the box and the curvature rows (the iteration of mincurv_pdip_kappa_kernel) ----
     const double m4 = 4.0 * n;
@@ -287,7 +361,7 @@ mincurv_dense_kernel(int n_max, int m, int dense_below, int banded, const int32_
     dense_Et(E, m, n, ED, ETV);
     double gmax = 0.0, fmaxv = 0.0;
     for (int i = threadIdx.x; i < n; i += DENSE_THREADS) {
-        gmax = fmax(gmax, fabs(ETV[i] + F[i]));
+        gmax = fmax(gmax, fabs(PROX ? ETV[i] + pmu * AL[i] + F[i] : ETV[i] + F[i]));
         fmaxv = fmax(fmaxv, fabs(F[i]));
     }
     gmax = block_reduce<1>(gmax, red);
@@ -295,7 +369,7 @@ mincurv_dense_kernel(int n_max, int m, int dense_below, int banded, const int32_
     const double lam0 = prm.lam0_rel * gmax + 1e-300;
     double musum = 0.0;
     for (int i = threadIdx.x; i < n; i += DENSE_THREADS) {
-        const double gi = ETV[i] + F[i];
+        const double gi = PROX ? ETV[i] + pmu * AL[i] + F[i] : ETV[i] + F[i];
         const double lu = fmax(-gi, 0.0) + lam0, ll = fmax(gi, 0.0) + lam0;
         const double a = AL[i], su = UB[i] - a, sl = a - LB[i];
         const double kl = KR[i] + ED[i];
@@ -315,12 +389,12 @@ mincurv_dense_kernel(int n_max, int m, int dense_below, int banded, const int32_
             const double s3 = S3[i], s4 = S4[i], l3 = L3[i], l4 = L4[i], kl = KL[i];
             const double rp3 = kl + s3 - kb, rp4 = -kl + s4 - kb;
             WK[i] = l3 / s3 + l4 / s4;
-            DD[i] = LU[i] / SU[i] + LL[i] / SL[i];
+            DD[i] = PROX ? LU[i] / SU[i] + LL[i] / SL[i] + pmu : LU[i] / SU[i] + LL[i] / SL[i];
             VV[i] = (kl - KR[i]) + l3 * rp3 / s3 - l4 * rp4 / s4;
         }
         __syncthreads();
         dense_Et(E, m, n, VV, ETV);
-        for (int i = threadIdx.x; i < n; i += DENSE_THREADS) RHS[i] = -F[i] - ETV[i];
+        for (int i = threadIdx.x; i < n; i += DENSE_THREADS) RHS[i] = PROX ? -F[i] - ETV[i] - pmu * AL[i] : -F[i] - ETV[i];
         if (!dense_factor(E, K, m, n, WK, DD)) {
             result = (mu <= 1e-7 * mu0 && rdmax <= 1e3 * rd_tol && rpmax <= 1e-6 * kb) ? 0 : 3;
             break;
@@ -366,7 +440,7 @@ mincurv_dense_kernel(int n_max, int m, int dense_below, int banded, const int32_
         }
         __syncthreads();
         dense_Et(E, m, n, VV, ETV);
-        for (int i = threadIdx.x; i < n; i += DENSE_THREADS) RHS[i] -= ETV[i];
+        for (int i = threadIdx.x; i < n; i += DENSE_THREADS) RHS[i] -= PROX ? ETV[i] + pmu * AL[i] : ETV[i];
         __syncthreads();
         dense_solve(K, m, n, RHS, DX);
         dense_E(E, m, n, DX, ED);
@@ -404,10 +478,11 @@ mincurv_dense_kernel(int n_max, int m, int dense_below, int banded, const int32_
         mu = block_reduce<0>(musum2, red) / m4;
         rpmax = block_reduce<1>(rpmax, red);
         __syncthreads();
-        // dual residual r_d = E^T (kl - k_ref + l3 - l4) + f + lu - ll
+        // dual residual r_d = E^T (kl - k_ref + l3 - l4) (+ mu a) + f + lu - ll
         dense_Et(E, m, n, VV, ETV);
         rdmax = 0.0;
-        for (int i = threadIdx.x; i < n; i += DENSE_THREADS) rdmax = fmax(rdmax, fabs(ETV[i] + F[i] + LU[i] - LL[i]));
+        for (int i = threadIdx.x; i < n; i += DENSE_THREADS)
+            rdmax = fmax(rdmax, fabs(PROX ? ETV[i] + pmu * AL[i] + F[i] + LU[i] - LL[i] : ETV[i] + F[i] + LU[i] - LL[i]));
         rdmax = block_reduce<1>(rdmax, red);
         if (mu <= prm.mu_rel * mu0 && rdmax <= rd_tol && rpmax <= 1e-8 * kb) { result = 0; ++it; break; }
         if (mu <= 1e-2 * prm.mu_rel * mu0) { result = (rdmax <= 1e3 * rd_tol && rpmax <= 1e-6 * kb) ? 0 : 2; ++it; break; }
@@ -427,49 +502,8 @@ mincurv_dense_kernel(int n_max, int m, int dense_below, int banded, const int32_
         if (threadIdx.x == 0) n_rows[b] = (int32_t)strong;
     }
 
-    // ---- post-solve quantities (mincurv_finalize_kernel) ----
-    double *U0 = dv(D_LU), *U1 = dv(D_LL), *W0 = dv(D_SU), *W1 = dv(D_SL), *ZX = dv(D_S3), *ZY = dv(D_S4);
-    __syncthreads();
-    for (int i = threadIdx.x; i < n; i += DENSE_THREADS) {
-        const int im1 = (i == 0) ? n - 1 : i - 1, ip1 = (i + 1 == n) ? 0 : i + 1;
-        const double hi = H[i], him = H[im1];
-        const double vx = NX[i] * AL[i], vxm = NX[im1] * AL[im1], vxp = NX[ip1] * AL[ip1];
-        const double vy = NY[i] * AL[i], vym = NY[im1] * AL[im1], vyp = NY[ip1] * AL[ip1];
-        U0[i] = 6.0 * ((vxp - vx) / hi - (vx - vxm) / him);
-        U1[i] = 6.0 * ((vyp - vy) / hi - (vy - vym) / him);
-    }
-    __syncthreads();
-    tri_solve2(LFW, INVD, H, U0, U1, W0, W1, ZX, ZY, n);
-    double kmax = 0.0, emax = 0.0, viol = 0.0;
-    bool nan_k = false, nan_e = false;           // (both maxima propagate a NaN, as in mincurv_finalize_kernel)
-    for (int i = threadIdx.x; i < n; i += DENSE_THREADS) {
-        const int ip1 = (i + 1 == n) ? 0 : i + 1;
-        const double hi = H[i], h2 = hi * hi;
-        const double zx = ZX[i], zy = ZY[i];
-        const double kl = fabs(KR[i] + SY[i] * zy - SX[i] * zx);
-        kmax = fmax(kmax, kl);
-        nan_k = nan_k || kl != kl;
-        if (!(kl <= kb * (1.0 + 1e-7))) viol = 1.0;         // (a NaN iterate counts as a violation)
-        const double ddx = h2 * (MX[i] + zx), ddy = h2 * (MY[i] + zy);
-        const double xp = XP[i], yp = YP[i];
-        double xc = xp, yc = yp;                // first derivatives of the centre line
-        if (LIN) {
-            xc = (PX[ip1] - PX[i]) - h2 * (2.0 * MX[i] + MX[ip1]) * (1.0 / 6.0);
-            yc = (PY[ip1] - PY[i]) - h2 * (2.0 * MY[i] + MY[ip1]) * (1.0 / 6.0);
-        }
-        const double xpt = xc + (NX[ip1] * AL[ip1] - NX[i] * AL[i]) - h2 * (2.0 * zx + ZX[ip1]) * (1.0 / 6.0);
-        const double ypt = yc + (NY[ip1] * AL[ip1] - NY[i] * AL[i]) - h2 * (2.0 * zy + ZY[ip1]) * (1.0 / 6.0);
-        const double q0 = xp * xp + yp * yp, q1 = xpt * xpt + ypt * ypt;
-        const double c0 = (xp * ddy - yp * ddx) / (q0 * sqrt(q0));
-        const double c1 = (xpt * ddy - ypt * ddx) / (q1 * sqrt(q1));
-        emax = fmax(emax, fabs(c1 - c0));
-        nan_e = nan_e || c1 - c0 != c1 - c0;
-    }
-    kmax = block_reduce<1>(kmax, red);
-    emax = block_reduce<1>(emax, red);
-    viol = block_reduce<1>(viol, red);
-    if (__syncthreads_or(nan_k)) kmax = NAN;
-    if (__syncthreads_or(nan_e)) emax = NAN;
+    double kmax, emax, viol;
+    dense_post_solve<LIN>(s_dense, m, n, kb, red, kmax, emax, viol);
     if constexpr (EXPORT) {
         if (result == 0 && viol > 0.0) export_zeros();
         if (threadIdx.x == 0) grad_status[b] = (viol > 0.0) ? 4 : result;
@@ -663,31 +697,108 @@ int mincurv_dense_adjoint(int B, int n_max, int dense_below, bool banded, const 
     return check_cuda("mincurv_dense_adjoint_kernel");
 }
 
-// launched after the banded stages (banded != 0), or alone when n_max < N_MIN
-int mincurv_dense(int B, int n_max, int dense_below, bool banded, const int32_t *n_pts, const double *reftrack,
-                  const double *normvec, const double *h, double kappa_bound, const double *kappa_bound_batch, double w_veh,
-                  const double *w_veh_batch, double f_scale, const int32_t *centre_id, const double *lin_alpha, double *alpha,
-                  double *curv_error_max, double *kappa_lin_max, int32_t *status, int32_t *iters, double *sens,
-                  int32_t *grad_status, double *sens_rows, int32_t *n_rows, void *stream) {
-    PdipParams prm;                     // those of the curvature-row phase (mincurv_kappa_phase)
+// ================================================================================================
+// K2e-v -- the post-solve quantities at a given alpha (mc_mincurv_finalize_batch with dense_below, for
+// raceline_refine.CurvatureProjection.evaluate): those of the finalize stage after the assembly, with its status rules,
+// for the instances with 3 <= n < dense_below,
+// n <= n_max: status -1 (a vehicle width that is not finite, or a limit that is not finite or not > 0) or 1 (lb > ub) with
+// both maxima 0; otherwise kappa_lin_max and curv_error_max of dense_post_solve (NaN-propagating) and status 4 iff
+// kappa_lin_max > kb (1 + 1e-7) (a NaN maximum leaves 0), else 0.
+template <bool LIN>
+__global__ void __launch_bounds__(DENSE_THREADS)
+mincurv_dense_eval_kernel(int n_max, int m, int dense_below, const int32_t *__restrict__ n_pts,
+                          const double *__restrict__ reftrack, const double *__restrict__ normvec,
+                          const double *__restrict__ hin, double kappa_bound, const double *__restrict__ kappa_bound_batch,
+                          double w_veh, const double *__restrict__ w_veh_batch, const double *__restrict__ lin_alpha,
+                          const double *__restrict__ alpha, double *__restrict__ curv_error_max,
+                          double *__restrict__ kappa_lin_max, int32_t *__restrict__ status) {
+    const int b = blockIdx.x;
+    const int n = n_pts ? n_pts[b] : n_max;
+    if (!(n >= 3 && n < dense_below && n <= n_max)) return;
+    __shared__ double red[32];
+    __shared__ int s_flag;
+    extern __shared__ __align__(16) double s_dense[];
+    const double wv = w_veh_batch ? w_veh_batch[b] : w_veh;
+    const double kb = kappa_bound_batch ? kappa_bound_batch[b] : kappa_bound;
+    int st = (fabs(wv) < INFINITY && kb > 0.0 && kb < INFINITY) ? 0 : -1;
+    if (st == 0 && !dense_assemble<LIN>(s_dense, m, n, reftrack + (size_t)b * n_max * 4, normvec + (size_t)b * n_max * 2,
+                                        hin + (size_t)b * n_max, LIN ? lin_alpha + (size_t)b * n_max : nullptr, wv, 1.0,
+                                        s_flag))
+        st = 1;
+    double kmax = 0.0, emax = 0.0, viol;
+    if (st == 0) {
+        double *AL = s_dense + 2 * (size_t)m * m + (size_t)D_AL * m;
+        const double *ab = alpha + (size_t)b * n_max;
+        for (int i = threadIdx.x; i < n; i += DENSE_THREADS) AL[i] = ab[i];
+        dense_post_solve<LIN>(s_dense, m, n, kb, red, kmax, emax, viol);
+        if (kmax > kb * (1.0 + 1e-7)) st = 4;
+    }
+    if (threadIdx.x == 0) {
+        curv_error_max[b] = emax;
+        kappa_lin_max[b] = kmax;
+        status[b] = st;
+    }
+}
+
+// one CTA per instance with dense_smem_bytes(m) of shared memory, m = min(n_max, dense_below - 1)
+template <typename Kernel, typename... Args>
+static int dense_launch(Kernel kernel, const char *name, int B, int n_max, int dense_below, void *stream, Args... args) {
+    const int m = n_max < dense_below - 1 ? n_max : dense_below - 1;
+    const int smem = (int)dense_smem_bytes(m);
+    // (per launch: the attribute is per device and a process may drive several)
+    if (cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) != cudaSuccess) return check_cuda(name);
+    kernel<<<B, DENSE_THREADS, smem, (cudaStream_t)stream>>>(n_max, m, dense_below, args...);
+    return check_cuda(name);
+}
+
+// the curvature-row phase's parameters (mincurv_kappa_phase)
+static PdipParams dense_params() {
+    PdipParams prm;
     prm.max_iter = 40;
     prm.mu_rel = 1e-11;
     prm.rd_rel = 1e-8;
     prm.eta = 0.995;
     prm.dx_rel = 0.0;
     prm.lam0_rel = 1e-2;
-    const int m = n_max < dense_below - 1 ? n_max : dense_below - 1;
-    const int smem = (int)dense_smem_bytes(m);
-    auto kernel = sens ? (lin_alpha ? mincurv_dense_kernel<true, true> : mincurv_dense_kernel<false, true>)
-                       : (lin_alpha ? mincurv_dense_kernel<true, false> : mincurv_dense_kernel<false, false>);
-    // (per launch: the attribute is per device and a process may drive several)
-    if (cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) != cudaSuccess)
-        return check_cuda("mincurv_dense_kernel: cudaFuncSetAttribute");
-    kernel<<<B, DENSE_THREADS, smem, (cudaStream_t)stream>>>(n_max, m, dense_below, banded ? 1 : 0, n_pts, reftrack, normvec,
-                                                             h, kappa_bound, kappa_bound_batch, w_veh, w_veh_batch, f_scale,
-                                                             centre_id, lin_alpha, prm, alpha, curv_error_max, kappa_lin_max,
-                                                             status, iters, sens, sens_rows, n_rows, grad_status);
-    return check_cuda("mincurv_dense_kernel");
+    return prm;
+}
+
+// launched after the banded stages (banded != 0), or alone when n_max < N_MIN
+int mincurv_dense(int B, int n_max, int dense_below, bool banded, const int32_t *n_pts, const double *reftrack,
+                  const double *normvec, const double *h, double kappa_bound, const double *kappa_bound_batch, double w_veh,
+                  const double *w_veh_batch, double f_scale, const int32_t *centre_id, const double *lin_alpha, double *alpha,
+                  double *curv_error_max, double *kappa_lin_max, int32_t *status, int32_t *iters, double *sens,
+                  int32_t *grad_status, double *sens_rows, int32_t *n_rows, void *stream) {
+    auto kernel = sens ? (lin_alpha ? mincurv_dense_kernel<true, true, false> : mincurv_dense_kernel<false, true, false>)
+                       : (lin_alpha ? mincurv_dense_kernel<true, false, false> : mincurv_dense_kernel<false, false, false>);
+    return dense_launch(kernel, "mincurv_dense_kernel", B, n_max, dense_below, stream, banded ? 1 : 0, n_pts, reftrack,
+                        normvec, h, kappa_bound, kappa_bound_batch, w_veh, w_veh_batch, f_scale, centre_id, lin_alpha,
+                        dense_params(), alpha, curv_error_max, kappa_lin_max, status, iters, sens, sens_rows, n_rows,
+                        grad_status, 0.0, (const double *)nullptr, (const double *)nullptr);
+}
+
+// the projection QP of mc_mincurv_solve_batch_ex(prox_x, prox_dense_below) on the small tracks alone
+int mincurv_dense_prox(int B, int n_max, int dense_below, const int32_t *n_pts, const double *reftrack,
+                       const double *normvec, const double *h, double kappa_bound, const double *kappa_bound_batch,
+                       double w_veh, const double *w_veh_batch, double prox_mu, const double *prox_x, const double *prox_q,
+                       const double *lin_alpha, double *alpha, double *curv_error_max, double *kappa_lin_max,
+                       int32_t *status, int32_t *iters, void *stream) {
+    auto kernel = lin_alpha ? mincurv_dense_kernel<true, false, true> : mincurv_dense_kernel<false, false, true>;
+    return dense_launch(kernel, "mincurv_dense_kernel (prox)", B, n_max, dense_below, stream, 1, n_pts, reftrack, normvec, h,
+                        kappa_bound, kappa_bound_batch, w_veh, w_veh_batch, 1.0, (const int32_t *)nullptr, lin_alpha,
+                        dense_params(), alpha, curv_error_max, kappa_lin_max, status, iters, (double *)nullptr,
+                        (double *)nullptr, (int32_t *)nullptr, (int32_t *)nullptr, prox_mu, prox_x, prox_q);
+}
+
+// the post-solve evaluation of mc_mincurv_finalize_batch(dense_below) on the small tracks alone
+int mincurv_dense_eval(int B, int n_max, int dense_below, const int32_t *n_pts, const double *reftrack,
+                       const double *normvec, const double *h, double kappa_bound, const double *kappa_bound_batch,
+                       double w_veh, const double *w_veh_batch, const double *lin_alpha, const double *alpha,
+                       double *curv_error_max, double *kappa_lin_max, int32_t *status, void *stream) {
+    auto kernel = lin_alpha ? mincurv_dense_eval_kernel<true> : mincurv_dense_eval_kernel<false>;
+    return dense_launch(kernel, "mincurv_dense_eval_kernel", B, n_max, dense_below, stream, n_pts, reftrack, normvec, h,
+                        kappa_bound, kappa_bound_batch, w_veh, w_veh_batch, lin_alpha, alpha, curv_error_max,
+                        kappa_lin_max, status);
 }
 
 }  // namespace mc

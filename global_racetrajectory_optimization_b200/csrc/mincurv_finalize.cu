@@ -188,7 +188,20 @@ extern "C" {
 
 int mc_mincurv_finalize_batch(int B, int n_max, const int32_t *n_pts, const double *alpha, double kappa_bound,
                               double *curv_error_max, double *kappa_lin_max, int32_t *status, int linearised,
-                              const double *kappa_bound_batch, void *workspace, size_t workspace_bytes, void *stream) {
+                              const double *kappa_bound_batch, const double *reftrack, const double *normvec,
+                              const double *h, double w_veh, const double *w_veh_batch, const double *lin_alpha,
+                              int dense_below, void *workspace, size_t workspace_bytes, void *stream) {
+    if (dense_below != 0) {     // the small tracks alone, assembled in the dense kernel; the workspace is not read
+        if (B <= 0 || n_max <= 0) return bad("mc_mincurv_finalize_batch: B <= 0 or n_max <= 0");
+        if (dense_below < mc::N_MIN || dense_below > MC_DENSE_N_MAX + 1)
+            return bad("mc_mincurv_finalize_batch: dense_below must be 0 or in [%d, %d]", mc::N_MIN, MC_DENSE_N_MAX + 1);
+        if (!alpha || !curv_error_max || !kappa_lin_max || !status || !reftrack || !normvec || !h)
+            return bad("mc_mincurv_finalize_batch: NULL argument");
+        if ((linearised != 0) != (lin_alpha != nullptr))
+            return bad("mc_mincurv_finalize_batch: with dense_below, linearised must be 1 with lin_alpha and 0 without");
+        return mc::mincurv_dense_eval(B, n_max, dense_below, n_pts, reftrack, normvec, h, kappa_bound, kappa_bound_batch,
+                                      w_veh, w_veh_batch, lin_alpha, alpha, curv_error_max, kappa_lin_max, status, stream);
+    }
     return mc::mincurv_finalize(B, n_max, n_pts, alpha, kappa_bound, curv_error_max, kappa_lin_max, status, linearised != 0,
                                 kappa_bound_batch, workspace, workspace_bytes, stream);
 }
@@ -199,7 +212,8 @@ int mc_mincurv_solve_batch(int B, int n_max, const int32_t *n_pts, const double 
                            void *workspace, size_t workspace_bytes, void *stream) {
     return mc_mincurv_solve_batch_ex(B, n_max, n_pts, reftrack, normvec, h, kappa_bound, w_veh, w_veh_batch, MC_F_SCALE_DEFAULT,
                                      alpha, curv_error_max, kappa_lin_max, status, iters, 0.0, nullptr, nullptr, nullptr,
-                                     nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, 0, workspace, workspace_bytes, stream);
+                                     nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, 0, 0, workspace, workspace_bytes,
+                                     stream);
 }
 
 // the projection QP: setup -> prox -> pdip -> finalize -> kappa (with prox_mu) -> finalize
@@ -273,8 +287,8 @@ int mc_mincurv_solve_batch_ex(int B, int n_max, const int32_t *n_pts, const doub
                               double *alpha, double *curv_error_max, double *kappa_lin_max, int32_t *status, int32_t *iters,
                               double prox_mu, const double *prox_x, const double *prox_q, const double *lin_alpha,
                               const double *kappa_bound_batch, const int32_t *centre_id, double *sens, int32_t *grad_status,
-                              double *sens_rows, int32_t *n_rows, int dense_below, void *workspace, size_t workspace_bytes,
-                              void *stream) {
+                              double *sens_rows, int32_t *n_rows, int dense_below, int prox_dense_below, void *workspace,
+                              size_t workspace_bytes, void *stream) {
     if (!sens != !grad_status) return bad("mc_mincurv_solve_batch_ex: sens and grad_status go together");
     if (!sens_rows != !n_rows || (sens_rows && !sens))
         return bad("mc_mincurv_solve_batch_ex: sens_rows and n_rows go together, and with sens");
@@ -289,6 +303,20 @@ int mc_mincurv_solve_batch_ex(int B, int n_max, const int32_t *n_pts, const doub
         if (!reftrack || !normvec || !h || !alpha || !curv_error_max || !status)
             return bad("mc_mincurv_solve_batch_ex: NULL argument");
         if (!(f_scale > 0.0)) return bad("mc_mincurv_solve_batch_ex: f_scale must be positive");
+    }
+    if (prox_dense_below != 0) {    // the small tracks' projection QP alone; the workspace is not read
+        if (prox_dense_below < mc::N_MIN || prox_dense_below > MC_DENSE_N_MAX + 1)
+            return bad("mc_mincurv_solve_batch_ex: prox_dense_below must be 0 or in [%d, %d]", mc::N_MIN, MC_DENSE_N_MAX + 1);
+        if (!prox_x) return bad("mc_mincurv_solve_batch_ex: prox_dense_below needs prox_x");
+        if (dense_below) return bad("mc_mincurv_solve_batch_ex: dense_below does not take prox_x");
+        if (B <= 0 || n_max <= 0) return bad("mc_mincurv_solve_batch_ex: B <= 0 or n_max <= 0");
+        if (!reftrack || !normvec || !h || !alpha || !curv_error_max || !status || !prox_q)
+            return bad("mc_mincurv_solve_batch_ex: NULL argument");
+        if (!(prox_mu > 0.0) || !(prox_mu < INFINITY))
+            return bad("mc_mincurv_solve_batch_ex: prox_mu must be finite and positive");
+        return mc::mincurv_dense_prox(B, n_max, prox_dense_below, n_pts, reftrack, normvec, h, kappa_bound, kappa_bound_batch,
+                                      w_veh, w_veh_batch, prox_mu, prox_x, prox_q, lin_alpha, alpha, curv_error_max,
+                                      kappa_lin_max, status, iters, stream);
     }
     if (prox_x)
         return mincurv_prox_solve(B, n_max, n_pts, reftrack, normvec, h, kappa_bound, w_veh, w_veh_batch, f_scale, alpha,

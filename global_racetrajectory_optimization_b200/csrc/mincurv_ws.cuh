@@ -100,6 +100,21 @@ int mincurv_dense(int B, int n_max, int dense_below, bool banded, const int32_t 
                   double *curv_error_max, double *kappa_lin_max, int32_t *status, int32_t *iters, double *sens,
                   int32_t *grad_status, double *sens_rows, int32_t *n_rows, void *stream);
 
+// the dense kernels of the lap-time refinement on the same instances (mincurv_dense.cu), each writing only them: the
+// projection QP of mc_mincurv_solve_batch_ex(prox_x, prox_dense_below) and the post-solve evaluation of
+// mc_mincurv_finalize_batch(dense_below).  Not exported.
+__attribute__((visibility("hidden")))
+int mincurv_dense_prox(int B, int n_max, int dense_below, const int32_t *n_pts, const double *reftrack,
+                       const double *normvec, const double *h, double kappa_bound, const double *kappa_bound_batch,
+                       double w_veh, const double *w_veh_batch, double prox_mu, const double *prox_x, const double *prox_q,
+                       const double *lin_alpha, double *alpha, double *curv_error_max, double *kappa_lin_max,
+                       int32_t *status, int32_t *iters, void *stream);
+__attribute__((visibility("hidden")))
+int mincurv_dense_eval(int B, int n_max, int dense_below, const int32_t *n_pts, const double *reftrack,
+                       const double *normvec, const double *h, double kappa_bound, const double *kappa_bound_batch,
+                       double w_veh, const double *w_veh_batch, const double *lin_alpha, const double *alpha,
+                       double *curv_error_max, double *kappa_lin_max, int32_t *status, void *stream);
+
 // the dense adjoint (mincurv_dense.cu) of mc_mincurv_adjoint_batch on the same instances.  Before the banded adjoint runs
 // on the batch, mincurv_dense_hold marks them (grad_status ^ DENSE_HOLD) so that it leaves them alone; the dense adjoint
 // (banded = true) restores their grad_status.  Not exported.

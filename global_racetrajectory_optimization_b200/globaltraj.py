@@ -58,7 +58,10 @@ def globaltraj_batch(reftrack: torch.Tensor, opt_type: str, pars: dict, ggv=None
 
     ``small_tracks``: the 'mincurv' and 'mincurv_iqp' QPs also solve the tracks below batch.N_MIN points (the dense
     small-track solver, batch.opt_min_curv_batch); without it those get status -1.  'shortest_path' takes every size
-    anyway.  With ``refine`` a solved short track is refined as the refinement documents for tracks below N_MIN."""
+    anyway.  With ``refine`` a solved short track is refined as the refinement documents for tracks below N_MIN: in the
+    curvature metric and under a curvature limit only with the refinement's own flag as well,
+    ``refine={"small_tracks": True, "metric_length": 10.0, "kappa_bound": 0.12}`` (the dense kernels then give such a
+    track its metric and projection; without it the metric falls back to the identity step and the projection fails)."""
     if opt_type not in ("mincurv", "mincurv_iqp", "shortest_path"):
         raise IOError("Unknown optimization type!" if opt_type != "mintime" else
                       "opt_type 'mintime' (CasADi/IPOPT NLP) is outside the CUDA path")

@@ -18,6 +18,11 @@ gradient is dominated by short wavelengths, which M damps like 1 / (1 + l^4 k^4)
 With kappa_bound as well, every step is taken inside the minimum-curvature QP's feasible set P = {lb <= alpha <= ub,
 |k_ref + E alpha| <= kappa_bound} instead of the box alone: the direction is the scaled projected gradient in M, one
 projection QP per iteration on the device (CurvatureProjection, mc_mincurv_solve_batch_ex with prox arguments).
+
+With small_tracks, the closed tracks of 3 .. N_MIN - 1 points, which the banded solver does not take, get the metric,
+the projection and its evaluation from the dense one-CTA kernels (DESIGN.md section 3.14): the dense adjoint of
+mc_mincurv_adjoint_batch(dense_below), mc_mincurv_solve_batch_ex(prox_x, prox_dense_below) and
+mc_mincurv_finalize_batch(dense_below).
 """
 from __future__ import annotations
 
@@ -98,6 +103,18 @@ def box(reftrack: torch.Tensor, w_veh: Union[float, torch.Tensor], n_pts: Option
     ub = torch.where(collapsed, mid + FIX_EPS, ub)
     zero = torch.zeros_like(lb)
     return torch.where(valid, lb, zero), torch.where(valid, ub, zero), empty
+
+
+def _dense_of(small_tracks: bool, dense_below: int) -> int:
+    """The dense_below of the C-ABI: 0 (none), N_MIN with small_tracks, or the tests-only override (N_MIN ..
+    N_DENSE_MAX + 1), which lets the dense kernels take tracks the banded ones would and the two be compared."""
+    return int(dense_below) if dense_below else (_b.N_MIN if small_tracks else 0)
+
+
+def _split(n_pts, dense_below: int):
+    """(banded, dense) bool [B]: the tracks the banded kernels take (n_pts >= N_MIN, and >= dense_below) and those the
+    dense ones take (3 <= n_pts < dense_below; none for dense_below 0)."""
+    return n_pts >= max(_b.N_MIN, dense_below), (n_pts >= 3) & (n_pts < dense_below)
 
 
 def _valid(n_pts, B, n_max, dev) -> torch.Tensor:
@@ -396,17 +413,28 @@ class CurvatureMetric:
     N_MIN points, are not launched (n_pts 0, grad_status -1: not ok); with n_max < N_MIN nothing is.  h, the chunk size
     and the chunk-local centre ids are computed once here, so a call does not synchronise the stream.  timer(name) as
     LapTime's ('metric').  lin_alpha [B, n_max] (None: the centre line): H is that of the QP linearised about the line
-    reftrack + lin_alpha * normvec (DESIGN.md section 3.2)."""
+    reftrack + lin_alpha * normvec (DESIGN.md section 3.2).
 
-    def __init__(self, reftrack, normvec, n_pts, length: float, lin_alpha: Optional[torch.Tensor] = None):
+    small_tracks: the tracks of 3 .. N_MIN - 1 points get the same two solves from the dense adjoint of
+    mc_mincurv_adjoint_batch(dense_below) (DESIGN.md section 3.14), with zero row weights: grad_w_right = d v, v =
+    (H + diag(d))^-1 rhs, without band truncation.  It runs in one call after the banded ones (which see those tracks at
+    n_pts 0) on the first m = min(n_max, dense_below - 1) points of every row, so that its banded stages, which need
+    n_max >= N_MIN, are not launched (nor a workspace needed) unless dense_below > N_MIN.  Its H about lin_alpha is that
+    of the line reftrack + lin_alpha * normvec taken as the centre line: the linearised QP's E is built from that line's
+    first derivatives, the normals and h (DESIGN.md section 3.2), which is what the dense adjoint assembles for it.
+    dense_below (tests only): see refine_raceline_batch."""
+
+    def __init__(self, reftrack, normvec, n_pts, length: float, lin_alpha: Optional[torch.Tensor] = None,
+                 small_tracks: bool = False, dense_below: int = 0):
         B, n_max, _ = reftrack.shape
         dev = reftrack.device
         self.mu = float(length) ** -4
         self.n_pts = n_pts if n_pts is not None else torch.full((B,), n_max, dtype=torch.int32, device=dev)
-        self.launchable = self.n_pts >= _b.N_MIN
+        self.dense_below = _dense_of(small_tracks, dense_below)
+        self.launchable, self.dense = _split(self.n_pts, self.dense_below)
         self.timer = lambda name: contextlib.nullcontext()
         self.chunk = None
-        if n_max < _b.N_MIN:
+        if n_max < _b.N_MIN and not self.dense_below:
             return
         _, _, _, h = _b.calc_splines_batch(reftrack, n_pts=n_pts, want_coeffs=False)
         valid = _valid(n_pts, B, n_max, dev)
@@ -416,19 +444,36 @@ class CurvatureMetric:
         self.reftrack = two(torch.cat((reftrack[:, :, :2], torch.ones_like(reftrack[:, :, 2:])), dim=2))
         self.normvec, self.h = two(normvec), two(h)
         self.lin = None if lin_alpha is None else two(lin_alpha.to(torch.float64))
+        if self.dense_below:                # the dense adjoint's rows: m points, the linearisation line as the centre line
+            m = self.m = min(n_max, self.dense_below - 1)
+            line = reftrack[:, :m, :2] if lin_alpha is None else \
+                reftrack[:, :m, :2] + lin_alpha[:, :m, None].to(torch.float64) * normvec[:, :m]
+            self.d_rt = two(torch.cat((line, torch.ones_like(line)), dim=2))
+            self.d_nv, self.d_h = two(normvec[:, :m]), two(h[:, :m])
+            self.d_zero = torch.zeros((2 * B, m), dtype=torch.float64, device=dev)        # sens[1] and the row weights
+            self.d_rows = torch.zeros((2 * B,), dtype=torch.int32, device=dev)
+            self.d_schur = torch.zeros((1,), dtype=torch.float64, device=dev)
+            self.d_ws = None if m < _b.N_MIN else \
+                _b._workspace("mincurv_dense_metric", _lib.load().mc_mincurv_workspace_bytes(2 * B, m), dev)
+        if n_max < _b.N_MIN:
+            return
         chunk = _b._chunk(2 * B, _lib.load().mc_mincurv_workspace_bytes(1, n_max), dev)
         self.chunk = max(2, chunk - chunk % 2)                           # (a track's two rows share a launch)
         r = torch.arange(2 * B, dtype=torch.int32, device=dev)
         self.centre_id = r % self.chunk - r % 2                          # row 2b + 1 owned by row 2b, chunk-local
 
+    def _rows(self, take, y):
+        """n_pts [2 B] of a launch: row 2b the track's count where take[b], row 2b + 1 too if y is given; 0 elsewhere."""
+        n_dir = torch.where(take, self.n_pts, torch.zeros_like(self.n_pts))
+        return torch.stack((n_dir, n_dir if y is not None else torch.zeros_like(n_dir)), dim=1).reshape(-1)
+
     def __call__(self, g, pin, y, mask):
         B, n_max = g.shape
-        if self.chunk is None:
+        if self.chunk is None and not self.dense_below:
             return g, y, torch.zeros_like(mask)
         with self.timer("metric"):
             go = mask & self.launchable
-            n_dir = torch.where(go, self.n_pts, torch.zeros_like(self.n_pts))
-            n_pts = torch.stack((n_dir, n_dir if y is not None else torch.zeros_like(n_dir)), dim=1).reshape(2 * B)
+            n_pts = self._rows(go, y)
             gs = torch.where(n_pts > 0, 0, -1).to(torch.int32)
             sens = torch.zeros((B, 2, 2, n_max), dtype=torch.float64, device=g.device)
             sens[:, 0, 0] = torch.where(pin, self.pin[:, None], self.mu)
@@ -436,14 +481,31 @@ class CurvatureMetric:
             sens = sens.reshape(2 * B, 2, n_max)
             rhs = torch.stack((g, y if y is not None else torch.zeros_like(g)), dim=1).reshape(2 * B, n_max)
             out = torch.empty((2 * B, n_max), dtype=torch.float64, device=g.device)
-            gwl = torch.empty_like(out)
-            gwv = torch.empty((2 * B,), dtype=torch.float64, device=g.device)
-            for s in range(0, 2 * B, self.chunk):
-                e = min(2 * B, s + self.chunk)
-                _b._mincurv_launch("mc_mincurv_adjoint_batch", e - s, n_pts[s:e], self.reftrack[s:e], self.normvec[s:e],
-                                   self.h[s:e], None, 0.0, None, _b.F_SCALE, self.centre_id[s:e], sens[s:e], gs[s:e],
-                                   rhs[s:e], out[s:e], gwl[s:e], gwv[s:e], None, None, None, 0,
-                                   None if self.lin is None else self.lin[s:e], 0)
+            if self.chunk is not None:
+                gwl = torch.empty_like(out)
+                gwv = torch.empty((2 * B,), dtype=torch.float64, device=g.device)
+                for s in range(0, 2 * B, self.chunk):
+                    e = min(2 * B, s + self.chunk)
+                    _b._mincurv_launch("mc_mincurv_adjoint_batch", e - s, n_pts[s:e], self.reftrack[s:e],
+                                       self.normvec[s:e], self.h[s:e], None, 0.0, None, _b.F_SCALE, self.centre_id[s:e],
+                                       sens[s:e], gs[s:e], rhs[s:e], out[s:e], gwl[s:e], gwv[s:e], None, None, None, 0,
+                                       None if self.lin is None else self.lin[s:e], 0)
+            if self.dense_below:                # (after the banded launches; on the first m points of every row)
+                gd = mask & self.dense
+                n_d = self._rows(gd, y)
+                m = self.m
+                gs_d = torch.where(n_d > 0, 0, -1).to(torch.int32)
+                sens_d = torch.stack((sens[:, 0, :m], self.d_zero), dim=1).contiguous()
+                u_d, gwl_d = torch.empty_like(self.d_zero), torch.empty_like(self.d_zero)
+                gwv_d = torch.empty((2 * B,), dtype=torch.float64, device=g.device)
+                ws = (None, 0) if self.d_ws is None else (self.d_ws, self.d_ws.numel())
+                _b._call("mc_mincurv_adjoint_batch", 2 * B, m, n_d, self.d_rt, self.d_nv, self.d_h, 0.0, None, _b.F_SCALE,
+                         None, sens_d, gs_d, rhs[:, :m].contiguous(), u_d, gwl_d, gwv_d, self.d_zero, self.d_rows,
+                         self.d_schur, 0, None, self.dense_below, *ws)
+                took = n_d > 0
+                out = torch.where(took[:, None], torch.nn.functional.pad(u_d, (0, n_max - m)), out)
+                gs = torch.where(took, gs_d, gs)
+                go = go | gd
             out, gs = out.reshape(B, 2, n_max), gs.reshape(B, 2)
             u, w = out[:, 0], (out[:, 1] if y is not None else None)
             ok = go & (gs[:, 0] == 0) & torch.isfinite(u).all(dim=1)
@@ -467,44 +529,64 @@ class CurvatureProjection:
     max |k_ref + E x| at x (assembly and the finalize stage); evaluate(x, mask) -> (kappa_lin_max, curv_error_max) [B].
     timer(name) as LapTime's ('projection').  lin_alpha [B, n_max] (None: the centre line): P and H are those of the QP
     linearised about the line reftrack + lin_alpha * normvec (DESIGN.md section 3.2).  kappa_bound: a float or a [B]
-    tensor (a limit per track, as for batch.opt_min_curv_batch)."""
+    tensor (a limit per track, as for batch.opt_min_curv_batch).
+
+    small_tracks: the tracks of 3 .. N_MIN - 1 points are projected by mc_mincurv_solve_batch_ex(prox_x,
+    prox_dense_below) (the same QP, solved by the dense interior point on the box and the rows together; DESIGN.md
+    section 3.14) and evaluated by mc_mincurv_finalize_batch(dense_below), each in one call after the banded ones (which
+    see them at n_pts 0) that writes only them; with n_max < N_MIN those calls are the only ones, without a workspace.
+    dense_below (tests only): see refine_raceline_batch."""
 
     def __init__(self, reftrack, normvec, n_pts, w_veh, kappa_bound: Union[float, torch.Tensor], length: float,
-                 lin_alpha: Optional[torch.Tensor] = None):
+                 lin_alpha: Optional[torch.Tensor] = None, small_tracks: bool = False, dense_below: int = 0):
         B, n_max, _ = reftrack.shape
         dev = reftrack.device
         self.mu = float(length) ** -4
         self.kb, self.kb_batch = _b._kappa_bound(kappa_bound, B, dev)
         self.n_pts = n_pts if n_pts is not None else torch.full((B,), n_max, dtype=torch.int32, device=dev)
-        self.launchable = self.n_pts >= _b.N_MIN
+        self.dense_below = _dense_of(small_tracks, dense_below)
+        self.launchable, self.dense = _split(self.n_pts, self.dense_below)
         self.w_scalar, self.w_batch = _b._wveh(w_veh, B, dev)
         self.timer = lambda name: contextlib.nullcontext()
         self.chunk = None
         self.lin = None if lin_alpha is None else lin_alpha.to(torch.float64).contiguous()
-        if n_max < _b.N_MIN:
+        if n_max < _b.N_MIN and not self.dense_below:
             return
         self.reftrack, self.normvec = reftrack.contiguous(), normvec.contiguous()
         _, _, _, self.h = _b.calc_splines_batch(self.reftrack, n_pts=n_pts, want_coeffs=False)
-        self.chunk = _b._chunk(B, _lib.load().mc_mincurv_workspace_bytes(1, n_max), dev)
+        if n_max >= _b.N_MIN:
+            self.chunk = _b._chunk(B, _lib.load().mc_mincurv_workspace_bytes(1, n_max), dev)
 
     def _n(self, mask):
         return torch.where(mask & self.launchable, self.n_pts, torch.zeros_like(self.n_pts))
+
+    def _n_dense(self, mask):
+        return torch.where(mask & self.dense, self.n_pts, torch.zeros_like(self.n_pts))
+
+    def _taken(self, mask):
+        return mask & (self.launchable | self.dense)
 
     def _ws(self):
         return _b._workspace("mincurv", _lib.load().mc_mincurv_workspace_bytes(self.chunk, self.h.shape[1]), self.h.device)
 
     def __call__(self, x, q, mask):
-        if self.chunk is None:
+        if self.chunk is None and not self.dense_below:
             return x, torch.zeros_like(mask)
         with self.timer("projection"):
             B, n_max = x.shape
             out = _b._mincurv_results(B, n_max, x.device)
-            _b._launch_chunks("mc_mincurv_solve_batch_ex", B, self.chunk, self._ws(), n_max,
-                              *map(_b._rows, (self._n(mask), self.reftrack, self.normvec, self.h)), self.kb, self.w_scalar,
-                              _b._rows(self.w_batch), _b.F_SCALE, *map(_b._rows, out.values()), self.mu,
-                              _b._rows(x.contiguous()), _b._rows(q.contiguous()), _b._rows(self.lin),
-                              _b._rows(self.kb_batch), *(None,) * 5, 0)
-            ok = mask & self.launchable & (out["status"] == 0) & torch.isfinite(out["alpha"]).all(dim=1)
+            x, q = x.contiguous(), q.contiguous()
+            if self.chunk is not None:
+                _b._launch_chunks("mc_mincurv_solve_batch_ex", B, self.chunk, self._ws(), n_max,
+                                  *map(_b._rows, (self._n(mask), self.reftrack, self.normvec, self.h)), self.kb,
+                                  self.w_scalar, _b._rows(self.w_batch), _b.F_SCALE, *map(_b._rows, out.values()), self.mu,
+                                  _b._rows(x), _b._rows(q), _b._rows(self.lin), _b._rows(self.kb_batch), *(None,) * 5, 0,
+                                  0)
+            if self.dense_below:
+                _b._call("mc_mincurv_solve_batch_ex", B, n_max, self._n_dense(mask), self.reftrack, self.normvec, self.h,
+                         self.kb, self.w_scalar, self.w_batch, _b.F_SCALE, *out.values(), self.mu, x, q, self.lin,
+                         self.kb_batch, *(None,) * 5, 0, self.dense_below, None, 0)
+            ok = self._taken(mask) & (out["status"] == 0) & torch.isfinite(out["alpha"]).all(dim=1)
             return out["alpha"], ok
 
     def kappa_lin(self, x, mask):
@@ -513,21 +595,26 @@ class CurvatureProjection:
     def evaluate(self, x, mask):
         B, n_max = x.shape
         kmax = torch.full((B,), math.nan, dtype=torch.float64, device=x.device)
-        if self.chunk is None:
+        if self.chunk is None and not self.dense_below:
             return kmax, kmax.clone()
         out = _b._mincurv_results(B, n_max, x.device)
-        n = self._n(mask)
-        ws = self._ws()
         x = x.contiguous()
-        for s in range(0, B, self.chunk):              # (assembly and finalize share the chunk's workspace)
-            e = min(B, s + self.chunk)
-            _b._call("mc_mincurv_setup_batch_ex", e - s, n_max, n[s:e], self.reftrack[s:e], self.normvec[s:e], self.h[s:e],
-                     self.w_scalar, None if self.w_batch is None else self.w_batch[s:e], _b.F_SCALE, out["status"][s:e],
-                     None if self.lin is None else self.lin[s:e], ws=ws)
-            _b._call("mc_mincurv_finalize_batch", e - s, n_max, n[s:e], x[s:e], self.kb, out["curv_error_max"][s:e],
-                     out["kappa_lin_max"][s:e], out["status"][s:e], int(self.lin is not None),
-                     None if self.kb_batch is None else self.kb_batch[s:e], ws=ws)
-        ok = mask & self.launchable & (out["status"] != 1) & (out["status"] >= 0)
+        if self.chunk is not None:
+            n = self._n(mask)
+            ws = self._ws()
+            for s in range(0, B, self.chunk):              # (assembly and finalize share the chunk's workspace)
+                e = min(B, s + self.chunk)
+                _b._call("mc_mincurv_setup_batch_ex", e - s, n_max, n[s:e], self.reftrack[s:e], self.normvec[s:e],
+                         self.h[s:e], self.w_scalar, None if self.w_batch is None else self.w_batch[s:e], _b.F_SCALE,
+                         out["status"][s:e], None if self.lin is None else self.lin[s:e], ws=ws)
+                _b._call("mc_mincurv_finalize_batch", e - s, n_max, n[s:e], x[s:e], self.kb, out["curv_error_max"][s:e],
+                         out["kappa_lin_max"][s:e], out["status"][s:e], int(self.lin is not None),
+                         None if self.kb_batch is None else self.kb_batch[s:e], None, None, None, 0.0, None, None, 0, ws=ws)
+        if self.dense_below:
+            _b._call("mc_mincurv_finalize_batch", B, n_max, self._n_dense(mask), x, self.kb, out["curv_error_max"],
+                     out["kappa_lin_max"], out["status"], int(self.lin is not None), self.kb_batch, self.reftrack,
+                     self.normvec, self.h, self.w_scalar, self.w_batch, self.lin, self.dense_below, None, 0)
+        ok = self._taken(mask) & (out["status"] != 1) & (out["status"] >= 0)
         return torch.where(ok, out["kappa_lin_max"], kmax), torch.where(ok, out["curv_error_max"], kmax)
 
 
@@ -540,7 +627,8 @@ def refine_raceline_batch(reftrack: torch.Tensor, normvec: torch.Tensor, alpha0:
                           callback: Optional[Callable] = None, objective: Optional[LapTime] = None,
                           metric_length: Optional[float] = None, kappa_bound: Union[None, float, torch.Tensor] = None,
                           relinearise: int = 0, curv_error_allowed: float = CURV_ERROR_ALLOWED,
-                          vehicles: Optional[_b.Vehicles] = None, veh_id=None) -> dict:
+                          vehicles: Optional[_b.Vehicles] = None, veh_id=None, small_tracks: bool = False,
+                          _dense_below: int = 0) -> dict:
     """Lowers the quasi-steady-state lap time of every track's raceline by moving alpha inside opt_min_curv's box.
 
     reftrack [B, n_max, 4], normvec [B, n_max, 2] and alpha0 [B, n_max] (normally the opt_min_curv_batch result) as for
@@ -586,9 +674,20 @@ def refine_raceline_batch(reftrack: torch.Tensor, normvec: torch.Tensor, alpha0:
     vehicles, veh_id: a vehicle per track (batch.Vehicles; veh_id [B], None for one vehicle per track), each track
     driven at its vehicle's v_max; ggv, ax_max_machines, v_max, drag_coeff and m_veh are then None.  Tracks are refined
     independently, so a track's result is that of the track refined alone with its vehicle.  A track whose vehicle the
-    kernels refuse gets no gradient (NO_GRADIENT)."""
+    kernels refuse gets no gradient (NO_GRADIENT).
+
+    small_tracks: the closed tracks of 3 .. N_MIN - 1 points, which the banded solver does not take, get the curvature
+    metric, the projection and its evaluation from the dense one-CTA kernels (DESIGN.md section 3.14): the same
+    quantities, so such a track is refined in the metric and under kappa_bound (and re-linearised) as a longer one is,
+    instead of taking the identity step in every iteration (metric_fallbacks) or stopping at alpha0 with NO_PROJECTION.
+    Tracks of N_MIN points or more get what they get without the flag, bit for bit.  _dense_below (tests only): the dense
+    kernels take the tracks below this count instead (N_MIN .. batch.N_DENSE_MAX + 1), so that the two paths can be
+    compared on the same track."""
     if int(relinearise) != relinearise or relinearise < 0:
         raise ValueError("refine_raceline_batch: relinearise must be an integer >= 0")
+    dense_below = _dense_of(small_tracks, _dense_below)
+    if dense_below and not _b.N_MIN <= dense_below <= _b.N_DENSE_MAX + 1:
+        raise ValueError(f"refine_raceline_batch: _dense_below must be 0 or in [{_b.N_MIN}, {_b.N_DENSE_MAX + 1}]")
     if relinearise and kappa_bound is None:
         raise ValueError("refine_raceline_batch: relinearise needs kappa_bound (it re-linearises the curvature rows)")
     if not (math.isfinite(float(curv_error_allowed)) and float(curv_error_allowed) >= 0.0):
@@ -639,7 +738,7 @@ def refine_raceline_batch(reftrack: torch.Tensor, normvec: torch.Tensor, alpha0:
         fun.start(x0, active)                   # (with the projection: at the projected start, by fun's first call)
     metric = project = None
     if metric_length is not None:
-        metric = CurvatureMetric(reftrack, normvec, n_pts, float(metric_length))
+        metric = CurvatureMetric(reftrack, normvec, n_pts, float(metric_length), dense_below=dense_below)
         metric.timer = fun.timer
     if kappa_bound is not None:
         if isinstance(kappa_bound, torch.Tensor):            # (checked and on the device once, for every round)
@@ -648,7 +747,8 @@ def refine_raceline_batch(reftrack: torch.Tensor, normvec: torch.Tensor, alpha0:
             kappa_bound = _b._kappa_bound(kappa_bound, B, dev)[1]
         else:
             kappa_bound = float(kappa_bound)
-        project = CurvatureProjection(reftrack, normvec, n_pts, w_veh, kappa_bound, float(metric_length))
+        project = CurvatureProjection(reftrack, normvec, n_pts, w_veh, kappa_bound, float(metric_length),
+                                      dense_below=dense_below)
         project.timer = fun.timer
     res = spg(fun, x0, lb, ub, active, max_iters=max_iters, pg_tol=pg_tol, memory=memory, gamma=gamma,
               lam_min=lam_min, lam_max=lam_max, max_halvings=max_halvings, callback=callback, metric=metric,
@@ -669,7 +769,8 @@ def refine_raceline_batch(reftrack: torch.Tensor, normvec: torch.Tensor, alpha0:
         if relinearise:
             _rounds(out, fun, reftrack, normvec, n_pts, w_veh, lb, ub, kept, int(relinearise), float(curv_error_allowed),
                     kappa_bound, float(metric_length), dict(max_iters=max_iters, pg_tol=pg_tol, memory=memory,
-                    gamma=gamma, lam_min=lam_min, lam_max=lam_max, max_halvings=max_halvings, callback=callback))
+                    gamma=gamma, lam_min=lam_min, lam_max=lam_max, max_halvings=max_halvings, callback=callback),
+                    dense_below)
         else:
             out["rounds"] = torch.zeros_like(out["iters"])
         rl = _b.create_raceline_batch(reftrack, normvec, out["alpha"], stepsize_interp,
@@ -682,7 +783,8 @@ def refine_raceline_batch(reftrack: torch.Tensor, normvec: torch.Tensor, alpha0:
     return out
 
 
-def _rounds(out, fun, reftrack, normvec, n_pts, w_veh, lb, ub, kept, relinearise, allowed, kb, length, spg_opts):
+def _rounds(out, fun, reftrack, normvec, n_pts, w_veh, lb, ub, kept, relinearise, allowed, kb, length, spg_opts,
+            dense_below=0):
     """The outer rounds of refine_raceline_batch(relinearise=...), updating out (round 0's result) in place."""
     B = kept.shape[0]
     rounds = torch.zeros((B,), dtype=torch.int32, device=kept.device)
@@ -692,8 +794,8 @@ def _rounds(out, fun, reftrack, normvec, n_pts, w_veh, lb, ub, kept, relinearise
         if not bool(go.any()):                                              # the round's one read
             break
         x0 = out["alpha"].clone()
-        project = CurvatureProjection(reftrack, normvec, n_pts, w_veh, kb, length, lin_alpha=x0)
-        metric = CurvatureMetric(reftrack, normvec, n_pts, length, lin_alpha=x0)
+        project = CurvatureProjection(reftrack, normvec, n_pts, w_veh, kb, length, lin_alpha=x0, dense_below=dense_below)
+        metric = CurvatureMetric(reftrack, normvec, n_pts, length, lin_alpha=x0, dense_below=dense_below)
         project.timer = metric.timer = fun.timer
         res = spg(fun, x0, lb, ub, go, metric=metric, project=project, **spg_opts)
         failed = go & (res["status"] == NO_PROJECTION) & (res["evals"] == 0)

@@ -57,6 +57,11 @@ extern "C" {
  * dense adjoint of small closed tracks (dense_below).  The binding lets a call leave out the MC_OPTIONAL5 parameters alone,
  * or them and each earlier group in turn. */
 #define MC_OPTIONAL5
+/* MC_OPTIONAL6 marks parameters added after the MC_OPTIONAL5 ones, alike 0 / NULL-able: on mc_mincurv_solve_batch_ex and
+ * mc_mincurv_finalize_batch, the lap-time refinement's projection QP and post-solve evaluation of small closed tracks by
+ * the dense kernels (prox_dense_below, dense_below).  The binding lets a call leave out the MC_OPTIONAL6 parameters alone,
+ * or them and each earlier group in turn. */
+#define MC_OPTIONAL6
 
 #define MC_STATUS_OK 0
 #define MC_STATUS_TOO_NARROW 1
@@ -164,7 +169,16 @@ int mc_mincurv_solve_batch(int B, int n_max, const int32_t *n_pts,
  *                    refused): the dense iterate always carries the curvature rows.  The banded stages export as
  *                    documented at mc_mincurv_solve_batch_sens, then the dense kernel overwrites the export of its
  *                    instances with that of its final iterate (ratios, row weights, strong-row count, grad_status =
- *                    status; zeros where the status is not 0), for mc_mincurv_adjoint_batch with the same dense_below. */
+ *                    status; zeros where the status is not 0), for mc_mincurv_adjoint_batch with the same dense_below.
+ *   prox_dense_below (0: none of this): with prox_x, the projection QP above of the closed tracks with 3 <= n_pts[b] <
+ *                    prox_dense_below (N_MIN <= prox_dense_below <= MC_DENSE_N_MAX + 1) by the dense kernel (DESIGN.md
+ *                    section 3.14), for raceline_refine.CurvatureProjection(small_tracks=True): Hessian H + prox_mu I and
+ *                    linear term c in the dense interior point on the box and the rows together; lin_alpha and
+ *                    kappa_bound_batch as above.  Only those instances are written (every other instance's outputs are
+ *                    left untouched, so that a mixed batch takes the banded call, with them at n_pts 0, and then this one)
+ *                    and the workspace is not read (NULL and 0 bytes are accepted), any n_max >= 1.  Statuses -1, 1, 2, 3
+ *                    as above, 4 when the rows are still violated at the end (whatever ended the iteration); kappa_lin_max
+ *                    and curv_error_max of the result.  dense_below must be 0 (it stays refused with prox_x). */
 int mc_mincurv_solve_batch_ex(int B, int n_max, const int32_t *n_pts,
                               const double *reftrack, const double *normvec, const double *h,
                               double kappa_bound, double w_veh, const double *w_veh_batch, double f_scale,
@@ -175,7 +189,7 @@ int mc_mincurv_solve_batch_ex(int B, int n_max, const int32_t *n_pts,
                               MC_OPTIONAL3 const double *kappa_bound_batch, MC_OPTIONAL3 const int32_t *centre_id,
                               MC_OPTIONAL3 double *sens, MC_OPTIONAL3 int32_t *grad_status, MC_OPTIONAL3 double *sens_rows,
                               MC_OPTIONAL3 int32_t *n_rows,
-                              MC_OPTIONAL4 int dense_below,
+                              MC_OPTIONAL4 int dense_below, MC_OPTIONAL6 int prox_dense_below,
                               void *workspace, size_t workspace_bytes, void *stream);
 
 /* the same for batches in which several instances share a centreline (x, y, normal vectors, h and n_pts identical, only
@@ -211,7 +225,14 @@ int mc_mincurv_setup_batch_shared(int B, int n_max, const int32_t *n_pts, const 
  * status (with kappa_bound_batch a limit that is not finite or not > 0 first turns a status >= 0 into -1); otherwise
  * kappa_lin_max = max |k_ref + E alpha| and curv_error_max = max |kappa_sol_lin - kappa_orig_lin| over the n points, each
  * NaN if any of its terms is NaN (as tph's np.amax; a NaN or infinite alpha makes both NaN), and status 0 becomes 4
- * iff kappa_lin_max > kappa_bound * (1 + 1e-7) in float64 (a NaN maximum leaves 0); statuses 2, 3 and 4 are kept. */
+ * iff kappa_lin_max > kappa_bound * (1 + 1e-7) in float64 (a NaN maximum leaves 0); statuses 2, 3 and 4 are kept.
+ * mc_mincurv_finalize_batch with dense_below (0: the above): the same quantities of the closed tracks with 3 <= n_pts[b] <
+ * dense_below (N_MIN <= dense_below <= MC_DENSE_N_MAX + 1) at alpha, for raceline_refine.CurvatureProjection.evaluate:
+ * each instance's QP is assembled by the dense kernel from reftrack, normvec, h, w_veh / w_veh_batch and lin_alpha (its
+ * linearisation point or NULL; linearised must be 1 with it, 0 without), and status is written, not read: -1 (a vehicle
+ * width that is not finite, or a limit that is not finite or not > 0) or 1 (lb > ub), both maxima 0; otherwise the maxima
+ * and 4 or 0 by the rule above.  Only those instances are written, the workspace is not read (NULL and 0 bytes are
+ * accepted), any n_max >= 1. */
 int mc_mincurv_setup_batch(int B, int n_max, const int32_t *n_pts, const double *reftrack, const double *normvec,
                            const double *h, double w_veh, const double *w_veh_batch, int32_t *status,
                            void *workspace, size_t workspace_bytes, void *stream);
@@ -225,6 +246,9 @@ int mc_mincurv_finalize_batch(int B, int n_max, const int32_t *n_pts, const doub
                               double *curv_error_max, double *kappa_lin_max, int32_t *status,
                               MC_OPTIONAL2 int linearised,
                               MC_OPTIONAL3 const double *kappa_bound_batch,
+                              MC_OPTIONAL6 const double *reftrack, MC_OPTIONAL6 const double *normvec,
+                              MC_OPTIONAL6 const double *h, MC_OPTIONAL6 double w_veh, MC_OPTIONAL6 const double *w_veh_batch,
+                              MC_OPTIONAL6 const double *lin_alpha, MC_OPTIONAL6 int dense_below,
                               void *workspace, size_t workspace_bytes, void *stream);
 
 /* Width sensitivities of this QP: alpha differentiated with respect to w_tr_right, w_tr_left and w_veh by one more
